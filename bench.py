@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- ns/day of the B200-native OpenMM hot path (BASELINE.json metric) + roofline of the dominant kernel.
+"""bench.py -- ns/day of the CUDA-native OpenMM hot path (BASELINE.json metric) + roofline of the dominant kernel.
 
     python bench.py --gpus N --steps K --warmup W            # our arm (CUDA, through the C-ABI)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's own CPU platform on the host cores
@@ -11,6 +11,9 @@ fused Langevin+SETTLE/SHAKE update.  Default workload `dhfr` = BASELINE.json con
 tools/make_benchmark_systems.py builds with the reference's own forcefield.py.  Others: `apoa1` (92,224 atoms, 88^3),
 `water24k` (S1 of SURVEY.md 8d), `water1m` (S4).
 N > 1 (torchrun, one process per GPU): the SAME system on N GPUs by force decomposition -> "scaling": "strong".
+--dump-outputs DIR: after the timed steps, what a caller of the step path receives (positions and velocities, float64
+[atoms, 3]) as DIR/<name>.npy; the inputs are fixed by the workload and seed, so that two builds can be compared output
+for output.
 """
 import argparse
 import json
@@ -47,7 +50,7 @@ def load_workload(name):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, index):
@@ -83,7 +86,19 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p))["hbm_gbs"], "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
+
+
+def dump_outputs(out_dir, out, max_bytes=64_000_000 - 4096):
+    """`out` = {name: float64 [atoms, 3]} after the last timed step; above `max_bytes` in all (64 MB less room for the
+    .npy headers), the rows of a fixed, seeded sample of the atoms, in atom order."""
+    os.makedirs(out_dir, exist_ok=True)
+    n = len(next(iter(out.values())))
+    if len(out)*n*3*8 > max_bytes:
+        idx = np.sort(np.random.default_rng(0).choice(n, max_bytes//(len(out)*3*8), replace=False))
+        out = {k: v[idx] for k, v in out.items()}
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def run_reference(args, rank, world):
@@ -130,6 +145,7 @@ def main():
     ap.add_argument("--ref-md-steps", type=int, default=10)
     ap.add_argument("--dt", type=float, default=0.002)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the state the timed steps computed as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -144,7 +160,7 @@ def main():
     from openmm_b200 import systems, Engine, _lib
     import ctypes as C
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 hot path has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device; the CUDA hot path has no CPU fallback")
     torch.cuda.set_device(local)
     comm = None
     if world > 1:
@@ -180,7 +196,7 @@ def main():
     eng = Engine(d, device=local, comm=comm)
     eng.set_integrator(systems.INT_LANGEVIN, args.dt, 300.0, 1.0, 7, 1e-5)
     stream = torch.cuda.ExternalStream(eng.stream(), device=local)
-    flush = torch.empty(256*1024*1024, dtype=torch.uint8, device="cuda")      # > 126 MB L2
+    flush = torch.empty(256*1024*1024, dtype=torch.uint8, device="cuda")      # > 50 MB L2 of an H100
 
     def barrier():
         torch.cuda.synchronize()
@@ -211,6 +227,11 @@ def main():
     ms = ev0.elapsed_time(ev1)
     sampler.stop_flag = True
     st1 = eng.stats()
+    if args.dump_outputs:
+        # collective in the multi-GPU engine (the velocities come from their owners): every rank reads, rank 0 writes
+        out = {"positions": eng.get_positions(), "velocities": eng.get_velocities()}
+        if rank == 0:
+            dump_outputs(args.dump_outputs, out)
     if world > 1:
         t = torch.tensor([ms])
         dist.all_reduce(t, op=dist.ReduceOp.MAX)

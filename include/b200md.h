@@ -1,4 +1,4 @@
-/* b200md.h -- the C-ABI of the B200-native OpenMM hot path (libb200md.so).
+/* b200md.h -- the C-ABI of the CUDA-native (sm_90a) OpenMM hot path (libb200md.so).
  *
  * This is the drop-in boundary.  Plain pointers and sizes only: no C++ types, no torch types.  Every entry
  * point replaces one method of the reference's abstract kernel interfaces (olla/include/openmm/kernels.h in

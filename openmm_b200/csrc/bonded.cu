@@ -1,5 +1,5 @@
 // bonded.cu -- harmonic bonds, harmonic angles, periodic torsions, 1-4 exceptions and the Ewald exclusion
-// correction in ONE launch (sm_100a).  Double precision arithmetic on fp32 positions: these terms are a few
+// correction in ONE launch (sm_90a).  Double precision arithmetic on fp32 positions: these terms are a few
 // thousand work items, far below any roofline, and double removes them from the 1e-4 parity budget.
 //
 // Restates ReferenceHarmonicBondIxn / ReferenceAngleBondIxn / ReferenceProperDihedralBond::calculateBondIxn,

@@ -1,4 +1,4 @@
-// comm.cu -- the peer-memory data plane of the multi-GPU engine (sm_100a, NVLink 5 / NVSwitch).
+// comm.cu -- the peer-memory data plane of the multi-GPU engine (sm_90a, NVLink / NVSwitch).
 //
 // What the reference does here: CudaParallelKernels.cpp:110-121, 177-252 -- every device computes a share of the forces
 // on ALL atoms, the host copies the partial force buffers to device 0 through pinned memory, device 0 sums and integrates

@@ -1,4 +1,4 @@
-// constraints.cu -- general constraint networks (CCMA) on the device, one CTA per connected component (sm_100a).
+// constraints.cu -- general constraint networks (CCMA) on the device, one CTA per connected component (sm_90a).
 //
 // Restates ReferenceCCMAAlgorithm::applyConstraints (ReferenceCCMAAlgorithm.cpp:235-316: positions and velocities) for the
 // constraints that are neither a rigid 3-atom molecule (SETTLE) nor an X-H_n cluster (SHAKE, both inside k_integrate):

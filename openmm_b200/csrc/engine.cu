@@ -160,7 +160,7 @@ static void check_flags(b200md_ctx* c);
 static void sync_velocities(b200md_ctx* c);
 static void sync_positions(b200md_ctx* c);
 
-extern "C" const char* b200md_version(void) { return "b200md 0.2 (sm_100a)"; }
+extern "C" const char* b200md_version(void) { return "b200md 0.2 (sm_90a)"; }
 extern "C" const char* b200md_last_error(const b200md_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
 
 extern "C" int b200md_create(b200md_ctx** out, int device, int natoms) {

@@ -1,4 +1,4 @@
-// fft.cu -- the bespoke grid-resident 3-D FFT for PME (sm_100a), fused with the reciprocal-space convolution.
+// fft.cu -- the bespoke grid-resident 3-D FFT for PME (sm_90a), fused with the reciprocal-space convolution.
 //
 // Replaces cufftExecR2C / cufftExecC2R + reciprocalConvolution + gridEvaluateEnergy of the reference CUDA
 // platform (CudaKernels.cpp:826-829,1228-1255; pme.cc:390-505); numerically it restates fftpack_exec_3d +

@@ -1,4 +1,4 @@
-// integrate.cu -- fused integrate + constrain step (sm_100a): one thread per integration unit
+// integrate.cu -- fused integrate + constrain step (sm_90a): one thread per integration unit
 // (a rigid 3-atom molecule, an X-H_n SHAKE cluster or a free atom), everything in registers, ONE launch.
 //
 // Restates ReferenceStochasticDynamics::update (ReferenceStochasticDynamics.cpp:89-194),
@@ -389,7 +389,7 @@ void launch_cm_prime(const NbDev& nb, const IntegDev& integ, const CommDev& cd, 
 }
 
 void launch_integrate(const NbDev& nb, const UnitDev& units, const IntegDev& integ, const CommDev& cd, cudaStream_t s) {
-    // 64-thread blocks: at DHFR size (8k units) 128-thread blocks fill only 65 of the 148 SMs
+    // 64-thread blocks: at DHFR size (8k units) 128-thread blocks fill only 65 of the 132 SMs of an H100
     const int n = cd.world > 1 ? cd.unitLo[cd.rank + 1] - cd.unitLo[cd.rank] : units.nunits;
     const int grid = std::max(1, (n + 63)/64);
     if (integ.kind == B200MD_INT_VERLET) k_integrate<B200MD_INT_VERLET><<<grid, 64, 0, s>>>(nb, units, integ, cd);

@@ -1,4 +1,4 @@
-// nonbonded.cu -- neighbour-list construction and the direct-space 32x32 tile kernel (sm_100a).
+// nonbonded.cu -- neighbour-list construction and the direct-space 32x32 tile kernel (sm_90a).
 //
 // Replaces (reference, platforms/cuda): findBlockBounds/sortBoxData/findBlocksWithInteractions
 // (findInteractingBlocks.cu:7,54,180), CudaSort (sort.cu), the host-side Hilbert reorder
@@ -757,7 +757,7 @@ void launch_list_build(const NbDev& nb, cudaStream_t s, int mode) {
     // kernels only (this sequence is also the body of a CUDA-graph conditional node); each returns immediately unless
     // its flag (counters[CT_REBUILD] / counters[CT_SOFT]) is set
     const int merged = list_build_merged() ? 1 : 0;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (merged) {
@@ -791,8 +791,8 @@ void launch_list_build(const NbDev& nb, cudaStream_t s, int mode) {
 //           E    = qi qj erfc(ar)/r + sw*eps (s^12 - s^6)
 //   cutoff: reaction field (ReferenceLJCoulombIxn.cpp:559-575): dEdR = qi qj (1/r^3 - 2 krf) ..., E = qi qj (1/r + krf r^2 - crf)
 //
-// B200 notes (profiles/r01_k_pair_v1_details.csv): the v1 loop was bound by the XU pipe (MUFU + FRND: rsqrt, ex2,
-// rcp and three rintf of the per-pair minimum image = 6 XU ops per pair slot, ~5 clk/SM each).  v2:
+// The v1 loop was bound by the XU pipe (MUFU + FRND: rsqrt, ex2, rcp and three rintf of the per-pair minimum image =
+// 6 XU ops per pair slot).  v2:
 //  * SHIFT mode: when every block satisfies halfExtent <= L/2 - cutoff - padding (checked on the device at list
 //    build) the j atoms of a tile are moved ONCE to the periodic image nearest the i-block centre, and the per-pair
 //    minimum image (3 FRND) disappears; pairs whose true image would differ are beyond the cutoff either way.
@@ -1019,7 +1019,9 @@ __device__ __forceinline__ void pair_tiles(const NbDev& nb, const ListDev& L, fl
                 else {
                     const float r = r2*y;
                     const float ar = nb.alpha*r;
-                    const float ex = __expf(-ar*ar);
+                    // accurate expf, not __expf: the ex2.approx form loses ulps with |ar^2| and pushed ApoA1 atoms whose net
+                    // force is a small difference of large direct and reciprocal parts over 1e-4 (no measurable cost here)
+                    const float ex = expf(-ar*ar);
                     // erfc: Abramowitz-Stegun 7.1.26, |err| < 1.5e-7 (same form as coulombLennardJones.cc:15-20)
                     const float tt = rcp_approx(fmaf(0.3275911f, ar, 1.0f));
                     const float erfcAr = (0.254829592f+(-0.284496736f+(1.421413741f+(-1.453152027f+1.061405429f*tt)*tt)*tt)*tt)*tt*ex;
@@ -1156,7 +1158,7 @@ __global__ void __launch_bounds__(256, ENERGY ? 2 : 4) k_pair(NbDev nb) {
 
 template <bool ENERGY>
 static void launch_pair_m(const NbDev& nb, cudaStream_t s) {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     // M waves of short-lived CTAs instead of one wave of persistent ones: SM slots are handed back while the kernel runs
@@ -1186,7 +1188,7 @@ __global__ void k_smid_probe(unsigned long long* bitmap) {
 int choose_pme_sms(int reserve, unsigned long long mask[4]) {
     mask[0] = mask[1] = mask[2] = mask[3] = 0ull;
     if (reserve <= 0) return 0;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     unsigned long long* d = nullptr;
@@ -1240,6 +1242,9 @@ __global__ void k_count_pairs(NbDev nb) {
 }
 
 void launch_count_pairs(const NbDev& nb, cudaStream_t s) {
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     cudaMemsetAsync(&nb.counters[CT_PAIRS], 0, sizeof(int), s);
-    k_count_pairs<<<148*4, 256, 0, s>>>(nb);
+    k_count_pairs<<<sms*4, 256, 0, s>>>(nb);
 }

@@ -1,4 +1,4 @@
-// pme.cu -- PME charge spreading, influence function and force interpolation (sm_100a).
+// pme.cu -- PME charge spreading, influence function and force interpolation (sm_90a).
 //
 // Restates pme_update_grid_index_and_fraction / pme_update_bsplines / pme_grid_spread_charge /
 // pme_grid_interpolate_force / pme_calculate_bsplines_moduli (ReferencePME.cpp:98-193, 206-405, 617-713);

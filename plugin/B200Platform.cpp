@@ -1,4 +1,4 @@
-// B200Platform.cpp -- libOpenMMB200.so: the OpenMM Platform plugin for the B200-native hot path.
+// B200Platform.cpp -- libOpenMMB200.so: the OpenMM Platform plugin for the CUDA-native (sm_90a) hot path.
 //
 // A thin C++ adapter: every KernelImpl below forwards one abstract kernel interface of the reference
 // (olla/include/openmm/kernels.h) to the C-ABI of libb200md.so (include/b200md.h), where all the CUDA lives.

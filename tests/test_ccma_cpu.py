@@ -1,6 +1,6 @@
 """CPU tests of the general-constraint (CCMA) path, no GPU needed:
- * oracle/md_oracle.c:orc_ccma restates ReferenceCCMAAlgorithm::applyConstraints and is pinned against the LIVE Reference platform
-   (Context::applyConstraints on a perturbed chain and on the real DHFR protein under constraints=AllBonds);
+ * oracle/md_oracle.c:orc_ccma restates ReferenceCCMAAlgorithm::applyConstraints and is pinned against the Reference platform
+   (Context::applyConstraints on the real DHFR protein under constraints=AllBonds, stored in tests/golden/reference_platform.npz);
  * the matrix the ENGINE builds on the host (b200md_ccma_setup_probe: coupling matrix as the reference builds it, inverse
    approximated from the constraints within three bonds) makes that iteration converge as fast as an exact inverse would need
    to, and to the same positions as the reference's own sparse-QR matrix."""
@@ -8,7 +8,7 @@ import ctypes as C
 import os
 import numpy as np
 import pytest
-from conftest import ROOT
+from conftest import ROOT, GOLDEN
 from openmm_b200 import systems, _lib
 from oracle import port
 
@@ -72,9 +72,6 @@ def test_chain_classification_components_and_convergence():
 
 @pytest.mark.parametrize("vel", [False, True])
 def test_dhfr_allbonds_matrix_and_iteration_against_the_live_reference(vel):
-    from oracle import omm
-    if not omm.available():
-        pytest.skip("oracle/_ref not built")
     d = systems.SystemDesc.load(os.path.join(ROOT, "data", "dhfr.npz"))
     have = set((min(i, j), max(i, j)) for i, j in zip(d.con_i, d.con_j))
     ci, cj, cd = list(d.con_i), list(d.con_j), list(d.con_d)
@@ -87,11 +84,13 @@ def test_dhfr_allbonds_matrix_and_iteration_against_the_live_reference(vel):
     assert ncomp >= 1 and 2000 < nprot < 3000                      # the protein's bonds; the waters stay with SETTLE
     nnz_per_row = (row[1:] - row[:-1])
     assert nnz_per_row.min() >= 1 and nnz_per_row.mean() < 20     # sparse: entries below the reference's 0.02 cut-off are dropped
-    # the Reference platform projects the PDB structure onto the constraints (ReferenceConstraints -> SETTLE + CCMA with ITS matrix)
-    sim = omm.Simulation(d, "Reference", integrator=(systems.INT_VERLET, 0, 0, 0.001), constraint_tol=1e-7, pme=d.pme_parameters())
+    # the Reference platform projects the PDB structure onto the constraints (ReferenceConstraints -> SETTLE + CCMA with ITS
+    # matrix, tolerance 1e-7); stored for the protein atoms as the displacement from the input positions
     x0 = np.array(d.positions, dtype=np.float64)
-    sim.apply_constraints(1e-7)
-    xref = sim.state(positions=True)["positions"]
+    dx = np.load(os.path.join(GOLDEN, "reference_platform.npz"))["ccma_cpu:dx"]
+    xref = x0.copy()
+    xref[:len(dx)] += dx
+    assert max(np.array(ci)[order].max(), np.array(cj)[order].max()) < len(dx)
     if vel:
         # velocities: project random velocities with the restated iteration and check the constraint velocities vanish
         v = np.random.default_rng(2).standard_normal(x0.shape)

@@ -85,12 +85,10 @@ def test_system_desc_roundtrip(tmp_path):
     assert e.natoms == d.natoms and np.array_equal(e.positions, d.positions) and e.method == d.method and np.array_equal(e.con_i, d.con_i)
 
 
-# ---- the restatement against the LIVE reference (oracle/_ref = the unmodified Reference platform built here) ----
-def _live():
-    from oracle import omm
-    if not omm.available():
-        pytest.skip("oracle/_ref is not built (needs /root/reference: run __graft_entry__.build() where it exists)")
-    return omm
+# ---- the restatement against the unmodified Reference platform: what it computed for these inputs, stored by
+# tests/golden/make_golden.py in reference_platform.npz ----
+def _ref():
+    return np.load(os.path.join(GOLDEN, "reference_platform.npz"))
 
 
 def _cases():
@@ -107,11 +105,11 @@ def _cases():
 def test_port_matches_live_reference_platform(name):
     """Every branch of the path the GPU parity tests lean on the port for: PME in a triclinic cell, reaction field, the
     switching function, no cutoff, bonded terms + exceptions + exclusion correction (ReferenceKernels.cpp:967-1014)."""
-    omm = _live()
+    ref = _ref()
     d = dict(_cases())[name]
     pme = d.pme_parameters() if d.method == systems.NB_PME else None
     f, e, _ = port.forces_energy(d, pme=pme)
-    fr, er = omm.Simulation(d, "Reference", pme=pme).forces_energy()
+    fr, er = ref["port_%s:f" % name], float(ref["port_%s:e" % name])
     assert relative_force_error(f, fr) < 1e-8
     assert abs(e - er) < 1e-8*max(1.0, abs(er))
 
@@ -121,18 +119,17 @@ def test_port_integrator_matches_live_reference(kind, friction):
     """Deterministic updates (Verlet; Langevin and LangevinMiddle at zero temperature, with and without friction) with
     SETTLE on positions and -- LangevinMiddle -- on velocities, 5 steps (ReferenceVerletDynamics.cpp,
     ReferenceStochasticDynamics.cpp:89-194, ReferenceLangevinMiddleDynamics.cpp:54-127, ReferenceSETTLEAlgorithm.cpp)."""
-    omm = _live()
+    ref = _ref()
     d = systems.water_box(3, cutoff=0.45).rounded()
     pme = d.pme_parameters()
-    sim = omm.Simulation(d, "Reference", integrator=(kind, 0.0, friction, 0.002), pme=pme, constraint_tol=1e-10)
     x = d.positions.copy()
     v = np.zeros_like(x)
     cl = port.settle_clusters(d)
     for _ in range(5):
         f, _, _ = port.forces_energy(d, positions=x, pme=pme)
         port.step(d, kind, 0.002, friction, x, v, f, cl)
-    sim.step(5)
-    st = sim.state(positions=True, velocities=True)
+    key = "port_integrate%d_%g:" % (kind, friction)
+    st = {"positions": ref[key + "x"], "velocities": ref[key + "v"]}
     # measured 4e-9 nm after 5 steps (the port integrates from its own forces, which differ from the reference's at 1e-9)
     assert np.abs(x - st["positions"]).max() < 1e-7
     assert np.abs(v - st["velocities"]).max() < 1e-4
@@ -161,7 +158,7 @@ def test_port_parameter_offsets_match_live_reference():
     ReferenceKernels.cpp:1077-1121): at the default values and after Context::setParameter, PME with bonded terms.  The two
     exception offsets sit on water O-H exclusions whose base parameters are zero (they must become live 1-4 terms,
     :873-895); the dispersion correction keeps the DEFAULT values (NonbondedForceImpl.cpp:241-258)."""
-    omm = _live()
+    ref = _ref()
     d = systems.water_box(3, cutoff=0.45, rigid=False).rounded()
     pme = d.pme_parameters()
     glob = {"lambda_q": 0.25, "lambda_lj": 1.0}
@@ -169,15 +166,13 @@ def test_port_parameter_offsets_match_live_reference():
              ("lambda_q", 6, 0.05, 0.0, 0.0)]
     e_off = [("lambda_lj", 0, 0.04, 0.2, 0.3), ("lambda_q", 4, -0.02, 0.15, 0.1)]
     assert d.exc_qq[0] == 0 and d.exc_eps[0] == 0
-    sim = omm.Simulation(d, "Reference", pme=pme, nb_globals=glob, particle_offsets=p_off, exception_offsets=e_off)
     disp = port.with_parameter_offsets(d, glob, p_off, e_off).dispersion_coefficient()
     seen = []
-    for values in (glob, {"lambda_q": -0.5, "lambda_lj": 0.4}):
-        for name, value in values.items():
-            sim.set_parameter(name, value)
+    for k, values in enumerate((glob, {"lambda_q": -0.5, "lambda_lj": 0.4})):
+        # the Reference platform after Context::setParameter of each value in turn
         eff = port.with_parameter_offsets(d, values, p_off, e_off)
         f, e, parts = port.forces_energy(eff, pme=pme, dispersion_coefficient=disp)
-        fr, er = sim.forces_energy()
+        fr, er = ref["port_offsets%d:f" % k], float(ref["port_offsets%d:e" % k])
         assert relative_force_error(f, fr) < 1e-8
         assert abs(e - er) < 1e-8*max(1.0, abs(er))
         seen.append(e)
@@ -246,18 +241,18 @@ def test_port_periodic_bonded_terms_match_live_reference():
     """Force::usesPeriodicBoundaryConditions on HarmonicBondForce / HarmonicAngleForce / PeriodicTorsionForce: the minimum
     image on every displacement (ReferenceHarmonicBondIxn.cpp:86-89, ReferenceAngleBondIxn.cpp:121-128,
     ReferenceProperDihedralBond.cpp:91-100), in a triclinic cell, with atoms of one molecule on different sides of a face."""
-    omm = _live()
+    ref = _ref()
     d = _wrapped_chains()
     pme = d.pme_parameters()
     # the molecules really are split: some bonded neighbours are more than half a cell apart before the minimum image
     raw = np.linalg.norm(d.positions[d.bond_i] - d.positions[d.bond_j], axis=1)
     assert (raw > 1.0).sum() >= 3
     f, e, parts = port.forces_energy(d, pme=pme, bonded_periodic=True)
-    fr, er = omm.Simulation(d, "Reference", pme=pme, bonded_periodic=True).forces_energy()
+    fr, er = ref["port_bonded_periodic:f"], float(ref["port_bonded_periodic:e"])
     assert relative_force_error(f, fr) < 1e-8
     assert abs(e - er) < 1e-8*max(1.0, abs(er))
     # and the flag matters: without it both sides agree with each other on a very different answer
     f0, e0, _ = port.forces_energy(d, pme=pme)
-    fr0, er0 = omm.Simulation(d, "Reference", pme=pme).forces_energy()
+    fr0, er0 = ref["port_bonded_nonperiodic:f"], float(ref["port_bonded_nonperiodic:e"])
     assert relative_force_error(f0, fr0) < 1e-8 and abs(e0 - er0) < 1e-8*abs(er0)
     assert e0 > 10*e

@@ -2,7 +2,7 @@
 // Forks one process per GPU (like torchrun does), exchanges cudaIpcMemHandles over pipes, maps every peer's window and
 // measures (a) a flag ping-pong between GPU 0 and GPU 1 driven entirely from kernels (store to peer + spin on local),
 // (b) the bandwidth of a kernel that copies a buffer into peer memory with plain coalesced stores.
-//   nvcc -O2 -gencode arch=compute_100a,code=sm_100a -o tools/ipc_probe tools/ipc_probe.cu && tools/ipc_probe 2
+//   nvcc -O2 -gencode arch=compute_90a,code=sm_90a -o tools/ipc_probe tools/ipc_probe.cu && tools/ipc_probe 2
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdlib>
@@ -109,11 +109,11 @@ int main(int argc, char** argv) {
         CK(cudaMalloc(&src, 32u << 20));
         CK(cudaMemset(src, rank + 1, 32u << 20));
         const int to = (rank + 1) % world;
-        for (int rep = 0; rep < 3; rep++) k_copy<<<148*4, 256>>>((const uint4*) src, (uint4*) (peer[to] + (16u << 20)), n);
+        for (int rep = 0; rep < 3; rep++) k_copy<<<132*4, 256>>>((const uint4*) src, (uint4*) (peer[to] + (16u << 20)), n);
         CK(cudaDeviceSynchronize());
         barrier();
         CK(cudaEventRecord(e0));
-        for (int rep = 0; rep < 10; rep++) k_copy<<<148*4, 256>>>((const uint4*) src, (uint4*) (peer[to] + (16u << 20)), n);
+        for (int rep = 0; rep < 10; rep++) k_copy<<<132*4, 256>>>((const uint4*) src, (uint4*) (peer[to] + (16u << 20)), n);
         CK(cudaEventRecord(e1));
         CK(cudaEventSynchronize(e1));
         float ms = 0; CK(cudaEventElapsedTime(&ms, e0, e1));

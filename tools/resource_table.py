@@ -3,7 +3,7 @@
 GPU needed): registers, shared memory, local-memory stack and spills (`--dump-resource-usage`), plus the count of the SASS
 mnemonics that prove a mechanism (UBLKCP = cp.async.bulk, SYNCS = mbarrier, ATOMG/RED = global atomics, MEMBAR.SYS = system
 fence, LDG.*.SYS / STG.*.SYS = system-scope acquire/release used by the peer-memory flags).
-    python tools/resource_table.py > profiles/r02_kernel_resources.md
+    python tools/resource_table.py > profiles/kernel_resources.md
 """
 import os
 import re
@@ -62,7 +62,7 @@ def main():
                 if re.search(p, line):
                     counts[cur][k] += 1
     names = demangle(sorted(rows))
-    print("# Static kernel resources of openmm_b200/libb200md.so (sm_100a cubin, cuobjdump; no GPU involved)\n")
+    print("# Static kernel resources of openmm_b200/libb200md.so (sm_90a cubin, cuobjdump; no GPU involved)\n")
     print("`python tools/resource_table.py`.  REG = registers per thread, SHARED = static shared memory (bytes), STACK = local-memory frame (bytes; 0 = no spills, no")
     print("local arrays), then counts of SASS instructions: UBLKCP = `cp.async.bulk` (TMA engine), SYNCS = mbarrier, ATOM/RED = global atomics, MEMBAR.SYS = system")
     print("fence, LD.SYS / ST.SYS = system-scope acquire loads / release stores of the peer-memory flags, DFMA / FFMA = double / single FMAs.\n")
@@ -80,12 +80,12 @@ Notes.
 * `k_pair<false, M>` (forces only; M = 0 no cutoff, 2 reaction field, 4 PME) is capped at 64 registers by `__launch_bounds__(256, 4)`: four CTAs per SM hide the
   latency of the shuffle-bound inner loop (four versus three resident CTAs was measured in round 1; the close-pair path would otherwise take 80).  The price is
   the 16..32-byte frame above (`-Xptxas -v`: 132 B of spill stores / 244 B of spill loads, static, for `<false, 4>`); the energy instantiations run at 2 CTAs/SM
-  and do not spill.  SHARED includes the 1 KiB the driver reserves per CTA on sm_100.
+  and do not spill.  SHARED includes the 1 KiB the driver reserves per CTA on sm_90.
 * `k_grid_push_tma`, `k_pos_push`, `k_force_push_tma` are the only kernels with UBLKCP / SYNCS: bulk copies into PEER memory through the TMA engine, completion
   on an mbarrier (DESIGN.md section 5).  There is no tcgen05 anywhere: nothing on this path is GEMM-shaped (DESIGN.md section 4).
 * System-scope traffic (MEMBAR.SYS, LD.SYS, ST.SYS) appears exactly in the kernels that talk to other GPUs; with one rank those branches are not taken.
 * DFMA in `k_pair<*, 4>` is the close-pair path (pairs under 0.36 nm, evaluated in double); in `k_pme_spread` / `k_pme_gather` it is the
-  double B-spline weights and sums (profiles/r02_parity_probe.md says why they are there).""")
+  double B-spline weights and sums (DESIGN.md section 4 says why they are there).""")
 
 
 if __name__ == "__main__":
