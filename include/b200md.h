@@ -124,6 +124,21 @@ int b200md_update_bonded_params(b200md_ctx* ctx, int kind, int n, const double* 
  * UpdateStateDataKernel (kernels.h:125-214).                                                         */
 int b200md_set_box(b200md_ctx* ctx, const double a[3], const double b[3], const double c[3]);
 int b200md_get_box(b200md_ctx* ctx, double a[3], double b[3], double c[3]);
+
+/* ---------------------------------------------------------------------------------------------------
+ * ApplyMonteCarloBarostatKernel (kernels.h:1425-1459), for MonteCarloBarostat and MonteCarloAnisotropicBarostat.  The host
+ * half (MonteCarloBarostatImpl) stays the caller's: it evaluates the energy, calls b200md_scale_coordinates, sets the scaled
+ * box with b200md_set_box, evaluates again and on rejection calls b200md_restore_coordinates and sets the old box.  One rank
+ * only: all three fail in a multi-GPU context.                                                        */
+/* ApplyMonteCarloBarostatKernel::initialize: the molecules of ContextImpl::getMolecules(), in that order, as CSR
+ * (start[nmol+1], atoms[start[nmol]]).                                                                */
+int b200md_set_barostat_molecules(b200md_ctx* ctx, int nmol, const int* start, const int* atoms);
+/* ApplyMonteCarloBarostatKernel::scaleCoordinates: save the positions and the force buffer, then move every molecule's centre
+ * into the first periodic box of the CURRENT box and scale it by (sx, sy, sz) (ReferenceMonteCarloBarostat.cpp:67-103).
+ * b200md_get_positions then returns the wrapped, scaled coordinates.                                  */
+int b200md_scale_coordinates(b200md_ctx* ctx, double sx, double sy, double sz);
+/* ApplyMonteCarloBarostatKernel::restoreCoordinates: positions and forces as before the last scale, bit for bit. */
+int b200md_restore_coordinates(b200md_ctx* ctx);
 int b200md_set_positions(b200md_ctx* ctx, const double* xyz);
 int b200md_get_positions(b200md_ctx* ctx, double* xyz);   /* continuous (unwrapped) trajectory, like the Reference platform's:
                                                              * internal molecule wrapping is undone (DESIGN.md section 4, "Long runs") */
@@ -191,6 +206,7 @@ typedef struct b200md_stats {
     int     overflow;             /* sticky: tile capacity exceeded at some point               */
     int     stale_list_steps;     /* B200MD_ASYNC_LIST=1 only: steps served by a list whose skin was exceeded
                                    * within that one step (see k_check_gather); 0 in any sane simulation */
+    int64_t graph_instantiations; /* executable step graphs instantiated so far (a box change updates them in place) */
 } b200md_stats;
 int b200md_get_stats(b200md_ctx* ctx, b200md_stats* out);
 /* mean device time (ms) of named phases measured with CUDA events on the engine's stream:

@@ -16,7 +16,8 @@ class Stats(C.Structure):
     _fields_ = [("natoms", C.c_int64), ("padded_atoms", C.c_int64), ("num_blocks", C.c_int64), ("num_tiles", C.c_int64),
                 ("num_mask_tiles", C.c_int64), ("list_builds", C.c_int64), ("force_evals", C.c_int64),
                 ("kernel_launches", C.c_int64), ("pairs_in_cutoff", C.c_int64), ("pme_grid", C.c_int*3),
-                ("ewald_alpha", C.c_double), ("overflow", C.c_int), ("stale_list_steps", C.c_int)]
+                ("ewald_alpha", C.c_double), ("overflow", C.c_int), ("stale_list_steps", C.c_int),
+                ("graph_instantiations", C.c_int64)]
 
 
 _P = C.c_void_p
@@ -47,6 +48,9 @@ SIGNATURES = {
     "b200md_update_bonded_params": (C.c_int, [_P, C.c_int, C.c_int, _D, _D, _I]),
     "b200md_set_box": (C.c_int, [_P, _D, _D, _D]),
     "b200md_get_box": (C.c_int, [_P, _D, _D, _D]),
+    "b200md_set_barostat_molecules": (C.c_int, [_P, C.c_int, _I, _I]),
+    "b200md_scale_coordinates": (C.c_int, [_P, C.c_double, C.c_double, C.c_double]),
+    "b200md_restore_coordinates": (C.c_int, [_P]),
     "b200md_set_positions": (C.c_int, [_P, _D]),
     "b200md_get_positions": (C.c_int, [_P, _D]),
     "b200md_set_velocities": (C.c_int, [_P, _D]),

@@ -128,11 +128,17 @@ struct b200md_ctx {
     int64_t stepCount = 0;
     double selfEnergy = 0, dispersionCoefficient = 0;
     // ---- stats ----
-    int64_t forceEvals = 0, kernelLaunches = 0;
+    int64_t forceEvals = 0, kernelLaunches = 0, graphInstantiations = 0;
+    // ---- Monte Carlo barostat (b200md_scale_coordinates / b200md_restore_coordinates) ----
+    DevBuf<int> baroStart, baroAtoms;    // molecules of ContextImpl::getMolecules(), CSR
+    int baroNmol = 0;
+    DevBuf<float4> savePosq; DevBuf<int> saveCellOffset; DevBuf<long long> saveForce;     // state before the last scale
+    bool haveSaved = false;
     // ---- graph ----
     cudaGraphExec_t stepGraph = nullptr;      // one MD step
     cudaGraphExec_t multiGraph = nullptr;     // graphSteps MD steps in one launch (host launch cost amortised)
-    bool graphValid = false;
+    bool graphValid = false;                  // stepGraph matches the current kernel parameters
+    bool multiValid = false;                  // multiGraph does
     bool useGraph = true;
     int graphSteps = 8;
     int stepLaunches = 0;
@@ -349,7 +355,10 @@ static void setup_cells(b200md_ctx* c) {
     }
 }
 
-static void invalidate_graph(b200md_ctx* c) { c->graphValid = false; }
+// The step graphs hold kernel parameters by value (box, tile-pool pointers, cell grid, integrator constants): whatever changes
+// one of them marks both graphs stale.  b200md_step captures them again and updates the executable graphs in place
+// (capture_steps), so a box change every few steps -- a barostat -- does not instantiate graphs.
+static void invalidate_graph(b200md_ctx* c) { c->graphValid = false; c->multiValid = false; }
 
 static void apply_box(b200md_ctx* c) {
     BoxDev& b = c->nb.box;
@@ -400,6 +409,68 @@ extern "C" int b200md_get_box(b200md_ctx* ctx, double a[3], double b[3], double 
     if (!ctx) return -1;
     for (int i = 0; i < 3; i++) { a[i] = ctx->boxA[i]; b[i] = ctx->boxB[i]; c[i] = ctx->boxC[i]; }
     return 0;
+}
+
+// ---------------------------------------------------------------- Monte Carlo barostat
+// ApplyMonteCarloBarostatKernel (kernels.h:1425-1459).  The host half (MonteCarloBarostatImpl: random volume change, the two
+// energy evaluations, acceptance, adaptive step) stays the reference's own; these three calls are the platform's part.
+static void require_single_rank(const b200md_ctx* c, const char* what) {
+    if (c->world > 1) throw std::runtime_error(std::string(what) + ": the Monte Carlo barostat is not supported in multi-GPU runs");
+}
+static void mark_list_dirty(b200md_ctx* c) {
+    const int one = 1;
+    CUDA_CHECK(cudaMemcpyAsync(&c->counters.p[CT_REBUILD], &one, sizeof(int), cudaMemcpyHostToDevice, c->stream)); c->listDirty = true;
+}
+
+extern "C" int b200md_set_barostat_molecules(b200md_ctx* ctx, int nmol, const int* start, const int* atoms) {
+    API_BEGIN(ctx)
+    require_single_rank(ctx, "set_barostat_molecules");
+    require(nmol >= 0 && start != nullptr && start[0] == 0 && start[nmol] <= ctx->natoms && (start[nmol] == 0 || atoms != nullptr),
+            "set_barostat_molecules: malformed molecule list");
+    for (int m = 0; m < nmol; m++) require(start[m+1] > start[m], "set_barostat_molecules: empty molecule");
+    for (int t = 0; t < start[nmol]; t++) require(atoms[t] >= 0 && atoms[t] < ctx->natoms, "set_barostat_molecules: atom index out of range");
+    ctx->baroStart.upload(std::vector<int>(start, start + nmol + 1));
+    ctx->baroAtoms.upload(std::vector<int>(atoms, atoms + start[nmol]));
+    ctx->baroNmol = nmol;
+    API_END(ctx)
+}
+
+extern "C" int b200md_scale_coordinates(b200md_ctx* ctx, double sx, double sy, double sz) {
+    API_BEGIN(ctx)
+    b200md_ctx* c = ctx;
+    require_single_rank(c, "scale_coordinates");
+    require(c->finalized && c->haveBox, "scale_coordinates before finalize / set_box");
+    require(c->baroStart.n > 0, "scale_coordinates before set_barostat_molecules");
+    const int NP = c->npad;
+    c->savePosq.alloc(NP); c->saveCellOffset.alloc((size_t) 3*NP); c->saveForce.alloc((size_t) 3*NP);
+    CUDA_CHECK(cudaMemcpyAsync(c->savePosq.p, c->posq.p, sizeof(float4)*NP, cudaMemcpyDeviceToDevice, c->stream));
+    CUDA_CHECK(cudaMemcpyAsync(c->saveCellOffset.p, c->cellOffset.p, sizeof(int)*3*NP, cudaMemcpyDeviceToDevice, c->stream));
+    CUDA_CHECK(cudaMemcpyAsync(c->saveForce.p, c->force.p, sizeof(long long)*3*NP, cudaMemcpyDeviceToDevice, c->stream));
+    c->haveSaved = true;
+    ScaleDev sc{};
+    sc.nmol = c->baroNmol; sc.molStart = c->baroStart.p; sc.molAtoms = c->baroAtoms.p;
+    for (int k = 0; k < 3; k++) { sc.a[k] = c->boxA[k]; sc.b[k] = c->boxB[k]; sc.c[k] = c->boxC[k]; }
+    sc.s[0] = sx; sc.s[1] = sy; sc.s[2] = sz;
+    launch_scale_molecules(c->nb, sc, c->stream);
+    c->kernelLaunches++;
+    CUDA_CHECK(cudaGetLastError());
+    mark_list_dirty(c);
+    c->stepStateValid = false;
+    API_END(ctx)
+}
+
+extern "C" int b200md_restore_coordinates(b200md_ctx* ctx) {
+    API_BEGIN(ctx)
+    b200md_ctx* c = ctx;
+    require_single_rank(c, "restore_coordinates");
+    require(c->haveSaved, "restore_coordinates without a preceding scale_coordinates");
+    const int NP = c->npad;
+    CUDA_CHECK(cudaMemcpyAsync(c->posq.p, c->savePosq.p, sizeof(float4)*NP, cudaMemcpyDeviceToDevice, c->stream));
+    CUDA_CHECK(cudaMemcpyAsync(c->cellOffset.p, c->saveCellOffset.p, sizeof(int)*3*NP, cudaMemcpyDeviceToDevice, c->stream));
+    CUDA_CHECK(cudaMemcpyAsync(c->force.p, c->saveForce.p, sizeof(long long)*3*NP, cudaMemcpyDeviceToDevice, c->stream));
+    mark_list_dirty(c);
+    c->stepStateValid = false;            // the force buffer holds forces again, not the zeros the fused step expects
+    API_END(ctx)
 }
 
 // per-atom and per-exception parameters -> device (computeParameters, ReferenceKernels.cpp:1077-1121)
@@ -1598,9 +1669,12 @@ extern "C" int b200md_integrate_only(b200md_ctx* ctx) {
     API_END(ctx)
 }
 
-static cudaGraphExec_t capture_steps(b200md_ctx* c, int nsteps, int* launches) {
+// Capture `nsteps` steps into *exec.  An executable graph that exists already is updated in place with cudaGraphExecUpdate (a
+// box change or a grown tile pool changes kernel parameters, not the topology) and instantiated anew only when the driver
+// refuses the update.  Graphs with conditional (IF) nodes -- B200MD_LIST_MERGED=0 or B200MD_ASYNC_LIST=1 -- are always
+// instantiated anew: every capture creates new conditional handles, which the kernels that set them carry as parameters.
+static void capture_steps(b200md_ctx* c, int nsteps, cudaGraphExec_t* exec, int* launches) {
     cudaGraph_t g;
-    cudaGraphExec_t exec = nullptr;
     CUDA_CHECK(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
     int l = 0;
     try { for (int k = 0; k < nsteps; k++) l += enqueue_step(c); } catch (...) { cudaStreamEndCapture(c->stream, &g); throw; }
@@ -1620,10 +1694,18 @@ static cudaGraphExec_t capture_steps(b200md_ctx* c, int nsteps, int* launches) {
             fprintf(stderr, "node %zu kernel priority %d (%s)\n", i, v.priority, cudaGetErrorString(e));
         }
     }
-    CUDA_CHECK(cudaGraphInstantiate(&exec, g, 0));
-    cudaGraphDestroy(g);
     *launches = l;
-    return exec;
+    const bool cond = c->useCond && (!list_build_merged() || (c->asyncList && c->softPad2 < c->nb.halfPad2));
+    if (*exec && !cond) {
+        cudaGraphExecUpdateResultInfo info;
+        if (cudaGraphExecUpdate(*exec, g, &info) == cudaSuccess) { cudaGraphDestroy(g); return; }
+        (void) cudaGetLastError();          // the refusal is not sticky: fall back to a new instantiation
+    }
+    if (*exec) { cudaGraphExecDestroy(*exec); *exec = nullptr; }
+    const cudaError_t e = cudaGraphInstantiate(exec, g, 0);
+    cudaGraphDestroy(g);
+    CUDA_CHECK(e);
+    c->graphInstantiations++;
 }
 
 extern "C" int b200md_step(b200md_ctx* ctx, int nsteps) {
@@ -1646,21 +1728,18 @@ extern "C" int b200md_step(b200md_ctx* ctx, int nsteps) {
         if (c->cmFreq > 1 && c->stepCount % c->cmFreq == 0) { sync_velocities(c); launch_remove_cm(c->nb, c->cmScratch.p, c->stream); c->kernelLaunches += 2; }
         int done = 1;
         if (c->useGraph) {
-            if (!c->graphValid) {
-                if (c->stepGraph) { cudaGraphExecDestroy(c->stepGraph); c->stepGraph = nullptr; }
-                if (c->multiGraph) { cudaGraphExecDestroy(c->multiGraph); c->multiGraph = nullptr; }
-                c->stepGraph = capture_steps(c, 1, &c->stepLaunches);
-                if (c->graphSteps > 1) { int l; c->multiGraph = capture_steps(c, c->graphSteps, &l); }
-                c->graphValid = true;
-            }
-            // the multi-step graph may not straddle a centre-of-mass removal that lives outside the graph
+            // the multi-step graph may not straddle a centre-of-mass removal that lives outside the graph; it is captured only
+            // when this call can use it (the plugin only ever steps one at a time)
             int untilCm = (c->cmFreq > 1) ? (int) (c->cmFreq - c->stepCount % c->cmFreq) : remaining;
-            if (c->multiGraph && remaining >= c->graphSteps && untilCm >= c->graphSteps) {
+            if (c->graphSteps > 1 && remaining >= c->graphSteps && untilCm >= c->graphSteps) {
+                if (!c->multiValid) { int l; capture_steps(c, c->graphSteps, &c->multiGraph, &l); c->stepLaunches = l/c->graphSteps; c->multiValid = true; }
                 CUDA_CHECK(cudaGraphLaunch(c->multiGraph, c->stream));
                 done = c->graphSteps;
             }
-            else
+            else {
+                if (!c->graphValid) { capture_steps(c, 1, &c->stepGraph, &c->stepLaunches); c->graphValid = true; }
                 CUDA_CHECK(cudaGraphLaunch(c->stepGraph, c->stream));
+            }
             c->kernelLaunches += (int64_t) c->stepLaunches*done;
         }
         else
@@ -1790,7 +1869,7 @@ extern "C" int b200md_get_stats(b200md_ctx* ctx, b200md_stats* out) {
         for (int r = 0; r < TILE_REGIONS; r++) masks += cur[LC_MASKS + r];
         out->num_tiles = cur[LC_USED]; out->num_mask_tiles = masks; out->overflow = h[CT_OVERFLOW]; out->list_builds = h[CT_BUILDS]; out->pairs_in_cutoff = h[CT_PAIRS]; out->stale_list_steps = h[CT_STALE];
     }
-    out->force_evals = ctx->forceEvals; out->kernel_launches = ctx->kernelLaunches;
+    out->force_evals = ctx->forceEvals; out->kernel_launches = ctx->kernelLaunches; out->graph_instantiations = ctx->graphInstantiations;
     out->pme_grid[0] = ctx->pme.nx; out->pme_grid[1] = ctx->pme.ny; out->pme_grid[2] = ctx->pme.nz; out->ewald_alpha = ctx->pme.alpha;
     API_END(ctx)
 }

@@ -340,6 +340,16 @@ __device__ __forceinline__ float3 gauss3(unsigned int seed, int atom, unsigned l
 
 #endif
 
+// Monte Carlo barostat move (k_scale_molecules): molecules as ContextImpl::getMolecules() forms them, the current box vectors in
+// double (reduced form, a = (a0,0,0), b = (b0,b1,0)) and the scale factor of each axis.
+struct ScaleDev {
+    int nmol;
+    const int* molStart;         // [nmol+1] CSR over molAtoms
+    const int* molAtoms;
+    double a[3], b[3], c[3];
+    double s[3];
+};
+
 // ---- launchers (defined in the .cu files) ----
 void launch_check_displacement(const NbDev& nb, const CommDev& cd, cudaStream_t s);
 bool list_build_merged();        // list build = 2 gated launches (k_list_prep with grid barriers + k_build_tiles); B200MD_LIST_MERGED=0: 7
@@ -376,6 +386,7 @@ void launch_constrain_positions(const NbDev& nb, const UnitDev& units, float tol
 void launch_constrain_velocities(const NbDev& nb, const UnitDev& units, float tol, cudaStream_t s);
 void launch_kinetic_energy(const NbDev& nb, const UnitDev& units, const IntegDev& integ, float shiftDt, cudaStream_t s);
 void launch_remove_cm(const NbDev& nb, double* scratch, cudaStream_t s);
+void launch_scale_molecules(const NbDev& nb, const ScaleDev& sc, cudaStream_t s);
 void launch_ccma_step(const NbDev& nb, const CcmaDev& cc, const IntegDev& in, cudaStream_t s);      // before launch_integrate in a step
 void launch_ccma_apply(const NbDev& nb, const CcmaDev& cc, bool velocities, float tol, cudaStream_t s);
 void launch_ccma_kinetic(const NbDev& nb, const CcmaDev& cc, float shiftDt, float tol, cudaStream_t s);

@@ -498,3 +498,51 @@ void launch_remove_cm(const NbDev& nb, double* scratch, cudaStream_t s) {
     k_cm_sum<<<(nb.natoms + 255)/256, 256, 0, s>>>(nb, scratch);
     k_cm_apply<<<(nb.natoms + 255)/256, 256, 0, s>>>(nb, scratch);
 }
+
+// ApplyMonteCarloBarostatKernel::scaleCoordinates (kernels.h:1425-1459) as ReferenceMonteCarloBarostat::applyBarostat does it
+// (ReferenceMonteCarloBarostat.cpp:67-103): the unweighted centre of each barostat molecule, in user coordinates (posq plus
+// cellOffset lattice vectors of the CURRENT box), is moved into the first periodic box (floor order c, b, a; origin 0), scaled,
+// and every atom of the molecule moves by the same offset.  posq receives the result in fp32 and cellOffset becomes zero.
+// One warp per molecule: lane l sums the atoms l, l+32, ... in double and an xor butterfly joins the lanes.  Addition is
+// commutative, so every lane ends with the same bits and the result does not depend on scheduling: no atomics, two runs are
+// bit-identical, and a 2,500-atom protein costs ~80 loads per lane instead of 2,500 on one thread.
+__global__ void __launch_bounds__(256) k_scale_molecules(NbDev nb, ScaleDev sc) {
+    const int m = (blockIdx.x*blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (m >= sc.nmol) return;                       // whole warps only: blockDim is a multiple of 32
+    const int begin = sc.molStart[m], end = sc.molStart[m + 1];
+    const int NP = nb.npad;
+    double cx = 0, cy = 0, cz = 0;
+    for (int t = begin + lane; t < end; t += 32) {
+        const int a = sc.molAtoms[t];
+        const float4 p = nb.posq[a];
+        const int kx = nb.cellOffset[a], ky = nb.cellOffset[a + NP], kz = nb.cellOffset[a + 2*NP];
+        cx += (double) p.x + (kx*sc.a[0] + ky*sc.b[0] + kz*sc.c[0]);
+        cy += (double) p.y + (ky*sc.b[1] + kz*sc.c[1]);
+        cz += (double) p.z + kz*sc.c[2];
+    }
+    for (int off = 16; off > 0; off >>= 1) {
+        cx += __shfl_xor_sync(0xffffffffu, cx, off); cy += __shfl_xor_sync(0xffffffffu, cy, off); cz += __shfl_xor_sync(0xffffffffu, cz, off);
+    }
+    const double inv = 1.0/(end - begin);           // Vec3::operator/= multiplies by the reciprocal
+    cx *= inv; cy *= inv; cz *= inv;
+    double x = cx, y = cy, z = cz, f;
+    f = floor(z/sc.c[2]); x -= sc.c[0]*f; y -= sc.c[1]*f; z -= sc.c[2]*f;
+    f = floor(y/sc.b[1]); x -= sc.b[0]*f; y -= sc.b[1]*f;
+    f = floor(x/sc.a[0]); x -= sc.a[0]*f;
+    const double ox = x*sc.s[0] - cx, oy = y*sc.s[1] - cy, oz = z*sc.s[2] - cz;
+    for (int t = begin + lane; t < end; t += 32) {
+        const int a = sc.molAtoms[t];
+        const float4 p = nb.posq[a];
+        const int kx = nb.cellOffset[a], ky = nb.cellOffset[a + NP], kz = nb.cellOffset[a + 2*NP];
+        const double ux = (double) p.x + (kx*sc.a[0] + ky*sc.b[0] + kz*sc.c[0]);
+        const double uy = (double) p.y + (ky*sc.b[1] + kz*sc.c[1]);
+        const double uz = (double) p.z + kz*sc.c[2];
+        nb.posq[a] = make_float4((float) (ux + ox), (float) (uy + oy), (float) (uz + oz), p.w);
+        nb.cellOffset[a] = 0; nb.cellOffset[a + NP] = 0; nb.cellOffset[a + 2*NP] = 0;
+    }
+}
+void launch_scale_molecules(const NbDev& nb, const ScaleDev& sc, cudaStream_t s) {
+    if (sc.nmol == 0) return;
+    k_scale_molecules<<<(sc.nmol + 7)/8, 256, 0, s>>>(nb, sc);
+}

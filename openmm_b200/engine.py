@@ -119,6 +119,29 @@ class Engine:
         b = _f64(box)
         self._ck(self.lib.b200md_set_box(self.h, _dp(b[0]), _dp(b[1]), _dp(b[2])))
 
+    def get_box(self):
+        a, b, c = np.empty(3), np.empty(3), np.empty(3)
+        self._ck(self.lib.b200md_get_box(self.h, _dp(a), _dp(b), _dp(c)))
+        return np.array([a, b, c])
+
+    # ---- ApplyMonteCarloBarostatKernel ----
+    def set_barostat_molecules(self, molecules=None):
+        """The molecules the barostat scales as rigid groups (default: desc.molecules(), as ContextImpl::getMolecules())."""
+        mols = self.desc.molecules() if molecules is None else molecules
+        start = np.zeros(len(mols) + 1, dtype=np.int32)
+        start[1:] = np.cumsum([len(m) for m in mols])
+        atoms = _i32([a for m in mols for a in m] or [0])
+        self._ck(self.lib.b200md_set_barostat_molecules(self.h, len(mols), _ip(start), _ip(atoms)))
+
+    def scale_coordinates(self, sx, sy, sz):
+        """Save positions and forces, then wrap every molecule's centre into the first periodic box and scale it.  The box
+        itself is unchanged: set_box(scaled box) follows, as in MonteCarloBarostatImpl::updateContextState."""
+        self._ck(self.lib.b200md_scale_coordinates(self.h, sx, sy, sz))
+
+    def restore_coordinates(self):
+        """Positions and forces as before the last scale_coordinates (a rejected move); set_box(old box) follows."""
+        self._ck(self.lib.b200md_restore_coordinates(self.h))
+
     # ---- CalcForcesAndEnergyKernel ----
     def compute(self, terms=TERM_ALL, energy=True):
         """Forces (get_forces()) and, if energy, the potential energy of the selected terms."""

@@ -90,6 +90,27 @@ class SystemDesc:
             return 0.0
         return dispersion_coefficient(self.sigmas, self.epsilons, self.cutoff, self.use_switch, self.switch_distance)
 
+    def molecules(self):
+        """The molecules a barostat moves as rigid groups, as ContextImpl::getMolecules() forms them: connected components of
+        the constraints and the HarmonicBondForce bonds (ContextImpl.cpp:351-383; angles, torsions and exceptions do not
+        join molecules).  Ordered by their lowest atom, atoms ascending (ContextImpl::findMolecules)."""
+        n = self.natoms
+        parent = np.arange(n)
+
+        def find(x):
+            while parent[x] != x:
+                parent[x] = parent[parent[x]]
+                x = parent[x]
+            return x
+        for i, j in zip(np.concatenate([self.con_i, self.bond_i]).tolist(), np.concatenate([self.con_j, self.bond_j]).tolist()):
+            a, b = find(i), find(j)
+            if a != b:
+                parent[max(a, b)] = min(a, b)
+        groups = {}
+        for i in range(n):
+            groups.setdefault(find(i), []).append(i)
+        return [groups[r] for r in sorted(groups)]
+
     def rounded(self):
         """Same system with fp32-representable positions: the identical inputs both the fp32 device path and the
         double-precision oracle are given in parity tests."""

@@ -8,7 +8,8 @@
 //
 // Supported: NonbondedForce (NoCutoff, CutoffNonPeriodic, CutoffPeriodic, PME; parameter offsets), HarmonicBondForce,
 // HarmonicAngleForce, PeriodicTorsionForce (any number of objects, each in its own force group), CMMotionRemover;
-// Verlet / Langevin / LangevinMiddle integrators; SETTLE + X-H_n SHAKE constraints.  A Force class without a kernel here
+// Verlet / Langevin / LangevinMiddle integrators; SETTLE + X-H_n SHAKE constraints; MonteCarloBarostat and
+// MonteCarloAnisotropicBarostat (ApplyMonteCarloBarostatKernel; MonteCarloMembraneBarostat is refused).  A Force class without a kernel here
 // makes Platform::supportsKernels() false; an unsupported OPTION of a supported class is rejected in contextCreated()
 // (validateSystem), which is the only place from which ContextImpl falls back to the next platform (ContextImpl.cpp:152-166).
 //
@@ -32,6 +33,7 @@
 #include "openmm/VerletIntegrator.h"
 #include "openmm/LangevinIntegrator.h"
 #include "openmm/LangevinMiddleIntegrator.h"
+#include "openmm/MonteCarloMembraneBarostat.h"
 #include "openmm/internal/ContextImpl.h"
 #include "openmm/internal/NonbondedForceImpl.h"
 #include "../include/b200md.h"
@@ -78,11 +80,17 @@ struct PlatformData {
     vector<int> angI, angJ, angK; vector<double> angT0, angKK;
     vector<int> torI, torJ, torK, torL, torN; vector<double> torPhase, torKK;
     map<string, string> props;
+    // a box b200md_set_box refused (smaller than twice the cutoff): the reference raises that at the next force evaluation
+    // (ReferenceKernels.cpp:983-985), not in setPeriodicBoxVectors; a later box that passes clears it
+    string boxError;
     int integratorKind = -1;
     double dt = 0, temperature = 0, friction = 0, tol = 0;
     int seed = 0;
     void check(int rc) const {
         if (rc != 0) throw OpenMMException(string("B200 platform: ") + b200md_last_error(ctx));
+    }
+    void checkBox() const {
+        if (!boxError.empty()) throw OpenMMException(boxError);
     }
     void ensureFinalized() {
         if (finalized) return;
@@ -120,6 +128,7 @@ public:
     void initialize(const System& system) {}
     void beginComputation(ContextImpl& context, bool includeForce, bool includeEnergy, int groups) {
         PlatformData& d = getData(context);
+        d.checkBox();
         d.ensureFinalized();
         d.dropForces();             // superseded by this evaluation
         d.pendingTerms = 0;
@@ -183,6 +192,7 @@ public:
     }
     void getForces(ContextImpl& context, vector<Vec3>& forces) {
         PlatformData& d = getData(context);
+        d.checkBox();
         d.ensureFinalized();
         d.flushForces();
         vector<double> x(3*d.numParticles);
@@ -200,7 +210,8 @@ public:
         PlatformData& d = getData(context);
         const double x[3] = {a[0], a[1], a[2]}, y[3] = {b[0], b[1], b[2]}, z[3] = {c[0], c[1], c[2]};
         d.dropForces();
-        d.check(b200md_set_box(d.ctx, x, y, z));
+        if (b200md_set_box(d.ctx, x, y, z) != 0) d.boxError = string("B200 platform: ") + b200md_last_error(d.ctx);
+        else d.boxError.clear();
     }
     void createCheckpoint(ContextImpl& context, ostream& stream) {
         PlatformData& d = getData(context);
@@ -484,6 +495,7 @@ void configureIntegrator(ContextImpl& context, int kind, double dt, double tempe
 // pending and covered the whole force field, forces + integration run as ONE replay of the captured step graph.
 void integrateStep(ContextImpl& context) {
     PlatformData& d = getData(context);
+    d.checkBox();
     d.ensureFinalized();
     const bool whole = d.lazyForces && d.lazyTerms == d.systemTerms && (d.bondedGroupsUsed & ~d.lazyGroups) == 0;
     if (whole && d.useFusedStep) {
@@ -534,6 +546,38 @@ public:
     double computeKineticEnergy(ContextImpl& context, const LangevinMiddleIntegrator& integrator) { configure(context, integrator); return kineticEnergy(context); }
 };
 
+// ------------------------------------------------------------------------------------------------ barostat
+// MonteCarloBarostat / MonteCarloAnisotropicBarostat: MonteCarloBarostatImpl (the reference's, untouched) draws the move, evaluates
+// the energy before and after, and accepts or rejects; the platform scales the molecules and restores them on rejection.
+class B200ApplyMonteCarloBarostatKernel : public ApplyMonteCarloBarostatKernel {
+public:
+    B200ApplyMonteCarloBarostatKernel(string name, const Platform& platform) : ApplyMonteCarloBarostatKernel(name, platform) {}
+    void initialize(const System& system, const Force& barostat) {}
+    void scaleCoordinates(ContextImpl& context, double scaleX, double scaleY, double scaleZ) {
+        PlatformData& d = getData(context);
+        d.ensureFinalized();
+        d.dropForces();
+        if (!haveMolecules) {
+            // ContextImpl::getMolecules() exists only once every ForceImpl is initialised: upload it at the first move, as
+            // CommonApplyMonteCarloBarostatKernel::scaleCoordinates does
+            const vector<vector<int> >& mols = context.getMolecules();
+            vector<int> start(1, 0), atoms;
+            for (const vector<int>& m : mols) { atoms.insert(atoms.end(), m.begin(), m.end()); start.push_back((int) atoms.size()); }
+            d.check(b200md_set_barostat_molecules(d.ctx, (int) mols.size(), start.data(), atoms.data()));
+            haveMolecules = true;
+        }
+        d.check(b200md_scale_coordinates(d.ctx, scaleX, scaleY, scaleZ));
+    }
+    void restoreCoordinates(ContextImpl& context) {
+        PlatformData& d = getData(context);
+        d.ensureFinalized();
+        d.dropForces();
+        d.check(b200md_restore_coordinates(d.ctx));
+    }
+private:
+    bool haveMolecules = false;
+};
+
 // ------------------------------------------------------------------------------------------------ factory + platform
 class B200KernelFactory : public KernelFactory {
 public:
@@ -550,6 +594,7 @@ public:
         if (name == IntegrateVerletStepKernel::Name()) return new B200IntegrateVerletStepKernel(name, platform);
         if (name == IntegrateLangevinStepKernel::Name()) return new B200IntegrateLangevinStepKernel(name, platform);
         if (name == IntegrateLangevinMiddleStepKernel::Name()) return new B200IntegrateLangevinMiddleStepKernel(name, platform);
+        if (name == ApplyMonteCarloBarostatKernel::Name()) return new B200ApplyMonteCarloBarostatKernel(name, platform);
         throw OpenMMException((string("Tried to create kernel with illegal kernel name '") + name + "'").c_str());
     }
 };
@@ -561,7 +606,7 @@ public:
         for (const string& n : {CalcForcesAndEnergyKernel::Name(), UpdateStateDataKernel::Name(), ApplyConstraintsKernel::Name(), VirtualSitesKernel::Name(),
                                 CalcNonbondedForceKernel::Name(), CalcHarmonicBondForceKernel::Name(), CalcHarmonicAngleForceKernel::Name(),
                                 CalcPeriodicTorsionForceKernel::Name(), RemoveCMMotionKernel::Name(), IntegrateVerletStepKernel::Name(),
-                                IntegrateLangevinStepKernel::Name(), IntegrateLangevinMiddleStepKernel::Name()})
+                                IntegrateLangevinStepKernel::Name(), IntegrateLangevinMiddleStepKernel::Name(), ApplyMonteCarloBarostatKernel::Name()})
             registerKernelFactory(n, factory);
         platformProperties.push_back(DeviceIndex());
         platformProperties.push_back(Precision());
@@ -601,6 +646,7 @@ public:
                 if (nb->getNumParticles() != system.getNumParticles()) throw OpenMMException("NonbondedForce must have exactly as many particles as the System it belongs to.");
             }
             if (force.getForceGroup() < 0 || force.getForceGroup() > 31) throw OpenMMException("B200 platform: force group out of range");
+            if (dynamic_cast<const MonteCarloMembraneBarostat*>(&force)) throw OpenMMException("B200 platform: MonteCarloMembraneBarostat is not supported");
         }
         const int nc = system.getNumConstraints();
         if (nc > 0) {
