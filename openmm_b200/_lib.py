@@ -43,6 +43,8 @@ SIGNATURES = {
     "b200md_ccma_setup_probe": (C.c_int, [C.c_int, _D, C.c_int, _I, _I, _D, C.c_int, _I, _I, _I, _D, _I, _I, _I, _I, _I, _F, C.c_int]),
     "b200md_set_cm_remover": (C.c_int, [_P, C.c_int]),
     "b200md_remove_cm_motion": (C.c_int, [_P]),
+    "b200md_set_precision": (C.c_int, [_P, C.c_int]),
+    "b200md_get_precision": (C.c_int, [_P]),
     "b200md_finalize": (C.c_int, [_P]),
     "b200md_update_nonbonded_params": (C.c_int, [_P, _D, _D, _D, C.c_int, _D, _D, _D, C.c_double]),
     "b200md_update_bonded_params": (C.c_int, [_P, C.c_int, C.c_int, _D, _D, _I]),

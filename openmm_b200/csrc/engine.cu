@@ -116,6 +116,12 @@ struct b200md_ctx {
     DevBuf<int> ccCompCon, ccCompAtom, ccRowStart, ccCol, ccAtoms, ccAStart, ccACon;
     DevBuf<int2> ccConAtoms; DevBuf<float> ccDist, ccRedMass, ccVal, ccDelta1, ccDelta2;
     DevBuf<float4> ccRij, ccXold, ccXunc;
+    // mixed precision (b200md_set_precision): low parts of the positions, double velocities, double constraint constants and
+    // CCMA scratch; unallocated in a single-precision context
+    int precision = B200MD_PRECISION_SINGLE;
+    DevBuf<float4> posqCorr; DevBuf<double4> velmD, unitParamsD;
+    DevBuf<double> ccDistD, ccRedMassD, ccDelta1D, ccDelta2D; DevBuf<double4> ccRijD, ccXoldD, ccXuncD, ccXposD;
+    bool mixed() const { return precision == B200MD_PRECISION_MIXED; }
     CcmaDev ccma{};
     NbDev nb{};
     PmeDev pme{};
@@ -132,7 +138,7 @@ struct b200md_ctx {
     // ---- Monte Carlo barostat (b200md_scale_coordinates / b200md_restore_coordinates) ----
     DevBuf<int> baroStart, baroAtoms;    // molecules of ContextImpl::getMolecules(), CSR
     int baroNmol = 0;
-    DevBuf<float4> savePosq; DevBuf<int> saveCellOffset; DevBuf<long long> saveForce;     // state before the last scale
+    DevBuf<float4> savePosq, savePosqCorr; DevBuf<int> saveCellOffset; DevBuf<long long> saveForce;     // state before the last scale
     bool haveSaved = false;
     // ---- graph ----
     cudaGraphExec_t stepGraph = nullptr;      // one MD step
@@ -153,7 +159,7 @@ struct b200md_ctx {
     DevBuf<unsigned long long> commCounters;   // [0] epoch, [1] posNeed
     DevBuf<unsigned int> commDone;             // [CH_COUNT]
     bool velStale = false;               // p2p: the velocities of foreign atoms are behind (only owners integrate)
-    std::vector<float4> hbuf4;
+    std::vector<float4> hbuf4, hcorr4;
     std::vector<int> hoffset;
     std::vector<long long> hforce;
 };
@@ -298,6 +304,18 @@ extern "C" int b200md_set_cm_remover(b200md_ctx* ctx, int freq) {
     ctx->cmFreq = freq;
     return 0;
 }
+
+extern "C" int b200md_set_precision(b200md_ctx* ctx, int precision) {
+    API_BEGIN(ctx)
+    require(!ctx->finalized, "set_precision after finalize");
+    require(precision == B200MD_PRECISION_SINGLE || precision == B200MD_PRECISION_MIXED,
+            "set_precision: unknown precision (B200MD_PRECISION_SINGLE or B200MD_PRECISION_MIXED)");
+    require(precision == B200MD_PRECISION_SINGLE || ctx->world == 1, "mixed precision is not supported in multi-GPU runs");
+    require(precision == B200MD_PRECISION_SINGLE || !ctx->pmeOnly, "mixed precision is not supported by the stand-alone PME provider");
+    ctx->precision = precision;
+    API_END(ctx)
+}
+extern "C" int b200md_get_precision(b200md_ctx* ctx) { return ctx ? ctx->precision : -1; }
 
 extern "C" int b200md_remove_cm_motion(b200md_ctx* ctx) {
     API_BEGIN(ctx)
@@ -446,6 +464,10 @@ extern "C" int b200md_scale_coordinates(b200md_ctx* ctx, double sx, double sy, d
     CUDA_CHECK(cudaMemcpyAsync(c->savePosq.p, c->posq.p, sizeof(float4)*NP, cudaMemcpyDeviceToDevice, c->stream));
     CUDA_CHECK(cudaMemcpyAsync(c->saveCellOffset.p, c->cellOffset.p, sizeof(int)*3*NP, cudaMemcpyDeviceToDevice, c->stream));
     CUDA_CHECK(cudaMemcpyAsync(c->saveForce.p, c->force.p, sizeof(long long)*3*NP, cudaMemcpyDeviceToDevice, c->stream));
+    if (c->mixed()) {
+        c->savePosqCorr.alloc(NP);
+        CUDA_CHECK(cudaMemcpyAsync(c->savePosqCorr.p, c->posqCorr.p, sizeof(float4)*NP, cudaMemcpyDeviceToDevice, c->stream));
+    }
     c->haveSaved = true;
     ScaleDev sc{};
     sc.nmol = c->baroNmol; sc.molStart = c->baroStart.p; sc.molAtoms = c->baroAtoms.p;
@@ -468,6 +490,7 @@ extern "C" int b200md_restore_coordinates(b200md_ctx* ctx) {
     CUDA_CHECK(cudaMemcpyAsync(c->posq.p, c->savePosq.p, sizeof(float4)*NP, cudaMemcpyDeviceToDevice, c->stream));
     CUDA_CHECK(cudaMemcpyAsync(c->cellOffset.p, c->saveCellOffset.p, sizeof(int)*3*NP, cudaMemcpyDeviceToDevice, c->stream));
     CUDA_CHECK(cudaMemcpyAsync(c->force.p, c->saveForce.p, sizeof(long long)*3*NP, cudaMemcpyDeviceToDevice, c->stream));
+    if (c->mixed()) CUDA_CHECK(cudaMemcpyAsync(c->posqCorr.p, c->savePosqCorr.p, sizeof(float4)*NP, cudaMemcpyDeviceToDevice, c->stream));
     mark_list_dirty(c);
     c->stepStateValid = false;            // the force buffer holds forces again, not the zeros the fused step expects
     API_END(ctx)
@@ -509,7 +532,8 @@ static void upload_params(b200md_ctx* c) {
 // Integration units: SETTLE waters, X-H_n SHAKE clusters, free atoms.  Pure host function so that the plugin can run it
 // as a dry run from Platform::contextCreated (b200md_check_constraints) before anything is allocated.
 static bool classify_units(int N, const double* mass, const std::vector<int>& conI, const std::vector<int>& conJ, const std::vector<double>& conD,
-                           std::vector<int4>& ua2, std::vector<int>& ut2, std::vector<float4>& up2, std::string& err, std::vector<int>* ccmaCons = nullptr) {
+                           std::vector<int4>& ua2, std::vector<int>& ut2, std::vector<float4>& up2, std::string& err, std::vector<int>* ccmaCons = nullptr,
+                           std::vector<double4>* upD2 = nullptr) {
     const int nc = (int) conI.size();
     std::vector<std::vector<std::pair<int, double> > > adj(N);
     for (int k = 0; k < nc; k++) {
@@ -520,7 +544,7 @@ static bool classify_units(int N, const double* mass, const std::vector<int>& co
         adj[conJ[k]].push_back(std::make_pair(conI[k], conD[k]));
     }
     std::vector<int> assigned(N, 0);
-    std::vector<int4> ua; std::vector<int> ut; std::vector<float4> up;
+    std::vector<int4> ua; std::vector<int> ut; std::vector<float4> up; std::vector<double4> upD;     // upD: the distances in double
     std::vector<std::pair<int, int> > order;      // (first atom, unit index) for sorting
     auto dist = [&](int a, int b) -> double { for (auto& pr : adj[a]) if (pr.first == b) return pr.second; return -1.0; };
     // SETTLE: closed triangles with two equal sides (compared as float, ReferenceConstraints.cpp:73-77,111-137)
@@ -530,15 +554,15 @@ static bool classify_units(int N, const double* mass, const std::vector<int>& co
         if (adj[b].size() != 2 || adj[d].size() != 2 || assigned[b] || assigned[d]) continue;
         if (dist(b, d) < 0) continue;
         const float dab = (float) dist(a, b), dad = (float) dist(a, d), dbd = (float) dist(b, d);
-        int apex, o1, o2; float d1, d2;
-        if (dab == dad) { apex = a; o1 = b; o2 = d; d1 = dab; d2 = dbd; }
-        else if (dab == dbd) { apex = b; o1 = a; o2 = d; d1 = dab; d2 = dad; }
-        else if (dad == dbd) { apex = d; o1 = a; o2 = b; d1 = dad; d2 = dab; }
+        int apex, o1, o2; float d1, d2; double d1D, d2D;
+        if (dab == dad) { apex = a; o1 = b; o2 = d; d1 = dab; d2 = dbd; d1D = dist(a, b); d2D = dist(b, d); }
+        else if (dab == dbd) { apex = b; o1 = a; o2 = d; d1 = dab; d2 = dad; d1D = dist(a, b); d2D = dist(a, d); }
+        else if (dad == dbd) { apex = d; o1 = a; o2 = b; d1 = dad; d2 = dab; d1D = dist(a, d); d2D = dist(a, b); }
         else continue;
         if (mass[apex] == 0 || mass[o1] == 0 || mass[o2] == 0) continue;
         assigned[a] = assigned[b] = assigned[d] = 1;
         order.push_back(std::make_pair(std::min(a, std::min(b, d)), (int) ua.size()));
-        ua.push_back(make_int4(apex, o1, o2, -1)); ut.push_back(1); up.push_back(make_float4(d1, d2, 0.f, 0.f));
+        ua.push_back(make_int4(apex, o1, o2, -1)); ut.push_back(1); up.push_back(make_float4(d1, d2, 0.f, 0.f)); upD.push_back(make_double4(d1D, d2D, 0, 0));
     }
     // SHAKE clusters: a centre whose partners are each constrained only to it (IntegrationUtilities.cpp:204-277)
     for (int a = 0; a < N; a++) {
@@ -551,11 +575,11 @@ static bool classify_units(int N, const double* mass, const std::vector<int>& co
             if (mass[b] > mass[a] || (mass[b] == mass[a] && b < a)) centre = false;
         }
         if (!centre) continue;
-        int at[4] = {a, -1, -1, -1}; float dd[3] = {0, 0, 0};
-        for (size_t k = 0; k < adj[a].size(); k++) { at[k+1] = adj[a][k].first; dd[k] = (float) adj[a][k].second; assigned[adj[a][k].first] = 1; }
+        int at[4] = {a, -1, -1, -1}; float dd[3] = {0, 0, 0}; double ddD[3] = {0, 0, 0};
+        for (size_t k = 0; k < adj[a].size(); k++) { at[k+1] = adj[a][k].first; dd[k] = (float) adj[a][k].second; ddD[k] = adj[a][k].second; assigned[adj[a][k].first] = 1; }
         assigned[a] = 1;
         order.push_back(std::make_pair(a, (int) ua.size()));
-        ua.push_back(make_int4(at[0], at[1], at[2], at[3])); ut.push_back(2); up.push_back(make_float4(dd[0], dd[1], dd[2], 0.f));
+        ua.push_back(make_int4(at[0], at[1], at[2], at[3])); ut.push_back(2); up.push_back(make_float4(dd[0], dd[1], dd[2], 0.f)); upD.push_back(make_double4(ddD[0], ddD[1], ddD[2], 0));
     }
     // everything else is a general constraint network: CCMA (ReferenceConstraints.cpp:148-184).  Its atoms get no
     // integration unit: k_ccma_step (constraints.cu) takes them through the step, one CTA per connected component.
@@ -571,20 +595,23 @@ static bool classify_units(int N, const double* mass, const std::vector<int>& co
         if (isCcma[a]) continue;
         if (!assigned[a]) {
             order.push_back(std::make_pair(a, (int) ua.size()));
-            ua.push_back(make_int4(a, -1, -1, -1)); ut.push_back(0); up.push_back(make_float4(0, 0, 0, 0));
+            ua.push_back(make_int4(a, -1, -1, -1)); ut.push_back(0); up.push_back(make_float4(0, 0, 0, 0)); upD.push_back(make_double4(0, 0, 0, 0));
         }
     }
     std::sort(order.begin(), order.end());
     ua2.resize(ua.size()); ut2.resize(ua.size()); up2.resize(ua.size());
     for (size_t k = 0; k < order.size(); k++) { ua2[k] = ua[order[k].second]; ut2[k] = ut[order[k].second]; up2[k] = up[order[k].second]; }
+    if (upD2) { upD2->resize(ua.size()); for (size_t k = 0; k < order.size(); k++) (*upD2)[k] = upD[order[k].second]; }
     return true;
 }
 
 static void build_units(b200md_ctx* c) {
-    std::vector<int4> ua2; std::vector<int> ut2; std::vector<float4> up2;
+    std::vector<int4> ua2; std::vector<int> ut2; std::vector<float4> up2; std::vector<double4> upD2;
     std::string err;
-    if (!classify_units(c->natoms, c->mass.data(), c->conI, c->conJ, c->conD, ua2, ut2, up2, err, &c->ccmaCons)) throw std::runtime_error("B200 platform: " + err);
+    if (!classify_units(c->natoms, c->mass.data(), c->conI, c->conJ, c->conD, ua2, ut2, up2, err, &c->ccmaCons, &upD2)) throw std::runtime_error("B200 platform: " + err);
     c->unitAtoms.upload(ua2); c->unitType.upload(ut2); c->unitParams.upload(up2);
+    if (c->mixed()) c->unitParamsD.upload(upD2);
+    c->units.unitParamsD = c->mixed() ? c->unitParamsD.p : nullptr;
     c->hUnitAtoms = ua2;
     c->units.nunits = (int) ua2.size();
     c->units.unitAtoms = c->unitAtoms.p; c->units.unitType = c->unitType.p; c->units.unitParams = c->unitParams.p;
@@ -609,6 +636,7 @@ struct CcmaHost {
     int ncomp = 0;
     std::vector<int> order, compCon, compAtom, atoms, aStart, aCon, rowStart, col;
     std::vector<int2> conAtoms; std::vector<float> dist, redMass, val;
+    std::vector<double> distD, redMassD;     // the same in double (mixed precision)
 };
 static void ccma_host_setup(const CcmaInput* c, CcmaHost& H) {
     const int nc = (int) c->ccmaCons.size();
@@ -621,13 +649,14 @@ static void ccma_host_setup(const CcmaInput* c, CcmaHost& H) {
     std::vector<int> order(nc);
     for (int k = 0; k < nc; k++) order[k] = k;
     std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return find(c->conI[c->ccmaCons[a]]) < find(c->conI[c->ccmaCons[b]]); });
-    std::vector<int2> conAtoms(nc); std::vector<float> dist(nc), redMass(nc); std::vector<double> distD(nc);
+    std::vector<int2> conAtoms(nc); std::vector<float> dist(nc), redMass(nc); std::vector<double> distD(nc), redMassD(nc);
     std::vector<int> compCon(1, 0), compOfCon(nc);
     for (int k = 0; k < nc; k++) {
         const int src = c->ccmaCons[order[k]];
         conAtoms[k] = make_int2(c->conI[src], c->conJ[src]);
         distD[k] = c->conD[src]; dist[k] = (float) distD[k];
-        redMass[k] = (float) (0.5/(1.0/c->mass[conAtoms[k].x] + 1.0/c->mass[conAtoms[k].y]));
+        redMassD[k] = 0.5/(1.0/c->mass[conAtoms[k].x] + 1.0/c->mass[conAtoms[k].y]);
+        redMass[k] = (float) redMassD[k];
         if (k > 0 && find(conAtoms[k].x) != find(conAtoms[k-1].x)) compCon.push_back(k);
         compOfCon[k] = (int) compCon.size() - 1;
     }
@@ -735,6 +764,7 @@ static void ccma_host_setup(const CcmaInput* c, CcmaHost& H) {
     H.ncomp = ncomp;
     H.order = order; H.compCon = compCon; H.compAtom = compAtom; H.atoms = atoms; H.aStart = aStart; H.aCon = aCon;
     H.rowStart = rowStart; H.col = col; H.conAtoms = conAtoms; H.dist = dist; H.redMass = redMass; H.val = val;
+    H.distD = distD; H.redMassD = redMassD;
 }
 
 static void build_ccma(b200md_ctx* c) {
@@ -755,6 +785,14 @@ static void build_ccma(b200md_ctx* c) {
     cc.rowStart = c->ccRowStart.p; cc.col = c->ccCol.p; cc.val = c->ccVal.p; cc.atoms = c->ccAtoms.p; cc.aStart = c->ccAStart.p; cc.aCon = c->ccACon.p;
     cc.rij = c->ccRij.p; cc.delta1 = c->ccDelta1.p; cc.delta2 = c->ccDelta2.p; cc.xold = c->ccXold.p; cc.xunc = c->ccXunc.p;
     cc.maxIter = 150;                   // ReferenceCCMAAlgorithm.cpp:55
+    if (c->mixed()) {
+        c->ccDistD.upload(H.distD); c->ccRedMassD.upload(H.redMassD);
+        c->ccRijD.alloc(nc); c->ccDelta1D.alloc(nc); c->ccDelta2D.alloc(nc);
+        c->ccXoldD.alloc(c->npad); c->ccXuncD.alloc(c->npad); c->ccXposD.alloc(c->npad);
+        cc.conDistD = c->ccDistD.p; cc.conRedMassD = c->ccRedMassD.p;
+        cc.rijD = c->ccRijD.p; cc.delta1D = c->ccDelta1D.p; cc.delta2D = c->ccDelta2D.p;
+        cc.xoldD = c->ccXoldD.p; cc.xuncD = c->ccXuncD.p; cc.xposD = c->ccXposD.p;
+    }
 }
 
 // CCMA host setup without a context or a device (tests): classification + approximate inverse of the coupling matrix.
@@ -1065,6 +1103,13 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     std::vector<float4> vm(NP, make_float4(0, 0, 0, 0));
     for (int i = 0; i < N; i++) vm[i].w = (c->mass[i] > 0) ? (float) (1.0/c->mass[i]) : 0.f;
     c->velm.upload(vm);
+    nb.posqCorr = nullptr; nb.velmD = nullptr;
+    if (c->mixed()) {
+        std::vector<double4> vd(NP, make_double4(0, 0, 0, 0));
+        for (int i = 0; i < N; i++) vd[i].w = (c->mass[i] > 0) ? 1.0/c->mass[i] : 0.0;
+        c->posqCorr.alloc(NP); c->posqCorr.zero(); c->velmD.upload(vd);
+        nb.posqCorr = c->posqCorr.p; nb.velmD = c->velmD.p;
+    }
     nb.posq = c->posq.p; nb.velm = c->velm.p; nb.sigeps = c->sigeps.p; nb.force = c->force.p; nb.energy = c->energy.p;
     nb.sortedOf = c->sortedOf.p;
     nb.refPos = c->refPos.p; nb.atomCell = c->atomCell.p; nb.tmpSorted = c->tmpSorted.p; nb.atomShift = c->atomShift.p;
@@ -1252,6 +1297,14 @@ extern "C" int b200md_set_positions(b200md_ctx* ctx, const double* x) {
     }
     sync_positions(ctx);          // the peers' stores of the last step must not land after this upload
     CUDA_CHECK(cudaMemcpyAsync(ctx->posq.p, ctx->hbuf4.data(), sizeof(float4)*ctx->npad, cudaMemcpyHostToDevice, ctx->stream));
+    if (ctx->mixed()) {           // low parts (engine.h: pos_split)
+        ctx->hcorr4.assign(ctx->npad, make_float4(0, 0, 0, 0));
+        for (int i = 0; i < N; i++) {
+            float hi; float4& l = ctx->hcorr4[i];       // hi: as uploaded to posq above
+            pos_split(x[3*i], hi, l.x); pos_split(x[3*i+1], hi, l.y); pos_split(x[3*i+2], hi, l.z);
+        }
+        CUDA_CHECK(cudaMemcpyAsync(ctx->posqCorr.p, ctx->hcorr4.data(), sizeof(float4)*ctx->npad, cudaMemcpyHostToDevice, ctx->stream));
+    }
     host_set_state(ctx);
     CUDA_CHECK(cudaMemsetAsync(ctx->cellOffset.p, 0, sizeof(int)*3*ctx->npad, ctx->stream));
     const int one = 1;
@@ -1264,8 +1317,17 @@ extern "C" int b200md_get_positions(b200md_ctx* ctx, double* x) {
     ctx->hbuf4.resize(ctx->npad);
     sync_positions(ctx);
     CUDA_CHECK(cudaMemcpyAsync(ctx->hbuf4.data(), ctx->posq.p, sizeof(float4)*ctx->npad, cudaMemcpyDeviceToHost, ctx->stream));
+    if (ctx->mixed()) {
+        ctx->hcorr4.resize(ctx->npad);
+        CUDA_CHECK(cudaMemcpyAsync(ctx->hcorr4.data(), ctx->posqCorr.p, sizeof(float4)*ctx->npad, cudaMemcpyDeviceToHost, ctx->stream));
+    }
     check_flags(ctx);
     for (int i = 0; i < ctx->natoms; i++) { x[3*i] = ctx->hbuf4[i].x; x[3*i+1] = ctx->hbuf4[i].y; x[3*i+2] = ctx->hbuf4[i].z; }
+    if (ctx->mixed())
+        for (int i = 0; i < ctx->natoms; i++) {
+            const float4 h = ctx->hbuf4[i], l = ctx->hcorr4[i];
+            x[3*i] = pos_join(h.x, l.x); x[3*i+1] = pos_join(h.y, l.y); x[3*i+2] = pos_join(h.z, l.z);
+        }
     if (ctx->nb.nmol > 0) {
         // undo the internal molecule wrapping: the caller sees the continuous trajectory, like the Reference platform's
         const int NP = ctx->npad;
@@ -1290,7 +1352,13 @@ extern "C" int b200md_set_velocities(b200md_ctx* ctx, const double* v) {
     for (int i = 0; i < ctx->npad; i++) ctx->hbuf4[i] = make_float4(0, 0, 0, 0);
     for (int i = 0; i < ctx->natoms; i++)
         ctx->hbuf4[i] = make_float4((float) v[3*i], (float) v[3*i+1], (float) v[3*i+2], ctx->mass[i] > 0 ? (float) (1.0/ctx->mass[i]) : 0.f);
-    CUDA_CHECK(cudaMemcpyAsync(ctx->velm.p, ctx->hbuf4.data(), sizeof(float4)*ctx->npad, cudaMemcpyHostToDevice, ctx->stream));
+    std::vector<double4> vd;
+    if (ctx->mixed()) {
+        vd.assign(ctx->npad, make_double4(0, 0, 0, 0));
+        for (int i = 0; i < ctx->natoms; i++) vd[i] = make_double4(v[3*i], v[3*i+1], v[3*i+2], ctx->mass[i] > 0 ? 1.0/ctx->mass[i] : 0.0);
+        CUDA_CHECK(cudaMemcpyAsync(ctx->velmD.p, vd.data(), sizeof(double4)*ctx->npad, cudaMemcpyHostToDevice, ctx->stream));
+    }
+    else CUDA_CHECK(cudaMemcpyAsync(ctx->velm.p, ctx->hbuf4.data(), sizeof(float4)*ctx->npad, cudaMemcpyHostToDevice, ctx->stream));
     ctx->velStale = false;
     CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
     API_END(ctx)
@@ -1299,9 +1367,17 @@ extern "C" int b200md_get_velocities(b200md_ctx* ctx, double* v) {
     API_BEGIN(ctx)
     ctx->hbuf4.resize(ctx->npad);
     sync_velocities(ctx);
-    CUDA_CHECK(cudaMemcpyAsync(ctx->hbuf4.data(), ctx->velm.p, sizeof(float4)*ctx->npad, cudaMemcpyDeviceToHost, ctx->stream));
-    check_flags(ctx);
-    for (int i = 0; i < ctx->natoms; i++) { v[3*i] = ctx->hbuf4[i].x; v[3*i+1] = ctx->hbuf4[i].y; v[3*i+2] = ctx->hbuf4[i].z; }
+    if (ctx->mixed()) {
+        std::vector<double4> vd(ctx->npad);
+        CUDA_CHECK(cudaMemcpyAsync(vd.data(), ctx->velmD.p, sizeof(double4)*ctx->npad, cudaMemcpyDeviceToHost, ctx->stream));
+        check_flags(ctx);
+        for (int i = 0; i < ctx->natoms; i++) { v[3*i] = vd[i].x; v[3*i+1] = vd[i].y; v[3*i+2] = vd[i].z; }
+    }
+    else {
+        CUDA_CHECK(cudaMemcpyAsync(ctx->hbuf4.data(), ctx->velm.p, sizeof(float4)*ctx->npad, cudaMemcpyDeviceToHost, ctx->stream));
+        check_flags(ctx);
+        for (int i = 0; i < ctx->natoms; i++) { v[3*i] = ctx->hbuf4[i].x; v[3*i+1] = ctx->hbuf4[i].y; v[3*i+2] = ctx->hbuf4[i].z; }
+    }
     API_END(ctx)
 }
 extern "C" int b200md_get_forces(b200md_ctx* ctx, double* f) {
@@ -1326,10 +1402,18 @@ extern "C" int b200md_synchronize(b200md_ctx* ctx) {
 }
 
 // ---------------------------------------------------------------- checkpoint
+// Version 2 (single precision): header | posq | velm | cellOffset.  Version 3 (mixed precision): header | posq | posqCorr |
+// velmD | cellOffset.  cellOffset stays last in both.  A blob is only loaded into a context of its own precision.
 struct CkptHeader { char magic[8]; int version; int natoms; double time; int64_t stepCount; double box[9]; unsigned long long rngStep; };
+static int ckpt_version(const b200md_ctx* c) { return c->mixed() ? 3 : 2; }
+static int64_t ckpt_bytes(const b200md_ctx* c) {
+    const int64_t NP = c->npad;
+    const int64_t state = c->mixed() ? 2*sizeof(float4)*NP + sizeof(double4)*NP : 2*sizeof(float4)*NP;
+    return sizeof(CkptHeader) + state + 3*sizeof(int)*NP;
+}
 extern "C" int64_t b200md_checkpoint_save(b200md_ctx* ctx, void* buf, int64_t cap) {
     if (!ctx) return -1;
-    const int64_t need = sizeof(CkptHeader) + 2*sizeof(float4)*(int64_t) ctx->npad + 3*sizeof(int)*(int64_t) ctx->npad;
+    const int64_t need = ckpt_bytes(ctx);
     if (!buf) return need;
     try {
         CUDA_CHECK(cudaSetDevice(ctx->device));
@@ -1337,13 +1421,17 @@ extern "C" int64_t b200md_checkpoint_save(b200md_ctx* ctx, void* buf, int64_t ca
         sync_positions(ctx); sync_velocities(ctx);
         CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
         CkptHeader h; memset(&h, 0, sizeof(h));
-        memcpy(h.magic, "B200MDCK", 8); h.version = 2; h.natoms = ctx->natoms; h.time = ctx->time; h.stepCount = ctx->stepCount;
+        memcpy(h.magic, "B200MDCK", 8); h.version = ckpt_version(ctx); h.natoms = ctx->natoms; h.time = ctx->time; h.stepCount = ctx->stepCount;
         for (int i = 0; i < 3; i++) { h.box[i] = ctx->boxA[i]; h.box[3+i] = ctx->boxB[i]; h.box[6+i] = ctx->boxC[i]; }
         CUDA_CHECK(cudaMemcpy(&h.rngStep, ctx->stepCounter.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
         char* p = (char*) buf;
         memcpy(p, &h, sizeof(h)); p += sizeof(h);
         CUDA_CHECK(cudaMemcpy(p, ctx->posq.p, sizeof(float4)*ctx->npad, cudaMemcpyDeviceToHost)); p += sizeof(float4)*ctx->npad;
-        CUDA_CHECK(cudaMemcpy(p, ctx->velm.p, sizeof(float4)*ctx->npad, cudaMemcpyDeviceToHost)); p += sizeof(float4)*ctx->npad;
+        if (ctx->mixed()) {
+            CUDA_CHECK(cudaMemcpy(p, ctx->posqCorr.p, sizeof(float4)*ctx->npad, cudaMemcpyDeviceToHost)); p += sizeof(float4)*ctx->npad;
+            CUDA_CHECK(cudaMemcpy(p, ctx->velmD.p, sizeof(double4)*ctx->npad, cudaMemcpyDeviceToHost)); p += sizeof(double4)*ctx->npad;
+        }
+        else { CUDA_CHECK(cudaMemcpy(p, ctx->velm.p, sizeof(float4)*ctx->npad, cudaMemcpyDeviceToHost)); p += sizeof(float4)*ctx->npad; }
         CUDA_CHECK(cudaMemcpy(p, ctx->cellOffset.p, sizeof(int)*3*ctx->npad, cudaMemcpyDeviceToHost));
         return need;
     } catch (std::exception& e) { ctx->err = e.what(); return -1; }
@@ -1352,17 +1440,23 @@ extern "C" int b200md_checkpoint_load(b200md_ctx* ctx, const void* buf, int64_t 
     API_BEGIN(ctx)
     ctx->stepStateValid = false;
     require(ctx->finalized, "checkpoint_load before finalize");
-    const int64_t need = sizeof(CkptHeader) + 2*sizeof(float4)*(int64_t) ctx->npad + 3*sizeof(int)*(int64_t) ctx->npad;
-    require(size >= need, "checkpoint blob too small");
+    require(size >= (int64_t) sizeof(CkptHeader), "checkpoint blob too small");
     CkptHeader h; memcpy(&h, buf, sizeof(h));
-    require(memcmp(h.magic, "B200MDCK", 8) == 0 && h.version == 2 && h.natoms == ctx->natoms, "checkpoint blob does not match this context");
+    require(memcmp(h.magic, "B200MDCK", 8) == 0 && (h.version == 2 || h.version == 3) && h.natoms == ctx->natoms, "checkpoint blob does not match this context");
+    require(h.version == ckpt_version(ctx), h.version == 3 ? "the checkpoint was written in mixed precision and this context is single precision"
+                                                           : "the checkpoint was written in single precision and this context is mixed precision");
+    require(size >= ckpt_bytes(ctx), "checkpoint blob too small");
     sync_positions(ctx);
     CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
     ctx->time = h.time; ctx->stepCount = h.stepCount;
     for (int i = 0; i < 3; i++) { ctx->boxA[i] = h.box[i]; ctx->boxB[i] = h.box[3+i]; ctx->boxC[i] = h.box[6+i]; }
     const char* p = (const char*) buf + sizeof(h);
     CUDA_CHECK(cudaMemcpy(ctx->posq.p, p, sizeof(float4)*ctx->npad, cudaMemcpyHostToDevice)); p += sizeof(float4)*ctx->npad;
-    CUDA_CHECK(cudaMemcpy(ctx->velm.p, p, sizeof(float4)*ctx->npad, cudaMemcpyHostToDevice)); p += sizeof(float4)*ctx->npad;
+    if (ctx->mixed()) {
+        CUDA_CHECK(cudaMemcpy(ctx->posqCorr.p, p, sizeof(float4)*ctx->npad, cudaMemcpyHostToDevice)); p += sizeof(float4)*ctx->npad;
+        CUDA_CHECK(cudaMemcpy(ctx->velmD.p, p, sizeof(double4)*ctx->npad, cudaMemcpyHostToDevice)); p += sizeof(double4)*ctx->npad;
+    }
+    else { CUDA_CHECK(cudaMemcpy(ctx->velm.p, p, sizeof(float4)*ctx->npad, cudaMemcpyHostToDevice)); p += sizeof(float4)*ctx->npad; }
     CUDA_CHECK(cudaMemcpy(ctx->cellOffset.p, p, sizeof(int)*3*ctx->npad, cudaMemcpyHostToDevice));
     CUDA_CHECK(cudaMemcpy(ctx->stepCounter.p, &h.rngStep, sizeof(unsigned long long), cudaMemcpyHostToDevice));
     host_set_state(ctx); ctx->velStale = false;
@@ -1634,6 +1728,9 @@ extern "C" int b200md_set_integrator(b200md_ctx* ctx, int kind, double dt, doubl
     in.vscale = (float) vscale;
     in.fscale = (float) (friction == 0 ? dt : (1-vscale)/friction);
     in.noisescale = (float) (kind == B200MD_INT_LANGEVIN_MIDDLE ? std::sqrt(1-vscale*vscale) : std::sqrt(kT*(1-vscale*vscale)));
+    in.dtD = dt; in.tolD = tol; in.kTD = kT; in.vscaleD = vscale;
+    in.fscaleD = friction == 0 ? dt : (1-vscale)/friction;
+    in.noisescaleD = kind == B200MD_INT_LANGEVIN_MIDDLE ? std::sqrt(1-vscale*vscale) : std::sqrt(kT*(1-vscale*vscale));
     in.stepCounter = ctx->stepCounter.p;
     in.fused = 0; in.cmEveryStep = 0; in.cmScratch = ctx->cmScratch.p; in.blocksDone = ctx->blocksDone.p;
     ctx->dt = dt; ctx->temperature = temperature; ctx->friction = friction;
@@ -1757,7 +1854,8 @@ extern "C" int b200md_step(b200md_ctx* ctx, int nsteps) {
 extern "C" int b200md_kinetic_energy(b200md_ctx* ctx, double* ke) {
     API_BEGIN(ctx)
     require(ctx->finalized, "kinetic_energy before finalize");
-    const float shift = (ctx->haveIntegrator && ctx->integ.kind != B200MD_INT_LANGEVIN_MIDDLE) ? 0.5f*ctx->integ.dt : 0.f;
+    const bool shifted = ctx->haveIntegrator && ctx->integ.kind != B200MD_INT_LANGEVIN_MIDDLE;
+    const double shift = !shifted ? 0.0 : ctx->mixed() ? 0.5*ctx->integ.dtD : (double) (0.5f*ctx->integ.dt);
     sync_positions(ctx); sync_velocities(ctx);
     CUDA_CHECK(cudaMemsetAsync(ctx->energy.p + EN_KE, 0, sizeof(double), ctx->stream));
     launch_kinetic_energy(ctx->nb, ctx->units, ctx->integ, shift, ctx->stream);
@@ -1770,8 +1868,8 @@ extern "C" int b200md_kinetic_energy(b200md_ctx* ctx, double* ke) {
 extern "C" int b200md_apply_constraints(b200md_ctx* ctx, double tol) {
     API_BEGIN(ctx)
     sync_positions(ctx);
-    launch_constrain_positions(ctx->nb, ctx->units, (float) tol, ctx->stream);
-    launch_ccma_apply(ctx->nb, ctx->ccma, false, (float) tol, ctx->stream);
+    launch_constrain_positions(ctx->nb, ctx->units, tol, ctx->stream);
+    launch_ccma_apply(ctx->nb, ctx->ccma, false, tol, ctx->stream);
     ctx->kernelLaunches++;
     CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
     API_END(ctx)
@@ -1780,8 +1878,8 @@ extern "C" int b200md_apply_velocity_constraints(b200md_ctx* ctx, double tol) {
     API_BEGIN(ctx)
     ctx->stepStateValid = false;
     sync_positions(ctx); sync_velocities(ctx);
-    launch_constrain_velocities(ctx->nb, ctx->units, (float) tol, ctx->stream);
-    launch_ccma_apply(ctx->nb, ctx->ccma, true, (float) tol, ctx->stream);
+    launch_constrain_velocities(ctx->nb, ctx->units, tol, ctx->stream);
+    launch_ccma_apply(ctx->nb, ctx->ccma, true, tol, ctx->stream);
     ctx->kernelLaunches++;
     CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
     API_END(ctx)
@@ -1796,6 +1894,7 @@ extern "C" int b200md_comm_unique_id(void* id128) {
 extern "C" int b200md_comm_init(b200md_ctx* ctx, int rank, int world, const void* id128) {
     API_BEGIN(ctx)
     require(!ctx->finalized, "comm_init must precede finalize");
+    require(!ctx->mixed() || world <= 1, "comm_init: mixed precision is not supported in multi-GPU runs (use Precision=single)");
     std::string err;
     if (!g_nccl.load(err)) throw std::runtime_error(err);
     NcclApi::Uid uid; memcpy(uid.b, id128, 128);
@@ -1888,20 +1987,30 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
     const int one = 1;
     double total = 0;
     // the integrate phase mutates the state: snapshot it and restore it after every repetition
-    DevBuf<float4> savePos, saveVel; unsigned long long saveStep = 0;
+    DevBuf<float4> savePos, saveVel, saveCorr; DevBuf<double4> saveVelD; unsigned long long saveStep = 0;
+    auto restoreState = [&]() {
+        CUDA_CHECK(cudaMemcpyAsync(c->posq.p, savePos.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
+        CUDA_CHECK(cudaMemcpyAsync(c->velm.p, saveVel.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
+        if (c->mixed()) {
+            CUDA_CHECK(cudaMemcpyAsync(c->posqCorr.p, saveCorr.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
+            CUDA_CHECK(cudaMemcpyAsync(c->velmD.p, saveVelD.p, sizeof(double4)*c->npad, cudaMemcpyDeviceToDevice, s));
+        }
+    };
     if (phase == 4) {
         require(c->haveIntegrator, "time_phase(integrate) before set_integrator");
         savePos.alloc(c->npad); saveVel.alloc(c->npad);
         CUDA_CHECK(cudaMemcpyAsync(savePos.p, c->posq.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
         CUDA_CHECK(cudaMemcpyAsync(saveVel.p, c->velm.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
+        if (c->mixed()) {
+            saveCorr.alloc(c->npad); saveVelD.alloc(c->npad);
+            CUDA_CHECK(cudaMemcpyAsync(saveCorr.p, c->posqCorr.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
+            CUDA_CHECK(cudaMemcpyAsync(saveVelD.p, c->velmD.p, sizeof(double4)*c->npad, cudaMemcpyDeviceToDevice, s));
+        }
         CUDA_CHECK(cudaMemcpyAsync(&saveStep, c->stepCounter.p, sizeof(saveStep), cudaMemcpyDeviceToHost, s));
         CUDA_CHECK(cudaStreamSynchronize(s));
     }
     for (int r = -2; r < reps; r++) {
-        if (phase == 4) {
-            CUDA_CHECK(cudaMemcpyAsync(c->posq.p, savePos.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
-            CUDA_CHECK(cudaMemcpyAsync(c->velm.p, saveVel.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
-        }
+        if (phase == 4) restoreState();
         if (phase == 5) CUDA_CHECK(cudaMemcpyAsync(&c->counters.p[CT_REBUILD], &one, sizeof(int), cudaMemcpyHostToDevice, s));
         if (phase == 0) { CUDA_CHECK(cudaMemsetAsync(&c->counters.p[CT_CURSOR], 0, sizeof(int), s)); CUDA_CHECK(cudaMemsetAsync(&c->counters.p[CT_PAIRSTART], 0, sizeof(int), s)); }      // the dynamic tile schedule starts from tile 0
         CUDA_CHECK(cudaEventRecord(e0, s));
@@ -1921,8 +2030,7 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
         if (r >= 0) total += ms;
     }
     if (phase == 4) {
-        CUDA_CHECK(cudaMemcpyAsync(c->posq.p, savePos.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
-        CUDA_CHECK(cudaMemcpyAsync(c->velm.p, saveVel.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
+        restoreState();
         CUDA_CHECK(cudaMemcpyAsync(c->stepCounter.p, &saveStep, sizeof(saveStep), cudaMemcpyHostToDevice, s));
         CUDA_CHECK(cudaStreamSynchronize(s));
     }

@@ -145,8 +145,14 @@ __device__ __forceinline__ void wrap_molecule(const NbDev& nb, int m) {
     const double sz = -(k[2]*(double) b.dcz);
     for (int t = begin; t < end; t++) {
         const int a = nb.molAtoms[t];
-        const float4 q = nb.posq[a];
-        nb.posq[a] = make_float4((float) ((double) q.x + sx), (float) ((double) q.y + sy), (float) ((double) q.z + sz), q.w);
+        if (nb.posqCorr) {          // mixed precision: hi + lo + shift in double, stored as hi / lo (no rounding to fp32)
+            const double4 q = load_pos<double>(nb, a);
+            store_pos<double>(nb, a, q.x + sx, q.y + sy, q.z + sz);
+        }
+        else {
+            const float4 q = nb.posq[a];
+            nb.posq[a] = make_float4((float) ((double) q.x + sx), (float) ((double) q.y + sy), (float) ((double) q.z + sz), q.w);
+        }
         nb.cellOffset[a] += k[0]; nb.cellOffset[a + nb.npad] += k[1]; nb.cellOffset[a + 2*nb.npad] += k[2];
     }
 }

@@ -29,12 +29,19 @@ def _i32(a):
     return np.ascontiguousarray(a, dtype=np.int32)
 
 
+PRECISIONS = {"single": 0, "mixed": 1}
+
+
 class Engine:
-    def __init__(self, desc: SystemDesc, device=0, comm=None):
-        """comm = (rank, world, unique_id_bytes) for the multi-GPU force decomposition."""
+    def __init__(self, desc: SystemDesc, device=0, comm=None, precision="single"):
+        """comm = (rank, world, unique_id_bytes) for the multi-GPU force decomposition.  precision: "single" (fp32 state) or
+        "mixed" (positions as fp32 hi + lo, velocities, integration and constraints in double; single GPU only)."""
+        if precision not in PRECISIONS:
+            raise ValueError("precision must be one of %s, not %r" % (sorted(PRECISIONS), precision))
         self.lib = _lib.load()
         self.desc = desc
         self.natoms = desc.natoms
+        self._precision = precision
         h = C.c_void_p()
         if self.lib.b200md_create(C.byref(h), device, self.natoms) != 0:
             raise EngineError(self.lib.b200md_last_error(None).decode())
@@ -55,6 +62,7 @@ class Engine:
             rank, world, uid = comm
             buf = C.create_string_buffer(bytes(uid), 128)
             self._ck(L.b200md_comm_init(self.h, rank, world, C.cast(buf, C.c_void_p)))
+        self._ck(L.b200md_set_precision(self.h, PRECISIONS[self._precision]))
         self._ck(L.b200md_set_masses(self.h, _dp(_f64(d.masses))))
         nd = _lib.NonbondedDesc()
         nd.method = d.method
@@ -89,6 +97,12 @@ class Engine:
             self._ck(L.b200md_set_box(self.h, _dp(b[0]), _dp(b[1]), _dp(b[2])))
         self._ck(L.b200md_finalize(self.h))
         self.set_positions(d.positions)
+
+    @property
+    def precision(self):
+        """"single" or "mixed", as the library reports it."""
+        p = self.lib.b200md_get_precision(self.h)
+        return {v: k for k, v in PRECISIONS.items()}[p]
 
     # ---- UpdateStateDataKernel ----
     def set_positions(self, x):

@@ -229,10 +229,13 @@ public:
         d.dropForces(); d.cmRequested = false;
         int64_t n = 0;
         stream.read((char*) &n, sizeof(n));
-        if (n <= 0 || n != b200md_checkpoint_save(d.ctx, nullptr, 0)) throw OpenMMException("B200 platform: checkpoint does not match this Context");
+        // a blob of the other precision differs in size; b200md_checkpoint_load reads its header and names the mismatch
+        const int64_t expect = b200md_checkpoint_save(d.ctx, nullptr, 0);
+        if (n <= 0 || n > 2*expect) throw OpenMMException("B200 platform: checkpoint does not match this Context");
         vector<char> buf(n);
         stream.read(buf.data(), n);
         d.check(b200md_checkpoint_load(d.ctx, buf.data(), n));
+        if (n != expect) throw OpenMMException("B200 platform: checkpoint does not match this Context");
     }
 };
 
@@ -665,13 +668,16 @@ public:
         try {
             string dev = properties.count(DeviceIndex()) ? properties.at(DeviceIndex()) : getPropertyDefaultValue(DeviceIndex());
             string prec = properties.count(Precision()) ? properties.at(Precision()) : getPropertyDefaultValue(Precision());
-            if (prec != "single") throw OpenMMException("B200 platform: only Precision=single is implemented");
+            // mixed: positions hi + lo, velocities, integration and constraints in double, forces in single precision (the
+            // reference GPU platforms' definition).  double is refused here, so OpenMM moves such a Context to another platform.
+            if (prec != "single" && prec != "mixed") throw OpenMMException("B200 platform: Precision=" + prec + " is not supported (single or mixed)");
             const System& system = context.getSystem();
             d->numParticles = system.getNumParticles();
             if (b200md_create(&d->ctx, atoi(dev.c_str()), d->numParticles) != 0)
                 throw OpenMMException(string("B200 platform: ") + b200md_last_error(nullptr));
             d->props[DeviceIndex()] = dev;
             d->props[Precision()] = prec;
+            d->check(b200md_set_precision(d->ctx, prec == "mixed" ? B200MD_PRECISION_MIXED : B200MD_PRECISION_SINGLE));
             vector<double> mass(d->numParticles);
             for (int i = 0; i < d->numParticles; i++) mass[i] = system.getParticleMass(i);
             d->check(b200md_set_masses(d->ctx, mass.data()));

@@ -11,10 +11,16 @@
 #include <iostream>
 #include <string>
 
+// -DB200_PRECISION='"mixed"' runs the same bodies with that Precision as the platform default, as
+// platforms/cuda/tests/CudaTests.h does with its precision argument
 static OpenMM::Platform& loadB200() {
     const char* path = getenv("B200_PLUGIN");
     OpenMM::Platform::loadPluginLibrary(path ? path : "libOpenMMB200.so");
-    return OpenMM::Platform::getPlatformByName("B200");
+    OpenMM::Platform& p = OpenMM::Platform::getPlatformByName("B200");
+#ifdef B200_PRECISION
+    p.setPropertyDefaultValue("Precision", B200_PRECISION);
+#endif
+    return p;
 }
 OpenMM::Platform& platform = loadB200();
 
