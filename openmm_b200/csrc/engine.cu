@@ -75,6 +75,11 @@ struct b200md_ctx {
     float softPad2 = 3e38f;
     bool overlapPme = true;
     bool useCond = true;
+    // brick path of the PME spread (pme.cu): B200MD_PME_BRICK=0 keeps the user-order kernel; B200MD_PME_BRICK_POINTS sets
+    // the brick capacity (a small one forces the global-memory fallback)
+    bool pmeBrick = true;
+    int brickAtoms = 64, brickPoints = 8192;
+    bool listBuilt = false;             // a neighbour list covers every atom (the brick path walks its sorted order)
     // ---- host copy of the system definition ----
     std::vector<double> mass, charge, sigma, epsilon;
     b200md_nonbonded_desc nbdesc{};
@@ -193,6 +198,8 @@ extern "C" int b200md_create(b200md_ctx** out, int device, int natoms) {
         CUDA_CHECK(cudaStreamCreateWithFlags(&c->stream2, cudaStreamNonBlocking));
         if (getenv("B200MD_NO_COND")) c->useCond = false;
         if (getenv("B200MD_NO_OVERLAP")) c->overlapPme = false;
+        if (getenv("B200MD_PME_BRICK")) c->pmeBrick = atoi(getenv("B200MD_PME_BRICK")) != 0;
+        if (getenv("B200MD_PME_BRICK_POINTS")) c->brickPoints = std::max(1, atoi(getenv("B200MD_PME_BRICK_POINTS")));
         int lo = 0, hi = 0;
         CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
         CUDA_CHECK(cudaStreamCreateWithPriority(&c->streamPme, cudaStreamNonBlocking, getenv("B200MD_PME_PRIO") && atoi(getenv("B200MD_PME_PRIO")) == 0 ? lo : hi));
@@ -881,6 +888,8 @@ static void setup_pme(b200md_ctx* c, int nx, int ny, int nz, double alpha) {
     cudaDeviceGetAttribute(&maxSmem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     if (fft_plane_smem_bytes(ny, nz) > (size_t) maxSmem || fft_line_smem_bytes(nx) > (size_t) maxSmem)
         throw std::runtime_error("B200 platform: PME grid plane does not fit in shared memory (max about 160x160 per slab)");
+    pme_brick_setup(maxSmem);
+    c->brickPoints = std::min(c->brickPoints, (maxSmem - 1024)/(int) sizeof(long long));
     c->grid.alloc((size_t) nx*ny*nz);
     c->gridFixed.alloc((size_t) nx*ny*nz);
     p.gridFixed = c->gridFixed.p;
@@ -1480,6 +1489,14 @@ static NbDev role_nb(const b200md_ctx* c) {
 }
 
 // ---------------------------------------------------------------- force evaluation
+// PME parameters of the next spread launch: the brick path needs a list that covers every atom on this GPU
+static PmeDev pme_for_launch(const b200md_ctx* c) {
+    PmeDev p = c->pme;
+    p.brickAtoms = (c->pmeBrick && c->world == 1 && !c->pmeOnly && c->listBuilt) ? c->brickAtoms : 0;
+    p.brickPoints = c->brickPoints;
+    return p;
+}
+
 // Enqueue one force evaluation on the stream (no host sync).  Returns the number of kernels launched.
 static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlreadyZero = false, bool inStep = false, unsigned int groupMask = 0xffffffffu) {
     int launches = 0;
@@ -1508,21 +1525,30 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     const bool fork = direct && recip && c->overlapPme && !(c->world > 1 && c->comm && !p2p);
     cudaStream_t sp = fork ? c->streamPme : s;
     if (p2p && !direct) { launch_pos_wait(c->nb, c->cd, s); launches++; }       // nobody else on this stream waits for the owners' position stores
-    if (fork) {
-        CUDA_CHECK(cudaEventRecord(c->evFork, s));
-        CUDA_CHECK(cudaStreamWaitEvent(sp, c->evFork, 0));
-    }
-    if (recip) {
-        launch_pme_spread(c->nb, c->pme, c->cd, sp); launches++;
-        if (p2p) { launch_grid_push(c->pme, c->cd, sp); launches++; }
-        else if (c->world > 1 && c->comm && !split) {
-            int rc = g_nccl.AllReduce(c->gridFixed.p, c->gridFixed.p, (size_t) c->pme.nx*c->pme.ny*c->pme.nz, NCCL_INT64, NCCL_SUM, c->comm, sp);
-            if (rc != 0) throw std::runtime_error("ncclAllReduce(grid) failed");
+    // The brick path of the spread walks the current list's sorted order, so when it runs beside direct space the
+    // fork comes after the list build: the list then cannot flip under it (a rebuild flips at the end of k_build_tiles,
+    // a successor built beside the step in k_integrate, after the join).  On one stream it runs before the build and reads
+    // the current list, which is complete even when stale.
+    const PmeDev pme = pme_for_launch(c);
+    const bool forkAfterList = fork && direct && pme.brickAtoms > 0;
+    auto launch_recip = [&]() {
+        if (fork) {
+            CUDA_CHECK(cudaEventRecord(c->evFork, s));
+            CUDA_CHECK(cudaStreamWaitEvent(sp, c->evFork, 0));
         }
-        launch_pme_fft_conv(c->nb, c->pme, c->cd, energy && (split || p2p || c->rank == 0), sp); launches += pme_fft_launch_count(c->pme);
-        launch_pme_gather(c->nb, c->pme, c->cd, sp); launches++;
-    }
-    if (fork) CUDA_CHECK(cudaEventRecord(c->evJoin, sp));
+        if (recip) {
+            launch_pme_spread(c->nb, pme, c->cd, sp); launches++;
+            if (p2p) { launch_grid_push(c->pme, c->cd, sp); launches++; }
+            else if (c->world > 1 && c->comm && !split) {
+                int rc = g_nccl.AllReduce(c->gridFixed.p, c->gridFixed.p, (size_t) c->pme.nx*c->pme.ny*c->pme.nz, NCCL_INT64, NCCL_SUM, c->comm, sp);
+                if (rc != 0) throw std::runtime_error("ncclAllReduce(grid) failed");
+            }
+            launch_pme_fft_conv(c->nb, c->pme, c->cd, energy && (split || p2p || c->rank == 0), sp); launches += pme_fft_launch_count(c->pme);
+            launch_pme_gather(c->nb, pme, c->cd, sp); launches++;
+        }
+        if (fork) CUDA_CHECK(cudaEventRecord(c->evJoin, sp));
+    };
+    if (!forkAfterList) launch_recip();
     bool joinList = false;
     if (direct) {
         cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
@@ -1596,6 +1622,7 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
             launch_list_build(c->nb, s); launches += list_build_launch_count();
         }
     }
+    if (forkAfterList) launch_recip();
     if (direct) { launch_pair(c->nb, energy, s); launches++; }
     int bterms = terms & (B200MD_TERM_BONDS | B200MD_TERM_ANGLES | B200MD_TERM_TORSIONS);
     if (c->haveNb) bterms |= terms & B200MD_TERM_NB_DIRECT;
@@ -1665,12 +1692,12 @@ static void prepare_list(b200md_ctx* c) {
         for (int r = 0; r < TILE_REGIONS; r++) worst = std::max(worst, cur[LC_TILES + r]);
         const int cap = c->nb.maxTiles/TILE_REGIONS;
         const bool overflow = h[CT_OVERFLOW] != 0;
-        if (!overflow && worst <= (int) (0.8*cap)) { c->listDirty = false; return; }
+        if (!overflow && worst <= (int) (0.8*cap)) { c->listDirty = false; c->listBuilt = true; return; }
         // grow: the counters keep counting past the capacity (flush_tile), so `worst` is the demand even after an overflow
         const int want = std::min(worst_pool_capacity(c), std::max(2*cap, (int) (1.5*worst) + 64));
         if (want <= cap) {
             if (overflow) throw std::runtime_error("B200 platform: neighbour-list tile capacity exceeded and cannot grow (" + std::to_string(c->nb.maxTiles) + " tiles)");
-            c->listDirty = false; return;
+            c->listDirty = false; c->listBuilt = true; return;
         }
         alloc_tile_pools(c, want);
         const int zero = 0, one = 1;
@@ -2016,9 +2043,9 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
         CUDA_CHECK(cudaEventRecord(e0, s));
         switch (phase) {
             case 0: launch_pair(nbv, false, s); break;
-            case 1: launch_pme_spread(nbv, c->pme, local, s); break;
+            case 1: launch_pme_spread(nbv, pme_for_launch(c), local, s); break;
             case 2: launch_pme_fft_conv(nbv, c->pme, local, false, s); break;
-            case 3: launch_pme_gather(nbv, c->pme, local, s); break;
+            case 3: launch_pme_gather(nbv, pme_for_launch(c), local, s); break;
             case 4: launch_integrate(nbv, c->units, c->integ, local, s); break;
             case 5: launch_list_build(nbv, s); break;
             case 6: launch_bonded(nbv, c->bd, B200MD_TERM_ALL, false, s); break;

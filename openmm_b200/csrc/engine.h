@@ -151,6 +151,11 @@ struct PmeDev {
     const double* moduli[3];
     FftPlanDev plan[3];          // x, y, z
     double alpha;
+    // brick path of the spread (pme.cu): each CTA takes brickAtoms consecutive atoms of the current neighbour list's sorted
+    // order and accumulates into a shared-memory box of at most brickPoints grid points.
+    // brickAtoms == 0: user atom order, straight to global memory (multi-GPU, stand-alone PME, no list built yet)
+    int brickAtoms;
+    int brickPoints;
 };
 
 struct BondedDev {
@@ -429,6 +434,7 @@ void launch_pme_eterm(const NbDev& nb, const PmeDev& pme, cudaStream_t s);
 void launch_pme_spread(const NbDev& nb, const PmeDev& pme, const CommDev& cd, cudaStream_t s);
 void launch_pme_fft_conv(const NbDev& nb, const PmeDev& pme, const CommDev& cd, bool energy, cudaStream_t s);
 void launch_pme_gather(const NbDev& nb, const PmeDev& pme, const CommDev& cd, cudaStream_t s);
+void pme_brick_setup(int maxSmem);
 void launch_grid_push(const PmeDev& pme, const CommDev& cd, cudaStream_t s);
 void launch_fft3d_r2c(const PmeDev& pme, cudaStream_t s);         // grid -> cgrid
 void launch_fft3d_c2r(const PmeDev& pme, cudaStream_t s);         // cgrid -> grid

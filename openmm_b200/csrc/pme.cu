@@ -7,6 +7,8 @@
 // forward-only stencil with periodic wrap, charges carry sqrt(ONE_4PI_EPS0).
 #include "engine.h"
 #include <algorithm>
+#include <climits>
+#include <stdexcept>
 
 #define ORDER B200MD_PME_ORDER
 
@@ -60,6 +62,124 @@ __device__ __forceinline__ bool grid_index(const float4& p, const NbDev& nb, con
     return ok;
 }
 
+// Shared-memory brick of the brick spread (launch_pme_spread with PmeDev::brickAtoms > 0): the box of grid points that the
+// stencils of one CTA's atoms touch.  Point (x, y, z) of the brick is grid point (org + (x, y, z)) mod n, z fastest.  A
+// contribution reaches the same grid point, with the same value, as in the user-order kernel, and the grid is an int64 sum,
+// so the regrouping changes no bit.
+struct Brick {
+    int ref[3];                  // grid index of the CTA's first contributing atom
+    int org[3];                  // brick origin, unwrapped (may lie outside [0, n))
+    int ext[3];                  // brick extent per axis
+    // periodic difference idx - ref on axis d, folded into (-n/2, n/2]
+    __device__ __forceinline__ int rel(const int* idx, int d, int n) const {
+        int r = idx[d] - ref[d];
+        if (2*r > n) r -= n; else if (2*r <= -n) r += n;
+        return r;
+    }
+    // brick coordinates of the stencil origin idx of an atom of this CTA
+    __device__ __forceinline__ int local(const int* idx, int d, int n) const { return ref[d] + rel(idx, d, n) - org[d]; }
+    __device__ __forceinline__ int points() const { return ext[0]*ext[1]*ext[2]; }
+    // grid index of brick coordinate u on axis d: org + u lies in (-n/2, 3n/2 + ORDER - 1), below 3n for n >= 3
+    __device__ __forceinline__ int wrap(int d, int u, int n) const {
+        int g = org[d] + u;
+        if (g < 0) g += n;
+        if (g >= n) g -= n;
+        if (g >= n) g -= n;
+        return g;
+    }
+};
+
+// slot k of the current list's sorted order: the user atom, or -1 when it contributes nothing (padding, zero charge)
+__device__ __forceinline__ int brick_atom(const NbDev& nb, const ListDev& L, int k, float4& p) {
+    if (k >= nb.npad) return -1;
+    const int a = L.sorig[k];
+    if (a < 0 || a >= nb.natoms) return -1;
+    p = nb.posq[a];
+    return p.w == 0.f ? -1 : a;
+}
+
+// Block-wide: bounds of the stencils of slots [k0, k0 + count) (count <= blockDim.x).  Indices are taken relative to the
+// first contributing atom with the periodic difference folded into (-n/2, n/2], so a run of atoms that straddles the
+// periodic boundary still gets a small brick.  Returns false (to all threads) when no slot contributes.
+__device__ __forceinline__ bool brick_bounds(const NbDev& nb, const PmeDev& pme, const ListDev& L, int k0, int count, Brick& B) {
+    __shared__ int sFirst, sRef[3], sLo[3], sHi[3];
+    const int n[3] = {pme.nx, pme.ny, pme.nz};
+    if (threadIdx.x == 0) {
+        sFirst = INT_MAX;
+        for (int d = 0; d < 3; d++) { sLo[d] = INT_MAX; sHi[d] = INT_MIN; }
+    }
+    __syncthreads();
+    int idx[3];
+    wreal fr[3];
+    float4 p;
+    const bool ok = (int) threadIdx.x < count && brick_atom(nb, L, k0 + threadIdx.x, p) >= 0 && grid_index(p, nb, pme, idx, fr);
+    if (ok) atomicMin(&sFirst, (int) threadIdx.x);
+    __syncthreads();
+    if (sFirst == INT_MAX) return false;
+    if ((int) threadIdx.x == sFirst) for (int d = 0; d < 3; d++) sRef[d] = idx[d];
+    __syncthreads();
+    for (int d = 0; d < 3; d++) B.ref[d] = sRef[d];
+    if (ok) {
+        for (int d = 0; d < 3; d++) {
+            const int r = B.rel(idx, d, n[d]);
+            atomicMin(&sLo[d], r); atomicMax(&sHi[d], r);
+        }
+    }
+    __syncthreads();
+    for (int d = 0; d < 3; d++) { B.org[d] = B.ref[d] + sLo[d]; B.ext[d] = sHi[d] - sLo[d] + ORDER; }
+    return true;
+}
+
+// 64-bit shared-memory add as two native 32-bit ATOMS.ADD with the carry of the low word moved into the high word: exact
+// modulo 2^64 whatever the order.  atomicAdd(unsigned long long*) on shared memory compiles to a compare-and-swap loop
+// (ATOMS.CAST.SPIN.64) on sm_90a, which retries whenever the atoms of one water hit the same point together.
+__device__ __forceinline__ void shared_add_u64(unsigned long long* p, unsigned long long v) {
+    unsigned int* w = (unsigned int*) p;
+    const unsigned int lo = (unsigned int) v;
+    const unsigned int old = atomicAdd(w, lo);
+    atomicAdd(w + 1, (unsigned int) (v >> 32) + (old + lo < old ? 1u : 0u));
+}
+
+// One atom's x-plane ix of the stencil: into the global grid, or (BRICK) into the CTA's brick.
+// integer accumulation: the grid (hence every force) is independent of the order of the atomics
+template <bool BRICK>
+__device__ __forceinline__ void spread_atom(const NbDev& nb, const PmeDev& pme, int a, const float4& p, int ix, unsigned long long* brick, const Brick& B) {
+    int idx[3];
+    wreal fr[3];
+    if (!grid_index(p, nb, pme, idx, fr)) return;
+    wreal tx[ORDER], ty[ORDER], tz[ORDER], dd[ORDER];
+    bspline(fr[0], tx, dd);
+    bspline(fr[1], ty, dd);
+    bspline(fr[2], tz, dd);
+    wreal txi = tx[0];
+#pragma unroll
+    for (int k = 1; k < ORDER; k++) if (ix == k) txi = tx[k];
+    int xi = idx[0] + ix; if (xi >= pme.nx) xi -= pme.nx;
+    const wreal qx = (nb.chargeD != nullptr ? nb.chargeD[a] : (double) p.w)*txi;
+    if (BRICK) {
+        unsigned long long* plane = brick + ((size_t) (B.local(idx, 0, pme.nx) + ix)*B.ext[1] + B.local(idx, 1, pme.ny))*B.ext[2] + B.local(idx, 2, pme.nz);
+#pragma unroll
+        for (int iy = 0; iy < ORDER; iy++) {
+            const wreal qxy = qx*ty[iy];
+#pragma unroll
+            for (int iz = 0; iz < ORDER; iz++)
+                shared_add_u64(plane + iy*B.ext[2] + iz, (unsigned long long) __double2ll_rn(qxy*tz[iz]*4294967296.0));
+        }
+        return;
+    }
+#pragma unroll
+    for (int iy = 0; iy < ORDER; iy++) {
+        int yi = idx[1] + iy; if (yi >= pme.ny) yi -= pme.ny;
+        const wreal qxy = qx*ty[iy];
+        long long* row = pme.gridFixed + ((size_t) xi*pme.ny + yi)*pme.nz;
+#pragma unroll
+        for (int iz = 0; iz < ORDER; iz++) {
+            int zi = idx[2] + iz; if (zi >= pme.nz) zi -= pme.nz;
+            atomicAdd((unsigned long long*) (row + zi), (unsigned long long) __double2ll_rn(qxy*tz[iz]*4294967296.0));
+        }
+    }
+}
+
 // 8 lanes per atom, lane ix < 5 owns one x-plane of the 5x5x5 stencil (25 grid points): five times more independent
 // atomics / loads in flight per atom than the one-thread-per-atom form (both kernels are L2-latency bound at 24k atoms).
 // Multi-GPU: every rank spreads the atoms it owns into its OWN full-size grid; k_grid_push then hands each x slab to its
@@ -78,29 +198,51 @@ __global__ void __launch_bounds__(128) k_pme_spread(NbDev nb, PmeDev pme, CommDe
     // the grid index/fraction is exact for fp32 inputs wherever the atom sits relative to the primary cell
     const float4 p = nb.posq[s];
     if (p.w == 0.f) return;
-    int idx[3];
-    wreal fr[3];
-    if (!grid_index(p, nb, pme, idx, fr)) return;
-    wreal tx[ORDER], ty[ORDER], tz[ORDER], dd[ORDER];
-    bspline(fr[0], tx, dd);
-    bspline(fr[1], ty, dd);
-    bspline(fr[2], tz, dd);
-    wreal txi = tx[0];
-#pragma unroll
-    for (int k = 1; k < ORDER; k++) if (ix == k) txi = tx[k];
-    int xi = idx[0] + ix; if (xi >= pme.nx) xi -= pme.nx;
-    const wreal qx = (nb.chargeD != nullptr ? nb.chargeD[s] : (double) p.w)*txi;
-#pragma unroll
-    for (int iy = 0; iy < ORDER; iy++) {
-        int yi = idx[1] + iy; if (yi >= pme.ny) yi -= pme.ny;
-        const wreal qxy = qx*ty[iy];
-        long long* row = pme.gridFixed + ((size_t) xi*pme.ny + yi)*pme.nz;
-#pragma unroll
-        for (int iz = 0; iz < ORDER; iz++) {
-            int zi = idx[2] + iz; if (zi >= pme.nz) zi -= pme.nz;
-            // integer accumulation: the grid (hence every force) is independent of the order of the atomics
-            atomicAdd((unsigned long long*) (row + zi), (unsigned long long) __double2ll_rn(qxy*tz[iz]*4294967296.0));
-        }
+    spread_atom<false>(nb, pme, s, p, ix, nullptr, Brick());
+}
+
+// Brick path of the spread (one GPU, a list exists): a CTA of 256 threads takes pme.brickAtoms consecutive slots of the
+// current list's sorted order, spatially compact, so their stencils fit a brick of a few thousand points.  The atoms go
+// into the brick in shared memory; then each non-zero brick point is added to the grid with ONE global atomic, coalesced
+// along z, instead of one per atom and stencil point.  A brick above pme.brickPoints (atoms that are not compact, e.g.
+// a stale order after set_positions moved molecules by lattice vectors) spreads those atoms straight to global memory.
+// The list must not flip while this runs: enqueue_forces forks the reciprocal-space stream after the list build.
+__global__ void __launch_bounds__(256) k_pme_spread_brick(NbDev nb, PmeDev pme) {
+    extern __shared__ unsigned long long brick[];
+    const ListDev& L = nb.list[nb.counters[CT_CUR] & 1];
+    const int count = pme.brickAtoms, k0 = blockIdx.x*count;
+    Brick B;
+    if (!brick_bounds(nb, pme, L, k0, count, B)) return;
+    const int npts = B.points();
+    const bool fits = npts <= pme.brickPoints;
+    if (fits) {
+        for (int c = threadIdx.x; c < npts; c += blockDim.x) brick[c] = 0ull;
+        __syncthreads();
+    }
+    const int ix = threadIdx.x & 7, g = threadIdx.x >> 3, ng = blockDim.x >> 3;
+    // the four atoms of a warp are ng/4 slots apart: consecutive slots (the atoms of one water) hit the same points
+    const int perm = (g & 3)*(ng >> 2) + (g >> 2);
+    for (int j = 0; j < count; j += ng) {
+        float4 p;
+        const int a = (j + perm < count && ix < ORDER) ? brick_atom(nb, L, k0 + j + perm, p) : -1;
+        if (a < 0) continue;
+        if (fits) spread_atom<true>(nb, pme, a, p, ix, brick, B);
+        else spread_atom<false>(nb, pme, a, p, ix, nullptr, B);
+    }
+    if (!fits) return;
+    __syncthreads();
+    // consecutive threads take consecutive points (coalesced along z); each thread steps its (x, y, z) by blockDim.x points
+    // with carries instead of dividing per point
+    int z = threadIdx.x % B.ext[2], y = threadIdx.x / B.ext[2], x = y / B.ext[1];
+    y -= x*B.ext[1];
+    const int dz = blockDim.x % B.ext[2], dy0 = blockDim.x / B.ext[2], dx = dy0 / B.ext[1], dy = dy0 - dx*B.ext[1];
+    for (int c = threadIdx.x; c < npts; c += blockDim.x) {
+        const unsigned long long v = brick[c];
+        if (v != 0ull)
+            atomicAdd((unsigned long long*) pme.gridFixed + ((size_t) B.wrap(0, x, pme.nx)*pme.ny + B.wrap(1, y, pme.ny))*pme.nz + B.wrap(2, z, pme.nz), v);
+        z += dz; y += dy; x += dx;
+        if (z >= B.ext[2]) { z -= B.ext[2]; y++; }
+        if (y >= B.ext[1]) { y -= B.ext[1]; x++; }
     }
 }
 
@@ -195,8 +337,20 @@ void launch_pme_eterm(const NbDev& nb, const PmeDev& pme, cudaStream_t s) {
     k_pme_eterm<<<(unsigned) ((total + 255)/256), 256, 0, s>>>(nb, pme);
 }
 
+// allows the brick spread all the dynamic shared memory a CTA can opt in to (maxSmem bytes with their static shared memory)
+// on the current device; each launch asks for what it uses
+void pme_brick_setup(int maxSmem) {
+    cudaFuncAttributes fa;
+    CUDA_CHECK(cudaFuncGetAttributes(&fa, k_pme_spread_brick));
+    CUDA_CHECK(cudaFuncSetAttribute(k_pme_spread_brick, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem - (int) fa.sharedSizeBytes));
+}
+
 void launch_pme_spread(const NbDev& nb, const PmeDev& pme, const CommDev& cd, cudaStream_t s) {
     cudaMemsetAsync(pme.gridFixed, 0, sizeof(long long)*(size_t) pme.nx*pme.ny*pme.nz, s);
+    if (pme.brickAtoms > 0) {
+        k_pme_spread_brick<<<(nb.npad + pme.brickAtoms - 1)/pme.brickAtoms, 256, sizeof(long long)*pme.brickPoints, s>>>(nb, pme);
+        return;
+    }
     const int per = cd.world > 1 ? cd.atomLo[cd.rank + 1] - cd.atomLo[cd.rank] : (nb.natoms + nb.world - 1)/nb.world;
     k_pme_spread<<<std::max(1, (per*8 + 127)/128), 128, 0, s>>>(nb, pme, cd);
 }
