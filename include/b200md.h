@@ -213,8 +213,6 @@ typedef struct b200md_stats {
     int     pme_grid[3];
     double  ewald_alpha;
     int     overflow;             /* sticky: tile capacity exceeded at some point               */
-    int     stale_list_steps;     /* B200MD_ASYNC_LIST=1 only: steps served by a list whose skin was exceeded
-                                   * within that one step (see k_check_gather); 0 in any sane simulation */
     int64_t graph_instantiations; /* executable step graphs instantiated so far (a box change updates them in place) */
 } b200md_stats;
 int b200md_get_stats(b200md_ctx* ctx, b200md_stats* out);

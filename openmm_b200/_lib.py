@@ -16,7 +16,7 @@ class Stats(C.Structure):
     _fields_ = [("natoms", C.c_int64), ("padded_atoms", C.c_int64), ("num_blocks", C.c_int64), ("num_tiles", C.c_int64),
                 ("num_mask_tiles", C.c_int64), ("list_builds", C.c_int64), ("force_evals", C.c_int64),
                 ("kernel_launches", C.c_int64), ("pairs_in_cutoff", C.c_int64), ("pme_grid", C.c_int*3),
-                ("ewald_alpha", C.c_double), ("overflow", C.c_int), ("stale_list_steps", C.c_int),
+                ("ewald_alpha", C.c_double), ("overflow", C.c_int),
                 ("graph_instantiations", C.c_int64)]
 
 

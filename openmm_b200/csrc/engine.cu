@@ -63,18 +63,11 @@ struct b200md_ctx {
     bool finalized = false;
     std::string err;
     cudaStream_t stream = nullptr;
-    cudaStream_t stream2 = nullptr;     // body capture of conditional graph nodes
     cudaStream_t streamPme = nullptr;   // reciprocal space runs concurrently with direct space (high priority: its kernels are small)
-    cudaStream_t streamList = nullptr;  // the successor neighbour list is built here, beside the tile kernel
-    cudaEvent_t evFork = nullptr, evJoin = nullptr, evListFork = nullptr, evListJoin = nullptr;
-    bool asyncList = false;             // B200MD_ASYNC_LIST=1: build the successor list beside the step (see enqueue_forces)
-    bool specPair = true;               // step graphs: the tile kernel does not wait for a rebuild IF node (needs asyncList)
+    cudaEvent_t evFork = nullptr, evJoin = nullptr;
     bool pmeOnly = false;               // b200md_pme_create: reciprocal space only, no neighbour list is ever built
     bool listDirty = true;              // state changed from outside: rebuild synchronously before the next step graph
-    double softFrac = 0.7;
-    float softPad2 = 3e38f;
     bool overlapPme = true;
-    bool useCond = true;
     // brick path of the PME spread (pme.cu): B200MD_PME_BRICK=0 keeps the user-order kernel; B200MD_PME_BRICK_POINTS sets
     // the brick capacity (a small one forces the global-memory fallback)
     bool pmeBrick = true;
@@ -195,22 +188,14 @@ extern "C" int b200md_create(b200md_ctx** out, int device, int natoms) {
         c->npad = ((natoms + 31)/32)*32;
         c->nblocks = c->npad/32;
         CUDA_CHECK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-        CUDA_CHECK(cudaStreamCreateWithFlags(&c->stream2, cudaStreamNonBlocking));
-        if (getenv("B200MD_NO_COND")) c->useCond = false;
         if (getenv("B200MD_NO_OVERLAP")) c->overlapPme = false;
         if (getenv("B200MD_PME_BRICK")) c->pmeBrick = atoi(getenv("B200MD_PME_BRICK")) != 0;
         if (getenv("B200MD_PME_BRICK_POINTS")) c->brickPoints = std::max(1, atoi(getenv("B200MD_PME_BRICK_POINTS")));
-        int lo = 0, hi = 0;
-        CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-        CUDA_CHECK(cudaStreamCreateWithPriority(&c->streamPme, cudaStreamNonBlocking, getenv("B200MD_PME_PRIO") && atoi(getenv("B200MD_PME_PRIO")) == 0 ? lo : hi));
+        int hi = 0;
+        CUDA_CHECK(cudaDeviceGetStreamPriorityRange(nullptr, &hi));
+        CUDA_CHECK(cudaStreamCreateWithPriority(&c->streamPme, cudaStreamNonBlocking, hi));
         CUDA_CHECK(cudaEventCreateWithFlags(&c->evFork, cudaEventDisableTiming));
         CUDA_CHECK(cudaEventCreateWithFlags(&c->evJoin, cudaEventDisableTiming));
-        CUDA_CHECK(cudaStreamCreateWithFlags(&c->streamList, cudaStreamNonBlocking));
-        CUDA_CHECK(cudaEventCreateWithFlags(&c->evListFork, cudaEventDisableTiming));
-        CUDA_CHECK(cudaEventCreateWithFlags(&c->evListJoin, cudaEventDisableTiming));
-        if (getenv("B200MD_ASYNC_LIST")) c->asyncList = atoi(getenv("B200MD_ASYNC_LIST")) != 0;
-        if (getenv("B200MD_SOFT_FRACTION")) c->softFrac = atof(getenv("B200MD_SOFT_FRACTION"));
-        if (getenv("B200MD_SPEC_PAIR")) c->specPair = atoi(getenv("B200MD_SPEC_PAIR")) != 0;
         c->mass.assign(natoms, 1.0);
         c->charge.assign(natoms, 0.0); c->sigma.assign(natoms, 1.0); c->epsilon.assign(natoms, 0.0);
         const char* pf = getenv("B200MD_PAD_FRACTION");
@@ -233,13 +218,9 @@ extern "C" void b200md_destroy(b200md_ctx* ctx) {
     for (int q = 0; q < B200MD_MAX_RANKS; q++) if (ctx->peerMapped[q]) cudaIpcCloseMemHandle(ctx->peerMapped[q]);
     if (ctx->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(ctx->comm);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
-    if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
     if (ctx->streamPme) cudaStreamDestroy(ctx->streamPme);
     if (ctx->evFork) cudaEventDestroy(ctx->evFork);
     if (ctx->evJoin) cudaEventDestroy(ctx->evJoin);
-    if (ctx->streamList) cudaStreamDestroy(ctx->streamList);
-    if (ctx->evListFork) cudaEventDestroy(ctx->evListFork);
-    if (ctx->evListJoin) cudaEventDestroy(ctx->evListJoin);
     char* window = ctx->window;
     delete ctx;
     if (window) cudaFree(window);
@@ -372,7 +353,7 @@ static void setup_cells(b200md_ctx* c) {
         std::vector<int> rank;
         cell_order(nc, rank);
         c->cellRank.upload(rank);
-        c->cellCount.alloc(ncells + 1); c->cellCount.zero();     // every list build leaves them zeroed again (k_block_bounds)
+        c->cellCount.alloc(ncells + 1); c->cellCount.zero();     // every list build leaves them zeroed again (k_list_prep)
         c->cellFill.alloc(ncells); c->cellFill.zero();
         c->nb.ncells = ncells;
         for (int d = 0; d < 3; d++) c->nb.ncell[d] = nc[d];
@@ -1067,12 +1048,10 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     c->cd = CommDev{}; c->cd.world = 1;
     c->p2p = c->world > 1 && c->comm && !(getenv("B200MD_MGPU") && std::string(getenv("B200MD_MGPU")) == "nccl");
     if (c->p2p) setup_window(c);
-    nb.useRational = getenv("B200MD_PAIR_RATIONAL") ? atoi(getenv("B200MD_PAIR_RATIONAL")) : 0;
-    nb.pairDynamic = getenv("B200MD_PAIR_DYNAMIC") ? atoi(getenv("B200MD_PAIR_DYNAMIC")) : 0;
     { const double cc = getenv("B200MD_CLOSE_NM") ? atof(getenv("B200MD_CLOSE_NM")) : 0.36; nb.closeCut2 = (float) (cc*cc); }
-    nb.packCull = getenv("B200MD_BT_PACK") ? atoi(getenv("B200MD_BT_PACK")) : 1;
     // SM partition between the tile kernel and the reciprocal-space chain (B200MD_PME_SMS=k reserves k SMs; 0 = off)
     for (int w = 0; w < 4; w++) nb.pmeSmMask[w] = 0ull;
+    nb.smPartition = false;
     // Off on one GPU (measured: the chain is latency bound and needs most SMs to be short, profiles/r02_sm_partition.md).
     // Multi-GPU (peer-memory data plane): the chain is a sequence of kernels that wait for the other ranks, and behind a tile
     // kernel that holds every SM it would only start when that has drained; here the default reserves as many SMs as the rank
@@ -1085,7 +1064,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
         if (getenv("B200MD_PME_SMS")) want = atoi(getenv("B200MD_PME_SMS"));
         const int got = want > 0 ? choose_pme_sms(want, nb.pmeSmMask) : 0;
         if (got > 0) {
-            nb.pairDynamic = 2;
+            nb.smPartition = true;
             const int planes = (c->nbdesc.grid[0] + c->world - 1)/c->world;
             fft_set_compact(planes > got ? 2 : 1);
         }
@@ -1127,14 +1106,11 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     const double rc = c->nbdesc.cutoff;
     if (nb.method == B200MD_NB_NOCUTOFF) {
         nb.cutoff = 1e18f; nb.cutoff2 = 3e38f; nb.paddedCutoff2 = 3e38f; nb.halfPad2 = 3e38f;
-        c->softPad2 = 3e38f;
     }
     else {
         const double pad = c->padFrac*rc;
         nb.cutoff = (float) rc; nb.cutoff2 = (float) (rc*rc); nb.paddedCutoff2 = (float) ((rc+pad)*(rc+pad)); nb.halfPad2 = (float) (0.25*pad*pad);
-        c->softPad2 = (float) (0.25*pad*pad*c->softFrac*c->softFrac);
     }
-    nb.softPad2 = 3e38f; nb.condAsync = 0ull;
     nb.useSwitch = c->nbdesc.use_switch; nb.switchDist = (float) c->nbdesc.switch_distance;
     nb.alpha = (float) c->nbdesc.ewald_alpha;
     if (nb.method == B200MD_NB_CUTOFF_PERIODIC || nb.method == B200MD_NB_CUTOFF_NONPERIODIC) {
@@ -1196,8 +1172,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     // and the reciprocal-space rank builds no list) ----
     c->cellOffset.alloc((size_t) 3*NP); c->cellOffset.zero();
     nb.cellOffset = c->cellOffset.p; nb.nmol = 0; nb.molStart = nullptr; nb.molAtoms = nullptr;
-    // (also off with B200MD_ASYNC_LIST=1: the side-stream build would move molecules while bonded / PME kernels read them)
-    if ((nb.method == B200MD_NB_CUTOFF_PERIODIC || nb.method == B200MD_NB_PME) && c->world == 1 && !c->pmeOnly && !c->asyncList && !getenv("B200MD_NO_WRAP")) {
+    if ((nb.method == B200MD_NB_CUTOFF_PERIODIC || nb.method == B200MD_NB_PME) && c->world == 1 && !c->pmeOnly) {
         std::vector<int> parent(N);
         for (int i = 0; i < N; i++) parent[i] = i;
         auto find = [&](int x) { while (parent[x] != x) { parent[x] = parent[parent[x]]; x = parent[x]; } return x; };
@@ -1516,7 +1491,7 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
         if (c->rank == pmeRank) direct = false; else recip = false;
         c->nb = role_nb(c);
     }
-    struct Restore { b200md_ctx* c; NbDev saved; ~Restore() { unsigned long long h = c->nb.condHandle; c->nb = saved; c->nb.condHandle = h; } } restore{c, nbSave};
+    struct Restore { b200md_ctx* c; NbDev saved; ~Restore() { c->nb = saved; } } restore{c, nbSave};
     // Reciprocal space (spread -> FFT/convolution -> gather, in USER atom order: independent of the neighbour list) and
     // direct space (list check / rebuild, tile kernel, bonded terms) are independent until the integrator: fork them onto
     // two streams (also inside the captured step graph).  Both accumulate into the same fixed-point force buffer, so the
@@ -1526,9 +1501,8 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     cudaStream_t sp = fork ? c->streamPme : s;
     if (p2p && !direct) { launch_pos_wait(c->nb, c->cd, s); launches++; }       // nobody else on this stream waits for the owners' position stores
     // The brick path of the spread walks the current list's sorted order, so when it runs beside direct space the
-    // fork comes after the list build: the list then cannot flip under it (a rebuild flips at the end of k_build_tiles,
-    // a successor built beside the step in k_integrate, after the join).  On one stream it runs before the build and reads
-    // the current list, which is complete even when stale.
+    // fork comes after the list build: the list then cannot flip under it (a rebuild flips at the end of k_build_tiles).
+    // On one stream it runs before the build and reads the current list, which is complete even when stale.
     const PmeDev pme = pme_for_launch(c);
     const bool forkAfterList = fork && direct && pme.brickAtoms > 0;
     auto launch_recip = [&]() {
@@ -1549,78 +1523,9 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
         if (fork) CUDA_CHECK(cudaEventRecord(c->evJoin, sp));
     };
     if (!forkAfterList) launch_recip();
-    bool joinList = false;
     if (direct) {
-        cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-        cudaGraph_t graph = nullptr;
-        const cudaGraphNode_t* deps = nullptr;
-        size_t ndeps = 0;
-        CUDA_CHECK(cudaStreamGetCaptureInfo_v2(s, &cap, nullptr, &graph, &deps, &ndeps));
-        // With the two-launch list build a NOT-taken rebuild costs ~4 us of gated kernels in front of the tile kernel, an IF
-        // node ~15 us: the IF nodes are kept for the 7-launch build and for the side-stream successor build only.
-        const bool wantCond = c->useCond && (!list_build_merged() || (inStep && c->asyncList && c->softPad2 < c->nb.halfPad2));
-        if (cap == cudaStreamCaptureStatusActive && wantCond) {
-            // the rebuild kernels live in an IF node of the step graph: zero launches on the (usual) steps without a rebuild
-            // Inside a step, a second IF node builds the SUCCESSOR list on a side stream as soon as some atom has used up
-            // softFrac of its allowance: the current list is still valid for this step's forces, the new one takes over when
-            // the integrator has finished (k_integrate's last block flips counters[CT_CUR]), so the rebuild leaves the
-            // critical path.  The first IF node remains as the synchronous fallback (state set from outside, or a
-            // displacement that jumps past the hard limit within one step).
-            const bool async = inStep && c->asyncList && c->softPad2 < c->nb.halfPad2;
-            // spec: no synchronous IF node at all in step graphs (an IF node costs ~15 us of latency on this driver, taken
-            // or not, and the tile kernel would sit behind it every step); b200md_step rebuilds eagerly after any
-            // outside change of the state, and k_check_gather documents the one-step corner case
-            const bool spec = async && c->specPair;
-            cudaGraphConditionalHandle h = 0, ha = 0;
-            if (!spec) CUDA_CHECK(cudaGraphConditionalHandleCreate(&h, graph, 0, cudaGraphCondAssignDefault));
-            if (async) CUDA_CHECK(cudaGraphConditionalHandleCreate(&ha, graph, 0, cudaGraphCondAssignDefault));
-            c->nb.condHandle = (unsigned long long) h;
-            c->nb.condAsync = async ? (unsigned long long) ha : 0ull;
-            c->nb.softPad2 = async ? c->softPad2 : 3e38f;
-            launch_check_displacement(c->nb, c->cd, s); launches++;
-            NbDev nbBody = c->nb;
-            cudaGraph_t tmp;
-            if (!spec) {
-                CUDA_CHECK(cudaStreamGetCaptureInfo_v2(s, &cap, nullptr, &graph, &deps, &ndeps));
-                cudaGraphNodeParams np = {cudaGraphNodeTypeConditional};
-                np.type = cudaGraphNodeTypeConditional;
-                np.conditional.handle = h;
-                np.conditional.type = cudaGraphCondTypeIf;
-                np.conditional.size = 1;
-                cudaGraphNode_t node;
-                CUDA_CHECK(cudaGraphAddNode(&node, graph, deps, ndeps, &np));
-                cudaGraph_t body = np.conditional.phGraph_out[0];
-                CUDA_CHECK(cudaStreamBeginCaptureToGraph(c->stream2, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
-                launch_list_build(nbBody, c->stream2);
-                CUDA_CHECK(cudaStreamEndCapture(c->stream2, &tmp));
-                CUDA_CHECK(cudaStreamUpdateCaptureDependencies(s, &node, 1, cudaStreamSetCaptureDependencies));
-            }
-            if (async) {
-                cudaStream_t sl = c->streamList;
-                CUDA_CHECK(cudaEventRecord(c->evListFork, s));
-                CUDA_CHECK(cudaStreamWaitEvent(sl, c->evListFork, 0));
-                CUDA_CHECK(cudaStreamGetCaptureInfo_v2(sl, &cap, nullptr, &graph, &deps, &ndeps));
-                cudaGraphNodeParams np2 = {cudaGraphNodeTypeConditional};
-                np2.type = cudaGraphNodeTypeConditional;
-                np2.conditional.handle = ha;
-                np2.conditional.type = cudaGraphCondTypeIf;
-                np2.conditional.size = 1;
-                cudaGraphNode_t node2;
-                CUDA_CHECK(cudaGraphAddNode(&node2, graph, deps, ndeps, &np2));
-                CUDA_CHECK(cudaStreamBeginCaptureToGraph(c->stream2, np2.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
-                launch_list_build(nbBody, c->stream2, 1);
-                CUDA_CHECK(cudaStreamEndCapture(c->stream2, &tmp));
-                CUDA_CHECK(cudaStreamUpdateCaptureDependencies(sl, &node2, 1, cudaStreamSetCaptureDependencies));
-                CUDA_CHECK(cudaEventRecord(c->evListJoin, sl));
-                joinList = true;
-            }
-            c->nb.condHandle = 0ull; c->nb.condAsync = 0ull; c->nb.softPad2 = 3e38f;
-        }
-        else {
-            c->nb.condHandle = 0ull;
-            launch_check_displacement(c->nb, c->cd, s); launches++;
-            launch_list_build(c->nb, s); launches += list_build_launch_count();
-        }
+        launch_check_displacement(c->nb, c->cd, s); launches++;
+        launch_list_build(c->nb, s); launches += LIST_BUILD_LAUNCHES;
     }
     if (forkAfterList) launch_recip();
     if (direct) { launch_pair(c->nb, energy, s); launches++; }
@@ -1634,7 +1539,6 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     const bool pushEarly = p2p && fork;
     if (pushEarly) { launch_force_push(c->nb, c->cd, s); launches++; }
     if (fork) CUDA_CHECK(cudaStreamWaitEvent(s, c->evJoin, 0));
-    if (joinList) CUDA_CHECK(cudaStreamWaitEvent(s, c->evListJoin, 0));
     if (p2p) {
         if (!pushEarly) { launch_force_push(c->nb, c->cd, s); launches++; }
         // in the step path k_integrate totals own partial + inboxes; here (energies, getState) the owners total and broadcast
@@ -1679,8 +1583,8 @@ static void prepare_list(b200md_ctx* c) {
     for (int attempt = 0; attempt < 8; attempt++) {
         const NbDev nb = role_nb(c);
         launch_check_displacement(nb, c->cd, c->stream);
-        launch_list_build(nb, c->stream, 0);
-        c->kernelLaunches += 1 + list_build_launch_count();
+        launch_list_build(nb, c->stream);
+        c->kernelLaunches += 1 + LIST_BUILD_LAUNCHES;
         int h[16], lc[2*LC_STRIDE];
         CUDA_CHECK(cudaMemcpyAsync(h, c->counters.p, sizeof(int)*16, cudaMemcpyDeviceToHost, c->stream));
         CUDA_CHECK(cudaMemcpyAsync(lc, c->listCounters.p, sizeof(lc), cudaMemcpyDeviceToHost, c->stream));
@@ -1795,32 +1699,15 @@ extern "C" int b200md_integrate_only(b200md_ctx* ctx) {
 
 // Capture `nsteps` steps into *exec.  An executable graph that exists already is updated in place with cudaGraphExecUpdate (a
 // box change or a grown tile pool changes kernel parameters, not the topology) and instantiated anew only when the driver
-// refuses the update.  Graphs with conditional (IF) nodes -- B200MD_LIST_MERGED=0 or B200MD_ASYNC_LIST=1 -- are always
-// instantiated anew: every capture creates new conditional handles, which the kernels that set them carry as parameters.
+// refuses the update.
 static void capture_steps(b200md_ctx* c, int nsteps, cudaGraphExec_t* exec, int* launches) {
     cudaGraph_t g;
     CUDA_CHECK(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
     int l = 0;
     try { for (int k = 0; k < nsteps; k++) l += enqueue_step(c); } catch (...) { cudaStreamEndCapture(c->stream, &g); throw; }
     CUDA_CHECK(cudaStreamEndCapture(c->stream, &g));
-    if (getenv("B200MD_DEBUG_PRIO")) {
-        size_t n = 0;
-        CUDA_CHECK(cudaGraphGetNodes(g, nullptr, &n));
-        std::vector<cudaGraphNode_t> nodes(n);
-        CUDA_CHECK(cudaGraphGetNodes(g, nodes.data(), &n));
-        for (size_t i = 0; i < n; i++) {
-            cudaGraphNodeType t;
-            CUDA_CHECK(cudaGraphNodeGetType(nodes[i], &t));
-            if (t != cudaGraphNodeTypeKernel) { fprintf(stderr, "node %zu type %d\n", i, (int) t); continue; }
-            cudaLaunchAttributeValue v;
-            memset(&v, 0, sizeof(v));
-            cudaError_t e = cudaGraphKernelNodeGetAttribute(nodes[i], cudaLaunchAttributePriority, &v);
-            fprintf(stderr, "node %zu kernel priority %d (%s)\n", i, v.priority, cudaGetErrorString(e));
-        }
-    }
     *launches = l;
-    const bool cond = c->useCond && (!list_build_merged() || (c->asyncList && c->softPad2 < c->nb.halfPad2));
-    if (*exec && !cond) {
+    if (*exec) {
         cudaGraphExecUpdateResultInfo info;
         if (cudaGraphExecUpdate(*exec, g, &info) == cudaSuccess) { cudaGraphDestroy(g); return; }
         (void) cudaGetLastError();          // the refusal is not sticky: fall back to a new instantiation
@@ -1993,7 +1880,7 @@ extern "C" int b200md_get_stats(b200md_ctx* ctx, b200md_stats* out) {
         const int* cur = lc + LC_STRIDE*(h[CT_CUR] & 1);
         int masks = 0;
         for (int r = 0; r < TILE_REGIONS; r++) masks += cur[LC_MASKS + r];
-        out->num_tiles = cur[LC_USED]; out->num_mask_tiles = masks; out->overflow = h[CT_OVERFLOW]; out->list_builds = h[CT_BUILDS]; out->pairs_in_cutoff = h[CT_PAIRS]; out->stale_list_steps = h[CT_STALE];
+        out->num_tiles = cur[LC_USED]; out->num_mask_tiles = masks; out->overflow = h[CT_OVERFLOW]; out->list_builds = h[CT_BUILDS]; out->pairs_in_cutoff = h[CT_PAIRS];
     }
     out->force_evals = ctx->forceEvals; out->kernel_launches = ctx->kernelLaunches; out->graph_instantiations = ctx->graphInstantiations;
     out->pme_grid[0] = ctx->pme.nx; out->pme_grid[1] = ctx->pme.ny; out->pme_grid[2] = ctx->pme.nz; out->ewald_alpha = ctx->pme.alpha;
@@ -2039,7 +1926,7 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
     for (int r = -2; r < reps; r++) {
         if (phase == 4) restoreState();
         if (phase == 5) CUDA_CHECK(cudaMemcpyAsync(&c->counters.p[CT_REBUILD], &one, sizeof(int), cudaMemcpyHostToDevice, s));
-        if (phase == 0) { CUDA_CHECK(cudaMemsetAsync(&c->counters.p[CT_CURSOR], 0, sizeof(int), s)); CUDA_CHECK(cudaMemsetAsync(&c->counters.p[CT_PAIRSTART], 0, sizeof(int), s)); }      // the dynamic tile schedule starts from tile 0
+        if (phase == 0) { CUDA_CHECK(cudaMemsetAsync(&c->counters.p[CT_CURSOR], 0, sizeof(int), s)); CUDA_CHECK(cudaMemsetAsync(&c->counters.p[CT_PAIRSTART], 0, sizeof(int), s)); }      // the SM-partitioned tile kernel's cursor starts from tile 0
         CUDA_CHECK(cudaEventRecord(e0, s));
         switch (phase) {
             case 0: launch_pair(nbv, false, s); break;

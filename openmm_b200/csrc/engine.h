@@ -69,7 +69,7 @@ enum { LC_TILES = 0, LC_MASKS = TILE_REGIONS, LC_MAXHALF = 2*TILE_REGIONS, LC_US
 
 // indices into NbDev::counters
 enum { CT_PAIRSTART = 0,      // SM partition: CTAs of the tile kernel that have started (see k_pair)
-       CT_REBUILD = 2, CT_OVERFLOW = 3, CT_BUILDS = 4, CT_PAIRS = 5, CT_LASTBLOCK = 8, CT_CUR = 10, CT_SOFT = 11, CT_PENDING = 12, CT_STALE = 13, CT_CURSOR = 14,
+       CT_REBUILD = 2, CT_OVERFLOW = 3, CT_BUILDS = 4, CT_PAIRS = 5, CT_CUR = 10, CT_CURSOR = 14,
        CT_BTDONE = 7, CT_BAR = 9, CT_BAREXIT = 15 };      // k_build_tiles completion count; grid barrier of k_list_prep
 
 struct NbDev {
@@ -94,8 +94,7 @@ struct NbDev {
     long long* force;            // [3][npad] fixed point, user order
     double* energy;              // [B200MD_NUM_ENERGY] accumulators
     // sorted (nonbonded) copies, blocks and tiles: two complete lists.  counters[CT_CUR] names the one the tile kernel reads;
-    // a rebuild always fills the other one and flips (at once when the current list is no longer valid, at the end of the
-    // step when the successor was built beside the step: see k_check_gather)
+    // a rebuild always fills the other one and flips at the end of k_build_tiles
     ListDev list[2];
     int* sortedOf;               // user atom -> sorted slot (of the list built last; list construction only)
     float4* refPos;              // user-order positions at the last list build
@@ -121,23 +120,17 @@ struct NbDev {
     const int* molAtoms;
     int* cellOffset;             // [3][npad] lattice vector counts to ADD when reporting positions
     float halfPad2;              // (padding/2)^2: beyond this displacement the current list is invalid
-    float softPad2;              // displacement^2 at which the successor list is built beside the step (3e38: never)
     // multi-GPU sharding of the tile list / PME atoms
     int rank, world;
     // origin of the primary periodic cell used for binning (chosen at set_positions so that a structure centred anywhere,
     // e.g. a PDB centred on 0, is binned WITHOUT lattice shifts: a shift costs one fp32 rounding of the coordinate)
     double origin[3];
-    // CUDA-graph conditional node that holds the list-rebuild kernels (0 = none: rebuild kernels are gated on counters[CT_REBUILD])
-    unsigned long long condHandle;
-    unsigned long long condAsync;   // second IF node: build of the successor list on a side stream
-    int packCull;                // k_build_tiles: exact cull on full warps (B200MD_BT_PACK)
-    int pairDynamic;             // tile kernel fetches tiles from a cursor instead of a static stride
     // SM partition: the tile kernel's CTAs that land on an SM whose bit is set here return at once, so those SMs stay free for
     // the reciprocal-space chain (spread -> FFT -> gather) that runs beside it; the other CTAs (one persistent wave) share ALL
-    // tiles through the cursor.  All zero: no partition.
+    // tiles through the cursor.  smPartition false (all bits zero): no partition, several waves, static tile stride.
     unsigned long long pmeSmMask[4];
+    bool smPartition;
     float closeCut2;             // pairs closer than this (squared) are evaluated in double from the exact coordinates (0: off)
-    int useRational;             // B200MD_PAIR_RATIONAL=1: rational Ewald kernel in the force-only tile loop (1 MUFU less, lower accuracy)
 };
 
 enum { EN_NB = 0, EN_RECIP = 1, EN_BOND = 2, EN_ANGLE = 3, EN_TORSION = 4, EN_EXC = 5, EN_KE = 6, B200MD_NUM_ENERGY = 8 };
@@ -423,12 +416,11 @@ struct ScaleDev {
 
 // ---- launchers (defined in the .cu files) ----
 void launch_check_displacement(const NbDev& nb, const CommDev& cd, cudaStream_t s);
-bool list_build_merged();        // list build = 2 gated launches (k_list_prep with grid barriers + k_build_tiles); B200MD_LIST_MERGED=0: 7
-void launch_list_build(const NbDev& nb, cudaStream_t s, int mode = 0);   // all list kernels, gated on counters[CT_REBUILD] (mode 0) or counters[CT_SOFT] (mode 1)
+const int LIST_BUILD_LAUNCHES = 2;
+void launch_list_build(const NbDev& nb, cudaStream_t s);     // k_list_prep (grid barriers) + k_build_tiles, gated on counters[CT_REBUILD]
 void launch_pair(const NbDev& nb, bool energy, cudaStream_t s);
 void launch_count_pairs(const NbDev& nb, cudaStream_t s);
 int choose_pme_sms(int reserve, unsigned long long mask[4]);     // SM partition of the tile kernel (NbDev::pmeSmMask)
-int  list_build_launch_count();
 
 void launch_pme_eterm(const NbDev& nb, const PmeDev& pme, cudaStream_t s);
 void launch_pme_spread(const NbDev& nb, const PmeDev& pme, const CommDev& cd, cudaStream_t s);

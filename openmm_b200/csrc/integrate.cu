@@ -348,7 +348,6 @@ __global__ void __launch_bounds__(128, sizeof(R) == 8 ? 1 : 0) k_integrate(NbDev
             *cd.posNeed = E;
             *cd.epoch = E;
             *in.stepCounter = step + 1ull;
-            if (nb.counters[CT_PENDING]) { nb.counters[CT_PENDING] = 0; nb.counters[CT_CUR] ^= 1; }
         }
         return;
     }
@@ -363,8 +362,6 @@ __global__ void __launch_bounds__(128, sizeof(R) == 8 ? 1 : 0) k_integrate(NbDev
     if (last && threadIdx.x == 0) {
         *in.blocksDone = 0u;
         *in.stepCounter = step + 1ull;
-        // a successor neighbour list built beside this step (nonbonded.cu: k_check_gather / k_list_done) becomes current
-        if (nb.counters[CT_PENDING]) { nb.counters[CT_PENDING] = 0; nb.counters[CT_CUR] ^= 1; }
     }
 }
 

@@ -313,37 +313,6 @@ def test_checkpoint_roundtrip(mods):
     assert np.abs(xa - eng.get_positions()).max() < 1e-4
 
 
-_ASYNC_SCRIPT = r"""
-import sys, os, numpy as np
-sys.path.insert(0, os.environ["B200MD_ROOT"])
-from openmm_b200 import systems, Engine
-d = systems.water_box(12, cutoff=0.9).rounded()
-eng = Engine(d)
-eng.set_integrator(systems.INT_LANGEVIN, 0.002, 300.0, 1.0, 11, 1e-5)
-eng.step(400)
-st = eng.stats()
-x = eng.get_positions()
-e = eng.compute(); f = eng.get_forces()          # through the (other) current list, after a synchronous check
-fresh = Engine(d); fresh.set_positions(x)
-e2 = fresh.compute(); f2 = fresh.get_forces()    # a list built from scratch at the same positions
-print("RESULT", st["list_builds"], st["stale_list_steps"], abs(e - e2), np.abs(f - f2).max(), np.isfinite(x).all())
-"""
-
-
-def test_successor_list_built_beside_the_step(mods):
-    """B200MD_ASYNC_LIST=1: the next neighbour list is built on a side stream while the current one still serves the tile
-    kernel, and k_integrate's last block flips them.  400 steps of a 5,184-atom box must rebuild many times, never serve a
-    stale list, and end in a state whose forces equal those of an engine that builds its list from scratch."""
-    import subprocess, sys
-    from conftest import ROOT
-    env = dict(os.environ, B200MD_ASYNC_LIST="1", B200MD_ROOT=ROOT)
-    out = subprocess.run([sys.executable, "-c", _ASYNC_SCRIPT], env=env, capture_output=True, text=True, timeout=300)
-    assert out.returncode == 0, out.stderr[-2000:]
-    builds, stale, de, df, finite = [l for l in out.stdout.splitlines() if l.startswith("RESULT")][0].split()[1:]
-    assert int(builds) > 50 and int(stale) == 0 and finite == "True"
-    assert float(de) < 0.05 and float(df) < 0.05      # fp32 summation order differs between two lists, nothing else
-
-
 def test_molecules_that_walk_away_are_wrapped_but_the_trajectory_stays_continuous(mods):
     """fp32 coordinates must stay small, the user's trajectory must stay continuous (the Reference platform never wraps:
     ReferenceUpdateStateDataKernel::getPositions).  A 648-atom water box is given a 40 nm/ps drift: in 300 steps of 1 fs

@@ -35,5 +35,5 @@ for name in names:
             best = min(best, 1e3*e0.elapsed_time(e1)/nst)
         st = eng.stats()
         ph = {k: round(1e3*eng.time_phase(k, 20), 2) for k in ["pair", "pme_spread", "pme_fft_conv", "pme_gather", "bonded", "integrate", "list_build"]} if mode == "timeph" else {}
-        print("%s %.1f us/step %.1f ns/day builds %d tiles %d %s env BT=%s PAD=%s" % (name, best, 172800.0/best, st.get("list_builds", -1), st.get("num_tiles", -1), ph,
-              os.environ.get("B200MD_BT_WARPS"), os.environ.get("B200MD_PAD_FRACTION")), flush=True)
+        print("%s %.1f us/step %.1f ns/day builds %d tiles %d %s env PAD=%s" % (name, best, 172800.0/best, st.get("list_builds", -1), st.get("num_tiles", -1), ph,
+              os.environ.get("B200MD_PAD_FRACTION")), flush=True)
