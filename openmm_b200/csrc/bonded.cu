@@ -1,8 +1,9 @@
-// bonded.cu -- harmonic bonds, harmonic angles, periodic torsions, 1-4 exceptions and the Ewald exclusion
-// correction in ONE launch (sm_90a).  Double precision arithmetic on fp32 positions: these terms are a few
-// thousand work items, far below any roofline, and double removes them from the 1e-4 parity budget.
+// bonded.cu -- harmonic bonds, harmonic angles, periodic torsions, Ryckaert-Bellemans torsions, CMAP terms, 1-4
+// exceptions and the Ewald exclusion correction in ONE launch (sm_90a).  Double precision arithmetic on fp32 positions:
+// these terms are a few thousand work items, far below any roofline, and double removes them from the 1e-4 parity budget.
 //
-// Restates ReferenceHarmonicBondIxn / ReferenceAngleBondIxn / ReferenceProperDihedralBond::calculateBondIxn,
+// Restates ReferenceHarmonicBondIxn / ReferenceAngleBondIxn / ReferenceProperDihedralBond / ReferenceRbDihedralBond::
+// calculateBondIxn, ReferenceCMAPTorsionIxn::calculateOneIxn,
 // ReferenceLJCoulomb14::calculateBondIxn (ReferenceLJCoulomb14.cpp:75-110) and the exclusion loop of
 // ReferenceLJCoulombIxn::calculateEwaldIxn (ReferenceLJCoulombIxn.cpp:462-523).  Replaces the generated
 // computeBondedForces kernel of CudaBondedUtilities.cpp:76-150 with pmeExclusions.cc / nonbondedExceptions.cc.
@@ -31,10 +32,53 @@ __device__ __forceinline__ D3 min_image_d(D3 d, const BoxDev& b) {
     return d;
 }
 
+// Dihedral of the atoms (x, y, z, w) (ReferenceBondIxn::getDihedralAngleBetweenThreeVectors): the three difference vectors,
+// the two plane normals and their squared norms, the clamped cosine of the angle and the signed angle in (-pi, pi].
+struct Dihedral { D3 v0, v1, v2, cp0, cp1; double n0, n1, c, theta; };
+__device__ __forceinline__ Dihedral dihedral(const NbDev& nb, const int4& at, bool periodic) {
+    Dihedral d;
+    d.v0 = sub(nb.posq[at.x], nb.posq[at.y]);
+    d.v1 = sub(nb.posq[at.z], nb.posq[at.y]);
+    d.v2 = sub(nb.posq[at.z], nb.posq[at.w]);
+    if (periodic) { d.v0 = min_image_d(d.v0, nb.box); d.v1 = min_image_d(d.v1, nb.box); d.v2 = min_image_d(d.v2, nb.box); }
+    d.cp0 = cross(d.v0, d.v1); d.cp1 = cross(d.v1, d.v2);
+    d.n0 = dot(d.cp0, d.cp0); d.n1 = dot(d.cp1, d.cp1);
+    double c = dot(d.cp0, d.cp1)/sqrt(d.n0*d.n1);
+    c = fmin(1.0, fmax(-1.0, c));
+    double theta;
+    if (c > 0.99 || c < -0.99) {
+        // near 0 / pi use the cross product for accuracy (ReferenceBondIxn::getAngleBetweenTwoVectors)
+        D3 cc = cross(d.cp0, d.cp1);
+        double sc = sqrt(dot(cc, cc)/(d.n0*d.n1));
+        theta = asin(fmin(1.0, sc));
+        if (c < 0) theta = 3.14159265358979323846 - theta;
+    }
+    else theta = acos(c);
+    if (dot(d.v0, d.cp1) < 0) theta = -theta;
+    d.c = c; d.theta = theta;
+    return d;
+}
+
+// Forces of an energy term of one dihedral with derivative dE = dE/dtheta, distributed over its four atoms as in
+// ReferenceProperDihedralBond::calculateBondIxn.
+__device__ __forceinline__ void torsion_force(const NbDev& nb, const int4& at, const Dihedral& d, double dE) {
+    const double nbc2 = dot(d.v1, d.v1), nbc = sqrt(nbc2);
+    const double ffx = -dE*nbc/d.n0, ffw = dE*nbc/d.n1;
+    const double ffy = dot(d.v0, d.v1)/nbc2, ffz = dot(d.v2, d.v1)/nbc2;
+    D3 f1 = scale(d.cp0, ffx), f4 = scale(d.cp1, ffw);
+    D3 s = {ffy*f1.x - ffz*f4.x, ffy*f1.y - ffz*f4.y, ffy*f1.z - ffz*f4.z};
+    add_force(nb, at.x, f1);
+    add_force(nb, at.y, {s.x-f1.x, s.y-f1.y, s.z-f1.z});
+    add_force(nb, at.z, {-s.x-f4.x, -s.y-f4.y, -s.z-f4.z});
+    add_force(nb, at.w, f4);
+}
+
 __global__ void __launch_bounds__(128) k_bonded(NbDev nb, BondedDev bd, int terms, int wantEnergy) {
     const int nB = (terms & B200MD_TERM_BONDS) ? bd.nbonds : 0;
     const int nA = (terms & B200MD_TERM_ANGLES) ? bd.nangles : 0;
     const int nT = (terms & B200MD_TERM_TORSIONS) ? bd.ntorsions : 0;
+    const int nR = (terms & B200MD_TERM_RB_TORSIONS) ? bd.nrb : 0;
+    const int nC = (terms & B200MD_TERM_CMAP) ? bd.ncmap : 0;
     // both the 1-4 pairs and the Ewald exclusion correction belong to the DIRECT-space group: the reference evaluates
     // the exclusion loop after `if (!includeDirect) return;` (ReferenceLJCoulombIxn.cpp:373-374, 462-523)
     const bool doDirect = (terms & B200MD_TERM_NB_DIRECT) != 0;
@@ -42,7 +86,7 @@ __global__ void __launch_bounds__(128) k_bonded(NbDev nb, BondedDev bd, int term
     const int nE = doDirect ? bd.nexc : 0;
     // the bonded work is sharded over ranks in the multi-GPU force decomposition
     const int gid = nb.rank + nb.world*(blockIdx.x*blockDim.x + threadIdx.x);
-    double eB = 0, eA = 0, eT = 0, eE = 0;
+    double eB = 0, eA = 0, eT = 0, eR = 0, eC = 0, eE = 0;
     int i = gid;
     // group byte of a bonded term: bits 0-4 force group, bit 7 = the Force uses periodic boundary conditions
     // (usesPeriodicBoundaryConditions: every difference vector takes the minimum image, ReferenceBondIxn / getDeltaRPeriodic)
@@ -85,38 +129,54 @@ __global__ void __launch_bounds__(128) k_bonded(NbDev nb, BondedDev bd, int term
     if (i >= 0 && i < nT && ((bd.groupMask >> (bd.torsionGroup[i] & 31)) & 1u)) {
         const int4 at = bd.torsionAtoms[i];
         const double4 pr = bd.torsionParams[i];   // k, phase, n
-        D3 v0 = sub(nb.posq[at.x], nb.posq[at.y]);
-        D3 v1 = sub(nb.posq[at.z], nb.posq[at.y]);
-        D3 v2 = sub(nb.posq[at.z], nb.posq[at.w]);
-        if (bd.torsionGroup[i] & 0x80) { v0 = min_image_d(v0, nb.box); v1 = min_image_d(v1, nb.box); v2 = min_image_d(v2, nb.box); }
-        D3 cp0 = cross(v0, v1), cp1 = cross(v1, v2);
-        const double n0 = dot(cp0, cp0), n1 = dot(cp1, cp1);
-        double c = dot(cp0, cp1)/sqrt(n0*n1);
-        c = fmin(1.0, fmax(-1.0, c));
-        double theta;
-        if (c > 0.99 || c < -0.99) {
-            // near 0 / pi use the cross product for accuracy (ReferenceBondIxn::getDihedralAngleBetweenThreeVectors)
-            D3 cc = cross(cp0, cp1);
-            double sc = sqrt(dot(cc, cc)/(n0*n1));
-            theta = asin(fmin(1.0, sc));
-            if (c < 0) theta = 3.14159265358979323846 - theta;
-        }
-        else theta = acos(c);
-        if (dot(v0, cp1) < 0) theta = -theta;
-        const double arg = pr.z*theta - pr.y;
+        const Dihedral d = dihedral(nb, at, bd.torsionGroup[i] & 0x80);
+        const double arg = pr.z*d.theta - pr.y;
         eT = pr.x*(1.0 + cos(arg));
-        const double dE = -pr.x*pr.z*sin(arg);
-        const double nbc2 = dot(v1, v1), nbc = sqrt(nbc2);
-        const double ffx = -dE*nbc/n0, ffw = dE*nbc/n1;
-        const double ffy = dot(v0, v1)/nbc2, ffz = dot(v2, v1)/nbc2;
-        D3 f1 = scale(cp0, ffx), f4 = scale(cp1, ffw);
-        D3 s = {ffy*f1.x - ffz*f4.x, ffy*f1.y - ffz*f4.y, ffy*f1.z - ffz*f4.z};
-        add_force(nb, at.x, f1);
-        add_force(nb, at.y, {s.x-f1.x, s.y-f1.y, s.z-f1.z});
-        add_force(nb, at.z, {-s.x-f4.x, -s.y-f4.y, -s.z-f4.z});
-        add_force(nb, at.w, f4);
+        torsion_force(nb, at, d, -pr.x*pr.z*sin(arg));
     }
     i -= nT;
+    if (i >= 0 && i < nR && ((bd.groupMask >> (bd.rbGroup[i] & 31)) & 1u)) {
+        // ReferenceRbDihedralBond::calculateBondIxn: polymer convention psi = phi - pi, E = sum_n c_n cos^n psi
+        const int4 at = bd.rbAtoms[i];
+        const double* cn = bd.rbParams + 6*i;
+        const Dihedral d = dihedral(nb, at, bd.rbGroup[i] & 0x80);
+        const double psi = d.theta < 0 ? d.theta + 3.14159265358979323846 : d.theta - 3.14159265358979323846;
+        const double cpsi = -d.c;
+        double dE = 0, e = cn[0], cf = 1.0;
+        for (int n = 1; n < 6; n++) {
+            dE -= n*cn[n]*cf;
+            cf *= cpsi;
+            e += cf*cn[n];
+        }
+        eR = e;
+        torsion_force(nb, at, d, dE*sin(psi));
+    }
+    i -= nR;
+    if (i >= 0 && i < nC && ((bd.groupMask >> (bd.cmapGroup[i] & 31)) & 1u)) {
+        // ReferenceCMAPTorsionIxn::calculateOneIxn: bicubic patch of the map at the two dihedrals, each taken in [0, 2 pi)
+        const int4 atA = bd.cmapAtoms[2*i], atB = bd.cmapAtoms[2*i+1];
+        const bool periodic = bd.cmapGroup[i] & 0x80;
+        // the second dihedral is evaluated again for its forces rather than kept across the spline: fewer live registers
+        const Dihedral dA = dihedral(nb, atA, periodic);
+        const double twoPi = 2.0*3.14159265358979323846;
+        const double angleA = fmod(dA.theta + twoPi, twoPi), angleB = fmod(dihedral(nb, atB, periodic).theta + twoPi, twoPi);
+        const int2 map = bd.cmapMaps[bd.cmapMap[i]];      // (first patch, size)
+        const double delta = twoPi/map.y;
+        const int s = (int) fmin(angleA/delta, (double) (map.y - 1));
+        const int t = (int) fmin(angleB/delta, (double) (map.y - 1));
+        const double* c = bd.cmapCoeff + 16*((size_t) map.x + s + map.y*t);
+        const double da = angleA/delta - s, db = angleB/delta - t;
+        double e = 0, dEdA = 0, dEdB = 0;
+        for (int k = 3; k >= 0; k--) {
+            e = da*e + ((c[k*4+3]*db + c[k*4+2])*db + c[k*4+1])*db + c[k*4+0];
+            dEdA = db*dEdA + (3.0*c[k+3*4]*da + 2.0*c[k+2*4])*da + c[k+1*4];
+            dEdB = da*dEdB + (3.0*c[k*4+3]*db + 2.0*c[k*4+2])*db + c[k*4+1];
+        }
+        eC = e;
+        torsion_force(nb, atA, dA, dEdA/delta);
+        torsion_force(nb, atB, dihedral(nb, atB, periodic), dEdB/delta);
+    }
+    i -= nC;
     if (i >= 0 && i < nE) {
         const int2 at = bd.excAtoms[i];
         const double4 pr = bd.excParams[i];       // (k qq14, sigma, 4 eps, k qi qj)
@@ -148,18 +208,18 @@ __global__ void __launch_bounds__(128) k_bonded(NbDev nb, BondedDev bd, int term
         add_force(nb, at.y, scale(d, -dEdR));
     }
     if (wantEnergy) {
-        // block reduction of the four partial energies
-        __shared__ double red[4][4];
-        double v[4] = {eB, eA, eT, eE};
-        for (int k = 0; k < 4; k++) {
+        // block reduction of the six partial energies
+        __shared__ double red[6][4];
+        double v[6] = {eB, eA, eT, eE, eR, eC};
+        for (int k = 0; k < 6; k++) {
             double x = v[k];
             for (int off = 16; off > 0; off >>= 1) x += __shfl_xor_sync(0xffffffffu, x, off);
             if ((threadIdx.x & 31) == 0) red[k][threadIdx.x >> 5] = x;
         }
         __syncthreads();
-        if (threadIdx.x < 4) {
+        if (threadIdx.x < 6) {
             double x = red[threadIdx.x][0] + red[threadIdx.x][1] + red[threadIdx.x][2] + red[threadIdx.x][3];
-            const int slot[4] = {EN_BOND, EN_ANGLE, EN_TORSION, EN_EXC};
+            const int slot[6] = {EN_BOND, EN_ANGLE, EN_TORSION, EN_EXC, EN_RBTORSION, EN_CMAP};
             if (x != 0.0) atomicAdd(&nb.energy[slot[threadIdx.x]], x);
         }
     }
@@ -170,6 +230,8 @@ void launch_bonded(const NbDev& nb, const BondedDev& bd, int terms, bool energy,
     if (terms & B200MD_TERM_BONDS) n += bd.nbonds;
     if (terms & B200MD_TERM_ANGLES) n += bd.nangles;
     if (terms & B200MD_TERM_TORSIONS) n += bd.ntorsions;
+    if (terms & B200MD_TERM_RB_TORSIONS) n += bd.nrb;
+    if (terms & B200MD_TERM_CMAP) n += bd.ncmap;
     if (terms & B200MD_TERM_NB_DIRECT) n += bd.nexc;
     if (n == 0) return;
     int per = (n + nb.world - 1)/nb.world;

@@ -81,7 +81,9 @@ struct b200md_ctx {
     std::vector<int> bondI, bondJ; std::vector<double> bondR0, bondK;
     std::vector<int> angI, angJ, angK; std::vector<double> angT0, angKK;
     std::vector<int> torI, torJ, torK, torL, torN; std::vector<double> torPhase, torKK;
-    std::vector<unsigned char> bondGroup, angGroup, torGroup;       // force group of every bonded element (default 0)
+    std::vector<int> rbI, rbJ, rbK, rbL; std::vector<double> rbC;  // rbC [n][6]
+    std::vector<int> cmapSize, cmapMap, cmapAtoms; std::vector<double> cmapCoeff;   // cmapAtoms [n][8], cmapCoeff [sum size^2][16]
+    std::vector<unsigned char> bondGroup, angGroup, torGroup, rbGroup, cmapGroup;   // force group of every bonded element (default 0)
     std::vector<int> conI, conJ; std::vector<double> conD;
     int cmFreq = 0;
     std::vector<int4> hUnitAtoms;        // host copy of the integration units (ownership cuts of the multi-GPU data plane)
@@ -108,7 +110,8 @@ struct b200md_ctx {
     DevBuf<int2> bondAtoms, excAtoms; DevBuf<double2> bondParams, angleParams;
     DevBuf<int4> angleAtoms, torsionAtoms, unitAtoms; DevBuf<double4> torsionParams, excParams;
     DevBuf<int> unitType; DevBuf<float4> unitParams;
-    DevBuf<unsigned char> bondGroupDev, angGroupDev, torGroupDev;
+    DevBuf<unsigned char> bondGroupDev, angGroupDev, torGroupDev, rbGroupDev, cmapGroupDev;
+    DevBuf<int4> rbAtoms, cmapAtomsDev; DevBuf<double> rbParams, cmapCoeffDev; DevBuf<int> cmapMapDev; DevBuf<int2> cmapMapsDev;
     // general constraint networks (CCMA, constraints.cu)
     std::vector<int> ccmaCons;           // indices into conI/conJ/conD
     DevBuf<int> ccCompCon, ccCompAtom, ccRowStart, ccCol, ccAtoms, ccAStart, ccACon;
@@ -272,11 +275,38 @@ extern "C" int b200md_set_torsions(b200md_ctx* ctx, int n, const int* p1, const 
     ctx->torN.assign(per, per+n); ctx->torPhase.assign(ph, ph+n); ctx->torKK.assign(k, k+n);
     API_END(ctx)
 }
+extern "C" int b200md_set_rb_torsions(b200md_ctx* ctx, int n, const int* p1, const int* p2, const int* p3, const int* p4, const double* c) {
+    API_BEGIN(ctx)
+    require(!ctx->finalized, "set_rb_torsions after finalize");
+    require(n >= 0, "set_rb_torsions: negative count");
+    ctx->rbI.assign(p1, p1+n); ctx->rbJ.assign(p2, p2+n); ctx->rbK.assign(p3, p3+n); ctx->rbL.assign(p4, p4+n);
+    ctx->rbC.assign(c, c + 6*(size_t) n);
+    API_END(ctx)
+}
+// the number of coefficients of the maps: 16 per patch, size^2 patches per map
+static size_t cmap_coeff_count(int nmaps, const int* size) {
+    size_t total = 0;
+    for (int m = 0; m < nmaps; m++) {
+        require(size[m] > 0, "CMAP: the size of a map must be positive");
+        total += 16*(size_t) size[m]*size[m];
+    }
+    return total;
+}
+extern "C" int b200md_set_cmap(b200md_ctx* ctx, int nmaps, const int* size, const double* coeff, int n, const int* map, const int* atoms) {
+    API_BEGIN(ctx)
+    require(!ctx->finalized, "set_cmap after finalize");
+    require(nmaps >= 0 && n >= 0, "set_cmap: negative count");
+    const size_t nc = cmap_coeff_count(nmaps, size);
+    ctx->cmapSize.assign(size, size + nmaps); ctx->cmapCoeff.assign(coeff, coeff + nc);
+    ctx->cmapMap.assign(map, map + n); ctx->cmapAtoms.assign(atoms, atoms + 8*(size_t) n);
+    API_END(ctx)
+}
 extern "C" int b200md_set_bonded_groups(b200md_ctx* ctx, int kind, int n, const int* group) {
     API_BEGIN(ctx)
     require(!ctx->finalized, "set_bonded_groups after finalize");
-    require(kind >= 0 && kind <= 2, "set_bonded_groups: kind must be 0 (bonds), 1 (angles) or 2 (torsions)");
-    std::vector<unsigned char>& g = kind == 0 ? ctx->bondGroup : (kind == 1 ? ctx->angGroup : ctx->torGroup);
+    require(kind >= 0 && kind <= 4, "set_bonded_groups: kind must be 0 (bonds), 1 (angles), 2 (torsions), 3 (RB torsions) or 4 (CMAP)");
+    std::vector<unsigned char>& g = kind == 0 ? ctx->bondGroup : kind == 1 ? ctx->angGroup : kind == 2 ? ctx->torGroup :
+                                    kind == 3 ? ctx->rbGroup : ctx->cmapGroup;
     g.resize(n);
     for (int i = 0; i < n; i++) { require(group[i] >= 0 && (group[i] & ~0x80) < 32, "force group out of range"); g[i] = (unsigned char) group[i]; }
     API_END(ctx)
@@ -1157,6 +1187,35 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
         c->bd.bondGroup = c->bondGroupDev.p; c->bd.angleGroup = c->angGroupDev.p; c->bd.torsionGroup = c->torGroupDev.p;
         c->bd.groupMask = 0xffffffffu;
     }
+    // ---- Ryckaert-Bellemans torsions and CMAP terms ----
+    {
+        const int nr = (int) c->rbI.size(), ncm = (int) c->cmapMap.size(), nmaps = (int) c->cmapSize.size();
+        auto atom_ok = [&](int a) { return a >= 0 && a < N; };
+        std::vector<int4> ra(nr);
+        for (int i = 0; i < nr; i++) {
+            require(atom_ok(c->rbI[i]) && atom_ok(c->rbJ[i]) && atom_ok(c->rbK[i]) && atom_ok(c->rbL[i]), "RB torsion: atom index out of range");
+            ra[i] = make_int4(c->rbI[i], c->rbJ[i], c->rbK[i], c->rbL[i]);
+        }
+        require(c->cmapCoeff.size() == cmap_coeff_count(nmaps, c->cmapSize.data()), "CMAP: the number of coefficients differs from 16 x the number of patches");
+        std::vector<int2> maps(nmaps);
+        for (int m = 0, first = 0; m < nmaps; m++) { maps[m] = make_int2(first, c->cmapSize[m]); first += c->cmapSize[m]*c->cmapSize[m]; }
+        std::vector<int4> ca(2*(size_t) ncm);
+        for (int i = 0; i < ncm; i++) {
+            require(c->cmapMap[i] >= 0 && c->cmapMap[i] < nmaps, "CMAP torsion: map index out of range");
+            const int* a = &c->cmapAtoms[8*(size_t) i];
+            for (int k = 0; k < 8; k++) require(atom_ok(a[k]), "CMAP torsion: atom index out of range");
+            ca[2*i] = make_int4(a[0], a[1], a[2], a[3]); ca[2*i+1] = make_int4(a[4], a[5], a[6], a[7]);
+        }
+        require((c->rbGroup.empty() || (int) c->rbGroup.size() == nr) && (c->cmapGroup.empty() || (int) c->cmapGroup.size() == ncm),
+                "set_bonded_groups: group array length differs from the number of terms");
+        c->rbGroup.resize(std::max(nr, 1), 0); c->cmapGroup.resize(std::max(ncm, 1), 0);
+        c->rbAtoms.upload(ra); c->rbParams.upload(c->rbC); c->rbGroupDev.upload(c->rbGroup);
+        c->cmapAtomsDev.upload(ca); c->cmapMapDev.upload(c->cmapMap); c->cmapMapsDev.upload(maps); c->cmapCoeffDev.upload(c->cmapCoeff);
+        c->cmapGroupDev.upload(c->cmapGroup);
+        c->bd.nrb = nr; c->bd.rbAtoms = c->rbAtoms.p; c->bd.rbParams = c->rbParams.p; c->bd.rbGroup = c->rbGroupDev.p;
+        c->bd.ncmap = ncm; c->bd.cmapAtoms = c->cmapAtomsDev.p; c->bd.cmapMap = c->cmapMapDev.p; c->bd.cmapMaps = c->cmapMapsDev.p;
+        c->bd.cmapCoeff = c->cmapCoeffDev.p; c->bd.cmapGroup = c->cmapGroupDev.p;
+    }
     upload_params(c);
     build_units(c);
     build_ccma(c);
@@ -1167,7 +1226,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
             require(fft_slab_path(probe), "multi-GPU: the PME grid plane does not fit the slab FFT kernels (B200MD_MGPU=nccl selects the NCCL scheme)");
         }
     }
-    // ---- molecules (connected components of bonds, angles, torsions, constraints and exceptions) for the wrap at list
+    // ---- molecules (connected components of bonds, angles, torsions, RB torsions, CMAP terms, constraints and exceptions) for the wrap at list
     // builds; off for non-periodic systems and with more than one rank (every rank would have to wrap in the same step,
     // and the reciprocal-space rank builds no list) ----
     c->cellOffset.alloc((size_t) 3*NP); c->cellOffset.zero();
@@ -1180,6 +1239,8 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
         for (size_t i = 0; i < c->bondI.size(); i++) join(c->bondI[i], c->bondJ[i]);
         for (size_t i = 0; i < c->angI.size(); i++) { join(c->angI[i], c->angJ[i]); join(c->angJ[i], c->angK[i]); }
         for (size_t i = 0; i < c->torI.size(); i++) { join(c->torI[i], c->torJ[i]); join(c->torJ[i], c->torK[i]); join(c->torK[i], c->torL[i]); }
+        for (size_t i = 0; i < c->rbI.size(); i++) { join(c->rbI[i], c->rbJ[i]); join(c->rbJ[i], c->rbK[i]); join(c->rbK[i], c->rbL[i]); }
+        for (size_t i = 0; i < c->cmapAtoms.size(); i++) join(c->cmapAtoms[i - i%8], c->cmapAtoms[i]);
         for (size_t i = 0; i < c->conI.size(); i++) join(c->conI[i], c->conJ[i]);
         for (size_t i = 0; i < c->excI.size(); i++) join(c->excI[i], c->excJ[i]);
         std::vector<int> molOf(N), count;
@@ -1242,6 +1303,31 @@ extern "C" int b200md_update_bonded_params(b200md_ctx* ctx, int kind, int n, con
         ctx->torsionParams.upload(p);
     }
     else throw std::runtime_error("unknown bonded kind");
+    API_END(ctx)
+}
+
+// Calc{RBTorsion,CMAPTorsion}ForceKernel::copyParametersToContext (kernels.h:480, 515): the device arrays keep their size,
+// so they are overwritten in place and captured step graphs stay valid.
+extern "C" int b200md_update_rb_torsion_params(b200md_ctx* ctx, int n, const double* c) {
+    API_BEGIN(ctx)
+    require(ctx->finalized, "update_rb_torsion_params before finalize");
+    require(n == ctx->bd.nrb, "updateParametersInContext: The number of torsions has changed");
+    CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+    ctx->rbC.assign(c, c + 6*(size_t) n);
+    ctx->rbParams.upload(ctx->rbC);
+    API_END(ctx)
+}
+extern "C" int b200md_update_cmap_params(b200md_ctx* ctx, int nmaps, const int* size, const double* coeff, int n, const int* map) {
+    API_BEGIN(ctx)
+    require(ctx->finalized, "update_cmap_params before finalize");
+    require(nmaps == (int) ctx->cmapSize.size(), "updateParametersInContext: The number of maps has changed");
+    require(n == ctx->bd.ncmap, "updateParametersInContext: The number of CMAP torsions has changed");
+    for (int m = 0; m < nmaps; m++) require(size[m] == ctx->cmapSize[m], "updateParametersInContext: The size of a map has changed");
+    for (int i = 0; i < n; i++) require(map[i] >= 0 && map[i] < nmaps, "CMAP torsion: map index out of range");
+    CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+    ctx->cmapCoeff.assign(coeff, coeff + ctx->cmapCoeff.size());
+    ctx->cmapMap.assign(map, map + n);
+    ctx->cmapCoeffDev.upload(ctx->cmapCoeff); ctx->cmapMapDev.upload(ctx->cmapMap);
     API_END(ctx)
 }
 
@@ -1529,9 +1615,9 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     }
     if (forkAfterList) launch_recip();
     if (direct) { launch_pair(c->nb, energy, s); launches++; }
-    int bterms = terms & (B200MD_TERM_BONDS | B200MD_TERM_ANGLES | B200MD_TERM_TORSIONS);
+    int bterms = terms & (B200MD_TERM_BONDS | B200MD_TERM_ANGLES | B200MD_TERM_TORSIONS | B200MD_TERM_RB_TORSIONS | B200MD_TERM_CMAP);
     if (c->haveNb) bterms |= terms & B200MD_TERM_NB_DIRECT;
-    const int nbonded = c->bd.nbonds + c->bd.nangles + c->bd.ntorsions + c->bd.nexc;
+    const int nbonded = c->bd.nbonds + c->bd.nangles + c->bd.ntorsions + c->bd.nrb + c->bd.ncmap + c->bd.nexc;
     if (bterms && nbonded > 0 && !(split && c->rank == pmeRank)) { BondedDev bd = c->bd; bd.groupMask = groupMask; launch_bonded(c->nb, bd, bterms, energy, s); launches++; }
     // p2p: partial forces of the atoms this rank does not own -> the owners' inboxes.  Reciprocal space only ever touches the
     // atoms this rank OWNS (k_pme_gather), so when it runs on its own stream the push does not have to wait for it: it goes
@@ -1633,6 +1719,8 @@ extern "C" int b200md_compute_groups(b200md_ctx* ctx, int terms, unsigned int bo
         if (terms & B200MD_TERM_BONDS) e += h[EN_BOND];
         if (terms & B200MD_TERM_ANGLES) e += h[EN_ANGLE];
         if (terms & B200MD_TERM_TORSIONS) e += h[EN_TORSION];
+        if (terms & B200MD_TERM_RB_TORSIONS) e += h[EN_RBTORSION];
+        if (terms & B200MD_TERM_CMAP) e += h[EN_CMAP];
         if (ctx->haveNb) {
             if (terms & B200MD_TERM_NB_DIRECT) {
                 e += h[EN_NB] + h[EN_EXC];

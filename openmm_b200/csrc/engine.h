@@ -133,7 +133,8 @@ struct NbDev {
     float closeCut2;             // pairs closer than this (squared) are evaluated in double from the exact coordinates (0: off)
 };
 
-enum { EN_NB = 0, EN_RECIP = 1, EN_BOND = 2, EN_ANGLE = 3, EN_TORSION = 4, EN_EXC = 5, EN_KE = 6, B200MD_NUM_ENERGY = 8 };
+enum { EN_NB = 0, EN_RECIP = 1, EN_BOND = 2, EN_ANGLE = 3, EN_TORSION = 4, EN_EXC = 5, EN_KE = 6, EN_RBTORSION = 7, EN_CMAP = 8,
+       B200MD_NUM_ENERGY = 9 };
 
 struct PmeDev {
     int nx, ny, nz, nzc;
@@ -152,15 +153,20 @@ struct PmeDev {
 };
 
 struct BondedDev {
-    int nbonds, nangles, ntorsions, nexc;
+    int nbonds, nangles, ntorsions, nrb, ncmap, nexc;
     const int2* bondAtoms; const double2* bondParams;           // (r0, k)
     const int4* angleAtoms; const double2* angleParams;         // (theta0, k)
     const int4* torsionAtoms; const double4* torsionParams;     // (k, phase, n, 0)
+    const int4* rbAtoms; const double* rbParams;                // [nrb][6] Ryckaert-Bellemans c0..c5
+    // CMAP: two dihedrals per term (atoms [2i], [2i+1]), a map index per term, per map (first patch, size), and the bicubic
+    // coefficients of every patch, [sum size^2][16] (CMAPTorsionForceImpl::calcMapDerivatives), patch s + size*t of a map
+    const int4* cmapAtoms; const int* cmapMap; const int2* cmapMaps; const double* cmapCoeff;
     const int2* excAtoms; const double4* excParams;             // (qq14*ONE_4PI_EPS0, sigma, 4 eps, 0)
     int excPeriodic;
-    // force group of every bond / angle / torsion (several Force objects of one class may sit in different groups,
+    // force group of every bonded term (several Force objects of one class may sit in different groups,
     // ContextImpl::calcForcesAndEnergy groups, ContextImpl.cpp:293-308); an element is evaluated iff bit `group` of groupMask is set
     const unsigned char* bondGroup; const unsigned char* angleGroup; const unsigned char* torsionGroup;
+    const unsigned char* rbGroup; const unsigned char* cmapGroup;
     unsigned int groupMask;
 };
 

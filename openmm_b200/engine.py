@@ -5,7 +5,10 @@ import numpy as np
 from . import _lib
 from .systems import SystemDesc, NB_PME
 
-TERM_BONDS, TERM_ANGLES, TERM_TORSIONS, TERM_NB_DIRECT, TERM_NB_RECIP, TERM_ALL = 1, 2, 4, 8, 16, 31
+TERM_BONDS, TERM_ANGLES, TERM_TORSIONS, TERM_NB_DIRECT, TERM_NB_RECIP = 1, 2, 4, 8, 16
+TERM_RB_TORSIONS, TERM_CMAP, TERM_ALL = 32, 64, 127
+# kinds of b200md_set_bonded_groups
+BONDED_KINDS = {"bonds": 0, "angles": 1, "torsions": 2, "rb_torsions": 3, "cmap": 4}
 PHASES = {"pair": 0, "pme_spread": 1, "pme_fft_conv": 2, "pme_gather": 3, "integrate": 4, "list_build": 5, "bonded": 6}
 
 
@@ -33,9 +36,11 @@ PRECISIONS = {"single": 0, "mixed": 1}
 
 
 class Engine:
-    def __init__(self, desc: SystemDesc, device=0, comm=None, precision="single"):
+    def __init__(self, desc: SystemDesc, device=0, comm=None, precision="single", bonded_groups=None):
         """comm = (rank, world, unique_id_bytes) for the multi-GPU force decomposition.  precision: "single" (fp32 state) or
-        "mixed" (positions as fp32 hi + lo, velocities, integration and constraints in double; single GPU only)."""
+        "mixed" (positions as fp32 hi + lo, velocities, integration and constraints in double; single GPU only).
+        bonded_groups = {kind: group byte per term} with kind a key of BONDED_KINDS: bits 0-4 the force group, bit 7 the
+        term takes minimum-image difference vectors (Force::setUsesPeriodicBoundaryConditions)."""
         if precision not in PRECISIONS:
             raise ValueError("precision must be one of %s, not %r" % (sorted(PRECISIONS), precision))
         self.lib = _lib.load()
@@ -46,6 +51,7 @@ class Engine:
         if self.lib.b200md_create(C.byref(h), device, self.natoms) != 0:
             raise EngineError(self.lib.b200md_last_error(None).decode())
         self.h = h
+        self._bonded_groups = bonded_groups or {}
         try:
             self._define(desc, comm)
         except Exception:
@@ -88,6 +94,15 @@ class Engine:
         if len(d.tor_i):
             self._ck(L.b200md_set_torsions(self.h, len(d.tor_i), _ip(_i32(d.tor_i)), _ip(_i32(d.tor_j)), _ip(_i32(d.tor_k)), _ip(_i32(d.tor_l)),
                                            _ip(_i32(d.tor_n)), _dp(_f64(d.tor_phase)), _dp(_f64(d.tor_kk))))
+        if len(d.rb_i):
+            self._ck(L.b200md_set_rb_torsions(self.h, len(d.rb_i), _ip(_i32(d.rb_i)), _ip(_i32(d.rb_j)), _ip(_i32(d.rb_k)), _ip(_i32(d.rb_l)),
+                                              _dp(_f64(d.rb_c))))
+        if len(d.cmap_map):
+            self._ck(L.b200md_set_cmap(self.h, len(d.cmap_size), _ip(_i32(d.cmap_size)), _dp(_f64(d.cmap_coeff)), len(d.cmap_map),
+                                       _ip(_i32(d.cmap_map)), _ip(_i32(d.cmap_atoms))))
+        for kind, g in self._bonded_groups.items():
+            g = _i32(g)
+            self._ck(L.b200md_set_bonded_groups(self.h, BONDED_KINDS[kind], len(g), _ip(g)))
         if len(d.con_i):
             self._ck(L.b200md_set_constraints(self.h, len(d.con_i), _ip(_i32(d.con_i)), _ip(_i32(d.con_j)), _dp(_f64(d.con_d))))
         if d.cm_frequency:
@@ -165,6 +180,21 @@ class Engine:
             return e.value
         self._ck(self.lib.b200md_compute(self.h, terms, 1, None))
         return None
+
+    def compute_groups(self, terms=TERM_ALL, groups=0xffffffff):
+        """compute() restricted to the bonded terms whose force group is in the `groups` bit mask; returns the energy."""
+        e = C.c_double()
+        self._ck(self.lib.b200md_compute_groups(self.h, terms, groups, 1, C.byref(e)))
+        return e.value
+
+    # ---- Calc{RBTorsion,CMAPTorsion}ForceKernel::copyParametersToContext ----
+    def update_rb_torsion_params(self, c):
+        c = _f64(c)
+        self._ck(self.lib.b200md_update_rb_torsion_params(self.h, len(c), _dp(c)))
+
+    def update_cmap_params(self, size, coeff, cmap_map):
+        size, coeff, cmap_map = _i32(size), _f64(coeff), _i32(cmap_map)
+        self._ck(self.lib.b200md_update_cmap_params(self.h, len(size), _ip(size), _dp(coeff), len(cmap_map), _ip(cmap_map)))
 
     # ---- Integrate*StepKernel ----
     def set_integrator(self, kind, dt, temperature=300.0, friction=1.0, seed=7, constraint_tol=1e-5):

@@ -60,6 +60,16 @@ class SystemDesc:
     tor_n: np.ndarray = field(default_factory=_i)
     tor_phase: np.ndarray = field(default_factory=_d)
     tor_kk: np.ndarray = field(default_factory=_d)
+    rb_i: np.ndarray = field(default_factory=_i)          # RBTorsionForce
+    rb_j: np.ndarray = field(default_factory=_i)
+    rb_k: np.ndarray = field(default_factory=_i)
+    rb_l: np.ndarray = field(default_factory=_i)
+    rb_c: np.ndarray = field(default_factory=lambda: np.zeros((0, 6)))       # [n,6] c0..c5, kJ/mol
+    cmap_size: np.ndarray = field(default_factory=_i)     # CMAPTorsionForce: [nmaps] map sizes
+    cmap_coeff: np.ndarray = field(default_factory=_d)    # [sum size^2, 16] bicubic coefficients (CMAPTorsionForceImpl::calcMapDerivatives)
+    cmap_energy: np.ndarray = field(default_factory=_d)   # [sum size^2] map energies, kJ/mol (what a CMAPTorsionForce is given)
+    cmap_map: np.ndarray = field(default_factory=_i)      # [n] map of each term
+    cmap_atoms: np.ndarray = field(default_factory=lambda: np.zeros((0, 8), dtype=np.int32))   # [n,8] the two dihedrals
     con_i: np.ndarray = field(default_factory=_i)
     con_j: np.ndarray = field(default_factory=_i)
     con_d: np.ndarray = field(default_factory=_d)
@@ -141,6 +151,72 @@ class SystemDesc:
             else:
                 kw[k] = v
         return SystemDesc(**kw)
+
+
+def periodic_to_rb(desc):
+    """The same System with every periodic torsion k (1 + cos(n phi - phase)), n <= 3 and phase 0 or pi, written as an exactly
+    equal Ryckaert-Bellemans torsion sum_m c_m cos^m psi, psi = phi - pi: cos(n phi) = T_n(cos phi) = (-1)^n T_n(cos psi)."""
+    import copy
+    cheb = {0: [1, 0, 0, 0], 1: [0, 1, 0, 0], 2: [-1, 0, 2, 0], 3: [0, -3, 0, 4]}
+    n, ph, k = np.asarray(desc.tor_n), np.asarray(desc.tor_phase, dtype=np.float64), np.asarray(desc.tor_kk, dtype=np.float64)
+    if len(n) and (n.max() > 3 or n.min() < 0):
+        raise ValueError("periodic_to_rb: periodicity above 3")
+    # force fields write pi with about 12 digits (3.14159265359): a phase that far from pi changes a force by ~1e-12 relative
+    sign = np.where(np.abs(ph) < 1e-9, 1.0, np.where(np.abs(ph - math.pi) < 1e-9, -1.0, np.nan))
+    if np.isnan(sign).any():
+        raise ValueError("periodic_to_rb: a phase is neither 0 nor pi")
+    c = np.zeros((len(n), 6))
+    c[:, 0] = k
+    for m in range(4):
+        c[:, m] += k*sign*np.array([cheb[int(x)][m]*(-1)**int(x) for x in n])
+    d = copy.copy(desc)
+    d.rb_i, d.rb_j, d.rb_k, d.rb_l = (np.array(a, dtype=np.int32) for a in (desc.tor_i, desc.tor_j, desc.tor_k, desc.tor_l))
+    d.rb_c = c
+    d.tor_i, d.tor_j, d.tor_k, d.tor_l, d.tor_n, d.tor_phase, d.tor_kk = _i(), _i(), _i(), _i(), _i(), _d(), _d()
+    return d
+
+
+def backbone_cmap_atoms(desc):
+    """[n,8] atoms of every backbone (phi, psi) pair: C(=O)-N-CA-C(=O)-N chains of the bond graph (bonds and constraints),
+    with elements told apart by mass.  Ordered by the CA atom."""
+    elem = np.select([np.abs(desc.masses - 12.011) < 0.1, np.abs(desc.masses - 14.007) < 0.1, np.abs(desc.masses - 15.999) < 0.1],
+                     ["C", "N", "O"], "X")
+    nbr = [set() for _ in range(desc.natoms)]
+    for i, j in zip(np.concatenate([desc.bond_i, desc.con_i]).tolist(), np.concatenate([desc.bond_j, desc.con_j]).tolist()):
+        nbr[i].add(j)
+        nbr[j].add(i)
+    carbonyl = [a for a in range(desc.natoms) if elem[a] == "C" and any(elem[o] == "O" and len(nbr[o]) == 1 for o in nbr[a])]
+    is_co = np.zeros(desc.natoms, bool)
+    is_co[carbonyl] = True
+    out = []
+    for c in carbonyl:                                  # C of residue i: ... N-CA-C(=O)-N(i+1)
+        for ca in nbr[c]:
+            if elem[ca] != "C" or is_co[ca]:
+                continue
+            for n in nbr[ca]:
+                if elem[n] != "N":
+                    continue
+                for cp in nbr[n]:
+                    if cp == ca or not is_co[cp]:
+                        continue
+                    for nn in nbr[c]:
+                        if elem[nn] == "N":
+                            out.append((cp, n, ca, c, n, ca, c, nn))
+    out.sort(key=lambda t: t[2])
+    return np.array(out, dtype=np.int32).reshape(-1, 8)
+
+
+def with_cmap(desc, size, energy, coeff):
+    """desc plus one CMAP term per backbone (phi, psi) pair (backbone_cmap_atoms), the maps assigned round robin.
+    size [nmaps], energy [sum size^2] and coeff [sum size^2, 16] describe the maps."""
+    import copy
+    d = copy.copy(desc)
+    d.cmap_atoms = backbone_cmap_atoms(desc)
+    d.cmap_size = np.asarray(size, dtype=np.int32)
+    d.cmap_energy = np.asarray(energy, dtype=np.float64)
+    d.cmap_coeff = np.asarray(coeff, dtype=np.float64).reshape(-1, 16)
+    d.cmap_map = (np.arange(len(d.cmap_atoms)) % len(d.cmap_size)).astype(np.int32)
+    return d
 
 
 def fft_size_ok(n):

@@ -7,7 +7,8 @@
 // (CudaPlatform.cpp:59-61).  Compiled against the reference's headers where they lie; no reference source is copied.
 //
 // Supported: NonbondedForce (NoCutoff, CutoffNonPeriodic, CutoffPeriodic, PME; parameter offsets), HarmonicBondForce,
-// HarmonicAngleForce, PeriodicTorsionForce (any number of objects, each in its own force group), CMMotionRemover;
+// HarmonicAngleForce, PeriodicTorsionForce, RBTorsionForce, CMAPTorsionForce (any number of objects, each in its own force
+// group), CMMotionRemover;
 // Verlet / Langevin / LangevinMiddle integrators; SETTLE + X-H_n SHAKE constraints; MonteCarloBarostat and
 // MonteCarloAnisotropicBarostat (ApplyMonteCarloBarostatKernel; MonteCarloMembraneBarostat is refused).  A Force class without a kernel here
 // makes Platform::supportsKernels() false; an unsupported OPTION of a supported class is rejected in contextCreated()
@@ -29,6 +30,8 @@
 #include "openmm/HarmonicBondForce.h"
 #include "openmm/HarmonicAngleForce.h"
 #include "openmm/PeriodicTorsionForce.h"
+#include "openmm/RBTorsionForce.h"
+#include "openmm/CMAPTorsionForce.h"
 #include "openmm/CMMotionRemover.h"
 #include "openmm/VerletIntegrator.h"
 #include "openmm/LangevinIntegrator.h"
@@ -36,7 +39,9 @@
 #include "openmm/MonteCarloMembraneBarostat.h"
 #include "openmm/internal/ContextImpl.h"
 #include "openmm/internal/NonbondedForceImpl.h"
+#include "openmm/internal/CMAPTorsionForceImpl.h"
 #include "../include/b200md.h"
+#include <algorithm>
 #include <map>
 #include <string>
 #include <vector>
@@ -74,11 +79,15 @@ struct PlatformData {
     int cmFrequency = 0;
     bool cmRequested = false;       // RemoveCMMotionKernel::execute seen since the last integrator step
     bool useFusedStep = true;       // B200MD_PLUGIN_FUSED=0: always compute + integrate_only (debugging)
-    vector<int> bondG, angG, torG;  // force group of every bonded element
+    vector<int> bondG, angG, torG, rbG, cmapG;  // force group of every bonded element
     // bonded terms are gathered over all force objects of a kind and sent at finalize
     vector<int> bondI, bondJ; vector<double> bondR0, bondK;
     vector<int> angI, angJ, angK; vector<double> angT0, angKK;
     vector<int> torI, torJ, torK, torL, torN; vector<double> torPhase, torKK;
+    vector<int> rbI, rbJ, rbK, rbL; vector<double> rbC;                     // rbC [n][6]
+    // CMAP: the maps of all objects one after the other (a term's map index counts from the first map of all objects);
+    // coefficients from CMAPTorsionForceImpl::calcMapDerivatives, [sum size^2][16]
+    vector<int> cmapSize, cmapMap, cmapAtoms; vector<double> cmapCoeff;
     map<string, string> props;
     // a box b200md_set_box refused (smaller than twice the cutoff): the reference raises that at the next force evaluation
     // (ReferenceKernels.cpp:983-985), not in setPeriodicBoxVectors; a later box that passes clears it
@@ -97,9 +106,13 @@ struct PlatformData {
         if (!bondI.empty()) check(b200md_set_bonds(ctx, (int) bondI.size(), bondI.data(), bondJ.data(), bondR0.data(), bondK.data()));
         if (!angI.empty()) check(b200md_set_angles(ctx, (int) angI.size(), angI.data(), angJ.data(), angK.data(), angT0.data(), angKK.data()));
         if (!torI.empty()) check(b200md_set_torsions(ctx, (int) torI.size(), torI.data(), torJ.data(), torK.data(), torL.data(), torN.data(), torPhase.data(), torKK.data()));
+        if (!rbI.empty()) check(b200md_set_rb_torsions(ctx, (int) rbI.size(), rbI.data(), rbJ.data(), rbK.data(), rbL.data(), rbC.data()));
+        if (!cmapMap.empty()) check(b200md_set_cmap(ctx, (int) cmapSize.size(), cmapSize.data(), cmapCoeff.data(), (int) cmapMap.size(), cmapMap.data(), cmapAtoms.data()));
         if (!bondG.empty()) check(b200md_set_bonded_groups(ctx, 0, (int) bondG.size(), bondG.data()));
         if (!angG.empty()) check(b200md_set_bonded_groups(ctx, 1, (int) angG.size(), angG.data()));
         if (!torG.empty()) check(b200md_set_bonded_groups(ctx, 2, (int) torG.size(), torG.data()));
+        if (!rbG.empty()) check(b200md_set_bonded_groups(ctx, 3, (int) rbG.size(), rbG.data()));
+        if (!cmapG.empty()) check(b200md_set_bonded_groups(ctx, 4, (int) cmapG.size(), cmapG.data()));
         check(b200md_finalize(ctx));
         finalized = true;
     }
@@ -468,6 +481,102 @@ private:
     int first = 0, count = 0;
 };
 
+class B200CalcRBTorsionForceKernel : public CalcRBTorsionForceKernel {
+public:
+    B200CalcRBTorsionForceKernel(string name, const Platform& platform, ContextImpl& context) : CalcRBTorsionForceKernel(name, platform), context(context) {}
+    void initialize(const System& system, const RBTorsionForce& force) {
+        PlatformData& d = getData(context);
+        if (d.finalized) throw OpenMMException("B200 platform: RBTorsionForce initialised after the Context was finalised");
+        first = (int) d.rbI.size(); count = force.getNumTorsions();
+        for (int i = 0; i < count; i++) {
+            int a, b, c, e; double c0, c1, c2, c3, c4, c5;
+            force.getTorsionParameters(i, a, b, c, e, c0, c1, c2, c3, c4, c5);
+            d.rbI.push_back(a); d.rbJ.push_back(b); d.rbK.push_back(c); d.rbL.push_back(e);
+            for (double x : {c0, c1, c2, c3, c4, c5}) d.rbC.push_back(x);
+            d.rbG.push_back(force.getForceGroup() | (force.usesPeriodicBoundaryConditions() ? 0x80 : 0));
+        }
+        d.systemTerms |= B200MD_TERM_RB_TORSIONS; d.bondedGroupsUsed |= 1u << force.getForceGroup();
+    }
+    double execute(ContextImpl& context, bool includeForces, bool includeEnergy) { getData(context).pendingTerms |= B200MD_TERM_RB_TORSIONS; return 0.0; }
+    void copyParametersToContext(ContextImpl& context, const RBTorsionForce& force) {
+        PlatformData& d = getData(context);
+        d.ensureFinalized();
+        d.dropForces();
+        if (force.getNumTorsions() != count) throw OpenMMException("updateParametersInContext: The number of torsions has changed");
+        for (int i = 0; i < count; i++) {
+            int p, q, r, t;
+            double* c = &d.rbC[6*(size_t) (first+i)];
+            force.getTorsionParameters(i, p, q, r, t, c[0], c[1], c[2], c[3], c[4], c[5]);
+            if (p != d.rbI[first+i] || q != d.rbJ[first+i] || r != d.rbK[first+i] || t != d.rbL[first+i]) throw OpenMMException("updateParametersInContext: The set of particles in a torsion has changed");
+        }
+        d.check(b200md_update_rb_torsion_params(d.ctx, (int) d.rbI.size(), d.rbC.data()));
+    }
+private:
+    ContextImpl& context;
+    int first = 0, count = 0;
+};
+
+// The library takes spline coefficients: the reference's own platform-independent fitter makes them (call, don't rewrite).
+class B200CalcCMAPTorsionForceKernel : public CalcCMAPTorsionForceKernel {
+public:
+    B200CalcCMAPTorsionForceKernel(string name, const Platform& platform, ContextImpl& context) : CalcCMAPTorsionForceKernel(name, platform), context(context) {}
+    // the coefficients of the maps of `force`, appended to coeff; their sizes appended to size
+    static void readMaps(const CMAPTorsionForce& force, vector<int>& size, vector<double>& coeff) {
+        vector<double> energy;
+        vector<vector<double> > c;
+        for (int m = 0; m < force.getNumMaps(); m++) {
+            int n;
+            force.getMapParameters(m, n, energy);
+            CMAPTorsionForceImpl::calcMapDerivatives(n, energy, c);
+            size.push_back(n);
+            for (const vector<double>& patch : c) coeff.insert(coeff.end(), patch.begin(), patch.end());
+        }
+    }
+    void initialize(const System& system, const CMAPTorsionForce& force) {
+        PlatformData& d = getData(context);
+        if (d.finalized) throw OpenMMException("B200 platform: CMAPTorsionForce initialised after the Context was finalised");
+        firstMap = (int) d.cmapSize.size(); numMaps = force.getNumMaps();
+        firstCoeff = d.cmapCoeff.size();
+        readMaps(force, d.cmapSize, d.cmapCoeff);
+        first = (int) d.cmapMap.size(); count = force.getNumTorsions();
+        for (int i = 0; i < count; i++) {
+            int m, a[8];
+            force.getTorsionParameters(i, m, a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7]);
+            d.cmapMap.push_back(firstMap + m);
+            d.cmapAtoms.insert(d.cmapAtoms.end(), a, a + 8);
+            d.cmapG.push_back(force.getForceGroup() | (force.usesPeriodicBoundaryConditions() ? 0x80 : 0));
+        }
+        d.systemTerms |= B200MD_TERM_CMAP; d.bondedGroupsUsed |= 1u << force.getForceGroup();
+    }
+    double execute(ContextImpl& context, bool includeForces, bool includeEnergy) { getData(context).pendingTerms |= B200MD_TERM_CMAP; return 0.0; }
+    void copyParametersToContext(ContextImpl& context, const CMAPTorsionForce& force) {
+        PlatformData& d = getData(context);
+        d.ensureFinalized();
+        d.dropForces();
+        if (force.getNumMaps() != numMaps) throw OpenMMException("updateParametersInContext: The number of maps has changed");
+        if (force.getNumTorsions() != count) throw OpenMMException("updateParametersInContext: The number of CMAP torsions has changed");
+        vector<int> size;
+        vector<double> coeff;
+        readMaps(force, size, coeff);
+        for (int m = 0; m < numMaps; m++)
+            if (size[m] != d.cmapSize[firstMap+m]) throw OpenMMException("updateParametersInContext: The size of a map has changed");
+        for (int i = 0; i < count; i++) {
+            int m, a[8];
+            force.getTorsionParameters(i, m, a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7]);
+            for (int k = 0; k < 8; k++)
+                if (a[k] != d.cmapAtoms[8*(size_t) (first+i) + k]) throw OpenMMException("updateParametersInContext: The set of particles in a CMAP torsion has changed");
+            if (m < 0 || m >= numMaps) throw OpenMMException("updateParametersInContext: CMAP torsion map index out of range");
+            d.cmapMap[first+i] = firstMap + m;
+        }
+        copy(coeff.begin(), coeff.end(), d.cmapCoeff.begin() + firstCoeff);
+        d.check(b200md_update_cmap_params(d.ctx, (int) d.cmapSize.size(), d.cmapSize.data(), d.cmapCoeff.data(), (int) d.cmapMap.size(), d.cmapMap.data()));
+    }
+private:
+    ContextImpl& context;
+    int first = 0, count = 0, firstMap = 0, numMaps = 0;
+    size_t firstCoeff = 0;
+};
+
 // RemoveCMMotionKernel::execute is called by CMMotionRemoverImpl::updateContextState in EVERY step; the frequency test is
 // the kernel's (ReferenceKernels.cpp:2712-2714).  The removal itself is deferred to the integrator step that follows (the
 // fused step graph removes the centre-of-mass motion itself) or to the next read of the velocities (PlatformData::flushCm).
@@ -593,6 +702,8 @@ public:
         if (name == CalcHarmonicBondForceKernel::Name()) return new B200CalcHarmonicBondForceKernel(name, platform, context);
         if (name == CalcHarmonicAngleForceKernel::Name()) return new B200CalcHarmonicAngleForceKernel(name, platform, context);
         if (name == CalcPeriodicTorsionForceKernel::Name()) return new B200CalcPeriodicTorsionForceKernel(name, platform, context);
+        if (name == CalcRBTorsionForceKernel::Name()) return new B200CalcRBTorsionForceKernel(name, platform, context);
+        if (name == CalcCMAPTorsionForceKernel::Name()) return new B200CalcCMAPTorsionForceKernel(name, platform, context);
         if (name == RemoveCMMotionKernel::Name()) return new B200RemoveCMMotionKernel(name, platform, context);
         if (name == IntegrateVerletStepKernel::Name()) return new B200IntegrateVerletStepKernel(name, platform);
         if (name == IntegrateLangevinStepKernel::Name()) return new B200IntegrateLangevinStepKernel(name, platform);
@@ -608,7 +719,8 @@ public:
         B200KernelFactory* factory = new B200KernelFactory();
         for (const string& n : {CalcForcesAndEnergyKernel::Name(), UpdateStateDataKernel::Name(), ApplyConstraintsKernel::Name(), VirtualSitesKernel::Name(),
                                 CalcNonbondedForceKernel::Name(), CalcHarmonicBondForceKernel::Name(), CalcHarmonicAngleForceKernel::Name(),
-                                CalcPeriodicTorsionForceKernel::Name(), RemoveCMMotionKernel::Name(), IntegrateVerletStepKernel::Name(),
+                                CalcPeriodicTorsionForceKernel::Name(), CalcRBTorsionForceKernel::Name(), CalcCMAPTorsionForceKernel::Name(),
+                                RemoveCMMotionKernel::Name(), IntegrateVerletStepKernel::Name(),
                                 IntegrateLangevinStepKernel::Name(), IntegrateLangevinMiddleStepKernel::Name(), ApplyMonteCarloBarostatKernel::Name()})
             registerKernelFactory(n, factory);
         platformProperties.push_back(DeviceIndex());
