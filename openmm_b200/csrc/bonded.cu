@@ -235,5 +235,5 @@ void launch_bonded(const NbDev& nb, const BondedDev& bd, int terms, bool energy,
     if (terms & B200MD_TERM_NB_DIRECT) n += bd.nexc;
     if (n == 0) return;
     int per = (n + nb.world - 1)/nb.world;
-    k_bonded<<<(per + 127)/128, 128, 0, s>>>(nb, bd, terms, energy ? 1 : 0);
+    launch_high(k_bonded, (per + 127)/128, 128, 0, s, nb, bd, terms, energy ? 1 : 0);
 }

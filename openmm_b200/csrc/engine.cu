@@ -64,7 +64,8 @@ struct b200md_ctx {
     std::string err;
     cudaStream_t stream = nullptr;
     cudaStream_t streamPme = nullptr;   // reciprocal space runs concurrently with direct space (high priority: its kernels are small)
-    cudaEvent_t evFork = nullptr, evJoin = nullptr;
+    cudaStream_t streamBonded = nullptr;    // one GPU: the bonded terms, beside both
+    cudaEvent_t evFork = nullptr, evJoin = nullptr, evJoinBonded = nullptr;
     bool pmeOnly = false;               // b200md_pme_create: reciprocal space only, no neighbour list is ever built
     bool listDirty = true;              // state changed from outside: rebuild synchronously before the next step graph
     bool overlapPme = true;
@@ -197,8 +198,10 @@ extern "C" int b200md_create(b200md_ctx** out, int device, int natoms) {
         int hi = 0;
         CUDA_CHECK(cudaDeviceGetStreamPriorityRange(nullptr, &hi));
         CUDA_CHECK(cudaStreamCreateWithPriority(&c->streamPme, cudaStreamNonBlocking, hi));
+        CUDA_CHECK(cudaStreamCreateWithPriority(&c->streamBonded, cudaStreamNonBlocking, hi));
         CUDA_CHECK(cudaEventCreateWithFlags(&c->evFork, cudaEventDisableTiming));
         CUDA_CHECK(cudaEventCreateWithFlags(&c->evJoin, cudaEventDisableTiming));
+        CUDA_CHECK(cudaEventCreateWithFlags(&c->evJoinBonded, cudaEventDisableTiming));
         c->mass.assign(natoms, 1.0);
         c->charge.assign(natoms, 0.0); c->sigma.assign(natoms, 1.0); c->epsilon.assign(natoms, 0.0);
         const char* pf = getenv("B200MD_PAD_FRACTION");
@@ -222,8 +225,10 @@ extern "C" void b200md_destroy(b200md_ctx* ctx) {
     if (ctx->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(ctx->comm);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
     if (ctx->streamPme) cudaStreamDestroy(ctx->streamPme);
+    if (ctx->streamBonded) cudaStreamDestroy(ctx->streamBonded);
     if (ctx->evFork) cudaEventDestroy(ctx->evFork);
     if (ctx->evJoin) cudaEventDestroy(ctx->evJoin);
+    if (ctx->evJoinBonded) cudaEventDestroy(ctx->evJoinBonded);
     char* window = ctx->window;
     delete ctx;
     if (window) cudaFree(window);
@@ -1065,6 +1070,12 @@ static void alloc_tile_pools(b200md_ctx* c, int poolCap) {
     }
 }
 
+// The reciprocal-space chain runs beside a tile kernel that holds every SM: one GPU, two streams, no SM partition.  Its FFT
+// then runs as small CTAs that fit the slots retiring tile CTAs hand back (fft.cu); everywhere else it keeps the larger ones.
+static bool fft_beside_tiles(const b200md_ctx* c) {
+    return c->world == 1 && !c->pmeOnly && c->overlapPme && !c->nb.smPartition && c->nbdesc.method == B200MD_NB_PME;
+}
+
 extern "C" int b200md_finalize(b200md_ctx* ctx) {
     API_BEGIN(ctx)
     require(!ctx->finalized, "finalize called twice");
@@ -1258,6 +1269,8 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
         nb.nmol = (int) count.size(); nb.molStart = c->molStart.p; nb.molAtoms = c->molAtoms.p;
     }
     if (nb.method == B200MD_NB_PME) setup_pme(c, c->nbdesc.grid[0], c->nbdesc.grid[1], c->nbdesc.grid[2], c->nbdesc.ewald_alpha);
+    // the chain's CTAs join SMs that run the tile kernel (the brick's static shared memory is a few words)
+    if (fft_beside_tiles(c)) pair_set_carveout(fft_cta_smem_bytes(c->pme), sizeof(long long)*(size_t) c->brickPoints + 64);
     c->finalized = true;
     try { apply_box(c); } catch (...) { c->finalized = false; throw; }      // e.g. box smaller than twice the cutoff: the caller may fix the box and finalize again
     c->integ.stepCounter = c->stepCounter.p;
@@ -1603,7 +1616,7 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
                 int rc = g_nccl.AllReduce(c->gridFixed.p, c->gridFixed.p, (size_t) c->pme.nx*c->pme.ny*c->pme.nz, NCCL_INT64, NCCL_SUM, c->comm, sp);
                 if (rc != 0) throw std::runtime_error("ncclAllReduce(grid) failed");
             }
-            launch_pme_fft_conv(c->nb, c->pme, c->cd, energy && (split || p2p || c->rank == 0), sp); launches += pme_fft_launch_count(c->pme);
+            launch_pme_fft_conv(c->nb, c->pme, c->cd, energy && (split || p2p || c->rank == 0), fft_beside_tiles(c), sp); launches += pme_fft_launch_count(c->pme);
             launch_pme_gather(c->nb, pme, c->cd, sp); launches++;
         }
         if (fork) CUDA_CHECK(cudaEventRecord(c->evJoin, sp));
@@ -1613,18 +1626,29 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
         launch_check_displacement(c->nb, c->cd, s); launches++;
         launch_list_build(c->nb, s); launches += LIST_BUILD_LAUNCHES;
     }
-    if (forkAfterList) launch_recip();
-    if (direct) { launch_pair(c->nb, energy, s); launches++; }
     int bterms = terms & (B200MD_TERM_BONDS | B200MD_TERM_ANGLES | B200MD_TERM_TORSIONS | B200MD_TERM_RB_TORSIONS | B200MD_TERM_CMAP);
     if (c->haveNb) bterms |= terms & B200MD_TERM_NB_DIRECT;
     const int nbonded = c->bd.nbonds + c->bd.nangles + c->bd.ntorsions + c->bd.nrb + c->bd.ncmap + c->bd.nexc;
-    if (bterms && nbonded > 0 && !(split && c->rank == pmeRank)) { BondedDev bd = c->bd; bd.groupMask = groupMask; launch_bonded(c->nb, bd, bterms, energy, s); launches++; }
+    const bool bonded = bterms && nbonded > 0 && !(split && c->rank == pmeRank);
+    auto launch_bonded_terms = [&](cudaStream_t sb) { BondedDev bd = c->bd; bd.groupMask = groupMask; launch_bonded(c->nb, bd, bterms, energy, sb); launches++; };
+    // The bonded terms need nothing from the tile kernel either: on one GPU they fork with the spread onto a stream of their
+    // own (not before the list build, whose wrap phase moves molecules in posq) and join before the integrator.
+    const bool forkBonded = forkAfterList && bonded;
+    if (forkAfterList) launch_recip();
+    if (forkBonded) {
+        CUDA_CHECK(cudaStreamWaitEvent(c->streamBonded, c->evFork, 0));
+        launch_bonded_terms(c->streamBonded);
+        CUDA_CHECK(cudaEventRecord(c->evJoinBonded, c->streamBonded));
+    }
+    if (direct) { launch_pair(c->nb, energy, s); launches++; }
+    if (bonded && !forkBonded) launch_bonded_terms(s);
     // p2p: partial forces of the atoms this rank does not own -> the owners' inboxes.  Reciprocal space only ever touches the
     // atoms this rank OWNS (k_pme_gather), so when it runs on its own stream the push does not have to wait for it: it goes
     // out right behind the tile kernel and the bonded terms, beside the FFT chain.
     const bool pushEarly = p2p && fork;
     if (pushEarly) { launch_force_push(c->nb, c->cd, s); launches++; }
     if (fork) CUDA_CHECK(cudaStreamWaitEvent(s, c->evJoin, 0));
+    if (forkBonded) CUDA_CHECK(cudaStreamWaitEvent(s, c->evJoinBonded, 0));
     if (p2p) {
         if (!pushEarly) { launch_force_push(c->nb, c->cd, s); launches++; }
         // in the step path k_integrate totals own partial + inboxes; here (energies, getState) the owners total and broadcast
@@ -1801,7 +1825,10 @@ static void capture_steps(b200md_ctx* c, int nsteps, cudaGraphExec_t* exec, int*
         (void) cudaGetLastError();          // the refusal is not sticky: fall back to a new instantiation
     }
     if (*exec) { cudaGraphExecDestroy(*exec); *exec = nullptr; }
-    const cudaError_t e = cudaGraphInstantiate(exec, g, 0);
+    // One GPU: the graph runs each kernel node at its own priority (launch_high), not at the priority of c->stream, so the
+    // reciprocal-space chain and the bonded terms take the SM slots that the tile kernel's CTAs hand back.  An update in
+    // place keeps the priorities: every capture gives the same nodes the same ones.
+    const cudaError_t e = cudaGraphInstantiate(exec, g, c->world == 1 ? cudaGraphInstantiateFlagUseNodePriority : 0);
     cudaGraphDestroy(g);
     CUDA_CHECK(e);
     c->graphInstantiations++;
@@ -2019,7 +2046,7 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
         switch (phase) {
             case 0: launch_pair(nbv, false, s); break;
             case 1: launch_pme_spread(nbv, pme_for_launch(c), local, s); break;
-            case 2: launch_pme_fft_conv(nbv, c->pme, local, false, s); break;
+            case 2: launch_pme_fft_conv(nbv, c->pme, local, false, fft_beside_tiles(c), s); break;
             case 3: launch_pme_gather(nbv, pme_for_launch(c), local, s); break;
             case 4: launch_integrate(nbv, c->units, c->integ, local, s); break;
             case 5: launch_list_build(nbv, s); break;

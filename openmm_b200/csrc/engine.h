@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdexcept>
 #include <string>
 #include <vector>
 
@@ -15,6 +16,25 @@
 #define B200MD_MAX_FFT_STAGES 8
 
 #define CUDA_CHECK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) throw std::runtime_error(std::string(#x) + ": " + cudaGetErrorString(e_)); } while (0)
+
+// Launch at the device's greatest stream priority, carried by the launch (cudaLaunchAttributePriority) rather than by the
+// stream, so that a node captured into a step graph keeps it: the single-GPU step graph is instantiated with
+// cudaGraphInstantiateFlagUseNodePriority.  The reciprocal-space chain and the bonded terms launch this way; the CTA
+// dispatcher then gives them the SM slots that retiring tile-kernel CTAs hand back before the tile kernel's queued CTAs.
+// Elsewhere the attribute changes nothing that matters: multi-GPU graphs are instantiated without the flag, so their nodes
+// run at the launch stream's priority as before, and outside graphs these kernels either run on the high-priority
+// reciprocal-space stream already or sit in one stream behind the kernels they depend on.
+template <typename... P, typename... A>
+inline void launch_high(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, A... args) {
+    static const int hi = [] { int lo = 0, h = 0; cudaDeviceGetStreamPriorityRange(&lo, &h); return h; }();
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributePriority;
+    at[0].val.priority = hi;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, args...));
+}
 
 // Periodic box, reduced lower-triangular form (ContextImpl.cpp:267-275): a=(ax,0,0) b=(bx,by,0) c=(cx,cy,cz).
 struct BoxDev {
@@ -425,12 +445,14 @@ void launch_check_displacement(const NbDev& nb, const CommDev& cd, cudaStream_t 
 const int LIST_BUILD_LAUNCHES = 2;
 void launch_list_build(const NbDev& nb, cudaStream_t s);     // k_list_prep (grid barriers) + k_build_tiles, gated on counters[CT_REBUILD]
 void launch_pair(const NbDev& nb, bool energy, cudaStream_t s);
+void pair_set_carveout(size_t fftSmem, size_t brickSmem);     // shared memory for a chain CTA beside the tile CTAs left on an SM
 void launch_count_pairs(const NbDev& nb, cudaStream_t s);
 int choose_pme_sms(int reserve, unsigned long long mask[4]);     // SM partition of the tile kernel (NbDev::pmeSmMask)
 
 void launch_pme_eterm(const NbDev& nb, const PmeDev& pme, cudaStream_t s);
 void launch_pme_spread(const NbDev& nb, const PmeDev& pme, const CommDev& cd, cudaStream_t s);
-void launch_pme_fft_conv(const NbDev& nb, const PmeDev& pme, const CommDev& cd, bool energy, cudaStream_t s);
+// besideTiles: one GPU, the chain shares every SM with the tile kernel (smaller FFT CTAs, fft.cu)
+void launch_pme_fft_conv(const NbDev& nb, const PmeDev& pme, const CommDev& cd, bool energy, bool besideTiles, cudaStream_t s);
 void launch_pme_gather(const NbDev& nb, const PmeDev& pme, const CommDev& cd, cudaStream_t s);
 void pme_brick_setup(int maxSmem);
 void launch_grid_push(const PmeDev& pme, const CommDev& cd, cudaStream_t s);
@@ -441,6 +463,7 @@ size_t fft_line_smem_bytes(int nx);
 bool fft_make_radices(int n, int* radix, int* nstages);
 int pme_fft_launch_count(const PmeDev& pme);
 void fft_set_compact(int on);                   // smaller FFT CTAs (the chain shares the GPU with the tile kernel)
+size_t fft_cta_smem_bytes(const PmeDev& pme);  // largest shared memory of one single-GPU FFT CTA of this grid (dynamic + static)
 bool fft_slab_path(const PmeDev& pme);          // the 3-launch slab pipeline is usable for this grid (precondition of the multi-GPU FFT)
 
 void launch_bonded(const NbDev& nb, const BondedDev& bd, int terms, bool energy, cudaStream_t s);

@@ -588,22 +588,23 @@ __global__ void __launch_bounds__(FFT_THREADS) k_fft_slab_inv(PmeDev pme, size_t
 
 // Threads per CTA.  The kernels are compiled for up to 512 threads at 128 registers, i.e. a 512-thread CTA owns a whole SM's
 // register file.  A (y,z) plane keeps 512 threads busy only in its load / store phases (a radix-11 stage of an 88-point
-// line has 8 butterflies per line), a batch of 16 x lines even less: when the reciprocal-space chain shares the GPU with
-// the tile kernel (SM partition, multi-GPU) smaller CTAs let 2-4 of them share one of the few SMs it has.
+// line has 8 butterflies per line), a batch of 16 x lines even less.  On one GPU (besideTiles) the chain runs beside the
+// tile kernel, whose four CTAs per SM hold the whole register file: a 128-thread CTA (about 13,000 registers) fits the
+// slot that one retiring tile CTA hands back, a 512-thread CTA would wait for an SM to drain.  With an SM partition
+// (multi-GPU) smaller CTAs let 2-4 of them share one of the few SMs the chain has.  Every butterfly is computed the same
+// way whichever thread takes it, so the shape does not change a bit of the result.
 // B200MD_FFT_THREADS / B200MD_FFTX_THREADS override (slab kernels / x-line kernel).
 static int g_fft_compact = 0;            // fft_set_compact(): the chain runs on a reserved subset of the SMs; 2 = fewer SMs than planes per rank
 void fft_set_compact(int on) { g_fft_compact = on; }
-static int fft_threads() {
+static int fft_threads(bool besideTiles) {
     static const int env = getenv("B200MD_FFT_THREADS") ? std::min(FFT_THREADS, std::max(64, atoi(getenv("B200MD_FFT_THREADS")))) : 0;
-    return env ? env : (g_fft_compact == 2 ? 256 : FFT_THREADS);       // a plane per SM when there is one: 512 threads finish it in ~2/3 of the time of 256
+    if (env) return env;
+    if (besideTiles) return 128;
+    return g_fft_compact == 2 ? 256 : FFT_THREADS;       // a plane per SM when there is one: 512 threads finish it in ~2/3 of the time of 256
 }
-static int fftx_threads() {
+static int fftx_threads(bool besideTiles) {
     static const int env = getenv("B200MD_FFTX_THREADS") ? std::min(FFT_THREADS, std::max(64, atoi(getenv("B200MD_FFTX_THREADS")))) : 0;
-    return env ? env : (g_fft_compact ? 128 : fft_threads());
-}
-static dim3 fft_block(int n, int maxLines) {
-    (void) n; (void) maxLines;
-    return dim3(fft_threads());
+    return env ? env : (g_fft_compact ? 128 : fft_threads(besideTiles));
 }
 
 struct FftLaunch {
@@ -611,7 +612,7 @@ struct FftLaunch {
     int zb, yb, xb;
     dim3 zt, yt, xt, st;
     bool slab;
-    FftLaunch(const PmeDev& p) {
+    FftLaunch(const PmeDev& p, bool besideTiles = false) {
         int dev = 0, maxSmem = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&maxSmem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
@@ -620,14 +621,14 @@ struct FftLaunch {
         const int nmax = p.ny > p.nz ? p.ny : p.nz;
         slab = ss <= (size_t) maxSmem && nmax <= 1024 && getenv("B200MD_FFT_NOSLAB") == nullptr;
         if (slab) {
-            st = dim3(fft_threads());
+            st = dim3(fft_threads(besideTiles));
             set_smem((const void*) k_fft_slab_fwd, ss);
             set_smem((const void*) k_fft_slab_inv, ss);
         }
         zs = (2*(size_t) (ZROWS/2)*p.nz + 3*p.nz)*sizeof(real2);
         ys = (2*(size_t) LINE_BATCH*p.ny + 3*p.ny)*sizeof(real2);
         xs = (2*(size_t) LINE_BATCH*p.nx + 3*p.nx)*sizeof(real2);
-        zt = fft_block(p.nz, ZROWS/2); yt = fft_block(p.ny, LINE_BATCH); xt = dim3(fftx_threads());
+        zt = yt = dim3(fft_threads(besideTiles)); xt = dim3(fftx_threads(besideTiles));
         zb = (p.nx*p.ny + ZROWS - 1)/ZROWS;
         yb = p.nx*((p.nzc + LINE_BATCH - 1)/LINE_BATCH);
         xb = (p.ny*p.nzc + LINE_BATCH - 1)/LINE_BATCH;
@@ -641,17 +642,17 @@ struct FftLaunch {
 
 static const CommDev g_single = [] { CommDev c{}; c.world = 1; return c; }();
 static void fwd_zy(const FftLaunch& L, const PmeDev& pme, cudaStream_t s) {
-    if (L.slab) k_fft_slab_fwd<<<pme.nx, L.st, L.ss, s>>>(pme, L.selems, g_single);
+    if (L.slab) launch_high(k_fft_slab_fwd, pme.nx, L.st, L.ss, s, pme, L.selems, g_single);
     else {
-        k_fft_z_fwd<<<L.zb, L.zt, L.zs, s>>>(pme);
-        k_fft_y<<<L.yb, L.yt, L.ys, s>>>(pme, 0);
+        launch_high(k_fft_z_fwd, L.zb, L.zt, L.zs, s, pme);
+        launch_high(k_fft_y, L.yb, L.yt, L.ys, s, pme, 0);
     }
 }
 static void inv_yz(const FftLaunch& L, const PmeDev& pme, cudaStream_t s) {
-    if (L.slab) k_fft_slab_inv<<<pme.nx, L.st, L.ss, s>>>(pme, L.selems, g_single);
+    if (L.slab) launch_high(k_fft_slab_inv, pme.nx, L.st, L.ss, s, pme, L.selems, g_single);
     else {
-        k_fft_y<<<L.yb, L.yt, L.ys, s>>>(pme, 1);
-        k_fft_z_inv<<<L.zb, L.zt, L.zs, s>>>(pme);
+        launch_high(k_fft_y, L.yb, L.yt, L.ys, s, pme, 1);
+        launch_high(k_fft_z_inv, L.zb, L.zt, L.zs, s, pme);
     }
 }
 
@@ -659,34 +660,46 @@ int pme_fft_launch_count(const PmeDev& pme) { FftLaunch L(pme); return L.slab ? 
 
 bool fft_slab_path(const PmeDev& pme) { FftLaunch L(pme); return L.slab; }
 
-void launch_pme_fft_conv(const NbDev& nb, const PmeDev& pme, const CommDev& cd, bool energy, cudaStream_t s) {
-    FftLaunch L(pme);
+size_t fft_cta_smem_bytes(const PmeDev& pme) {
+    FftLaunch L(pme, true);
+    const void* kernels[] = {(const void*) k_fft_slab_fwd, (const void*) k_fft_slab_inv, (const void*) k_fft_x_conv<true>,
+                             (const void*) k_fft_x_conv<false>, (const void*) k_fft_z_fwd, (const void*) k_fft_z_inv, (const void*) k_fft_y};
+    size_t stat = 0;
+    for (const void* k : kernels) {
+        cudaFuncAttributes fa;
+        CUDA_CHECK(cudaFuncGetAttributes(&fa, k));
+        stat = std::max(stat, fa.sharedSizeBytes);
+    }
+    const size_t dyn = L.slab ? std::max(L.ss, L.xs) : std::max(L.zs, std::max(L.ys, L.xs));
+    return dyn + stat;
+}
+
+void launch_pme_fft_conv(const NbDev& nb, const PmeDev& pme, const CommDev& cd, bool energy, bool besideTiles, cudaStream_t s) {
+    FftLaunch L(pme, besideTiles);
     if (cd.world > 1) {
         // slab-decomposed over the ranks (the slab path is a precondition, checked when the communicator is set up)
         const int planes = cd.xLo[cd.rank + 1] - cd.xLo[cd.rank];
         const int plane = pme.ny*pme.nzc;
         const int mcount = std::max(0, std::min(cd.lineChunk, plane - cd.rank*cd.lineChunk));
         const int xb = std::max(1, (mcount + LINE_BATCH - 1)/LINE_BATCH);
-        k_fft_slab_fwd<<<std::max(1, planes), L.st, L.ss, s>>>(pme, L.selems, cd);
-        if (energy) k_fft_x_conv<true><<<xb, L.xt, L.xs, s>>>(pme, nb.energy + EN_RECIP, 0, cd);
-        else k_fft_x_conv<false><<<xb, L.xt, L.xs, s>>>(pme, nb.energy + EN_RECIP, 0, cd);
-        k_fft_slab_inv<<<std::max(1, planes), L.st, L.ss, s>>>(pme, L.selems, cd);
+        launch_high(k_fft_slab_fwd, std::max(1, planes), L.st, L.ss, s, pme, L.selems, cd);
+        launch_high(energy ? k_fft_x_conv<true> : k_fft_x_conv<false>, xb, L.xt, L.xs, s, pme, nb.energy + EN_RECIP, 0, cd);
+        launch_high(k_fft_slab_inv, std::max(1, planes), L.st, L.ss, s, pme, L.selems, cd);
         return;
     }
     fwd_zy(L, pme, s);
-    if (energy) k_fft_x_conv<true><<<L.xb, L.xt, L.xs, s>>>(pme, nb.energy + EN_RECIP, 0, g_single);
-    else k_fft_x_conv<false><<<L.xb, L.xt, L.xs, s>>>(pme, nb.energy + EN_RECIP, 0, g_single);
+    launch_high(energy ? k_fft_x_conv<true> : k_fft_x_conv<false>, L.xb, L.xt, L.xs, s, pme, nb.energy + EN_RECIP, 0, g_single);
     inv_yz(L, pme, s);
 }
 
 void launch_fft3d_r2c(const PmeDev& pme, cudaStream_t s) {
     FftLaunch L(pme);
     fwd_zy(L, pme, s);
-    k_fft_x_conv<false><<<L.xb, L.xt, L.xs, s>>>(pme, nullptr, 1, g_single);
+    launch_high(k_fft_x_conv<false>, L.xb, L.xt, L.xs, s, pme, (double*) nullptr, 1, g_single);
 }
 
 void launch_fft3d_c2r(const PmeDev& pme, cudaStream_t s) {
     FftLaunch L(pme);
-    k_fft_x_conv<false><<<L.xb, L.xt, L.xs, s>>>(pme, nullptr, 2, g_single);
+    launch_high(k_fft_x_conv<false>, L.xb, L.xt, L.xs, s, pme, (double*) nullptr, 2, g_single);
     inv_yz(L, pme, s);
 }

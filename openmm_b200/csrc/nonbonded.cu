@@ -1002,16 +1002,39 @@ static void launch_pair_m(const NbDev& nb, cudaStream_t s) {
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    // M waves of short-lived CTAs instead of one wave of persistent ones: SM slots are handed back while the kernel runs
-    // and the reciprocal-space kernels queued behind it start in its tail instead of after it (measured 1-2 %: DHFR
-    // 119.3 -> 117.6 us/step, ApoA1 352 -> 343; the CTA dispatcher is FIFO over launched grids, stream priority does not
-    // let a later grid overtake CTAs that are already queued)
+    // M waves of short-lived CTAs instead of one wave of persistent ones: SM slots are handed back while the kernel runs.
+    // On one GPU the reciprocal-space chain and the bonded terms are graph nodes of a higher priority (launch_high, and the
+    // step graph is instantiated with cudaGraphInstantiateFlagUseNodePriority); the FFT, gather and bonded CTAs fit one
+    // such slot (in registers; shared memory through pair_set_carveout), so they take the slots as they come free and run
+    // inside the tile kernel's span rather than after it.  The spread brick takes two slots.
     const int waves = 4, perSm = 4;
     dim3 grid(sms*perSm*(nb.smPartition ? 1 : waves)), block(256);       // partitioned: ONE persistent wave, tiles from the cursor
     switch (nb.method) {
         case B200MD_NB_PME: k_pair<ENERGY, B200MD_NB_PME><<<grid, block, 0, s>>>(nb); break;
         case B200MD_NB_NOCUTOFF: k_pair<ENERGY, B200MD_NB_NOCUTOFF><<<grid, block, 0, s>>>(nb); break;
         default: k_pair<ENERGY, B200MD_NB_CUTOFF_PERIODIC><<<grid, block, 0, s>>>(nb); break;
+    }
+}
+
+// Shared-memory carve-out of the PME tile kernel.  Left to itself the driver may configure an SM that runs four tile CTAs
+// (a few KiB of shared memory each) with a small carve-out; a chain CTA that needs tens of KiB could then join that SM only
+// after it drained and was reconfigured, and while such a high-priority CTA waits, SMs drain for it.  An FFT CTA (fftSmem
+// bytes, at most 16,384 registers) joins an SM as soon as one tile CTA retires, so it needs room beside three tile CTAs;
+// a spread-brick CTA (brickSmem bytes, 20,480 registers) joins once two have retired, beside two.  Ask for the larger of
+// the two; a percentage between two supported capacities selects the larger one.
+void pair_set_carveout(size_t fftSmem, size_t brickSmem) {
+    int dev = 0, perSm = 0, reserved = 0;
+    CUDA_CHECK(cudaGetDevice(&dev));
+    CUDA_CHECK(cudaDeviceGetAttribute(&perSm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
+    CUDA_CHECK(cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev));
+    const void* kernels[] = {(const void*) k_pair<false, B200MD_NB_PME>, (const void*) k_pair<true, B200MD_NB_PME>};
+    for (const void* k : kernels) {
+        cudaFuncAttributes fa;
+        CUDA_CHECK(cudaFuncGetAttributes(&fa, k));
+        const size_t tile = fa.sharedSizeBytes + reserved;
+        const size_t need = std::max(3*tile + fftSmem, 2*tile + brickSmem) + reserved;
+        const int percent = std::min(100, (int) ((100*need + perSm - 1)/perSm));
+        CUDA_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, percent));
     }
 }
 
