@@ -65,7 +65,7 @@ struct b200md_ctx {
     cudaStream_t stream = nullptr;
     cudaStream_t streamPme = nullptr;   // reciprocal space runs concurrently with direct space (high priority: its kernels are small)
     cudaStream_t streamBonded = nullptr;    // one GPU: the bonded terms, beside both
-    cudaEvent_t evFork = nullptr, evJoin = nullptr, evJoinBonded = nullptr;
+    cudaEvent_t evFork = nullptr, evJoin = nullptr, evJoinBonded = nullptr, evForkGrid = nullptr;
     bool pmeOnly = false;               // b200md_pme_create: reciprocal space only, no neighbour list is ever built
     bool listDirty = true;              // state changed from outside: rebuild synchronously before the next step graph
     bool overlapPme = true;
@@ -202,6 +202,7 @@ extern "C" int b200md_create(b200md_ctx** out, int device, int natoms) {
         CUDA_CHECK(cudaEventCreateWithFlags(&c->evFork, cudaEventDisableTiming));
         CUDA_CHECK(cudaEventCreateWithFlags(&c->evJoin, cudaEventDisableTiming));
         CUDA_CHECK(cudaEventCreateWithFlags(&c->evJoinBonded, cudaEventDisableTiming));
+        CUDA_CHECK(cudaEventCreateWithFlags(&c->evForkGrid, cudaEventDisableTiming));
         c->mass.assign(natoms, 1.0);
         c->charge.assign(natoms, 0.0); c->sigma.assign(natoms, 1.0); c->epsilon.assign(natoms, 0.0);
         const char* pf = getenv("B200MD_PAD_FRACTION");
@@ -229,6 +230,7 @@ extern "C" void b200md_destroy(b200md_ctx* ctx) {
     if (ctx->evFork) cudaEventDestroy(ctx->evFork);
     if (ctx->evJoin) cudaEventDestroy(ctx->evJoin);
     if (ctx->evJoinBonded) cudaEventDestroy(ctx->evJoinBonded);
+    if (ctx->evForkGrid) cudaEventDestroy(ctx->evForkGrid);
     char* window = ctx->window;
     delete ctx;
     if (window) cudaFree(window);
@@ -1610,7 +1612,7 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
             CUDA_CHECK(cudaStreamWaitEvent(sp, c->evFork, 0));
         }
         if (recip) {
-            launch_pme_spread(c->nb, pme, c->cd, sp); launches++;
+            launch_pme_spread(c->nb, pme, c->cd, sp, !forkAfterList); launches++;
             if (p2p) { launch_grid_push(c->pme, c->cd, sp); launches++; }
             else if (c->world > 1 && c->comm && !split) {
                 int rc = g_nccl.AllReduce(c->gridFixed.p, c->gridFixed.p, (size_t) c->pme.nx*c->pme.ny*c->pme.nz, NCCL_INT64, NCCL_SUM, c->comm, sp);
@@ -1622,6 +1624,14 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
         if (fork) CUDA_CHECK(cudaEventRecord(c->evJoin, sp));
     };
     if (!forkAfterList) launch_recip();
+    // When the chain forks after the list build, the charge grid is zeroed at the head of the step on the chain's stream,
+    // beside the list check and build: it needs nothing from them, and as the spread's first node it sat on the chain, which
+    // is the step's longest path (DHFR: memset 1.6 us plus a node gap before the spread).
+    if (forkAfterList && recip) {
+        CUDA_CHECK(cudaEventRecord(c->evForkGrid, s));
+        CUDA_CHECK(cudaStreamWaitEvent(sp, c->evForkGrid, 0));
+        CUDA_CHECK(cudaMemsetAsync(pme.gridFixed, 0, sizeof(long long)*(size_t) pme.nx*pme.ny*pme.nz, sp));
+    }
     if (direct) {
         launch_check_displacement(c->nb, c->cd, s); launches++;
         launch_list_build(c->nb, s); launches += LIST_BUILD_LAUNCHES;

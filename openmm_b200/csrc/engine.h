@@ -450,7 +450,8 @@ void launch_count_pairs(const NbDev& nb, cudaStream_t s);
 int choose_pme_sms(int reserve, unsigned long long mask[4]);     // SM partition of the tile kernel (NbDev::pmeSmMask)
 
 void launch_pme_eterm(const NbDev& nb, const PmeDev& pme, cudaStream_t s);
-void launch_pme_spread(const NbDev& nb, const PmeDev& pme, const CommDev& cd, cudaStream_t s);
+// zeroGrid = false: the caller has zeroed pme.gridFixed on this stream already (the single-GPU step does it at its head)
+void launch_pme_spread(const NbDev& nb, const PmeDev& pme, const CommDev& cd, cudaStream_t s, bool zeroGrid = true);
 // besideTiles: one GPU, the chain shares every SM with the tile kernel (smaller FFT CTAs, fft.cu)
 void launch_pme_fft_conv(const NbDev& nb, const PmeDev& pme, const CommDev& cd, bool energy, bool besideTiles, cudaStream_t s);
 void launch_pme_gather(const NbDev& nb, const PmeDev& pme, const CommDev& cd, cudaStream_t s);

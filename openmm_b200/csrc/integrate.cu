@@ -1,4 +1,4 @@
-// integrate.cu -- fused integrate + constrain step (sm_90a): one thread per integration unit
+// integrate.cu -- fused integrate + constrain step (sm_90a): one lane per atom, 4 lanes per integration unit
 // (a rigid 3-atom molecule, an X-H_n SHAKE cluster or a free atom), everything in registers, ONE launch.
 //
 // Restates ReferenceStochasticDynamics::update (ReferenceStochasticDynamics.cpp:89-194),
@@ -215,6 +215,29 @@ __device__ __forceinline__ void constrain_vel(const Unit<R>& U, V3<R>* v, R tol)
     else if (U.type == 2) shake_velocities(U.x, v, U.invM, U.n-1, tol);
 }
 
+// Work mapping of k_integrate: 4 lanes per unit, lane k of the group owns atom k of the unit (lanes past the unit's atom
+// count only join the shuffles).  Loads, force zeroing, CM-velocity removal, noise, the velocity update and the stores are
+// per atom; for the constraint solve every lane of the group gathers the whole unit by warp shuffle and runs the same
+// SETTLE / SHAKE code on the same operands (so all four hold the same bits) and keeps its own atom's result.  A group never
+// straddles a warp (8 units per warp).  A block covers INTEG_UNITS units, the same 64 as the one-thread-per-unit kernel it
+// replaced, so its centre-of-mass partial is summed over the same units in the same order.
+constexpr int INTEG_LANES = 4;
+constexpr int INTEG_UNITS = 64;
+constexpr int INTEG_THREADS = INTEG_LANES*INTEG_UNITS;
+
+__device__ __forceinline__ float shfl_r(float x, int src) { return __shfl_sync(0xffffffffu, x, src); }
+__device__ __forceinline__ double shfl_r(double x, int src) { return __shfl_sync(0xffffffffu, x, src); }
+template <class R>
+__device__ __forceinline__ V3<R> shfl_v3(V3<R> a, int src) { return {shfl_r(a.x, src), shfl_r(a.y, src), shfl_r(a.z, src)}; }
+
+// this lane's atom out of a per-unit array (unrolled selects: a dynamic index would put the array in local memory)
+template <class T>
+__device__ __forceinline__ T pick(const T* w, int k) {
+    T r = w[0];
+    _Pragma("unroll") for (int j = 1; j < 4; j++) if (k == j) r = w[j];
+    return r;
+}
+
 // Fused epilogue work (in.fused != 0, the b200md_step path):
 //  * centre-of-mass motion removal (CMMotionRemover, frequency 1): the momentum of the velocities this kernel WRITES is
 //    reduced into cm[(step+1)%3]; the next step subtracts cm[step%3]/mass before integrating (same velocities, so the same
@@ -227,18 +250,18 @@ __device__ __forceinline__ void constrain_vel(const Unit<R>& U, V3<R>* v, R tol)
 // NVLink -- the integrate step IS the position all-gather.  The last block hands its momentum sums to everybody and
 // publishes CH_POS.
 template <int KIND, class R>
-__global__ void __launch_bounds__(128, sizeof(R) == 8 ? 1 : 0) k_integrate(NbDev nb, UnitDev un, IntegDev in, CommDev cd) {
+__global__ void __launch_bounds__(INTEG_THREADS, 1) k_integrate(NbDev nb, UnitDev un, IntegDev in, CommDev cd) {
     const bool multi = cd.world > 1;
     const bool useInbox = multi && in.fused;       // step path; after b200md_compute the force buffer already holds the totals
     const unsigned long long E = multi ? *cd.epoch + 1ull : 0ull;
     if (useInbox) comm_wait(cd, CH_FORCE, E);
-    const int u = (multi ? cd.unitLo[cd.rank] : 0) + blockIdx.x*blockDim.x + threadIdx.x;
+    const int ka = threadIdx.x & (INTEG_LANES - 1);                     // this lane's atom in its unit
+    const int g = threadIdx.x & 31 & ~(INTEG_LANES - 1);               // the group's first lane in the warp
+    const int ub = threadIdx.x / INTEG_LANES;                          // the unit's index in the block
+    const int u = (multi ? cd.unitLo[cd.rank] : 0) + blockIdx.x*INTEG_UNITS + ub;
     const bool active = u < (multi ? cd.unitLo[cd.rank + 1] : un.nunits);
     const unsigned long long step = *in.stepCounter;
     const IntegR<R> ic = integ_r<R>(in);
-    Unit<R> U;
-    U.n = 0;
-    V3<R> d[4];
     const R invDt = R(1)/ic.dt;
     const bool cmFused = in.fused && in.cmEveryStep;
     V3<R> vcm = {R(0), R(0), R(0)};
@@ -254,55 +277,103 @@ __global__ void __launch_bounds__(128, sizeof(R) == 8 ? 1 : 0) k_integrate(NbDev
         const double im = (c[3] > 0.0) ? 1.0/c[3] : 0.0;
         vcm = {(R) (c[0]*im), (R) (c[1]*im), (R) (c[2]*im)};
     }
+    // the unit's constraint data (every lane of the group reads the same words) and this lane's atom
+    Unit<R> U;
+    U.n = 0; U.type = 0;
+    int a = -1;
     if (active) {
-    load_unit(nb, un, u, U, true, useInbox ? &cd : nullptr);
-    if (in.fused) {
-        _Pragma("unroll") for (int k = 0; k < 4; k++) if (k < U.n) {
-            const int a = U.atom[k];
+        const int4 at = un.unitAtoms[u];
+        U.n = at.w >= 0 ? 4 : at.z >= 0 ? 3 : at.y >= 0 ? 2 : at.x >= 0 ? 1 : 0;
+        a = ka == 0 ? at.x : ka == 1 ? at.y : ka == 2 ? at.z : at.w;
+        U.type = un.unitType[u];
+        U.prm = unit_params<R>(un, u);
+    }
+    const bool own = a >= 0;
+    V3<R> x = {R(0), R(0), R(0)}, v = x, f = x, d = x;
+    R invM = R(0), m = R(0);
+    if (own) {
+        const R4<R> p = load_pos<R>(nb, a);
+        const R4<R> vm = vel_array<R>(nb)[a];
+        x = {p.x, p.y, p.z};
+        v = {vm.x, vm.y, vm.z};
+        invM = vm.w;
+        m = (vm.w > R(0)) ? R(1)/vm.w : R(0);
+        long long fx = nb.force[a], fy = nb.force[a + nb.npad], fz = nb.force[a + 2*nb.npad];
+        if (useInbox) {
+            // owner: total = own partial + what the other ranks pushed into the inboxes (exact int64 sums, any order)
+            const long long* inbox = (const long long*) (cd.peer[cd.rank] + cd.offFinbox);
+            for (int q = 0; q < cd.world; q++) if (q != cd.rank) {
+                const long long* iq = inbox + (size_t) q*3*nb.npad;
+                fx += iq[a]; fy += iq[a + nb.npad]; fz += iq[a + 2*nb.npad];
+            }
+        }
+        f = {fixed_to_real<R>(fx), fixed_to_real<R>(fy), fixed_to_real<R>(fz)};
+        if (in.fused) {
             nb.force[a] = 0; nb.force[a + nb.npad] = 0; nb.force[a + 2*nb.npad] = 0;
-            if (U.invM[k] > R(0)) U.v[k] = U.v[k] - vcm;
+            if (invM > R(0)) v = v - vcm;
         }
     }
-    if (KIND == B200MD_INT_LANGEVIN_MIDDLE) {
-        _Pragma("unroll") for (int k = 0; k < 4; k++) if (k < U.n) U.v[k] = U.v[k] + U.f[k]*(ic.dt*U.invM[k]);
-        constrain_vel(U, U.v, ic.tol);
-        V3<R> du[4];
-        _Pragma("unroll") for (int k = 0; k < 4; k++) if (k < U.n) {
-            d[k] = U.v[k]*(R(0.5)*ic.dt);
-            if (U.invM[k] > R(0)) {
-                const float3 g = gauss3(in.seed, U.atom[k], step);
-                const R ns = ic.noisescale*sqrt_r(ic.kT*U.invM[k]);
-                U.v[k] = U.v[k]*ic.vscale + V3<R>{g.x, g.y, g.z}*ns;
-            }
-            d[k] = d[k] + U.v[k]*(R(0.5)*ic.dt);
-            if (U.invM[k] == R(0)) d[k] = {R(0), R(0), R(0)};
-            du[k] = d[k];
+    // the group's old positions and masses for the solve (whole warps take part; a warp of free atoms skips it)
+    const bool solve = __any_sync(0xffffffffu, U.type != 0);
+    if (solve) {
+        _Pragma("unroll") for (int j = 0; j < 4; j++) {
+            U.x[j] = shfl_v3(x, g + j);
+            U.invM[j] = shfl_r(invM, g + j);
+            U.m[j] = shfl_r(m, g + j);
         }
-        constrain_pos(U, d, ic.tol);
-        _Pragma("unroll") for (int k = 0; k < 4; k++) if (k < U.n) U.v[k] = U.v[k] + (d[k] - du[k])*invDt;
+    }
+    V3<R> uw[4];
+    if (KIND == B200MD_INT_LANGEVIN_MIDDLE) {
+        if (own) v = v + f*(ic.dt*invM);
+        if (solve) {
+            _Pragma("unroll") for (int j = 0; j < 4; j++) uw[j] = shfl_v3(v, g + j);
+            constrain_vel(U, uw, ic.tol);
+            v = pick(uw, ka);
+        }
+        V3<R> du = d;
+        if (own) {
+            d = v*(R(0.5)*ic.dt);
+            if (invM > R(0)) {
+                const float3 gn = gauss3(in.seed, a, step);
+                const R ns = ic.noisescale*sqrt_r(ic.kT*invM);
+                v = v*ic.vscale + V3<R>{gn.x, gn.y, gn.z}*ns;
+            }
+            d = d + v*(R(0.5)*ic.dt);
+            if (invM == R(0)) d = {R(0), R(0), R(0)};
+            du = d;
+        }
+        if (solve) {
+            _Pragma("unroll") for (int j = 0; j < 4; j++) uw[j] = shfl_v3(d, g + j);
+            constrain_pos(U, uw, ic.tol);
+            d = pick(uw, ka);
+        }
+        if (own) v = v + (d - du)*invDt;
     }
     else {
-        _Pragma("unroll") for (int k = 0; k < 4; k++) if (k < U.n) {
+        if (own) {
             V3<R> vn;
             if (KIND == B200MD_INT_LANGEVIN) {
-                vn = U.v[k]*ic.vscale + U.f[k]*(ic.fscale*U.invM[k]);
-                if (U.invM[k] > R(0) && ic.noisescale > R(0)) {
-                    const float3 g = gauss3(in.seed, U.atom[k], step);
-                    vn = vn + V3<R>{g.x, g.y, g.z}*(ic.noisescale*sqrt_r(U.invM[k]));
+                vn = v*ic.vscale + f*(ic.fscale*invM);
+                if (invM > R(0) && ic.noisescale > R(0)) {
+                    const float3 gn = gauss3(in.seed, a, step);
+                    vn = vn + V3<R>{gn.x, gn.y, gn.z}*(ic.noisescale*sqrt_r(invM));
                 }
             }
             else
-                vn = U.v[k] + U.f[k]*(ic.dt*U.invM[k]);
-            if (U.invM[k] == R(0)) vn = U.v[k];
-            d[k] = (U.invM[k] == R(0)) ? V3<R>{R(0), R(0), R(0)} : vn*ic.dt;
+                vn = v + f*(ic.dt*invM);
+            if (invM == R(0)) vn = v;
+            d = (invM == R(0)) ? V3<R>{R(0), R(0), R(0)} : vn*ic.dt;
         }
-        constrain_pos(U, d, ic.tol);
-        _Pragma("unroll") for (int k = 0; k < 4; k++) if (k < U.n) if (U.invM[k] > R(0)) U.v[k] = d[k]*invDt;
+        if (solve) {
+            _Pragma("unroll") for (int j = 0; j < 4; j++) uw[j] = shfl_v3(d, g + j);
+            constrain_pos(U, uw, ic.tol);
+            d = pick(uw, ka);
+        }
+        if (own && invM > R(0)) v = d*invDt;
     }
-    _Pragma("unroll") for (int k = 0; k < 4; k++) if (k < U.n) {
-        const int a = U.atom[k];
-        store_pos<R>(nb, a, U.x[k].x + d[k].x, U.x[k].y + d[k].y, U.x[k].z + d[k].z);
-        vel_array<R>(nb)[a] = make_r4(U.v[k].x, U.v[k].y, U.v[k].z, U.invM[k]);
+    if (own) {
+        store_pos<R>(nb, a, x.x + d.x, x.y + d.y, x.z + d.z);
+        vel_array<R>(nb)[a] = make_r4(v.x, v.y, v.z, invM);
         if (multi && !cd.posByPush) {
             const float4 pn = nb.posq[a];
             for (int k = 1; k < cd.world; k++) {            // staggered: rank r starts with peer r+1, so the ranks do not all hit peer 0 first
@@ -311,24 +382,35 @@ __global__ void __launch_bounds__(128, sizeof(R) == 8 ? 1 : 0) k_integrate(NbDev
             }
         }
     }
-    }   // active
     if (!in.fused && !(multi && !cd.posByPush)) return;
     if (cmFused) {
-        double px = 0, py = 0, pz = 0, m = 0;
-        _Pragma("unroll") for (int k = 0; k < 4; k++) if (k < U.n && U.invM[k] > R(0)) {
-            const double mk = U.m[k];
-            px += mk*U.v[k].x; py += mk*U.v[k].y; pz += mk*U.v[k].z; m += mk;
+        // the block's momentum sum, grouped as one thread per unit grouped it: per unit in atom order, a 32-unit xor
+        // butterfly, then the sum of the 2 groups of 32 units
+        // (the same px += mk*v form as there, so the compiler contracts it the same way)
+        const bool mine = own && invM > R(0);
+        double px = 0, py = 0, pz = 0, pm = 0;
+        _Pragma("unroll") for (int j = 0; j < 4; j++) {
+            const int cj = __shfl_sync(0xffffffffu, (int) mine, g + j);
+            const double mk = shfl_r((double) m, g + j);
+            const V3<R> vj = shfl_v3(v, g + j);
+            if (cj) { px += mk*vj.x; py += mk*vj.y; pz += mk*vj.z; pm += mk; }
         }
-        for (int off = 16; off > 0; off >>= 1) {
-            px += __shfl_xor_sync(0xffffffffu, px, off); py += __shfl_xor_sync(0xffffffffu, py, off);
-            pz += __shfl_xor_sync(0xffffffffu, pz, off); m += __shfl_xor_sync(0xffffffffu, m, off);
+        __shared__ double unitP[INTEG_UNITS][4];
+        if (ka == 0) { unitP[ub][0] = px; unitP[ub][1] = py; unitP[ub][2] = pz; unitP[ub][3] = pm; }
+        __shared__ double red[INTEG_UNITS/32][4];
+        __syncthreads();
+        if (threadIdx.x < INTEG_UNITS) {
+            px = unitP[threadIdx.x][0]; py = unitP[threadIdx.x][1]; pz = unitP[threadIdx.x][2]; pm = unitP[threadIdx.x][3];
+            for (int off = 16; off > 0; off >>= 1) {
+                px += __shfl_xor_sync(0xffffffffu, px, off); py += __shfl_xor_sync(0xffffffffu, py, off);
+                pz += __shfl_xor_sync(0xffffffffu, pz, off); pm += __shfl_xor_sync(0xffffffffu, pm, off);
+            }
+            if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5][0] = px; red[threadIdx.x >> 5][1] = py; red[threadIdx.x >> 5][2] = pz; red[threadIdx.x >> 5][3] = pm; }
         }
-        __shared__ double red[4][4];
-        if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5][0] = px; red[threadIdx.x >> 5][1] = py; red[threadIdx.x >> 5][2] = pz; red[threadIdx.x >> 5][3] = m; }
         __syncthreads();
         if (threadIdx.x < 4) {
             double t = 0;
-            for (int w = 0; w < (int) (blockDim.x >> 5); w++) t += red[w][threadIdx.x];
+            for (int w = 0; w < INTEG_UNITS/32; w++) t += red[w][threadIdx.x];
             atomicAdd(&in.cmScratch[4*((step + 1ull) % 3ull) + threadIdx.x], t);
             if (blockIdx.x == 0) in.cmScratch[4*((step + 2ull) % 3ull) + threadIdx.x] = 0.0;
         }
@@ -407,14 +489,14 @@ void launch_cm_prime(const NbDev& nb, const IntegDev& integ, const CommDev& cd, 
 
 template <int KIND>
 static void launch_integrate_kind(int grid, const NbDev& nb, const UnitDev& units, const IntegDev& integ, const CommDev& cd, cudaStream_t s) {
-    if (nb.velmD) k_integrate<KIND, double><<<grid, 64, 0, s>>>(nb, units, integ, cd);
-    else k_integrate<KIND, float><<<grid, 64, 0, s>>>(nb, units, integ, cd);
+    if (nb.velmD) k_integrate<KIND, double><<<grid, INTEG_THREADS, 0, s>>>(nb, units, integ, cd);
+    else k_integrate<KIND, float><<<grid, INTEG_THREADS, 0, s>>>(nb, units, integ, cd);
 }
 
 void launch_integrate(const NbDev& nb, const UnitDev& units, const IntegDev& integ, const CommDev& cd, cudaStream_t s) {
-    // 64-thread blocks: at DHFR size (8k units) 128-thread blocks fill only 65 of the 132 SMs of an H100
+    // 64 units (256 threads) per block: DHFR's 8k units give 128 blocks of 8 warps, one per SM of an H100 (132)
     const int n = cd.world > 1 ? cd.unitLo[cd.rank + 1] - cd.unitLo[cd.rank] : units.nunits;
-    const int grid = std::max(1, (n + 63)/64);
+    const int grid = std::max(1, (n + INTEG_UNITS - 1)/INTEG_UNITS);
     if (integ.kind == B200MD_INT_VERLET) launch_integrate_kind<B200MD_INT_VERLET>(grid, nb, units, integ, cd, s);
     else if (integ.kind == B200MD_INT_LANGEVIN) launch_integrate_kind<B200MD_INT_LANGEVIN>(grid, nb, units, integ, cd, s);
     else launch_integrate_kind<B200MD_INT_LANGEVIN_MIDDLE>(grid, nb, units, integ, cd, s);

@@ -347,8 +347,8 @@ void pme_brick_setup(int maxSmem) {
     CUDA_CHECK(cudaFuncSetAttribute(k_pme_spread_brick, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem - (int) fa.sharedSizeBytes));
 }
 
-void launch_pme_spread(const NbDev& nb, const PmeDev& pme, const CommDev& cd, cudaStream_t s) {
-    cudaMemsetAsync(pme.gridFixed, 0, sizeof(long long)*(size_t) pme.nx*pme.ny*pme.nz, s);
+void launch_pme_spread(const NbDev& nb, const PmeDev& pme, const CommDev& cd, cudaStream_t s, bool zeroGrid) {
+    if (zeroGrid) cudaMemsetAsync(pme.gridFixed, 0, sizeof(long long)*(size_t) pme.nx*pme.ny*pme.nz, s);
     if (pme.brickAtoms > 0) {
         launch_high(k_pme_spread_brick, (nb.npad + pme.brickAtoms - 1)/pme.brickAtoms, 256, sizeof(long long)*pme.brickPoints, s, nb, pme);
         return;
