@@ -28,6 +28,41 @@ template <class T> struct DevBuf {
     ~DevBuf() { free(); }
 };
 
+static void require(bool cond, const char* msg) { if (!cond) throw std::runtime_error(msg); }
+
+// Every atom index of a packed term table lies in [0, natoms): every int component, the 0 that pads an angle's int4 included.
+template <class A> static void check_atoms(int natoms, const std::vector<A>& a, const char* cls) {
+    const int* q = (const int*) a.data();
+    for (size_t k = 0; k < a.size()*sizeof(A)/sizeof(int); k++)
+        if (q[k] < 0 || q[k] >= natoms) throw std::runtime_error(std::string(cls) + ": atom index out of range");
+}
+
+// One bonded term class in the layout BondedDev reads: n terms' atoms and parameters, each term's force group (none set =
+// group 0) and the device copies.  set_* fills it through set(), finalize uploads it, update_* rewrites `params` and uploads
+// them into the same buffers (same size: captured step graphs keep their pointers).
+template <class A, class P> struct TermTable {
+    int n = 0;
+    std::vector<A> atoms; std::vector<P> params; std::vector<unsigned char> group;
+    DevBuf<A> atomsDev; DevBuf<P> paramsDev; DevBuf<unsigned char> groupDev;
+    void set(int natoms, const char* cls, int count, std::vector<A>& a, std::vector<P>& p) {
+        check_atoms(natoms, a, cls);
+        n = count; atoms.swap(a); params.swap(p);
+    }
+    // finalize: upload, and point the BondedDev fields at the copies (groups may come before or after the terms)
+    void upload(int& count, const A*& a, const P*& p, const unsigned char*& g) {
+        require(group.empty() || (int) group.size() == n, "set_bonded_groups: group array length differs from the number of terms");
+        std::vector<unsigned char> gr(group); gr.resize(std::max(n, 1), 0);
+        atomsDev.upload(atoms); paramsDev.upload(params); groupDev.upload(gr);
+        count = n; a = atomsDev.p; p = paramsDev.p; g = groupDev.p;
+    }
+};
+// CMAP: two int4 (the two dihedrals) per term, params = the coefficients of every patch [sum size^2][16]; besides, the map
+// index of every term and per map (first patch, size)
+struct CmapTable : TermTable<int4, double> {
+    std::vector<int> map; std::vector<int2> maps;
+    DevBuf<int> mapDev; DevBuf<int2> mapsDev;
+};
+
 // ---- minimal NCCL binding, resolved at run time so that libb200md.so has no link-time NCCL dependency ----
 struct NcclUid { char b[128]; };      // ncclUniqueId is passed BY VALUE to ncclCommInitRank
 struct NcclApi {
@@ -78,13 +113,13 @@ struct b200md_ctx {
     std::vector<double> mass, charge, sigma, epsilon;
     b200md_nonbonded_desc nbdesc{};
     bool haveNb = false;
-    std::vector<int> excI, excJ; std::vector<double> excQQ, excSig, excEps;
-    std::vector<int> bondI, bondJ; std::vector<double> bondR0, bondK;
-    std::vector<int> angI, angJ, angK; std::vector<double> angT0, angKK;
-    std::vector<int> torI, torJ, torK, torL, torN; std::vector<double> torPhase, torKK;
-    std::vector<int> rbI, rbJ, rbK, rbL; std::vector<double> rbC;  // rbC [n][6]
-    std::vector<int> cmapSize, cmapMap, cmapAtoms; std::vector<double> cmapCoeff;   // cmapAtoms [n][8], cmapCoeff [sum size^2][16]
-    std::vector<unsigned char> bondGroup, angGroup, torGroup, rbGroup, cmapGroup;   // force group of every bonded element (default 0)
+    // exceptions keep (qq, sigma, eps) as given: the device double4 also holds the product of the charges (upload_params)
+    struct { std::vector<int2> atoms; std::vector<double3> params; DevBuf<int2> atomsDev; DevBuf<double4> paramsDev; } exc;
+    TermTable<int2, double2> bonds;         // (r0, k)
+    TermTable<int4, double2> angles;        // atoms (i, j, k, 0), (theta0, k)
+    TermTable<int4, double4> torsions;      // (k, phase, n, 0)
+    TermTable<int4, double> rb;             // [n][6] c0..c5
+    CmapTable cmap;
     std::vector<int> conI, conJ; std::vector<double> conD;
     int cmFreq = 0;
     std::vector<int4> hUnitAtoms;        // host copy of the integration units (ownership cuts of the multi-GPU data plane)
@@ -108,11 +143,7 @@ struct b200md_ctx {
     DevBuf<real2> cgrid;
     DevBuf<real2> tw[3];
     DevBuf<double> moduli[3];
-    DevBuf<int2> bondAtoms, excAtoms; DevBuf<double2> bondParams, angleParams;
-    DevBuf<int4> angleAtoms, torsionAtoms, unitAtoms; DevBuf<double4> torsionParams, excParams;
-    DevBuf<int> unitType; DevBuf<float4> unitParams;
-    DevBuf<unsigned char> bondGroupDev, angGroupDev, torGroupDev, rbGroupDev, cmapGroupDev;
-    DevBuf<int4> rbAtoms, cmapAtomsDev; DevBuf<double> rbParams, cmapCoeffDev; DevBuf<int> cmapMapDev; DevBuf<int2> cmapMapsDev;
+    DevBuf<int4> unitAtoms; DevBuf<int> unitType; DevBuf<float4> unitParams;
     // general constraint networks (CCMA, constraints.cu)
     std::vector<int> ccmaCons;           // indices into conI/conJ/conD
     DevBuf<int> ccCompCon, ccCompAtom, ccRowStart, ccCol, ccAtoms, ccAStart, ccACon;
@@ -169,7 +200,6 @@ struct b200md_ctx {
 #define API_BEGIN(ctx) if (!(ctx)) return -1; try { CUDA_CHECK(cudaSetDevice((ctx)->device));
 #define API_END(ctx) } catch (std::exception& e) { (ctx)->err = e.what(); return -1; } return 0;
 
-static void require(bool cond, const char* msg) { if (!cond) throw std::runtime_error(msg); }
 static void check_flags(b200md_ctx* c);
 static void sync_velocities(b200md_ctx* c);
 static void sync_positions(b200md_ctx* c);
@@ -256,71 +286,82 @@ extern "C" int b200md_set_nonbonded(b200md_ctx* ctx, const b200md_nonbonded_desc
     API_END(ctx)
 }
 
+// The topology: every set_* call below refuses a call after finalize and a negative count.  The bonded ones also refuse an
+// atom index outside [0, natoms) before they replace their term class's table, so no kernel and no host loop ever indexes
+// with an unchecked atom (constraints are checked by classify_units).
+static void check_set(const b200md_ctx* c, const char* call, int n) {
+    if (c->finalized) throw std::runtime_error(std::string(call) + " after finalize");
+    if (n < 0) throw std::runtime_error(std::string(call) + ": negative count");
+}
 extern "C" int b200md_set_exceptions(b200md_ctx* ctx, int n, const int* p1, const int* p2, const double* qq, const double* sig, const double* eps) {
     API_BEGIN(ctx)
-    require(!ctx->finalized, "set_exceptions after finalize");
-    ctx->excI.assign(p1, p1+n); ctx->excJ.assign(p2, p2+n);
-    ctx->excQQ.assign(qq, qq+n); ctx->excSig.assign(sig, sig+n); ctx->excEps.assign(eps, eps+n);
+    check_set(ctx, "set_exceptions", n);
+    std::vector<int2> a(n); std::vector<double3> p(n);
+    for (int i = 0; i < n; i++) { a[i] = make_int2(p1[i], p2[i]); p[i] = make_double3(qq[i], sig[i], eps[i]); }
+    check_atoms(ctx->natoms, a, "exception");
+    ctx->exc.atoms.swap(a); ctx->exc.params.swap(p);
     API_END(ctx)
 }
 extern "C" int b200md_set_bonds(b200md_ctx* ctx, int n, const int* p1, const int* p2, const double* len, const double* k) {
     API_BEGIN(ctx)
-    require(!ctx->finalized, "set_bonds after finalize");
-    ctx->bondI.assign(p1, p1+n); ctx->bondJ.assign(p2, p2+n); ctx->bondR0.assign(len, len+n); ctx->bondK.assign(k, k+n);
+    check_set(ctx, "set_bonds", n);
+    std::vector<int2> a(n); std::vector<double2> p(n);
+    for (int i = 0; i < n; i++) { a[i] = make_int2(p1[i], p2[i]); p[i] = make_double2(len[i], k[i]); }
+    ctx->bonds.set(ctx->natoms, "bond", n, a, p);
     API_END(ctx)
 }
-extern "C" int b200md_set_angles(b200md_ctx* ctx, int n, const int* p1, const int* p2, const int* p3, const double* a, const double* k) {
+extern "C" int b200md_set_angles(b200md_ctx* ctx, int n, const int* p1, const int* p2, const int* p3, const double* t0, const double* k) {
     API_BEGIN(ctx)
-    require(!ctx->finalized, "set_angles after finalize");
-    ctx->angI.assign(p1, p1+n); ctx->angJ.assign(p2, p2+n); ctx->angK.assign(p3, p3+n); ctx->angT0.assign(a, a+n); ctx->angKK.assign(k, k+n);
+    check_set(ctx, "set_angles", n);
+    std::vector<int4> a(n); std::vector<double2> p(n);
+    for (int i = 0; i < n; i++) { a[i] = make_int4(p1[i], p2[i], p3[i], 0); p[i] = make_double2(t0[i], k[i]); }
+    ctx->angles.set(ctx->natoms, "angle", n, a, p);
     API_END(ctx)
 }
 extern "C" int b200md_set_torsions(b200md_ctx* ctx, int n, const int* p1, const int* p2, const int* p3, const int* p4, const int* per, const double* ph, const double* k) {
     API_BEGIN(ctx)
-    require(!ctx->finalized, "set_torsions after finalize");
-    ctx->torI.assign(p1, p1+n); ctx->torJ.assign(p2, p2+n); ctx->torK.assign(p3, p3+n); ctx->torL.assign(p4, p4+n);
-    ctx->torN.assign(per, per+n); ctx->torPhase.assign(ph, ph+n); ctx->torKK.assign(k, k+n);
+    check_set(ctx, "set_torsions", n);
+    std::vector<int4> a(n); std::vector<double4> p(n);
+    for (int i = 0; i < n; i++) { a[i] = make_int4(p1[i], p2[i], p3[i], p4[i]); p[i] = make_double4(k[i], ph[i], (double) per[i], 0); }
+    ctx->torsions.set(ctx->natoms, "periodic torsion", n, a, p);
     API_END(ctx)
 }
 extern "C" int b200md_set_rb_torsions(b200md_ctx* ctx, int n, const int* p1, const int* p2, const int* p3, const int* p4, const double* c) {
     API_BEGIN(ctx)
-    require(!ctx->finalized, "set_rb_torsions after finalize");
-    require(n >= 0, "set_rb_torsions: negative count");
-    ctx->rbI.assign(p1, p1+n); ctx->rbJ.assign(p2, p2+n); ctx->rbK.assign(p3, p3+n); ctx->rbL.assign(p4, p4+n);
-    ctx->rbC.assign(c, c + 6*(size_t) n);
+    check_set(ctx, "set_rb_torsions", n);
+    std::vector<int4> a(n); std::vector<double> p(c, c + 6*(size_t) n);
+    for (int i = 0; i < n; i++) a[i] = make_int4(p1[i], p2[i], p3[i], p4[i]);
+    ctx->rb.set(ctx->natoms, "RB torsion", n, a, p);
     API_END(ctx)
-}
-// the number of coefficients of the maps: 16 per patch, size^2 patches per map
-static size_t cmap_coeff_count(int nmaps, const int* size) {
-    size_t total = 0;
-    for (int m = 0; m < nmaps; m++) {
-        require(size[m] > 0, "CMAP: the size of a map must be positive");
-        total += 16*(size_t) size[m]*size[m];
-    }
-    return total;
 }
 extern "C" int b200md_set_cmap(b200md_ctx* ctx, int nmaps, const int* size, const double* coeff, int n, const int* map, const int* atoms) {
     API_BEGIN(ctx)
-    require(!ctx->finalized, "set_cmap after finalize");
-    require(nmaps >= 0 && n >= 0, "set_cmap: negative count");
-    const size_t nc = cmap_coeff_count(nmaps, size);
-    ctx->cmapSize.assign(size, size + nmaps); ctx->cmapCoeff.assign(coeff, coeff + nc);
-    ctx->cmapMap.assign(map, map + n); ctx->cmapAtoms.assign(atoms, atoms + 8*(size_t) n);
+    check_set(ctx, "set_cmap", std::min(nmaps, n));
+    std::vector<int2> maps(nmaps); size_t patches = 0;      // per map (first patch, size); size^2 patches of 16 coefficients
+    for (int m = 0; m < nmaps; m++) {
+        require(size[m] > 0, "CMAP: the size of a map must be positive");
+        maps[m] = make_int2((int) patches, size[m]); patches += (size_t) size[m]*size[m];
+    }
+    for (int i = 0; i < n; i++) require(map[i] >= 0 && map[i] < nmaps, "CMAP torsion: map index out of range");
+    std::vector<int4> a(2*(size_t) n); std::vector<double> p(coeff, coeff + 16*patches);
+    for (size_t d = 0; d < a.size(); d++) a[d] = make_int4(atoms[4*d], atoms[4*d+1], atoms[4*d+2], atoms[4*d+3]);
+    ctx->cmap.set(ctx->natoms, "CMAP torsion", n, a, p);
+    ctx->cmap.map.assign(map, map + n); ctx->cmap.maps.swap(maps);
     API_END(ctx)
 }
 extern "C" int b200md_set_bonded_groups(b200md_ctx* ctx, int kind, int n, const int* group) {
     API_BEGIN(ctx)
-    require(!ctx->finalized, "set_bonded_groups after finalize");
+    check_set(ctx, "set_bonded_groups", n);
     require(kind >= 0 && kind <= 4, "set_bonded_groups: kind must be 0 (bonds), 1 (angles), 2 (torsions), 3 (RB torsions) or 4 (CMAP)");
-    std::vector<unsigned char>& g = kind == 0 ? ctx->bondGroup : kind == 1 ? ctx->angGroup : kind == 2 ? ctx->torGroup :
-                                    kind == 3 ? ctx->rbGroup : ctx->cmapGroup;
+    std::vector<unsigned char>& g = kind == 0 ? ctx->bonds.group : kind == 1 ? ctx->angles.group : kind == 2 ? ctx->torsions.group :
+                                    kind == 3 ? ctx->rb.group : ctx->cmap.group;
     g.resize(n);
     for (int i = 0; i < n; i++) { require(group[i] >= 0 && (group[i] & ~0x80) < 32, "force group out of range"); g[i] = (unsigned char) group[i]; }
     API_END(ctx)
 }
 extern "C" int b200md_set_constraints(b200md_ctx* ctx, int n, const int* p1, const int* p2, const double* d) {
     API_BEGIN(ctx)
-    require(!ctx->finalized, "set_constraints after finalize");
+    check_set(ctx, "set_constraints", n);
     ctx->conI.assign(p1, p1+n); ctx->conJ.assign(p2, p2+n); ctx->conD.assign(d, d+n);
     API_END(ctx)
 }
@@ -539,15 +580,14 @@ static void upload_params(b200md_ctx* c) {
     CUDA_CHECK(cudaMemcpy(p.data(), c->posq.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToHost));
     for (int i = 0; i < N; i++) p[i].w = (float) (c->charge[i]*sk);
     CUDA_CHECK(cudaMemcpy(c->posq.p, p.data(), sizeof(float4)*c->npad, cudaMemcpyHostToDevice));
-    const int ne = (int) c->excI.size();
-    std::vector<int2> ea(ne); std::vector<double4> ep(ne);
+    const int ne = (int) c->exc.atoms.size();
+    std::vector<double4> ep(ne);
     for (int e = 0; e < ne; e++) {
-        ea[e] = make_int2(c->excI[e], c->excJ[e]);
-        ep[e] = make_double4(B200MD_ONE_4PI_EPS0*c->excQQ[e], c->excSig[e], 4.0*c->excEps[e],
-                             B200MD_ONE_4PI_EPS0*c->charge[c->excI[e]]*c->charge[c->excJ[e]]);
+        const int2 a = c->exc.atoms[e]; const double3 p = c->exc.params[e];
+        ep[e] = make_double4(B200MD_ONE_4PI_EPS0*p.x, p.y, 4.0*p.z, B200MD_ONE_4PI_EPS0*c->charge[a.x]*c->charge[a.y]);
     }
-    c->excAtoms.upload(ea); c->excParams.upload(ep);
-    c->bd.nexc = ne; c->bd.excAtoms = c->excAtoms.p; c->bd.excParams = c->excParams.p;
+    c->exc.atomsDev.upload(c->exc.atoms); c->exc.paramsDev.upload(ep);
+    c->bd.nexc = ne; c->bd.excAtoms = c->exc.atomsDev.p; c->bd.excParams = c->exc.paramsDev.p;
     double self = 0;
     if (c->nbdesc.method == B200MD_NB_PME)
         for (int i = 0; i < N; i++) self -= B200MD_ONE_4PI_EPS0*c->charge[i]*c->charge[i]*c->nbdesc.ewald_alpha/std::sqrt(M_PI);
@@ -655,7 +695,7 @@ struct CcmaInput {
     int natoms;
     const std::vector<double>& mass;
     const std::vector<int>& ccmaCons; const std::vector<int>& conI; const std::vector<int>& conJ; const std::vector<double>& conD;
-    const std::vector<int>& angI; const std::vector<int>& angJ; const std::vector<int>& angK; const std::vector<double>& angT0;
+    const std::vector<int4>& angAtoms; const std::vector<double2>& angParams;     // the layout of b200md_ctx::angles
 };
 struct CcmaHost {
     int ncomp = 0;
@@ -699,7 +739,7 @@ static void ccma_host_setup(const CcmaInput* c, CcmaHost& H) {
     }
     // ---- coupling matrix ----
     std::vector<std::vector<int> > atomAngles(N);
-    for (size_t i = 0; i < c->angJ.size(); i++) atomAngles[c->angJ[i]].push_back((int) i);
+    for (size_t i = 0; i < c->angAtoms.size(); i++) atomAngles[c->angAtoms[i].y].push_back((int) i);
     std::vector<std::vector<std::pair<int, double> > > M(nc);
     auto consOf = [&](int a) { std::vector<int> v; for (int code : atomCons[a]) v.push_back(std::abs(code) - 1); return v; };
     for (int j = 0; j < nc; j++) {
@@ -727,8 +767,8 @@ static void ccma_host_setup(const CcmaInput* c, CcmaHost& H) {
                 }
             if (!found)
                 for (int cand : atomAngles[ab])
-                    if ((c->angI[cand] == aa && c->angK[cand] == ac) || (c->angK[cand] == aa && c->angI[cand] == ac)) {
-                        M[j].push_back(std::make_pair(k, scale*std::cos(c->angT0[cand])));
+                    if ((c->angAtoms[cand].x == aa && c->angAtoms[cand].z == ac) || (c->angAtoms[cand].z == aa && c->angAtoms[cand].x == ac)) {
+                        M[j].push_back(std::make_pair(k, scale*std::cos(c->angParams[cand].x)));
                         break;
                     }
         }
@@ -797,7 +837,7 @@ static void build_ccma(b200md_ctx* c) {
     c->ccma = CcmaDev{};
     if (nc == 0) return;
     require(!c->p2p && c->world == 1, "general (CCMA) constraint networks are not supported in multi-GPU runs");
-    const CcmaInput in{c->natoms, c->mass, c->ccmaCons, c->conI, c->conJ, c->conD, c->angI, c->angJ, c->angK, c->angT0};
+    const CcmaInput in{c->natoms, c->mass, c->ccmaCons, c->conI, c->conJ, c->conD, c->angles.atoms, c->angles.params};
     CcmaHost H;
     ccma_host_setup(&in, H);
     // ---- device ----
@@ -827,15 +867,16 @@ extern "C" int b200md_ccma_setup_probe(int natoms, const double* mass, int ncon,
                                        int nangles, const int* a1, const int* a2, const int* a3, const double* theta0,
                                        int* out_ncomp, int* out_nccma, int* out_order, int* row_start, int* col, float* val, int cap) {
     try {
-        std::vector<double> m(mass, mass + natoms), cd(dist, dist + ncon), t0(theta0, theta0 + nangles);
-        std::vector<int> ci(p1, p1 + ncon), cj(p2, p2 + ncon), ai(a1, a1 + nangles), aj(a2, a2 + nangles), ak(a3, a3 + nangles);
+        std::vector<double> m(mass, mass + natoms), cd(dist, dist + ncon);
+        std::vector<int> ci(p1, p1 + ncon), cj(p2, p2 + ncon); std::vector<int4> aa(nangles); std::vector<double2> ap(nangles);
+        for (int i = 0; i < nangles; i++) { aa[i] = make_int4(a1[i], a2[i], a3[i], 0); ap[i] = make_double2(theta0[i], 0.0); }
         std::vector<int4> ua; std::vector<int> ut; std::vector<float4> up; std::vector<int> ccmaCons;
         std::string err;
         if (!classify_units(natoms, m.data(), ci, cj, cd, ua, ut, up, err, &ccmaCons)) { g_create_error = err; return -1; }
         *out_nccma = (int) ccmaCons.size();
         *out_ncomp = 0;
         if (ccmaCons.empty()) { row_start[0] = 0; return 0; }
-        const CcmaInput in{natoms, m, ccmaCons, ci, cj, cd, ai, aj, ak, t0};
+        const CcmaInput in{natoms, m, ccmaCons, ci, cj, cd, aa, ap};
         CcmaHost H;
         ccma_host_setup(&in, H);
         *out_ncomp = H.ncomp;
@@ -1164,7 +1205,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     // ---- exclusions (every exception is an exclusion) ----
     {
         std::vector<std::vector<int> > ex(N);
-        for (size_t e = 0; e < c->excI.size(); e++) { ex[c->excI[e]].push_back(c->excJ[e]); ex[c->excJ[e]].push_back(c->excI[e]); }
+        for (const int2& a : c->exc.atoms) { ex[a.x].push_back(a.y); ex[a.y].push_back(a.x); }
         std::vector<int> start(N+1, 0), list;
         for (int i = 0; i < N; i++) {
             std::sort(ex[i].begin(), ex[i].end());
@@ -1178,57 +1219,16 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     }
     // ---- tile capacity: TILE_REGIONS equal slot pools, i-block ib allocates from pool ib % TILE_REGIONS (flush_tile) ----
     alloc_tile_pools(c, initial_pool_capacity(c));
-    // ---- bonded ----
-    {
-        const int nbnd = (int) c->bondI.size(), na = (int) c->angI.size(), nt = (int) c->torI.size();
-        std::vector<int2> ba(nbnd); std::vector<double2> bp(nbnd);
-        for (int i = 0; i < nbnd; i++) { ba[i] = make_int2(c->bondI[i], c->bondJ[i]); bp[i] = make_double2(c->bondR0[i], c->bondK[i]); }
-        std::vector<int4> aa(na); std::vector<double2> ap(na);
-        for (int i = 0; i < na; i++) { aa[i] = make_int4(c->angI[i], c->angJ[i], c->angK[i], 0); ap[i] = make_double2(c->angT0[i], c->angKK[i]); }
-        std::vector<int4> ta(nt); std::vector<double4> tp(nt);
-        for (int i = 0; i < nt; i++) { ta[i] = make_int4(c->torI[i], c->torJ[i], c->torK[i], c->torL[i]); tp[i] = make_double4(c->torKK[i], c->torPhase[i], (double) c->torN[i], 0); }
-        c->bondAtoms.upload(ba); c->bondParams.upload(bp); c->angleAtoms.upload(aa); c->angleParams.upload(ap);
-        c->torsionAtoms.upload(ta); c->torsionParams.upload(tp);
-        c->bd.nbonds = nbnd; c->bd.nangles = na; c->bd.ntorsions = nt;
-        c->bd.bondAtoms = c->bondAtoms.p; c->bd.bondParams = c->bondParams.p; c->bd.angleAtoms = c->angleAtoms.p; c->bd.angleParams = c->angleParams.p;
-        c->bd.torsionAtoms = c->torsionAtoms.p; c->bd.torsionParams = c->torsionParams.p;
-        c->bd.excPeriodic = c->nbdesc.exceptions_periodic;
-        require((c->bondGroup.empty() || (int) c->bondGroup.size() == nbnd) && (c->angGroup.empty() || (int) c->angGroup.size() == na) &&
-                (c->torGroup.empty() || (int) c->torGroup.size() == nt), "set_bonded_groups: group array length differs from the number of terms");
-        c->bondGroup.resize(std::max(nbnd, 1), 0); c->angGroup.resize(std::max(na, 1), 0); c->torGroup.resize(std::max(nt, 1), 0);
-        c->bondGroupDev.upload(c->bondGroup); c->angGroupDev.upload(c->angGroup); c->torGroupDev.upload(c->torGroup);
-        c->bd.bondGroup = c->bondGroupDev.p; c->bd.angleGroup = c->angGroupDev.p; c->bd.torsionGroup = c->torGroupDev.p;
-        c->bd.groupMask = 0xffffffffu;
-    }
-    // ---- Ryckaert-Bellemans torsions and CMAP terms ----
-    {
-        const int nr = (int) c->rbI.size(), ncm = (int) c->cmapMap.size(), nmaps = (int) c->cmapSize.size();
-        auto atom_ok = [&](int a) { return a >= 0 && a < N; };
-        std::vector<int4> ra(nr);
-        for (int i = 0; i < nr; i++) {
-            require(atom_ok(c->rbI[i]) && atom_ok(c->rbJ[i]) && atom_ok(c->rbK[i]) && atom_ok(c->rbL[i]), "RB torsion: atom index out of range");
-            ra[i] = make_int4(c->rbI[i], c->rbJ[i], c->rbK[i], c->rbL[i]);
-        }
-        require(c->cmapCoeff.size() == cmap_coeff_count(nmaps, c->cmapSize.data()), "CMAP: the number of coefficients differs from 16 x the number of patches");
-        std::vector<int2> maps(nmaps);
-        for (int m = 0, first = 0; m < nmaps; m++) { maps[m] = make_int2(first, c->cmapSize[m]); first += c->cmapSize[m]*c->cmapSize[m]; }
-        std::vector<int4> ca(2*(size_t) ncm);
-        for (int i = 0; i < ncm; i++) {
-            require(c->cmapMap[i] >= 0 && c->cmapMap[i] < nmaps, "CMAP torsion: map index out of range");
-            const int* a = &c->cmapAtoms[8*(size_t) i];
-            for (int k = 0; k < 8; k++) require(atom_ok(a[k]), "CMAP torsion: atom index out of range");
-            ca[2*i] = make_int4(a[0], a[1], a[2], a[3]); ca[2*i+1] = make_int4(a[4], a[5], a[6], a[7]);
-        }
-        require((c->rbGroup.empty() || (int) c->rbGroup.size() == nr) && (c->cmapGroup.empty() || (int) c->cmapGroup.size() == ncm),
-                "set_bonded_groups: group array length differs from the number of terms");
-        c->rbGroup.resize(std::max(nr, 1), 0); c->cmapGroup.resize(std::max(ncm, 1), 0);
-        c->rbAtoms.upload(ra); c->rbParams.upload(c->rbC); c->rbGroupDev.upload(c->rbGroup);
-        c->cmapAtomsDev.upload(ca); c->cmapMapDev.upload(c->cmapMap); c->cmapMapsDev.upload(maps); c->cmapCoeffDev.upload(c->cmapCoeff);
-        c->cmapGroupDev.upload(c->cmapGroup);
-        c->bd.nrb = nr; c->bd.rbAtoms = c->rbAtoms.p; c->bd.rbParams = c->rbParams.p; c->bd.rbGroup = c->rbGroupDev.p;
-        c->bd.ncmap = ncm; c->bd.cmapAtoms = c->cmapAtomsDev.p; c->bd.cmapMap = c->cmapMapDev.p; c->bd.cmapMaps = c->cmapMapsDev.p;
-        c->bd.cmapCoeff = c->cmapCoeffDev.p; c->bd.cmapGroup = c->cmapGroupDev.p;
-    }
+    // ---- bonded (exceptions: upload_params) ----
+    BondedDev& bd = c->bd;
+    c->bonds.upload(bd.nbonds, bd.bondAtoms, bd.bondParams, bd.bondGroup);
+    c->angles.upload(bd.nangles, bd.angleAtoms, bd.angleParams, bd.angleGroup);
+    c->torsions.upload(bd.ntorsions, bd.torsionAtoms, bd.torsionParams, bd.torsionGroup);
+    c->rb.upload(bd.nrb, bd.rbAtoms, bd.rbParams, bd.rbGroup);
+    c->cmap.upload(bd.ncmap, bd.cmapAtoms, bd.cmapCoeff, bd.cmapGroup);
+    c->cmap.mapDev.upload(c->cmap.map); c->cmap.mapsDev.upload(c->cmap.maps); bd.cmapMap = c->cmap.mapDev.p; bd.cmapMaps = c->cmap.mapsDev.p;
+    bd.excPeriodic = c->nbdesc.exceptions_periodic;
+    bd.groupMask = 0xffffffffu;
     upload_params(c);
     build_units(c);
     build_ccma(c);
@@ -1249,13 +1249,12 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
         for (int i = 0; i < N; i++) parent[i] = i;
         auto find = [&](int x) { while (parent[x] != x) { parent[x] = parent[parent[x]]; x = parent[x]; } return x; };
         auto join = [&](int a, int b) { a = find(a); b = find(b); if (a != b) parent[std::max(a, b)] = std::min(a, b); };
-        for (size_t i = 0; i < c->bondI.size(); i++) join(c->bondI[i], c->bondJ[i]);
-        for (size_t i = 0; i < c->angI.size(); i++) { join(c->angI[i], c->angJ[i]); join(c->angJ[i], c->angK[i]); }
-        for (size_t i = 0; i < c->torI.size(); i++) { join(c->torI[i], c->torJ[i]); join(c->torJ[i], c->torK[i]); join(c->torK[i], c->torL[i]); }
-        for (size_t i = 0; i < c->rbI.size(); i++) { join(c->rbI[i], c->rbJ[i]); join(c->rbJ[i], c->rbK[i]); join(c->rbK[i], c->rbL[i]); }
-        for (size_t i = 0; i < c->cmapAtoms.size(); i++) join(c->cmapAtoms[i - i%8], c->cmapAtoms[i]);
+        for (const int2& a : c->bonds.atoms) join(a.x, a.y);
+        for (const int4& a : c->angles.atoms) { join(a.x, a.y); join(a.y, a.z); }
+        for (auto* t : {&c->torsions.atoms, &c->rb.atoms, &c->cmap.atoms}) for (const int4& a : *t) { join(a.x, a.y); join(a.y, a.z); join(a.z, a.w); }
+        for (size_t d = 1; d < c->cmap.atoms.size(); d += 2) join(c->cmap.atoms[d-1].x, c->cmap.atoms[d].x);     // a CMAP term's two dihedrals
         for (size_t i = 0; i < c->conI.size(); i++) join(c->conI[i], c->conJ[i]);
-        for (size_t i = 0; i < c->excI.size(); i++) join(c->excI[i], c->excJ[i]);
+        for (const int2& a : c->exc.atoms) join(a.x, a.y);
         std::vector<int> molOf(N), count;
         std::map<int, int> id;
         for (int i = 0; i < N; i++) {
@@ -1284,9 +1283,9 @@ extern "C" int b200md_update_nonbonded_params(b200md_ctx* ctx, const double* q, 
                                               int nexc, const double* eqq, const double* esig, const double* eeps, double dispCoef) {
     API_BEGIN(ctx)
     require(ctx->finalized, "update params before finalize");
-    require(nexc == (int) ctx->excI.size(), "update_nonbonded_params: the number of exceptions cannot change");
+    require(nexc == (int) ctx->exc.atoms.size(), "update_nonbonded_params: the number of exceptions cannot change");
     ctx->charge.assign(q, q + ctx->natoms); ctx->sigma.assign(sig, sig + ctx->natoms); ctx->epsilon.assign(eps, eps + ctx->natoms);
-    if (nexc) { ctx->excQQ.assign(eqq, eqq+nexc); ctx->excSig.assign(esig, esig+nexc); ctx->excEps.assign(eeps, eeps+nexc); }
+    for (int e = 0; e < nexc; e++) ctx->exc.params[e] = make_double3(eqq[e], esig[e], eeps[e]);
     ctx->dispersionCoefficient = dispCoef;
     CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
     upload_params(ctx);
@@ -1303,19 +1302,19 @@ extern "C" int b200md_update_bonded_params(b200md_ctx* ctx, int kind, int n, con
     require(ctx->finalized, "update_bonded_params before finalize");
     CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
     if (kind == 0) {
-        require(n == ctx->bd.nbonds, "the number of bonds cannot change");
-        std::vector<double2> p(n); for (int i = 0; i < n; i++) p[i] = make_double2(a[i], b[i]);
-        ctx->bondParams.upload(p);
+        require(n == ctx->bonds.n, "the number of bonds cannot change");
+        for (int i = 0; i < n; i++) ctx->bonds.params[i] = make_double2(a[i], b[i]);
+        ctx->bonds.paramsDev.upload(ctx->bonds.params);
     }
     else if (kind == 1) {
-        require(n == ctx->bd.nangles, "the number of angles cannot change");
-        std::vector<double2> p(n); for (int i = 0; i < n; i++) p[i] = make_double2(a[i], b[i]);
-        ctx->angleParams.upload(p);
+        require(n == ctx->angles.n, "the number of angles cannot change");
+        for (int i = 0; i < n; i++) ctx->angles.params[i] = make_double2(a[i], b[i]);
+        ctx->angles.paramsDev.upload(ctx->angles.params);
     }
     else if (kind == 2) {
-        require(n == ctx->bd.ntorsions, "the number of torsions cannot change");
-        std::vector<double4> p(n); for (int i = 0; i < n; i++) p[i] = make_double4(b[i], a[i], (double) periodicity[i], 0);
-        ctx->torsionParams.upload(p);
+        require(n == ctx->torsions.n, "the number of torsions cannot change");
+        for (int i = 0; i < n; i++) ctx->torsions.params[i] = make_double4(b[i], a[i], (double) periodicity[i], 0);
+        ctx->torsions.paramsDev.upload(ctx->torsions.params);
     }
     else throw std::runtime_error("unknown bonded kind");
     API_END(ctx)
@@ -1326,23 +1325,23 @@ extern "C" int b200md_update_bonded_params(b200md_ctx* ctx, int kind, int n, con
 extern "C" int b200md_update_rb_torsion_params(b200md_ctx* ctx, int n, const double* c) {
     API_BEGIN(ctx)
     require(ctx->finalized, "update_rb_torsion_params before finalize");
-    require(n == ctx->bd.nrb, "updateParametersInContext: The number of torsions has changed");
+    require(n == ctx->rb.n, "updateParametersInContext: The number of torsions has changed");
     CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-    ctx->rbC.assign(c, c + 6*(size_t) n);
-    ctx->rbParams.upload(ctx->rbC);
+    ctx->rb.params.assign(c, c + 6*(size_t) n);
+    ctx->rb.paramsDev.upload(ctx->rb.params);
     API_END(ctx)
 }
 extern "C" int b200md_update_cmap_params(b200md_ctx* ctx, int nmaps, const int* size, const double* coeff, int n, const int* map) {
     API_BEGIN(ctx)
     require(ctx->finalized, "update_cmap_params before finalize");
-    require(nmaps == (int) ctx->cmapSize.size(), "updateParametersInContext: The number of maps has changed");
-    require(n == ctx->bd.ncmap, "updateParametersInContext: The number of CMAP torsions has changed");
-    for (int m = 0; m < nmaps; m++) require(size[m] == ctx->cmapSize[m], "updateParametersInContext: The size of a map has changed");
+    require(nmaps == (int) ctx->cmap.maps.size(), "updateParametersInContext: The number of maps has changed");
+    require(n == ctx->cmap.n, "updateParametersInContext: The number of CMAP torsions has changed");
+    for (int m = 0; m < nmaps; m++) require(size[m] == ctx->cmap.maps[m].y, "updateParametersInContext: The size of a map has changed");
     for (int i = 0; i < n; i++) require(map[i] >= 0 && map[i] < nmaps, "CMAP torsion: map index out of range");
     CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-    ctx->cmapCoeff.assign(coeff, coeff + ctx->cmapCoeff.size());
-    ctx->cmapMap.assign(map, map + n);
-    ctx->cmapCoeffDev.upload(ctx->cmapCoeff); ctx->cmapMapDev.upload(ctx->cmapMap);
+    ctx->cmap.params.assign(coeff, coeff + ctx->cmap.params.size());
+    ctx->cmap.map.assign(map, map + n);
+    ctx->cmap.paramsDev.upload(ctx->cmap.params); ctx->cmap.mapDev.upload(ctx->cmap.map);
     API_END(ctx)
 }
 
