@@ -130,8 +130,8 @@ struct b200md_ctx {
     // ---- device state ----
     DevBuf<float4> posq, velm, sposq[2], swrap[2], refPos, atomShift, blockCenter[2], blockHalf[2], superCenter[2], superHalf[2];
     DevBuf<float2> sigeps, ssigeps[2];
-    DevBuf<double> chargeD; DevBuf<double2> sigepsD;
-    DevBuf<long long> force;
+    DevBuf<double> chargeD, schargeD[2]; DevBuf<double2> sigepsD, ssigepsD[2];
+    DevBuf<long long> force, forceS;
     DevBuf<double> energy, cmScratch;
     DevBuf<int> molStart, molAtoms, cellOffset, sorig[2], sortedOf, cellRank, cellCount, cellFill, atomCell, tmpSorted, tileI[2], tileJ[2], tileMask[2], listCounters, counters, exclStart, exclList;
     DevBuf<unsigned int> maskPool[2];
@@ -1160,13 +1160,15 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     for (int l = 0; l < 2; l++) {
         c->sposq[l].alloc(NP); c->sposq[l].zero(); c->swrap[l].alloc(NP); c->swrap[l].zero(); c->ssigeps[l].alloc(NP); c->ssigeps[l].zero();
         c->sorig[l].alloc(NP); c->sorig[l].zero(); c->blockCenter[l].alloc(c->nblocks); c->blockHalf[l].alloc(c->nblocks);
+        c->schargeD[l].alloc(NP); c->schargeD[l].zero(); c->ssigepsD[l].alloc(NP); c->ssigepsD[l].zero();
         ListDev& L = c->nb.list[l];
         L.sposq = c->sposq[l].p; L.ssigeps = c->ssigeps[l].p; L.swrap = c->swrap[l].p; L.sorig = c->sorig[l].p;
+        L.schargeD = c->schargeD[l].p; L.ssigepsD = c->ssigepsD[l].p;
         c->superCenter[l].alloc((c->nblocks + 31)/32); c->superHalf[l].alloc((c->nblocks + 31)/32);
         L.superCenter = c->superCenter[l].p; L.superHalf = c->superHalf[l].p;
         L.blockCenter = c->blockCenter[l].p; L.blockHalf = c->blockHalf[l].p; L.lc = c->listCounters.p + LC_STRIDE*l;
     }
-    c->force.alloc((size_t) 3*NP); c->force.zero();
+    c->force.alloc((size_t) 3*NP); c->force.zero(); c->forceS.alloc((size_t) 3*NP); c->forceS.zero();
     c->energy.alloc(B200MD_NUM_ENERGY); c->energy.zero(); c->cmScratch.alloc(12); c->cmScratch.zero();
     c->blocksDone.alloc(1); c->blocksDone.zero();
     c->sortedOf.alloc(NP); c->atomCell.alloc(NP); c->tmpSorted.alloc(NP);
@@ -1182,7 +1184,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
         c->posqCorr.alloc(NP); c->posqCorr.zero(); c->velmD.upload(vd);
         nb.posqCorr = c->posqCorr.p; nb.velmD = c->velmD.p;
     }
-    nb.posq = c->posq.p; nb.velm = c->velm.p; nb.sigeps = c->sigeps.p; nb.force = c->force.p; nb.energy = c->energy.p;
+    nb.posq = c->posq.p; nb.velm = c->velm.p; nb.sigeps = c->sigeps.p; nb.force = c->force.p; nb.forceS = c->forceS.p; nb.energy = c->energy.p;
     nb.sortedOf = c->sortedOf.p;
     nb.refPos = c->refPos.p; nb.atomCell = c->atomCell.p; nb.tmpSorted = c->tmpSorted.p; nb.atomShift = c->atomShift.p;
     nb.counters = c->counters.p;
@@ -1649,7 +1651,7 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
         launch_bonded_terms(c->streamBonded);
         CUDA_CHECK(cudaEventRecord(c->evJoinBonded, c->streamBonded));
     }
-    if (direct) { launch_pair(c->nb, energy, s); launches++; }
+    if (direct) { launch_pair(c->nb, energy, s); launches += PAIR_LAUNCHES; }
     if (bonded && !forkBonded) launch_bonded_terms(s);
     // p2p: partial forces of the atoms this rank does not own -> the owners' inboxes.  Reciprocal space only ever touches the
     // atoms this rank OWNS (k_pme_gather), so when it runs on its own stream the push does not have to wait for it: it goes

@@ -71,6 +71,8 @@ struct FftPlanDev {      // 1-D mixed-radix Stockham plan for one grid dimension
 struct ListDev {
     float4* sposq;               // sorted positions (exact user coordinates, refreshed every step) + charge
     float2* ssigeps;
+    double* schargeD;            // sorted copies of NbDev::chargeD / sigepsD (the double-precision close-pair path)
+    double2* ssigepsD;
     float4* swrap;               // sorted positions wrapped into the anchored cell at the build (list build only)
     int* sorig;                  // sorted slot -> user atom (-1 for padding)
     float4* blockCenter;
@@ -112,6 +114,9 @@ struct NbDev {
     const double* chargeD;       // the same parameters in double (user order): the double-precision close-pair path
     const double2* sigepsD;
     long long* force;            // [3][npad] fixed point, user order
+    // [3][npad] fixed point, sorted order of the current list: the tile kernel accumulates here (a warp's atomics land on
+    // contiguous addresses), and k_fold_sorted, launched right behind it, adds it into `force` and zeroes it again
+    long long* forceS;
     double* energy;              // [B200MD_NUM_ENERGY] accumulators
     // sorted (nonbonded) copies, blocks and tiles: two complete lists.  counters[CT_CUR] names the one the tile kernel reads;
     // a rebuild always fills the other one and flips at the end of k_build_tiles
@@ -444,7 +449,8 @@ struct ScaleDev {
 void launch_check_displacement(const NbDev& nb, const CommDev& cd, cudaStream_t s);
 const int LIST_BUILD_LAUNCHES = 2;
 void launch_list_build(const NbDev& nb, cudaStream_t s);     // k_list_prep (grid barriers) + k_build_tiles, gated on counters[CT_REBUILD]
-void launch_pair(const NbDev& nb, bool energy, cudaStream_t s);
+const int PAIR_LAUNCHES = 2;
+void launch_pair(const NbDev& nb, bool energy, cudaStream_t s);        // k_pair + k_fold_sorted (sorted -> user-order forces)
 void pair_set_carveout(size_t fftSmem, size_t brickSmem);     // shared memory for a chain CTA beside the tile CTAs left on an SM
 void launch_count_pairs(const NbDev& nb, cudaStream_t s);
 int choose_pme_sms(int reserve, unsigned long long mask[4]);     // SM partition of the tile kernel (NbDev::pmeSmMask)

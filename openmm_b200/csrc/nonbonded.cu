@@ -14,7 +14,8 @@
 // A build is two launches, k_list_prep and k_build_tiles, that return at once unless counters[CT_REBUILD] is raised.
 // The tile kernel (k_pair) is fp32 with two exceptions that the parity against the Reference platform asked for: pairs closer
 // than NbDev::closeCut2 are queued per warp and evaluated in double from the exact coordinates (close_pair_double), and the
-// fp32 force sums are folded every 8 terms (the j atoms rotate in four octets): see the comments at pair_tiles.
+// fp32 force sums are folded every 8 terms (the j atoms rotate in four octets): see the comments at pair_tiles.  The tile
+// kernel's forces go to a sorted-order buffer (NbDev::forceS) that k_fold_sorted adds into the user-order one.
 #include "engine.h"
 #include "../../include/b200md.h"
 #include <algorithm>
@@ -210,12 +211,16 @@ __device__ __forceinline__ void finalize_slot(const NbDev& nb, const ListDev& L,
         L.swrap[s] = make_float4(p.x+sh.x, p.y+sh.y, p.z+sh.z, p.w);   // wrapped into the anchored cell: list build only
         L.sposq[s] = p;
         L.ssigeps[s] = nb.sigeps[a];
+        L.schargeD[s] = nb.chargeD[a];
+        L.ssigepsD[s] = nb.sigepsD[a];
         nb.refPos[a] = p;
         if (s == 0) L.lc[LC_MAXHALF] = 0;        // max block half extent, filled by the block-bounds phase
     }
     else {
         L.sorig[s] = -1;
         L.ssigeps[s] = make_float2(0, 0);
+        L.schargeD[s] = 0.0;
+        L.ssigepsD[s] = make_double2(0.0, 0.0);
         // position is filled by the block-bounds phase with a copy of a real atom of the same block
     }
 }
@@ -712,11 +717,10 @@ __device__ __forceinline__ float ewald_g(float w);
 template <bool ENERGY, int METHOD, bool SWITCH>
 __device__ __forceinline__ void close_pair_double(const NbDev& nb, const ListDev& L, int si, int sj, double& energyD) {
     const float4 a = L.sposq[si], b = L.sposq[sj];
-    const int ai = L.sorig[si], aj = L.sorig[sj];
-    // parameters in double from the user-order tables: the fp32 copies (q sqrt(k), sigma/2, 2 sqrt(eps)) carry a relative
-    // rounding of 6e-8 each, i.e. up to 7e-7 on the r^-12 term of a pair whose force is in the hundreds
-    const double qq = nb.chargeD[ai]*nb.chargeD[aj];
-    const double2 sa = nb.sigepsD[ai], sb = nb.sigepsD[aj];
+    // parameters in double (sorted copies of the user-order tables): the fp32 copies (q sqrt(k), sigma/2, 2 sqrt(eps)) carry
+    // a relative rounding of 6e-8 each, i.e. up to 7e-7 on the r^-12 term of a pair whose force is in the hundreds
+    const double qq = L.schargeD[si]*L.schargeD[sj];
+    const double2 sa = L.ssigepsD[si], sb = L.ssigepsD[sj];
     double dx = (double) b.x - (double) a.x, dy = (double) b.y - (double) a.y, dz = (double) b.z - (double) a.z;
     const BoxDev& bx = nb.box;
     if (bx.periodic) {
@@ -767,12 +771,12 @@ __device__ __forceinline__ void close_pair_double(const NbDev& nb, const ListDev
     dEdR += ljF;
     if (ENERGY) energyD += e + ljE;
     const long long fx = __double2ll_rn(dx*dEdR*B200MD_FORCE_SCALE), fy = __double2ll_rn(dy*dEdR*B200MD_FORCE_SCALE), fz = __double2ll_rn(dz*dEdR*B200MD_FORCE_SCALE);
-    atomicAdd((unsigned long long*) &nb.force[ai], (unsigned long long) (-fx));
-    atomicAdd((unsigned long long*) &nb.force[ai + nb.npad], (unsigned long long) (-fy));
-    atomicAdd((unsigned long long*) &nb.force[ai + 2*nb.npad], (unsigned long long) (-fz));
-    atomicAdd((unsigned long long*) &nb.force[aj], (unsigned long long) fx);
-    atomicAdd((unsigned long long*) &nb.force[aj + nb.npad], (unsigned long long) fy);
-    atomicAdd((unsigned long long*) &nb.force[aj + 2*nb.npad], (unsigned long long) fz);
+    atomicAdd((unsigned long long*) &nb.forceS[si], (unsigned long long) (-fx));
+    atomicAdd((unsigned long long*) &nb.forceS[si + nb.npad], (unsigned long long) (-fy));
+    atomicAdd((unsigned long long*) &nb.forceS[si + 2*nb.npad], (unsigned long long) (-fz));
+    atomicAdd((unsigned long long*) &nb.forceS[sj], (unsigned long long) fx);
+    atomicAdd((unsigned long long*) &nb.forceS[sj + nb.npad], (unsigned long long) fy);
+    atomicAdd((unsigned long long*) &nb.forceS[sj + 2*nb.npad], (unsigned long long) fz);
 }
 
 template <bool ENERGY, int METHOD, bool SHIFT, bool SWITCH, bool CLOSE>
@@ -932,18 +936,18 @@ __device__ __forceinline__ void pair_tiles(const NbDev& nb, const ListDev& L, fl
             }
             __syncwarp();
         }
-        // after 4 x 8 rotations every lane holds its own j again
-        const int ai = L.sorig[si];
-        if (ai >= 0) {
-            atomicAdd((unsigned long long*) &nb.force[ai], (unsigned long long) float_to_fixed(fiTx));
-            atomicAdd((unsigned long long*) &nb.force[ai + nb.npad], (unsigned long long) float_to_fixed(fiTy));
-            atomicAdd((unsigned long long*) &nb.force[ai + 2*nb.npad], (unsigned long long) float_to_fixed(fiTz));
+        // after 4 x 8 rotations every lane holds its own j again.  The totals go to the SORTED-order buffer: the warp's 32
+        // i-atoms are one contiguous run per component and the j-atoms of a tile ascend, so the atomics of a warp land on
+        // a few L2 lines instead of 32 scattered ones (k_fold_sorted moves them to user order once per evaluation)
+        if (si < nb.natoms) {
+            atomicAdd((unsigned long long*) &nb.forceS[si], (unsigned long long) float_to_fixed(fiTx));
+            atomicAdd((unsigned long long*) &nb.forceS[si + nb.npad], (unsigned long long) float_to_fixed(fiTy));
+            atomicAdd((unsigned long long*) &nb.forceS[si + 2*nb.npad], (unsigned long long) float_to_fixed(fiTz));
         }
         if (jidx >= 0) {
-            const int aj = L.sorig[jidx];
-            atomicAdd((unsigned long long*) &nb.force[aj], (unsigned long long) float_to_fixed(fjTx));
-            atomicAdd((unsigned long long*) &nb.force[aj + nb.npad], (unsigned long long) float_to_fixed(fjTy));
-            atomicAdd((unsigned long long*) &nb.force[aj + 2*nb.npad], (unsigned long long) float_to_fixed(fjTz));
+            atomicAdd((unsigned long long*) &nb.forceS[jidx], (unsigned long long) float_to_fixed(fjTx));
+            atomicAdd((unsigned long long*) &nb.forceS[jidx + nb.npad], (unsigned long long) float_to_fixed(fjTy));
+            atomicAdd((unsigned long long*) &nb.forceS[jidx + 2*nb.npad], (unsigned long long) float_to_fixed(fjTz));
         }
     }
     if (ENERGY && CLOSE && energyD != 0.0) atomicAdd(&nb.energy[EN_NB], energyD);
@@ -1070,8 +1074,25 @@ int choose_pme_sms(int reserve, unsigned long long mask[4]) {
     return taken;
 }
 
+// The tile kernel's forces, sorted order -> user order: one thread per sorted slot of the list k_pair read.  Atomic, because
+// the gather and the bonded terms may be adding to `force` on other streams; forceS is left zeroed for the next evaluation.
+__global__ void __launch_bounds__(256) k_fold_sorted(NbDev nb) {
+    const int s = blockIdx.x*blockDim.x + threadIdx.x;
+    if (s >= nb.natoms) return;
+    const ListDev& L = nb.list[nb.counters[CT_CUR] & 1];
+    const int a = L.sorig[s];
+    for (int c = 0; c < 3; c++) {
+        const long long v = nb.forceS[s + c*nb.npad];
+        if (v != 0) {
+            atomicAdd((unsigned long long*) &nb.force[a + c*nb.npad], (unsigned long long) v);
+            nb.forceS[s + c*nb.npad] = 0;
+        }
+    }
+}
+
 void launch_pair(const NbDev& nb, bool energy, cudaStream_t s) {
     if (energy) launch_pair_m<true>(nb, s); else launch_pair_m<false>(nb, s);
+    k_fold_sorted<<<(nb.natoms + 255)/256, 256, 0, s>>>(nb);
 }
 
 // diagnostic: number of pairs inside the true cutoff that the list evaluates (tile efficiency accounting)
