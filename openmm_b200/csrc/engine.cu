@@ -30,6 +30,24 @@ template <class T> struct DevBuf {
 
 static void require(bool cond, const char* msg) { if (!cond) throw std::runtime_error(msg); }
 
+// A device-side copy of some of the context's arrays (`parts`), packed into one buffer.
+struct DevSpan { void* p; size_t bytes; };
+struct Snapshot {
+    std::vector<DevSpan> parts;
+    DevBuf<char> buf;
+    void save(cudaStream_t s) {
+        size_t total = 0;
+        for (const DevSpan& q : parts) total += q.bytes;
+        if (buf.n != total) buf.alloc(total);
+        char* d = buf.p;
+        for (const DevSpan& q : parts) { CUDA_CHECK(cudaMemcpyAsync(d, q.p, q.bytes, cudaMemcpyDeviceToDevice, s)); d += q.bytes; }
+    }
+    void restore(cudaStream_t s) const {
+        const char* d = buf.p;
+        for (const DevSpan& q : parts) { CUDA_CHECK(cudaMemcpyAsync(q.p, d, q.bytes, cudaMemcpyDeviceToDevice, s)); d += q.bytes; }
+    }
+};
+
 // Every atom index of a packed term table lies in [0, natoms): every int component, the 0 that pads an angle's int4 included.
 template <class A> static void check_atoms(int natoms, const std::vector<A>& a, const char* cls) {
     const int* q = (const int*) a.data();
@@ -61,6 +79,28 @@ template <class A, class P> struct TermTable {
 struct CmapTable : TermTable<int4, double> {
     std::vector<int> map; std::vector<int2> maps;
     DevBuf<int> mapDev; DevBuf<int2> mapsDev;
+};
+
+// The buffers of one neighbour list (ListDev): the sorted copies and the block boxes, sized by the atoms; the tile pools,
+// sized by the tile capacity and grown by prepare_list.
+struct ListBufs {
+    DevBuf<float4> sposq, swrap, blockCenter, blockHalf, superCenter, superHalf;
+    DevBuf<float2> ssigeps; DevBuf<double> schargeD; DevBuf<double2> ssigepsD;
+    DevBuf<int> sorig, tileI, tileJ, tileMask; DevBuf<unsigned int> maskPool;
+    void alloc(int npad, int nblocks) {
+        sposq.alloc(npad); sposq.zero(); swrap.alloc(npad); swrap.zero(); ssigeps.alloc(npad); ssigeps.zero();
+        sorig.alloc(npad); sorig.zero(); blockCenter.alloc(nblocks); blockHalf.alloc(nblocks);
+        schargeD.alloc(npad); schargeD.zero(); ssigepsD.alloc(npad); ssigepsD.zero();
+        superCenter.alloc((nblocks + 31)/32); superHalf.alloc((nblocks + 31)/32);
+    }
+    void alloc_tiles(int maxTiles) {
+        tileI.alloc(maxTiles); tileJ.alloc((size_t) maxTiles*32); tileMask.alloc(maxTiles); maskPool.alloc((size_t) maxTiles*32);
+    }
+    void bind(ListDev& L, int* lc) const {
+        L.sposq = sposq.p; L.ssigeps = ssigeps.p; L.schargeD = schargeD.p; L.ssigepsD = ssigepsD.p; L.swrap = swrap.p; L.sorig = sorig.p;
+        L.blockCenter = blockCenter.p; L.blockHalf = blockHalf.p; L.superCenter = superCenter.p; L.superHalf = superHalf.p;
+        L.tileI = tileI.p; L.tileJ = tileJ.p; L.tileMask = tileMask.p; L.maskPool = maskPool.p; L.lc = lc;
+    }
 };
 
 // ---- minimal NCCL binding, resolved at run time so that libb200md.so has no link-time NCCL dependency ----
@@ -128,13 +168,13 @@ struct b200md_ctx {
     bool haveOrigin = false;
     double padFrac = 0.10;
     // ---- device state ----
-    DevBuf<float4> posq, velm, sposq[2], swrap[2], refPos, atomShift, blockCenter[2], blockHalf[2], superCenter[2], superHalf[2];
-    DevBuf<float2> sigeps, ssigeps[2];
-    DevBuf<double> chargeD, schargeD[2]; DevBuf<double2> sigepsD, ssigepsD[2];
+    DevBuf<float4> posq, velm, refPos, atomShift;
+    DevBuf<float2> sigeps;
+    DevBuf<double> chargeD; DevBuf<double2> sigepsD;
+    ListBufs lists[2];
     DevBuf<long long> force, forceS;
     DevBuf<double> energy, cmScratch;
-    DevBuf<int> molStart, molAtoms, cellOffset, sorig[2], sortedOf, cellRank, cellCount, cellFill, atomCell, tmpSorted, tileI[2], tileJ[2], tileMask[2], listCounters, counters, exclStart, exclList;
-    DevBuf<unsigned int> maskPool[2];
+    DevBuf<int> molStart, molAtoms, cellOffset, sortedOf, cellRank, cellCount, cellFill, atomCell, tmpSorted, listCounters, counters, exclStart, exclList;
     DevBuf<unsigned long long> stepCounter;
     DevBuf<unsigned int> blocksDone;
     bool stepStateValid = false;         // fused step path: force buffer zeroed and cm accumulator primed
@@ -171,8 +211,7 @@ struct b200md_ctx {
     // ---- Monte Carlo barostat (b200md_scale_coordinates / b200md_restore_coordinates) ----
     DevBuf<int> baroStart, baroAtoms;    // molecules of ContextImpl::getMolecules(), CSR
     int baroNmol = 0;
-    DevBuf<float4> savePosq, savePosqCorr; DevBuf<int> saveCellOffset; DevBuf<long long> saveForce;     // state before the last scale
-    bool haveSaved = false;
+    Snapshot baroSave;                   // positions, cellOffset and forces before the last scale (no parts: no scale yet)
     // ---- graph ----
     cudaGraphExec_t stepGraph = nullptr;      // one MD step
     cudaGraphExec_t multiGraph = nullptr;     // graphSteps MD steps in one launch (host launch cost amortised)
@@ -444,6 +483,13 @@ static void setup_cells(b200md_ctx* c) {
 // (capture_steps), so a box change every few steps -- a barostat -- does not instantiate graphs.
 static void invalidate_graph(b200md_ctx* c) { c->graphValid = false; c->multiValid = false; }
 
+static void set_counter(b200md_ctx* c, int index, int value) {
+    CUDA_CHECK(cudaMemcpyAsync(&c->counters.p[index], &value, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+}
+// The state was changed from outside: the next evaluation rebuilds the list, synchronously and before any step graph
+// (prepare_list), which then trusts it.
+static void request_rebuild(b200md_ctx* c) { set_counter(c, CT_REBUILD, 1); c->listDirty = true; }
+
 static void apply_box(b200md_ctx* c) {
     BoxDev& b = c->nb.box;
     const int m = c->nbdesc.method;
@@ -475,8 +521,7 @@ static void apply_box(b200md_ctx* c) {
     if (c->finalized) {
         setup_cells(c);
         if (m == B200MD_NB_PME) { launch_pme_eterm(c->nb, c->pme, c->stream); c->kernelLaunches++; }
-        const int one = 1;
-        CUDA_CHECK(cudaMemcpyAsync(&c->counters.p[CT_REBUILD], &one, sizeof(int), cudaMemcpyHostToDevice, c->stream)); c->listDirty = true;
+        request_rebuild(c);
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
         invalidate_graph(c);
     }
@@ -495,15 +540,40 @@ extern "C" int b200md_get_box(b200md_ctx* ctx, double a[3], double b[3], double 
     return 0;
 }
 
+// ---------------------------------------------------------------- the per-atom dynamic state
+enum { ST_POS = 1, ST_VEL = 2, ST_CELL = 4, ST_ALL = 7 };
+// The context's state arrays for its precision, in checkpoint order: posq | posqCorr (mixed) | velm (single) or velmD
+// (mixed) | cellOffset.  `what` selects the positions, the velocities and cellOffset.
+static std::vector<DevSpan> state_spans(const b200md_ctx* c, int what = ST_ALL) {
+    const size_t NP = c->npad;
+    std::vector<DevSpan> s;
+    if (what & ST_POS) {
+        s.push_back({c->posq.p, sizeof(float4)*NP});
+        if (c->mixed()) s.push_back({c->posqCorr.p, sizeof(float4)*NP});
+    }
+    if (what & ST_VEL) s.push_back(c->mixed() ? DevSpan{c->velmD.p, sizeof(double4)*NP} : DevSpan{c->velm.p, sizeof(float4)*NP});
+    if (what & ST_CELL) s.push_back({c->cellOffset.p, sizeof(int)*3*NP});
+    return s;
+}
+
+// Velocities v (nullptr: zero) with 1/mass in w (0 for a massless atom), into velm (V = float4) or velmD (V = double4).
+template <class V> static void upload_velocities(b200md_ctx* c, V* dst, const double* v) {
+    typedef decltype(V::x) E;
+    const double none[3] = {0, 0, 0};
+    std::vector<V> h(c->npad, V{});
+    for (int i = 0; i < c->natoms; i++) {
+        const double* u = v ? v + 3*i : none;
+        h[i] = V{(E) u[0], (E) u[1], (E) u[2], c->mass[i] > 0 ? (E) (1.0/c->mass[i]) : (E) 0};
+    }
+    CUDA_CHECK(cudaMemcpyAsync(dst, h.data(), sizeof(V)*c->npad, cudaMemcpyHostToDevice, c->stream));
+    CUDA_CHECK(cudaStreamSynchronize(c->stream));
+}
+
 // ---------------------------------------------------------------- Monte Carlo barostat
 // ApplyMonteCarloBarostatKernel (kernels.h:1425-1459).  The host half (MonteCarloBarostatImpl: random volume change, the two
 // energy evaluations, acceptance, adaptive step) stays the reference's own; these three calls are the platform's part.
 static void require_single_rank(const b200md_ctx* c, const char* what) {
     if (c->world > 1) throw std::runtime_error(std::string(what) + ": the Monte Carlo barostat is not supported in multi-GPU runs");
-}
-static void mark_list_dirty(b200md_ctx* c) {
-    const int one = 1;
-    CUDA_CHECK(cudaMemcpyAsync(&c->counters.p[CT_REBUILD], &one, sizeof(int), cudaMemcpyHostToDevice, c->stream)); c->listDirty = true;
 }
 
 extern "C" int b200md_set_barostat_molecules(b200md_ctx* ctx, int nmol, const int* start, const int* atoms) {
@@ -525,16 +595,10 @@ extern "C" int b200md_scale_coordinates(b200md_ctx* ctx, double sx, double sy, d
     require_single_rank(c, "scale_coordinates");
     require(c->finalized && c->haveBox, "scale_coordinates before finalize / set_box");
     require(c->baroStart.n > 0, "scale_coordinates before set_barostat_molecules");
-    const int NP = c->npad;
-    c->savePosq.alloc(NP); c->saveCellOffset.alloc((size_t) 3*NP); c->saveForce.alloc((size_t) 3*NP);
-    CUDA_CHECK(cudaMemcpyAsync(c->savePosq.p, c->posq.p, sizeof(float4)*NP, cudaMemcpyDeviceToDevice, c->stream));
-    CUDA_CHECK(cudaMemcpyAsync(c->saveCellOffset.p, c->cellOffset.p, sizeof(int)*3*NP, cudaMemcpyDeviceToDevice, c->stream));
-    CUDA_CHECK(cudaMemcpyAsync(c->saveForce.p, c->force.p, sizeof(long long)*3*NP, cudaMemcpyDeviceToDevice, c->stream));
-    if (c->mixed()) {
-        c->savePosqCorr.alloc(NP);
-        CUDA_CHECK(cudaMemcpyAsync(c->savePosqCorr.p, c->posqCorr.p, sizeof(float4)*NP, cudaMemcpyDeviceToDevice, c->stream));
-    }
-    c->haveSaved = true;
+    // the velocities are not saved: the move does not touch them
+    c->baroSave.parts = state_spans(c, ST_POS | ST_CELL);
+    c->baroSave.parts.push_back({c->force.p, sizeof(long long)*3*c->npad});
+    c->baroSave.save(c->stream);
     ScaleDev sc{};
     sc.nmol = c->baroNmol; sc.molStart = c->baroStart.p; sc.molAtoms = c->baroAtoms.p;
     for (int k = 0; k < 3; k++) { sc.a[k] = c->boxA[k]; sc.b[k] = c->boxB[k]; sc.c[k] = c->boxC[k]; }
@@ -542,7 +606,7 @@ extern "C" int b200md_scale_coordinates(b200md_ctx* ctx, double sx, double sy, d
     launch_scale_molecules(c->nb, sc, c->stream);
     c->kernelLaunches++;
     CUDA_CHECK(cudaGetLastError());
-    mark_list_dirty(c);
+    request_rebuild(c);
     c->stepStateValid = false;
     API_END(ctx)
 }
@@ -551,13 +615,9 @@ extern "C" int b200md_restore_coordinates(b200md_ctx* ctx) {
     API_BEGIN(ctx)
     b200md_ctx* c = ctx;
     require_single_rank(c, "restore_coordinates");
-    require(c->haveSaved, "restore_coordinates without a preceding scale_coordinates");
-    const int NP = c->npad;
-    CUDA_CHECK(cudaMemcpyAsync(c->posq.p, c->savePosq.p, sizeof(float4)*NP, cudaMemcpyDeviceToDevice, c->stream));
-    CUDA_CHECK(cudaMemcpyAsync(c->cellOffset.p, c->saveCellOffset.p, sizeof(int)*3*NP, cudaMemcpyDeviceToDevice, c->stream));
-    CUDA_CHECK(cudaMemcpyAsync(c->force.p, c->saveForce.p, sizeof(long long)*3*NP, cudaMemcpyDeviceToDevice, c->stream));
-    if (c->mixed()) CUDA_CHECK(cudaMemcpyAsync(c->posqCorr.p, c->savePosqCorr.p, sizeof(float4)*NP, cudaMemcpyDeviceToDevice, c->stream));
-    mark_list_dirty(c);
+    require(!c->baroSave.parts.empty(), "restore_coordinates without a preceding scale_coordinates");
+    c->baroSave.restore(c->stream);
+    request_rebuild(c);
     c->stepStateValid = false;            // the force buffer holds forces again, not the zeros the fused step expects
     API_END(ctx)
 }
@@ -1106,11 +1166,7 @@ static int worst_pool_capacity(const b200md_ctx* c) {
 static void alloc_tile_pools(b200md_ctx* c, int poolCap) {
     NbDev& nb = c->nb;
     nb.maxTiles = poolCap*TILE_REGIONS;
-    for (int l = 0; l < 2; l++) {
-        c->tileI[l].alloc(nb.maxTiles); c->tileJ[l].alloc((size_t) nb.maxTiles*32); c->tileMask[l].alloc(nb.maxTiles); c->maskPool[l].alloc((size_t) nb.maxTiles*32);
-        ListDev& L = nb.list[l];
-        L.tileI = c->tileI[l].p; L.tileJ = c->tileJ[l].p; L.tileMask = c->tileMask[l].p; L.maskPool = c->maskPool[l].p;
-    }
+    for (int l = 0; l < 2; l++) { c->lists[l].alloc_tiles(nb.maxTiles); c->lists[l].bind(nb.list[l], c->listCounters.p + LC_STRIDE*l); }
 }
 
 // The reciprocal-space chain runs beside a tile kernel that holds every SM: one GPU, two streams, no SM partition.  Its FFT
@@ -1154,34 +1210,20 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
         }
     }
     // ---- state arrays ----
-    c->posq.alloc(NP); c->posq.zero(); c->velm.alloc(NP); c->velm.zero();
+    c->posq.alloc(NP); c->posq.zero(); c->velm.alloc(NP);
     c->refPos.alloc(NP); c->refPos.zero(); c->atomShift.alloc(NP); c->sigeps.alloc(NP);
     c->listCounters.alloc(2*LC_STRIDE); c->listCounters.zero();
-    for (int l = 0; l < 2; l++) {
-        c->sposq[l].alloc(NP); c->sposq[l].zero(); c->swrap[l].alloc(NP); c->swrap[l].zero(); c->ssigeps[l].alloc(NP); c->ssigeps[l].zero();
-        c->sorig[l].alloc(NP); c->sorig[l].zero(); c->blockCenter[l].alloc(c->nblocks); c->blockHalf[l].alloc(c->nblocks);
-        c->schargeD[l].alloc(NP); c->schargeD[l].zero(); c->ssigepsD[l].alloc(NP); c->ssigepsD[l].zero();
-        ListDev& L = c->nb.list[l];
-        L.sposq = c->sposq[l].p; L.ssigeps = c->ssigeps[l].p; L.swrap = c->swrap[l].p; L.sorig = c->sorig[l].p;
-        L.schargeD = c->schargeD[l].p; L.ssigepsD = c->ssigepsD[l].p;
-        c->superCenter[l].alloc((c->nblocks + 31)/32); c->superHalf[l].alloc((c->nblocks + 31)/32);
-        L.superCenter = c->superCenter[l].p; L.superHalf = c->superHalf[l].p;
-        L.blockCenter = c->blockCenter[l].p; L.blockHalf = c->blockHalf[l].p; L.lc = c->listCounters.p + LC_STRIDE*l;
-    }
+    for (int l = 0; l < 2; l++) c->lists[l].alloc(NP, c->nblocks);      // bound to nb.list[l] with the tile pools (alloc_tile_pools)
     c->force.alloc((size_t) 3*NP); c->force.zero(); c->forceS.alloc((size_t) 3*NP); c->forceS.zero();
     c->energy.alloc(B200MD_NUM_ENERGY); c->energy.zero(); c->cmScratch.alloc(12); c->cmScratch.zero();
     c->blocksDone.alloc(1); c->blocksDone.zero();
     c->sortedOf.alloc(NP); c->atomCell.alloc(NP); c->tmpSorted.alloc(NP);
     c->counters.alloc(16); c->counters.zero();
     c->stepCounter.alloc(1); c->stepCounter.zero();
-    std::vector<float4> vm(NP, make_float4(0, 0, 0, 0));
-    for (int i = 0; i < N; i++) vm[i].w = (c->mass[i] > 0) ? (float) (1.0/c->mass[i]) : 0.f;
-    c->velm.upload(vm);
+    upload_velocities(c, c->velm.p, nullptr);        // in a mixed context too: nothing reads it there, but nothing is left uninitialised
     nb.posqCorr = nullptr; nb.velmD = nullptr;
     if (c->mixed()) {
-        std::vector<double4> vd(NP, make_double4(0, 0, 0, 0));
-        for (int i = 0; i < N; i++) vd[i].w = (c->mass[i] > 0) ? 1.0/c->mass[i] : 0.0;
-        c->posqCorr.alloc(NP); c->posqCorr.zero(); c->velmD.upload(vd);
+        c->posqCorr.alloc(NP); c->posqCorr.zero(); c->velmD.alloc(NP); upload_velocities(c, c->velmD.p, nullptr);
         nb.posqCorr = c->posqCorr.p; nb.velmD = c->velmD.p;
     }
     nb.posq = c->posq.p; nb.velm = c->velm.p; nb.sigeps = c->sigeps.p; nb.force = c->force.p; nb.forceS = c->forceS.p; nb.energy = c->energy.p;
@@ -1291,8 +1333,7 @@ extern "C" int b200md_update_nonbonded_params(b200md_ctx* ctx, const double* q, 
     ctx->dispersionCoefficient = dispCoef;
     CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
     upload_params(ctx);
-    const int one = 1;
-    CUDA_CHECK(cudaMemcpy(&ctx->counters.p[CT_REBUILD], &one, sizeof(int), cudaMemcpyHostToDevice)); ctx->listDirty = true;   // sorted copies of the parameters
+    request_rebuild(ctx);         // the list holds sorted copies of the parameters
     invalidate_graph(ctx);
     API_END(ctx)
 }
@@ -1393,8 +1434,7 @@ extern "C" int b200md_set_positions(b200md_ctx* ctx, const double* x) {
     }
     host_set_state(ctx);
     CUDA_CHECK(cudaMemsetAsync(ctx->cellOffset.p, 0, sizeof(int)*3*ctx->npad, ctx->stream));
-    const int one = 1;
-    CUDA_CHECK(cudaMemcpyAsync(&ctx->counters.p[CT_REBUILD], &one, sizeof(int), cudaMemcpyHostToDevice, ctx->stream)); ctx->listDirty = true;
+    request_rebuild(ctx);
     CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
     API_END(ctx)
 }
@@ -1434,19 +1474,9 @@ extern "C" int b200md_set_velocities(b200md_ctx* ctx, const double* v) {
     API_BEGIN(ctx)
     ctx->stepStateValid = false;
     require(ctx->finalized, "set_velocities before finalize");
-    ctx->hbuf4.resize(ctx->npad);
-    for (int i = 0; i < ctx->npad; i++) ctx->hbuf4[i] = make_float4(0, 0, 0, 0);
-    for (int i = 0; i < ctx->natoms; i++)
-        ctx->hbuf4[i] = make_float4((float) v[3*i], (float) v[3*i+1], (float) v[3*i+2], ctx->mass[i] > 0 ? (float) (1.0/ctx->mass[i]) : 0.f);
-    std::vector<double4> vd;
-    if (ctx->mixed()) {
-        vd.assign(ctx->npad, make_double4(0, 0, 0, 0));
-        for (int i = 0; i < ctx->natoms; i++) vd[i] = make_double4(v[3*i], v[3*i+1], v[3*i+2], ctx->mass[i] > 0 ? 1.0/ctx->mass[i] : 0.0);
-        CUDA_CHECK(cudaMemcpyAsync(ctx->velmD.p, vd.data(), sizeof(double4)*ctx->npad, cudaMemcpyHostToDevice, ctx->stream));
-    }
-    else CUDA_CHECK(cudaMemcpyAsync(ctx->velm.p, ctx->hbuf4.data(), sizeof(float4)*ctx->npad, cudaMemcpyHostToDevice, ctx->stream));
+    if (ctx->mixed()) upload_velocities(ctx, ctx->velmD.p, v);
+    else upload_velocities(ctx, ctx->velm.p, v);
     ctx->velStale = false;
-    CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
     API_END(ctx)
 }
 extern "C" int b200md_get_velocities(b200md_ctx* ctx, double* v) {
@@ -1488,14 +1518,14 @@ extern "C" int b200md_synchronize(b200md_ctx* ctx) {
 }
 
 // ---------------------------------------------------------------- checkpoint
-// Version 2 (single precision): header | posq | velm | cellOffset.  Version 3 (mixed precision): header | posq | posqCorr |
-// velmD | cellOffset.  cellOffset stays last in both.  A blob is only loaded into a context of its own precision.
+// Header, then state_spans: version 2 (single precision) posq | velm | cellOffset, version 3 (mixed precision) posq | posqCorr
+// | velmD | cellOffset.  cellOffset stays last in both.  A blob is only loaded into a context of its own precision.
 struct CkptHeader { char magic[8]; int version; int natoms; double time; int64_t stepCount; double box[9]; unsigned long long rngStep; };
 static int ckpt_version(const b200md_ctx* c) { return c->mixed() ? 3 : 2; }
 static int64_t ckpt_bytes(const b200md_ctx* c) {
-    const int64_t NP = c->npad;
-    const int64_t state = c->mixed() ? 2*sizeof(float4)*NP + sizeof(double4)*NP : 2*sizeof(float4)*NP;
-    return sizeof(CkptHeader) + state + 3*sizeof(int)*NP;
+    int64_t n = sizeof(CkptHeader);
+    for (const DevSpan& s : state_spans(c)) n += s.bytes;
+    return n;
 }
 extern "C" int64_t b200md_checkpoint_save(b200md_ctx* ctx, void* buf, int64_t cap) {
     if (!ctx) return -1;
@@ -1512,13 +1542,7 @@ extern "C" int64_t b200md_checkpoint_save(b200md_ctx* ctx, void* buf, int64_t ca
         CUDA_CHECK(cudaMemcpy(&h.rngStep, ctx->stepCounter.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
         char* p = (char*) buf;
         memcpy(p, &h, sizeof(h)); p += sizeof(h);
-        CUDA_CHECK(cudaMemcpy(p, ctx->posq.p, sizeof(float4)*ctx->npad, cudaMemcpyDeviceToHost)); p += sizeof(float4)*ctx->npad;
-        if (ctx->mixed()) {
-            CUDA_CHECK(cudaMemcpy(p, ctx->posqCorr.p, sizeof(float4)*ctx->npad, cudaMemcpyDeviceToHost)); p += sizeof(float4)*ctx->npad;
-            CUDA_CHECK(cudaMemcpy(p, ctx->velmD.p, sizeof(double4)*ctx->npad, cudaMemcpyDeviceToHost)); p += sizeof(double4)*ctx->npad;
-        }
-        else { CUDA_CHECK(cudaMemcpy(p, ctx->velm.p, sizeof(float4)*ctx->npad, cudaMemcpyDeviceToHost)); p += sizeof(float4)*ctx->npad; }
-        CUDA_CHECK(cudaMemcpy(p, ctx->cellOffset.p, sizeof(int)*3*ctx->npad, cudaMemcpyDeviceToHost));
+        for (const DevSpan& s : state_spans(ctx)) { CUDA_CHECK(cudaMemcpy(p, s.p, s.bytes, cudaMemcpyDeviceToHost)); p += s.bytes; }
         return need;
     } catch (std::exception& e) { ctx->err = e.what(); return -1; }
 }
@@ -1537,18 +1561,11 @@ extern "C" int b200md_checkpoint_load(b200md_ctx* ctx, const void* buf, int64_t 
     ctx->time = h.time; ctx->stepCount = h.stepCount;
     for (int i = 0; i < 3; i++) { ctx->boxA[i] = h.box[i]; ctx->boxB[i] = h.box[3+i]; ctx->boxC[i] = h.box[6+i]; }
     const char* p = (const char*) buf + sizeof(h);
-    CUDA_CHECK(cudaMemcpy(ctx->posq.p, p, sizeof(float4)*ctx->npad, cudaMemcpyHostToDevice)); p += sizeof(float4)*ctx->npad;
-    if (ctx->mixed()) {
-        CUDA_CHECK(cudaMemcpy(ctx->posqCorr.p, p, sizeof(float4)*ctx->npad, cudaMemcpyHostToDevice)); p += sizeof(float4)*ctx->npad;
-        CUDA_CHECK(cudaMemcpy(ctx->velmD.p, p, sizeof(double4)*ctx->npad, cudaMemcpyHostToDevice)); p += sizeof(double4)*ctx->npad;
-    }
-    else { CUDA_CHECK(cudaMemcpy(ctx->velm.p, p, sizeof(float4)*ctx->npad, cudaMemcpyHostToDevice)); p += sizeof(float4)*ctx->npad; }
-    CUDA_CHECK(cudaMemcpy(ctx->cellOffset.p, p, sizeof(int)*3*ctx->npad, cudaMemcpyHostToDevice));
+    for (const DevSpan& s : state_spans(ctx)) { CUDA_CHECK(cudaMemcpy(s.p, p, s.bytes, cudaMemcpyHostToDevice)); p += s.bytes; }
     CUDA_CHECK(cudaMemcpy(ctx->stepCounter.p, &h.rngStep, sizeof(unsigned long long), cudaMemcpyHostToDevice));
     host_set_state(ctx); ctx->velStale = false;
     if (ctx->haveBox) apply_box(ctx);
-    const int one = 1;
-    CUDA_CHECK(cudaMemcpy(&ctx->counters.p[CT_REBUILD], &one, sizeof(int), cudaMemcpyHostToDevice)); ctx->listDirty = true;
+    request_rebuild(ctx);
     API_END(ctx)
 }
 
@@ -1679,22 +1696,33 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     return launches;
 }
 
+// The device flags (NbDev::counters) and, if read, the lists' counters, once the stream has finished its work.
+struct DevFlags {
+    int ct[16], lc[2*LC_STRIDE];
+    const int* cur() const { return lc + LC_STRIDE*(ct[CT_CUR] & 1); }       // the current list's counters
+};
+static DevFlags read_flags(b200md_ctx* c, bool lists) {
+    DevFlags f;
+    CUDA_CHECK(cudaMemcpyAsync(f.ct, c->counters.p, sizeof(f.ct), cudaMemcpyDeviceToHost, c->stream));
+    if (lists) CUDA_CHECK(cudaMemcpyAsync(f.lc, c->listCounters.p, sizeof(f.lc), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_CHECK(cudaStreamSynchronize(c->stream));
+    return f;
+}
+// CT_OVERFLOW codes 2 and 3: a device-side wait gave up
+static void raise_timeouts(const DevFlags& f) {
+    if (f.ct[CT_OVERFLOW] == 2) throw std::runtime_error("B200 platform: neighbour-list construction timed out at a grid barrier (k_list_prep)");
+    if (f.ct[CT_OVERFLOW] == 3) throw std::runtime_error("B200 platform: multi-GPU exchange timed out waiting for a peer rank (every rank must issue the same sequence of calls)");
+}
+
 // Sticky device flags are read at EVERY point where the host synchronises with the stream anyway (energy reads, state
 // reads, b200md_synchronize), so a problem inside a run of b200md_step calls surfaces at the next state read instead of
 // silently dropping pair interactions.
 static void check_flags(b200md_ctx* c) {
     if (!c->finalized) return;
-    int h[8];
-    CUDA_CHECK(cudaMemcpyAsync(h, c->counters.p, sizeof(int)*8, cudaMemcpyDeviceToHost, c->stream));
-    CUDA_CHECK(cudaStreamSynchronize(c->stream));
-    if (h[CT_OVERFLOW] == 2) throw std::runtime_error("B200 platform: neighbour-list construction timed out at a grid barrier (k_list_prep)");
-    if (h[CT_OVERFLOW] == 3) throw std::runtime_error("B200 platform: multi-GPU exchange timed out waiting for a peer rank (every rank must issue the same sequence of calls)");
-    if (h[CT_OVERFLOW]) throw std::runtime_error("B200 platform: neighbour-list tile capacity exceeded (" + std::to_string(c->nb.maxTiles) + " tiles) during the preceding steps; the trajectory since the last state read is invalid");
+    const DevFlags f = read_flags(c, false);
+    raise_timeouts(f);
+    if (f.ct[CT_OVERFLOW]) throw std::runtime_error("B200 platform: neighbour-list tile capacity exceeded (" + std::to_string(c->nb.maxTiles) + " tiles) during the preceding steps; the trajectory since the last state read is invalid");
 }
-
-static bool role_split(const b200md_ctx* c);
-static NbDev role_nb(const b200md_ctx* c);
-static void invalidate_graph(b200md_ctx* c);
 
 // After the state was changed from outside (positions, box, parameters, checkpoint): build the list now, synchronously,
 // and size the tile pools from what the build actually used.  The step graphs trust the current list and never grow it.
@@ -1706,17 +1734,12 @@ static void prepare_list(b200md_ctx* c) {
         launch_check_displacement(nb, c->cd, c->stream);
         launch_list_build(nb, c->stream);
         c->kernelLaunches += 1 + LIST_BUILD_LAUNCHES;
-        int h[16], lc[2*LC_STRIDE];
-        CUDA_CHECK(cudaMemcpyAsync(h, c->counters.p, sizeof(int)*16, cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK(cudaMemcpyAsync(lc, c->listCounters.p, sizeof(lc), cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
-        if (h[CT_OVERFLOW] == 2) throw std::runtime_error("B200 platform: neighbour-list construction timed out at a grid barrier (k_list_prep)");
-        if (h[CT_OVERFLOW] == 3) throw std::runtime_error("B200 platform: multi-GPU exchange timed out waiting for a peer rank (every rank must issue the same sequence of calls)");
-        const int* cur = lc + LC_STRIDE*(h[CT_CUR] & 1);
+        const DevFlags f = read_flags(c, true);
+        raise_timeouts(f);
         int worst = 0;
-        for (int r = 0; r < TILE_REGIONS; r++) worst = std::max(worst, cur[LC_TILES + r]);
+        for (int r = 0; r < TILE_REGIONS; r++) worst = std::max(worst, f.cur()[LC_TILES + r]);
         const int cap = c->nb.maxTiles/TILE_REGIONS;
-        const bool overflow = h[CT_OVERFLOW] != 0;
+        const bool overflow = f.ct[CT_OVERFLOW] != 0;
         if (!overflow && worst <= (int) (0.8*cap)) { c->listDirty = false; c->listBuilt = true; return; }
         // grow: the counters keep counting past the capacity (flush_tile), so `worst` is the demand even after an overflow
         const int want = std::min(worst_pool_capacity(c), std::max(2*cap, (int) (1.5*worst) + 64));
@@ -1725,9 +1748,7 @@ static void prepare_list(b200md_ctx* c) {
             c->listDirty = false; c->listBuilt = true; return;
         }
         alloc_tile_pools(c, want);
-        const int zero = 0, one = 1;
-        CUDA_CHECK(cudaMemcpy(&c->counters.p[CT_OVERFLOW], &zero, sizeof(int), cudaMemcpyHostToDevice));
-        CUDA_CHECK(cudaMemcpy(&c->counters.p[CT_REBUILD], &one, sizeof(int), cudaMemcpyHostToDevice));
+        set_counter(c, CT_OVERFLOW, 0); set_counter(c, CT_REBUILD, 1);
         invalidate_graph(c);
     }
     throw std::runtime_error("B200 platform: neighbour-list tile pools did not converge");
@@ -1999,14 +2020,10 @@ extern "C" int b200md_get_stats(b200md_ctx* ctx, b200md_stats* out) {
     out->natoms = ctx->natoms; out->padded_atoms = ctx->npad; out->num_blocks = ctx->nblocks;
     if (ctx->finalized) {
         launch_count_pairs(ctx->nb, ctx->stream);
-        int h[16], lc[2*LC_STRIDE];
-        CUDA_CHECK(cudaMemcpyAsync(h, ctx->counters.p, sizeof(int)*16, cudaMemcpyDeviceToHost, ctx->stream));
-        CUDA_CHECK(cudaMemcpyAsync(lc, ctx->listCounters.p, sizeof(lc), cudaMemcpyDeviceToHost, ctx->stream));
-        CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-        const int* cur = lc + LC_STRIDE*(h[CT_CUR] & 1);
+        const DevFlags f = read_flags(ctx, true);
         int masks = 0;
-        for (int r = 0; r < TILE_REGIONS; r++) masks += cur[LC_MASKS + r];
-        out->num_tiles = cur[LC_USED]; out->num_mask_tiles = masks; out->overflow = h[CT_OVERFLOW]; out->list_builds = h[CT_BUILDS]; out->pairs_in_cutoff = h[CT_PAIRS];
+        for (int r = 0; r < TILE_REGIONS; r++) masks += f.cur()[LC_MASKS + r];
+        out->num_tiles = f.cur()[LC_USED]; out->num_mask_tiles = masks; out->overflow = f.ct[CT_OVERFLOW]; out->list_builds = f.ct[CT_BUILDS]; out->pairs_in_cutoff = f.ct[CT_PAIRS];
     }
     out->force_evals = ctx->forceEvals; out->kernel_launches = ctx->kernelLaunches; out->graph_instantiations = ctx->graphInstantiations;
     out->pme_grid[0] = ctx->pme.nx; out->pme_grid[1] = ctx->pme.ny; out->pme_grid[2] = ctx->pme.nz; out->ewald_alpha = ctx->pme.alpha;
@@ -2024,34 +2041,18 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
     CommDev local{}; local.world = 1;   // phases are timed rank-locally (no peer traffic, no waits)
     cudaEvent_t e0, e1;
     CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
-    const int one = 1;
     double total = 0;
-    // the integrate phase mutates the state: snapshot it and restore it after every repetition
-    DevBuf<float4> savePos, saveVel, saveCorr; DevBuf<double4> saveVelD; unsigned long long saveStep = 0;
-    auto restoreState = [&]() {
-        CUDA_CHECK(cudaMemcpyAsync(c->posq.p, savePos.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
-        CUDA_CHECK(cudaMemcpyAsync(c->velm.p, saveVel.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
-        if (c->mixed()) {
-            CUDA_CHECK(cudaMemcpyAsync(c->posqCorr.p, saveCorr.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
-            CUDA_CHECK(cudaMemcpyAsync(c->velmD.p, saveVelD.p, sizeof(double4)*c->npad, cudaMemcpyDeviceToDevice, s));
-        }
-    };
+    // the integrate phase mutates the state: positions and velocities are restored before every repetition, the step
+    // counter (which each repetition advances, as a step does) once at the end
+    Snapshot state, counter;
     if (phase == 4) {
         require(c->haveIntegrator, "time_phase(integrate) before set_integrator");
-        savePos.alloc(c->npad); saveVel.alloc(c->npad);
-        CUDA_CHECK(cudaMemcpyAsync(savePos.p, c->posq.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
-        CUDA_CHECK(cudaMemcpyAsync(saveVel.p, c->velm.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
-        if (c->mixed()) {
-            saveCorr.alloc(c->npad); saveVelD.alloc(c->npad);
-            CUDA_CHECK(cudaMemcpyAsync(saveCorr.p, c->posqCorr.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToDevice, s));
-            CUDA_CHECK(cudaMemcpyAsync(saveVelD.p, c->velmD.p, sizeof(double4)*c->npad, cudaMemcpyDeviceToDevice, s));
-        }
-        CUDA_CHECK(cudaMemcpyAsync(&saveStep, c->stepCounter.p, sizeof(saveStep), cudaMemcpyDeviceToHost, s));
-        CUDA_CHECK(cudaStreamSynchronize(s));
+        state.parts = state_spans(c, ST_POS | ST_VEL); state.save(s);
+        counter.parts = {{c->stepCounter.p, sizeof(unsigned long long)}}; counter.save(s);
     }
     for (int r = -2; r < reps; r++) {
-        if (phase == 4) restoreState();
-        if (phase == 5) CUDA_CHECK(cudaMemcpyAsync(&c->counters.p[CT_REBUILD], &one, sizeof(int), cudaMemcpyHostToDevice, s));
+        if (phase == 4) state.restore(s);
+        if (phase == 5) set_counter(c, CT_REBUILD, 1);     // the list is not marked dirty: the next step adds no synchronous rebuild
         if (phase == 0) { CUDA_CHECK(cudaMemsetAsync(&c->counters.p[CT_CURSOR], 0, sizeof(int), s)); CUDA_CHECK(cudaMemsetAsync(&c->counters.p[CT_PAIRSTART], 0, sizeof(int), s)); }      // the SM-partitioned tile kernel's cursor starts from tile 0
         CUDA_CHECK(cudaEventRecord(e0, s));
         switch (phase) {
@@ -2070,8 +2071,7 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
         if (r >= 0) total += ms;
     }
     if (phase == 4) {
-        restoreState();
-        CUDA_CHECK(cudaMemcpyAsync(c->stepCounter.p, &saveStep, sizeof(saveStep), cudaMemcpyHostToDevice, s));
+        state.restore(s); counter.restore(s);
         CUDA_CHECK(cudaStreamSynchronize(s));
     }
     cudaEventDestroy(e0); cudaEventDestroy(e1);
