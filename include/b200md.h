@@ -40,7 +40,30 @@ typedef struct b200md_ctx b200md_ctx;
 #define B200MD_TERM_NB_RECIP   16   /* includeReciprocal */
 #define B200MD_TERM_RB_TORSIONS 32
 #define B200MD_TERM_CMAP       64
-#define B200MD_TERM_ALL        127
+#define B200MD_TERM_CUSTOM_TORSIONS 128
+#define B200MD_TERM_ALL        255
+
+/* ---- instructions of a custom-torsion expression program (b200md_set_custom_torsions) ----
+ * One instruction = (opcode, operand index, double immediate).  A program is the flat stack program of a Lepton
+ * ExpressionProgram (lepton/ExpressionProgram.h), one instruction per Lepton::Operation, in the same order and with the same
+ * argument order: an operation of k arguments reads them from the top of the stack, argument 0 being the value pushed LAST,
+ * and replaces them with its result (ExpressionProgram::evaluate).  Each opcode computes exactly what the Operation of the
+ * same name computes.  THETA pushes the dihedral in (-pi, pi], PARAM k the term's k-th parameter, GLOBAL s the context's
+ * global value in slot s; CONST, ADD_CONST, MUL_CONST and POW_CONST take their constant from the immediate. */
+enum {
+    B200MD_OP_CONST = 0, B200MD_OP_THETA, B200MD_OP_PARAM, B200MD_OP_GLOBAL,
+    B200MD_OP_ADD, B200MD_OP_SUB, B200MD_OP_MUL, B200MD_OP_DIV, B200MD_OP_POW, B200MD_OP_NEG, B200MD_OP_SQRT, B200MD_OP_EXP,
+    B200MD_OP_LOG, B200MD_OP_SIN, B200MD_OP_COS, B200MD_OP_SEC, B200MD_OP_CSC, B200MD_OP_TAN, B200MD_OP_COT, B200MD_OP_ASIN,
+    B200MD_OP_ACOS, B200MD_OP_ATAN, B200MD_OP_ATAN2, B200MD_OP_SINH, B200MD_OP_COSH, B200MD_OP_TANH, B200MD_OP_ERF,
+    B200MD_OP_ERFC, B200MD_OP_STEP, B200MD_OP_DELTA, B200MD_OP_SQUARE, B200MD_OP_CUBE, B200MD_OP_RECIP, B200MD_OP_ADD_CONST,
+    B200MD_OP_MUL_CONST, B200MD_OP_POW_CONST, B200MD_OP_MIN, B200MD_OP_MAX, B200MD_OP_ABS, B200MD_OP_FLOOR, B200MD_OP_CEIL,
+    B200MD_OP_SELECT,
+    B200MD_OP_COUNT
+};
+/* hard limits of a custom-torsion program: stack depth, instructions per program, parameters per term */
+#define B200MD_CUSTOM_MAX_STACK  16
+#define B200MD_CUSTOM_MAX_CODE   256
+#define B200MD_CUSTOM_MAX_PARAMS 16
 
 /* ---- integrators (kernels.h:1033-1060 Verlet, :1160-1188 Langevin, :1192-1220 LangevinMiddle) ---- */
 #define B200MD_INT_VERLET          0
@@ -91,10 +114,22 @@ int b200md_set_rb_torsions(b200md_ctx* ctx, int n, const int* p1, const int* p2,
  * spline coefficients of CMAPTorsionForceImpl::calcMapDerivatives, maps one after the other, [size^2 patches][16] each;
  * n terms, term i uses map[i] and the two dihedrals atoms[i][0..3] and atoms[i][4..7].                                */
 int b200md_set_cmap(b200md_ctx* ctx, int nmaps, const int* size, const double* coeff, int n, const int* map, const int* atoms);
+/* CalcCustomTorsionForceKernel::initialize (kernels.h:521): nprog expressions as instruction programs (B200MD_OP_*), program
+ * 2p the energy of expression p and program 2p+1 its derivative dE/dtheta; program q is the instructions
+ * [prog_start[q], prog_start[q+1]) of op / arg / imm (prog_start has 2*nprog+1 entries).  n terms: term i evaluates
+ * expression prog[i] on the dihedral atoms[4i..4i+3] with the parameters params[i*param_stride ..].  Every program is
+ * checked here (opcodes, operand indices, the stack simulated on the host); GLOBAL operands are checked against the number
+ * of global values at finalize.  Single GPU only.                                                                        */
+int b200md_set_custom_torsions(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                               int param_stride, int n, const int* prog, const int* atoms, const double* params);
+/* The global parameter values the GLOBAL instructions read (slot s = values[s]).  Before finalize it sets the number of
+ * slots; after it, a stream-ordered copy of n == that number of values into the same device buffer, so a captured step
+ * graph keeps running with the new values and is never instantiated again.                                               */
+int b200md_set_custom_globals(b200md_ctx* ctx, int n, const double* values);
 /* Force group (Force::getForceGroup, openmmapi/include/openmm/Force.h) of every bonded term, so that
  * several Force objects of one class may live in different groups (ContextImpl::calcForcesAndEnergy,
  * ContextImpl.cpp:293-308; tests/TestLocalEnergyMinimizer.h:234 testForceGroups).  kind 0 bonds, 1 angles, 2 torsions,
- * 3 Ryckaert-Bellemans torsions, 4 CMAP terms; default group 0.  group[i] | 0x80 marks a term of a Force with usesPeriodicBoundaryConditions(): its
+ * 3 Ryckaert-Bellemans torsions, 4 CMAP terms, 5 custom torsions; default group 0.  group[i] | 0x80 marks a term of a Force with usesPeriodicBoundaryConditions(): its
  * difference vectors take the minimum image (ReferenceForce::getDeltaRPeriodic, ReferenceForce.cpp:90-101).          */
 int b200md_set_bonded_groups(b200md_ctx* ctx, int kind, int n, const int* group);
 /* System::getConstraintParameters; supported topologies: 3-atom rigid molecules (SETTLE,
@@ -140,6 +175,15 @@ int b200md_update_rb_torsion_params(b200md_ctx* ctx, int n, const double* c);
 /* CalcCMAPTorsionForceKernel::copyParametersToContext (kernels.h:515): same number of maps and map sizes, same terms
  * (atoms); new coefficients and new map index per term.                                                              */
 int b200md_update_cmap_params(b200md_ctx* ctx, int nmaps, const int* size, const double* coeff, int n, const int* map);
+/* CalcCustomTorsionForceKernel::copyParametersToContext (kernels.h:544): same terms, same program per term, new parameters
+ * params[n][param_stride], written into the same device buffers.                                                         */
+int b200md_update_custom_torsion_params(b200md_ctx* ctx, int n, const double* params);
+/* Test hook, no context and no device: program `which` of a b200md_set_custom_torsions program set, checked as that call
+ * checks it (nglobals = the number of global slots), evaluated at (theta, params, globals) on the host by the interpreter
+ * source the device kernel runs.  0 and *out on success, -1 with the reason in msg.                                       */
+int b200md_custom_program_probe(int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                int param_stride, int nglobals, int which, double theta, const double* params,
+                                const double* globals, double* out, char* msg, int msglen);
 
 /* ---------------------------------------------------------------------------------------------------
  * UpdateStateDataKernel (kernels.h:125-214).                                                         */
@@ -231,7 +275,8 @@ typedef struct b200md_stats {
 int b200md_get_stats(b200md_ctx* ctx, b200md_stats* out);
 /* mean device time (ms) of named phases measured with CUDA events on the engine's stream:
  * phase: 0 pair kernel, 1 pme spread, 2 fft+convolution, 3 pme gather, 4 integrate+constrain, 5 list build,
- * 6 bonded+exceptions.  Runs `reps` isolated launches of that phase on the current state.           */
+ * 6 bonded+exceptions (k_bonded and, with custom torsions, k_custom_torsion), 7 custom torsions alone (k_custom_torsion).
+ * Runs `reps` isolated launches of that phase on the current state.                                  */
 int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* ms_mean);
 /* stand-alone 3-D FFT entry (the bespoke FFT alone, for parity against fftpack / numpy):
  * in: real [nx][ny][nz] floats (host), out: complex [nx][ny][nz/2+1] (re,im) floats (host).          */

@@ -39,6 +39,8 @@ SIGNATURES = {
     "b200md_set_torsions": (C.c_int, [_P, C.c_int, _I, _I, _I, _I, _I, _D, _D]),
     "b200md_set_rb_torsions": (C.c_int, [_P, C.c_int, _I, _I, _I, _I, _D]),
     "b200md_set_cmap": (C.c_int, [_P, C.c_int, _I, _D, C.c_int, _I, _I]),
+    "b200md_set_custom_torsions": (C.c_int, [_P, C.c_int, _I, _I, _I, _D, C.c_int, C.c_int, _I, _I, _D]),
+    "b200md_set_custom_globals": (C.c_int, [_P, C.c_int, _D]),
     "b200md_set_bonded_groups": (C.c_int, [_P, C.c_int, C.c_int, _I]),
     "b200md_set_constraints": (C.c_int, [_P, C.c_int, _I, _I, _D]),
     "b200md_check_constraints": (C.c_int, [C.c_int, _D, C.c_int, _I, _I, _D, C.c_char_p, C.c_int]),
@@ -52,6 +54,9 @@ SIGNATURES = {
     "b200md_update_bonded_params": (C.c_int, [_P, C.c_int, C.c_int, _D, _D, _I]),
     "b200md_update_rb_torsion_params": (C.c_int, [_P, C.c_int, _D]),
     "b200md_update_cmap_params": (C.c_int, [_P, C.c_int, _I, _D, C.c_int, _I]),
+    "b200md_update_custom_torsion_params": (C.c_int, [_P, C.c_int, _D]),
+    "b200md_custom_program_probe": (C.c_int, [C.c_int, _I, _I, _I, _D, C.c_int, C.c_int, C.c_int, C.c_double, _D, _D, _D,
+                                              C.c_char_p, C.c_int]),
     "b200md_set_box": (C.c_int, [_P, _D, _D, _D]),
     "b200md_get_box": (C.c_int, [_P, _D, _D, _D]),
     "b200md_set_barostat_molecules": (C.c_int, [_P, C.c_int, _I, _I]),

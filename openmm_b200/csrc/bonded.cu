@@ -1,6 +1,7 @@
 // bonded.cu -- harmonic bonds, harmonic angles, periodic torsions, Ryckaert-Bellemans torsions, CMAP terms, 1-4
-// exceptions and the Ewald exclusion correction in ONE launch (sm_90a).  Double precision arithmetic on fp32 positions:
-// these terms are a few thousand work items, far below any roofline, and double removes them from the 1e-4 parity budget.
+// exceptions and the Ewald exclusion correction in ONE launch (sm_90a); custom torsions in a second launch behind it.
+// Double precision arithmetic on fp32 positions: these terms are a few thousand work items, far below any roofline, and
+// double removes them from the 1e-4 parity budget.
 //
 // Restates ReferenceHarmonicBondIxn / ReferenceAngleBondIxn / ReferenceProperDihedralBond / ReferenceRbDihedralBond::
 // calculateBondIxn, ReferenceCMAPTorsionIxn::calculateOneIxn,
@@ -8,6 +9,7 @@
 // ReferenceLJCoulombIxn::calculateEwaldIxn (ReferenceLJCoulombIxn.cpp:462-523).  Replaces the generated
 // computeBondedForces kernel of CudaBondedUtilities.cpp:76-150 with pmeExclusions.cc / nonbondedExceptions.cc.
 #include "engine.h"
+#include "custom_interp.h"
 #include "../../include/b200md.h"
 
 struct D3 { double x, y, z; };
@@ -225,7 +227,42 @@ __global__ void __launch_bounds__(128) k_bonded(NbDev nb, BondedDev bd, int term
     }
 }
 
-void launch_bonded(const NbDev& nb, const BondedDev& bd, int terms, bool energy, cudaStream_t s) {
+// One thread per custom torsion (CustomTorsionForce, restating ReferenceCustomTorsionIxn::calculateBondIxn): the dihedral as
+// for every other torsion, dE/dtheta from the term's derivative program, the forces through torsion_force, and the energy
+// program only when the energy is asked for.  A kernel of its own rather than a segment of k_bonded: the interpreter's stack
+// and registers would otherwise weigh on every bonded term of every System.
+__global__ void __launch_bounds__(128) k_custom_torsion(NbDev nb, CustomTorsionDev ct, int wantEnergy) {
+    const int i = blockIdx.x*blockDim.x + threadIdx.x;
+    double e = 0;
+    if (i < ct.nslots) {
+        const int p = ct.prog[i];          // uniform across the warp: the terms of one expression fill whole warps
+        const unsigned char g = ct.group[i];
+        if (p >= 0 && ((ct.groupMask >> (g & 31)) & 1u)) {
+            const int4 at = ct.atoms[i];
+            const Dihedral d = dihedral(nb, at, g & 0x80);
+            const double* par = ct.params + (size_t) i*ct.paramStride;
+            const double dE = custom_run(ct.code, ct.imm, ct.progStart[2*p+1], ct.progStart[2*p+2], d.theta, par, ct.globals);
+            torsion_force(nb, at, d, dE);
+            if (wantEnergy) e = custom_run(ct.code, ct.imm, ct.progStart[2*p], ct.progStart[2*p+1], d.theta, par, ct.globals);
+        }
+    }
+    if (wantEnergy) {
+        __shared__ double red[4];
+        for (int off = 16; off > 0; off >>= 1) e += __shfl_xor_sync(0xffffffffu, e, off);
+        if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = e;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            const double x = red[0] + red[1] + red[2] + red[3];
+            if (x != 0.0) atomicAdd(&nb.energy[EN_CUSTOM_TORSION], x);
+        }
+    }
+}
+
+void launch_custom_torsion(const NbDev& nb, const CustomTorsionDev& ct, bool energy, cudaStream_t s) {
+    launch_high(k_custom_torsion, (ct.nslots + 127)/128, 128, 0, s, nb, ct, energy ? 1 : 0);
+}
+
+void launch_bonded(const NbDev& nb, const BondedDev& bd, const CustomTorsionDev& ct, int terms, bool energy, cudaStream_t s) {
     int n = 0;
     if (terms & B200MD_TERM_BONDS) n += bd.nbonds;
     if (terms & B200MD_TERM_ANGLES) n += bd.nangles;
@@ -233,7 +270,9 @@ void launch_bonded(const NbDev& nb, const BondedDev& bd, int terms, bool energy,
     if (terms & B200MD_TERM_RB_TORSIONS) n += bd.nrb;
     if (terms & B200MD_TERM_CMAP) n += bd.ncmap;
     if (terms & B200MD_TERM_NB_DIRECT) n += bd.nexc;
-    if (n == 0) return;
-    int per = (n + nb.world - 1)/nb.world;
-    launch_high(k_bonded, (per + 127)/128, 128, 0, s, nb, bd, terms, energy ? 1 : 0);
+    if (n > 0) {
+        int per = (n + nb.world - 1)/nb.world;
+        launch_high(k_bonded, (per + 127)/128, 128, 0, s, nb, bd, terms, energy ? 1 : 0);
+    }
+    if ((terms & B200MD_TERM_CUSTOM_TORSIONS) && ct.nslots > 0) launch_custom_torsion(nb, ct, energy, s);
 }

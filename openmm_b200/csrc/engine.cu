@@ -1,6 +1,7 @@
 // engine.cu -- host side of libb200md.so: the C-ABI of include/b200md.h over the CUDA kernels of this directory.
 // No CPU fallback exists: every compute entry point needs a CUDA device and fails loudly without one.
 #include "engine.h"
+#include "custom_interp.h"
 #include "../../include/b200md.h"
 #include <stdexcept>
 #include <algorithm>
@@ -79,6 +80,21 @@ template <class A, class P> struct TermTable {
 struct CmapTable : TermTable<int4, double> {
     std::vector<int> map; std::vector<int2> maps;
     DevBuf<int> mapDev; DevBuf<int2> mapsDev;
+};
+// Custom torsions: atoms, params [n][stride] and groups in the caller's term order; besides, the programs (code = (opcode,
+// operand), imm, progStart), the expression of every term and the global values.  finalize lays the terms out as
+// k_custom_torsion reads them: grouped by expression, each group padded to whole warps; slot[i] is the slot of term i.
+struct CustomTorsionTable : TermTable<int4, double> {
+    int stride = 0, nprog = 0, nslots = 0;
+    std::vector<int2> code; std::vector<double> imm; std::vector<int> progStart, prog, slot;
+    std::vector<double> globals;
+    DevBuf<int2> codeDev; DevBuf<double> immDev, globalsDev; DevBuf<int> progStartDev, progDev;
+    // params in the slot layout (padding slots 0)
+    std::vector<double> slot_params() const {
+        std::vector<double> p((size_t) nslots*stride, 0.0);
+        for (int i = 0; i < n; i++) std::copy(params.begin() + (size_t) i*stride, params.begin() + (size_t) (i+1)*stride, p.begin() + (size_t) slot[i]*stride);
+        return p;
+    }
 };
 
 // The buffers of one neighbour list (ListDev): the sorted copies and the block boxes, sized by the atoms; the tile pools,
@@ -160,6 +176,7 @@ struct b200md_ctx {
     TermTable<int4, double4> torsions;      // (k, phase, n, 0)
     TermTable<int4, double> rb;             // [n][6] c0..c5
     CmapTable cmap;
+    CustomTorsionTable custom;
     std::vector<int> conI, conJ; std::vector<double> conD;
     int cmFreq = 0;
     std::vector<int4> hUnitAtoms;        // host copy of the integration units (ownership cuts of the multi-GPU data plane)
@@ -199,6 +216,7 @@ struct b200md_ctx {
     NbDev nb{};
     PmeDev pme{};
     BondedDev bd{};
+    CustomTorsionDev ctd{};
     UnitDev units{};
     IntegDev integ{};
     bool haveIntegrator = false;
@@ -388,12 +406,68 @@ extern "C" int b200md_set_cmap(b200md_ctx* ctx, int nmaps, const int* size, cons
     ctx->cmap.map.assign(map, map + n); ctx->cmap.maps.swap(maps);
     API_END(ctx)
 }
+// A custom-torsion program set (b200md_set_custom_torsions): prog_start well formed and every program passing
+// custom_check_program (nglobals < 0: GLOBAL operands are checked at finalize).  Returns the instructions as (opcode, operand).
+static std::vector<int2> check_programs(int nprog, const int* prog_start, const int* op, const int* arg, int stride, int nglobals) {
+    require(nprog >= 0, "set_custom_torsions: negative number of programs");
+    require(stride >= 0 && stride <= B200MD_CUSTOM_MAX_PARAMS, "set_custom_torsions: more than 16 parameters per torsion");
+    require(nprog == 0 || prog_start[0] == 0, "set_custom_torsions: prog_start[0] must be 0");
+    for (int q = 0; q < 2*nprog; q++) require(prog_start[q+1] >= prog_start[q], "set_custom_torsions: prog_start must not decrease");
+    const int total = nprog ? prog_start[2*nprog] : 0;
+    std::vector<int2> code(total);
+    for (int k = 0; k < total; k++) code[k] = make_int2(op[k], arg[k]);
+    for (int q = 0; q < 2*nprog; q++) {
+        const char* why = custom_check_program(code.data(), prog_start[q], prog_start[q+1], stride, nglobals);
+        if (why) throw std::runtime_error(std::string(why) + " (program " + std::to_string(q) + ")");
+    }
+    return code;
+}
+extern "C" int b200md_set_custom_torsions(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                          int stride, int n, const int* prog, const int* atoms, const double* params) {
+    API_BEGIN(ctx)
+    check_set(ctx, "set_custom_torsions", n);
+    require(ctx->world == 1, "custom torsions are not supported in multi-GPU runs");
+    std::vector<int2> code = check_programs(nprog, prog_start, op, arg, stride, -1);
+    for (int i = 0; i < n; i++) require(prog[i] >= 0 && prog[i] < nprog, "custom torsion: program index out of range");
+    std::vector<int4> a(n); std::vector<double> p(params, params + (size_t) n*stride);
+    for (int i = 0; i < n; i++) a[i] = make_int4(atoms[4*i], atoms[4*i+1], atoms[4*i+2], atoms[4*i+3]);
+    CustomTorsionTable& t = ctx->custom;
+    t.set(ctx->natoms, "custom torsion", n, a, p);
+    t.stride = stride; t.nprog = nprog; t.code.swap(code);
+    t.imm.assign(imm, imm + t.code.size()); t.progStart.assign(prog_start, prog_start + (nprog ? 2*nprog + 1 : 0)); t.prog.assign(prog, prog + n);
+    API_END(ctx)
+}
+extern "C" int b200md_set_custom_globals(b200md_ctx* ctx, int n, const double* values) {
+    API_BEGIN(ctx)
+    require(n >= 0, "set_custom_globals: negative count");
+    CustomTorsionTable& t = ctx->custom;
+    if (!ctx->finalized) { t.globals.assign(values, values + n); return 0; }
+    require(n == (int) t.globals.size(), "set_custom_globals: the number of global parameters cannot change after finalize");
+    t.globals.assign(values, values + n);
+    // stream ordered, into the buffer the step graphs read: no graph is captured or instantiated again
+    if (n) CUDA_CHECK(cudaMemcpyAsync(t.globalsDev.p, t.globals.data(), sizeof(double)*n, cudaMemcpyHostToDevice, ctx->stream));
+    API_END(ctx)
+}
+extern "C" int b200md_custom_program_probe(int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                           int stride, int nglobals, int which, double theta, const double* params,
+                                           const double* globals, double* out, char* msg, int msglen) {
+    try {
+        require(nglobals >= 0, "custom_program_probe: negative number of globals");
+        const std::vector<int2> code = check_programs(nprog, prog_start, op, arg, stride, nglobals);
+        require(which >= 0 && which < 2*nprog, "custom_program_probe: program index out of range");
+        *out = custom_run(code.data(), imm, prog_start[which], prog_start[which+1], theta, params, globals);
+        return 0;
+    } catch (std::exception& e) {
+        if (msg && msglen > 0) { strncpy(msg, e.what(), msglen - 1); msg[msglen - 1] = 0; }
+        return -1;
+    }
+}
 extern "C" int b200md_set_bonded_groups(b200md_ctx* ctx, int kind, int n, const int* group) {
     API_BEGIN(ctx)
     check_set(ctx, "set_bonded_groups", n);
-    require(kind >= 0 && kind <= 4, "set_bonded_groups: kind must be 0 (bonds), 1 (angles), 2 (torsions), 3 (RB torsions) or 4 (CMAP)");
+    require(kind >= 0 && kind <= 5, "set_bonded_groups: kind must be 0 (bonds), 1 (angles), 2 (torsions), 3 (RB torsions), 4 (CMAP) or 5 (custom torsions)");
     std::vector<unsigned char>& g = kind == 0 ? ctx->bonds.group : kind == 1 ? ctx->angles.group : kind == 2 ? ctx->torsions.group :
-                                    kind == 3 ? ctx->rb.group : ctx->cmap.group;
+                                    kind == 3 ? ctx->rb.group : kind == 4 ? ctx->cmap.group : ctx->custom.group;
     g.resize(n);
     for (int i = 0; i < n; i++) { require(group[i] >= 0 && (group[i] & ~0x80) < 32, "force group out of range"); g[i] = (unsigned char) group[i]; }
     API_END(ctx)
@@ -1175,6 +1249,44 @@ static bool fft_beside_tiles(const b200md_ctx* c) {
     return c->world == 1 && !c->pmeOnly && c->overlapPme && !c->nb.smPartition && c->nbdesc.method == B200MD_NB_PME;
 }
 
+// finalize: the custom torsions in the layout of k_custom_torsion (CustomTorsionDev): grouped by expression, each group padded
+// to whole warps, and the programs, checked once more now that the number of global slots is final
+static void upload_custom_torsions(b200md_ctx* c) {
+    CustomTorsionTable& t = c->custom;
+    CustomTorsionDev& d = c->ctd;
+    d = CustomTorsionDev{};
+    d.groupMask = 0xffffffffu;
+    // the global values get their buffer even without terms: a CustomTorsionForce with no torsions may still name globals, and
+    // b200md_set_custom_globals copies into this buffer after finalize
+    t.globalsDev.alloc(std::max<size_t>(t.globals.size(), 1)); t.globalsDev.upload(t.globals);
+    d.globals = t.globalsDev.p;
+    if (t.n == 0) return;
+    require(c->world == 1, "custom torsions are not supported in multi-GPU runs");
+    require(t.group.empty() || (int) t.group.size() == t.n, "set_bonded_groups: group array length differs from the number of terms");
+    for (int q = 0; q < 2*t.nprog; q++) {
+        const char* why = custom_check_program(t.code.data(), t.progStart[q], t.progStart[q+1], t.stride, (int) t.globals.size());
+        if (why) throw std::runtime_error(std::string(why) + " (program " + std::to_string(q) + ")");
+    }
+    t.slot.assign(t.n, 0);
+    int cursor = 0;
+    for (int p = 0; p < t.nprog; p++) {
+        for (int i = 0; i < t.n; i++) if (t.prog[i] == p) t.slot[i] = cursor++;
+        cursor = (cursor + 31)/32*32;
+    }
+    t.nslots = cursor;
+    std::vector<int4> atoms(cursor, make_int4(0, 0, 0, 0));
+    std::vector<unsigned char> group(cursor, 0);
+    std::vector<int> prog(cursor, -1);
+    for (int i = 0; i < t.n; i++) { atoms[t.slot[i]] = t.atoms[i]; group[t.slot[i]] = t.group.empty() ? 0 : t.group[i]; prog[t.slot[i]] = t.prog[i]; }
+    t.atomsDev.upload(atoms); t.groupDev.upload(group); t.progDev.upload(prog);
+    const std::vector<double> par = t.slot_params();
+    t.paramsDev.alloc(std::max<size_t>(par.size(), 1)); t.paramsDev.upload(par);
+    t.codeDev.upload(t.code); t.immDev.upload(t.imm); t.progStartDev.upload(t.progStart);
+    d.nslots = t.nslots; d.paramStride = t.stride;
+    d.atoms = t.atomsDev.p; d.params = t.paramsDev.p; d.group = t.groupDev.p; d.prog = t.progDev.p;
+    d.code = t.codeDev.p; d.imm = t.immDev.p; d.progStart = t.progStartDev.p;
+}
+
 extern "C" int b200md_finalize(b200md_ctx* ctx) {
     API_BEGIN(ctx)
     require(!ctx->finalized, "finalize called twice");
@@ -1273,6 +1385,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     c->cmap.mapDev.upload(c->cmap.map); c->cmap.mapsDev.upload(c->cmap.maps); bd.cmapMap = c->cmap.mapDev.p; bd.cmapMaps = c->cmap.mapsDev.p;
     bd.excPeriodic = c->nbdesc.exceptions_periodic;
     bd.groupMask = 0xffffffffu;
+    upload_custom_torsions(c);
     upload_params(c);
     build_units(c);
     build_ccma(c);
@@ -1283,7 +1396,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
             require(fft_slab_path(probe), "multi-GPU: the PME grid plane does not fit the slab FFT kernels (B200MD_MGPU=nccl selects the NCCL scheme)");
         }
     }
-    // ---- molecules (connected components of bonds, angles, torsions, RB torsions, CMAP terms, constraints and exceptions) for the wrap at list
+    // ---- molecules (connected components of bonds, angles, torsions, RB torsions, CMAP terms, custom torsions, constraints and exceptions) for the wrap at list
     // builds; off for non-periodic systems and with more than one rank (every rank would have to wrap in the same step,
     // and the reciprocal-space rank builds no list) ----
     c->cellOffset.alloc((size_t) 3*NP); c->cellOffset.zero();
@@ -1295,7 +1408,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
         auto join = [&](int a, int b) { a = find(a); b = find(b); if (a != b) parent[std::max(a, b)] = std::min(a, b); };
         for (const int2& a : c->bonds.atoms) join(a.x, a.y);
         for (const int4& a : c->angles.atoms) { join(a.x, a.y); join(a.y, a.z); }
-        for (auto* t : {&c->torsions.atoms, &c->rb.atoms, &c->cmap.atoms}) for (const int4& a : *t) { join(a.x, a.y); join(a.y, a.z); join(a.z, a.w); }
+        for (auto* t : {&c->torsions.atoms, &c->rb.atoms, &c->cmap.atoms, &c->custom.atoms}) for (const int4& a : *t) { join(a.x, a.y); join(a.y, a.z); join(a.z, a.w); }
         for (size_t d = 1; d < c->cmap.atoms.size(); d += 2) join(c->cmap.atoms[d-1].x, c->cmap.atoms[d].x);     // a CMAP term's two dihedrals
         for (size_t i = 0; i < c->conI.size(); i++) join(c->conI[i], c->conJ[i]);
         for (const int2& a : c->exc.atoms) join(a.x, a.y);
@@ -1385,6 +1498,19 @@ extern "C" int b200md_update_cmap_params(b200md_ctx* ctx, int nmaps, const int* 
     ctx->cmap.params.assign(coeff, coeff + ctx->cmap.params.size());
     ctx->cmap.map.assign(map, map + n);
     ctx->cmap.paramsDev.upload(ctx->cmap.params); ctx->cmap.mapDev.upload(ctx->cmap.map);
+    API_END(ctx)
+}
+
+// CalcCustomTorsionForceKernel::copyParametersToContext (kernels.h:544): same terms and programs, new parameters, into the
+// same device buffer.
+extern "C" int b200md_update_custom_torsion_params(b200md_ctx* ctx, int n, const double* params) {
+    API_BEGIN(ctx)
+    require(ctx->finalized, "update_custom_torsion_params before finalize");
+    CustomTorsionTable& t = ctx->custom;
+    require(n == t.n, "updateParametersInContext: The number of torsions has changed");
+    CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+    t.params.assign(params, params + (size_t) n*t.stride);
+    if (n) t.paramsDev.upload(t.slot_params());
     API_END(ctx)
 }
 
@@ -1654,11 +1780,21 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
         launch_check_displacement(c->nb, c->cd, s); launches++;
         launch_list_build(c->nb, s); launches += LIST_BUILD_LAUNCHES;
     }
-    int bterms = terms & (B200MD_TERM_BONDS | B200MD_TERM_ANGLES | B200MD_TERM_TORSIONS | B200MD_TERM_RB_TORSIONS | B200MD_TERM_CMAP);
+    int bterms = terms & (B200MD_TERM_BONDS | B200MD_TERM_ANGLES | B200MD_TERM_TORSIONS | B200MD_TERM_RB_TORSIONS | B200MD_TERM_CMAP |
+                          B200MD_TERM_CUSTOM_TORSIONS);
     if (c->haveNb) bterms |= terms & B200MD_TERM_NB_DIRECT;
     const int nbonded = c->bd.nbonds + c->bd.nangles + c->bd.ntorsions + c->bd.nrb + c->bd.ncmap + c->bd.nexc;
-    const bool bonded = bterms && nbonded > 0 && !(split && c->rank == pmeRank);
-    auto launch_bonded_terms = [&](cudaStream_t sb) { BondedDev bd = c->bd; bd.groupMask = groupMask; launch_bonded(c->nb, bd, bterms, energy, sb); launches++; };
+    // the k_bonded branch is counted as one launch whenever it is taken (even when the selected classes have no terms and
+    // launch_bonded skips the kernel); k_custom_torsion is counted when it runs
+    const bool classic = (bterms & ~B200MD_TERM_CUSTOM_TORSIONS) && nbonded > 0;
+    const bool custom = (bterms & B200MD_TERM_CUSTOM_TORSIONS) && c->ctd.nslots > 0;
+    const bool bonded = (classic || custom) && !(split && c->rank == pmeRank);
+    auto launch_bonded_terms = [&](cudaStream_t sb) {
+        BondedDev bd = c->bd; bd.groupMask = groupMask;
+        CustomTorsionDev ct = c->ctd; ct.groupMask = groupMask;
+        launch_bonded(c->nb, bd, ct, bterms, energy, sb);
+        launches += (classic ? 1 : 0) + (custom ? 1 : 0);
+    };
     // The bonded terms need nothing from the tile kernel either: on one GPU they fork with the spread onto a stream of their
     // own (not before the list build, whose wrap phase moves molecules in posq) and join before the integrator.
     const bool forkBonded = forkAfterList && bonded;
@@ -1777,6 +1913,7 @@ extern "C" int b200md_compute_groups(b200md_ctx* ctx, int terms, unsigned int bo
         if (terms & B200MD_TERM_TORSIONS) e += h[EN_TORSION];
         if (terms & B200MD_TERM_RB_TORSIONS) e += h[EN_RBTORSION];
         if (terms & B200MD_TERM_CMAP) e += h[EN_CMAP];
+        if (terms & B200MD_TERM_CUSTOM_TORSIONS) e += h[EN_CUSTOM_TORSION];
         if (ctx->haveNb) {
             if (terms & B200MD_TERM_NB_DIRECT) {
                 e += h[EN_NB] + h[EN_EXC];
@@ -2045,6 +2182,7 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
     // the integrate phase mutates the state: positions and velocities are restored before every repetition, the step
     // counter (which each repetition advances, as a step does) once at the end
     Snapshot state, counter;
+    require(phase != 7 || c->ctd.nslots > 0, "time_phase(custom torsions): the System has none");
     if (phase == 4) {
         require(c->haveIntegrator, "time_phase(integrate) before set_integrator");
         state.parts = state_spans(c, ST_POS | ST_VEL); state.save(s);
@@ -2062,7 +2200,8 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
             case 3: launch_pme_gather(nbv, pme_for_launch(c), local, s); break;
             case 4: launch_integrate(nbv, c->units, c->integ, local, s); break;
             case 5: launch_list_build(nbv, s); break;
-            case 6: launch_bonded(nbv, c->bd, B200MD_TERM_ALL, false, s); break;
+            case 6: launch_bonded(nbv, c->bd, c->ctd, B200MD_TERM_ALL, false, s); break;
+            case 7: launch_custom_torsion(nbv, c->ctd, false, s); break;
             default: throw std::runtime_error("unknown phase");
         }
         CUDA_CHECK(cudaEventRecord(e1, s));

@@ -159,7 +159,7 @@ struct NbDev {
 };
 
 enum { EN_NB = 0, EN_RECIP = 1, EN_BOND = 2, EN_ANGLE = 3, EN_TORSION = 4, EN_EXC = 5, EN_KE = 6, EN_RBTORSION = 7, EN_CMAP = 8,
-       B200MD_NUM_ENERGY = 9 };
+       EN_CUSTOM_TORSION = 9, B200MD_NUM_ENERGY = 10 };
 
 struct PmeDev {
     int nx, ny, nz, nzc;
@@ -192,6 +192,19 @@ struct BondedDev {
     // ContextImpl::calcForcesAndEnergy groups, ContextImpl.cpp:293-308); an element is evaluated iff bit `group` of groupMask is set
     const unsigned char* bondGroup; const unsigned char* angleGroup; const unsigned char* torsionGroup;
     const unsigned char* rbGroup; const unsigned char* cmapGroup;
+    unsigned int groupMask;
+};
+
+// Custom torsions (k_custom_torsion, bonded.cu): a kernel and a parameter block of their own, so that BondedDev and k_bonded
+// stay as they are.  The terms are stored grouped by expression, each group padded to whole warps (prog = -1 in a padding
+// slot), so that every warp runs one program and reads its code with uniform loads.  Program 2p is expression p's energy,
+// program 2p+1 its dE/dtheta: the instructions [progStart[q], progStart[q+1]) of code (opcode, operand) and imm.
+struct CustomTorsionDev {
+    int nslots;                  // terms + padding
+    int paramStride;             // parameters per slot
+    const int4* atoms; const double* params; const unsigned char* group; const int* prog;
+    const int2* code; const double* imm; const int* progStart;
+    const double* globals;       // the values of the global parameter slots (b200md_set_custom_globals)
     unsigned int groupMask;
 };
 
@@ -473,7 +486,10 @@ void fft_set_compact(int on);                   // smaller FFT CTAs (the chain s
 size_t fft_cta_smem_bytes(const PmeDev& pme);  // largest shared memory of one single-GPU FFT CTA of this grid (dynamic + static)
 bool fft_slab_path(const PmeDev& pme);          // the 3-launch slab pipeline is usable for this grid (precondition of the multi-GPU FFT)
 
-void launch_bonded(const NbDev& nb, const BondedDev& bd, int terms, bool energy, cudaStream_t s);
+// k_bonded (when the classes in `terms` have terms) and, when `terms` has B200MD_TERM_CUSTOM_TORSIONS and there are custom
+// torsions, k_custom_torsion behind it on the same stream
+void launch_bonded(const NbDev& nb, const BondedDev& bd, const CustomTorsionDev& ct, int terms, bool energy, cudaStream_t s);
+void launch_custom_torsion(const NbDev& nb, const CustomTorsionDev& ct, bool energy, cudaStream_t s);
 
 void launch_integrate(const NbDev& nb, const UnitDev& units, const IntegDev& integ, const CommDev& cd, cudaStream_t s);
 void launch_force_push(const NbDev& nb, const CommDev& cd, cudaStream_t s);          // partial forces of foreign atoms -> owners' inboxes

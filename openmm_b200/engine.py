@@ -6,10 +6,11 @@ from . import _lib
 from .systems import SystemDesc, NB_PME
 
 TERM_BONDS, TERM_ANGLES, TERM_TORSIONS, TERM_NB_DIRECT, TERM_NB_RECIP = 1, 2, 4, 8, 16
-TERM_RB_TORSIONS, TERM_CMAP, TERM_ALL = 32, 64, 127
+TERM_RB_TORSIONS, TERM_CMAP, TERM_CUSTOM_TORSIONS, TERM_ALL = 32, 64, 128, 255
 # kinds of b200md_set_bonded_groups
-BONDED_KINDS = {"bonds": 0, "angles": 1, "torsions": 2, "rb_torsions": 3, "cmap": 4}
-PHASES = {"pair": 0, "pme_spread": 1, "pme_fft_conv": 2, "pme_gather": 3, "integrate": 4, "list_build": 5, "bonded": 6}
+BONDED_KINDS = {"bonds": 0, "angles": 1, "torsions": 2, "rb_torsions": 3, "cmap": 4, "custom_torsions": 5}
+PHASES = {"pair": 0, "pme_spread": 1, "pme_fft_conv": 2, "pme_gather": 3, "integrate": 4, "list_build": 5, "bonded": 6,
+          "custom_torsions": 7}
 
 
 class EngineError(RuntimeError):
@@ -100,6 +101,16 @@ class Engine:
         if len(d.cmap_map):
             self._ck(L.b200md_set_cmap(self.h, len(d.cmap_size), _ip(_i32(d.cmap_size)), _dp(_f64(d.cmap_coeff)), len(d.cmap_map),
                                        _ip(_i32(d.cmap_map)), _ip(_i32(d.cmap_atoms))))
+        if len(d.custom_prog):
+            if not len(d.custom_op):
+                raise EngineError("custom torsions without programs: compile desc.custom_energy into custom_op / custom_arg / "
+                                  "custom_imm / custom_prog_start first (the plugin's expression translator)")
+            params = _f64(d.custom_params).reshape(len(d.custom_prog), -1)
+            self._ck(L.b200md_set_custom_torsions(self.h, len(d.custom_prog_start)//2, _ip(_i32(d.custom_prog_start)), _ip(_i32(d.custom_op)),
+                                                  _ip(_i32(d.custom_arg)), _dp(_f64(d.custom_imm)), params.shape[1], len(d.custom_prog),
+                                                  _ip(_i32(d.custom_prog)), _ip(_i32(d.custom_atoms)), _dp(params)))
+        if len(d.custom_global_values):
+            self._ck(L.b200md_set_custom_globals(self.h, len(d.custom_global_values), _dp(_f64(d.custom_global_values))))
         for kind, g in self._bonded_groups.items():
             g = _i32(g)
             self._ck(L.b200md_set_bonded_groups(self.h, BONDED_KINDS[kind], len(g), _ip(g)))
@@ -195,6 +206,17 @@ class Engine:
     def update_cmap_params(self, size, coeff, cmap_map):
         size, coeff, cmap_map = _i32(size), _f64(coeff), _i32(cmap_map)
         self._ck(self.lib.b200md_update_cmap_params(self.h, len(size), _ip(size), _dp(coeff), len(cmap_map), _ip(cmap_map)))
+
+    # ---- CalcCustomTorsionForceKernel::copyParametersToContext and the global parameters of its expressions ----
+    def update_custom_torsion_params(self, params):
+        """New per-torsion parameters [n, param_stride] for the same torsions and expressions."""
+        p = _f64(params)
+        self._ck(self.lib.b200md_update_custom_torsion_params(self.h, len(p), _dp(p)))
+
+    def set_custom_globals(self, values):
+        """The values of the global parameter slots the expressions read (the number of slots is fixed at definition)."""
+        v = _f64(values)
+        self._ck(self.lib.b200md_set_custom_globals(self.h, len(v), _dp(v)))
 
     # ---- Integrate*StepKernel ----
     def set_integrator(self, kind, dt, temperature=300.0, friction=1.0, seed=7, constraint_tol=1e-5):

@@ -70,6 +70,21 @@ class SystemDesc:
     cmap_energy: np.ndarray = field(default_factory=_d)   # [sum size^2] map energies, kJ/mol (what a CMAPTorsionForce is given)
     cmap_map: np.ndarray = field(default_factory=_i)      # [n] map of each term
     cmap_atoms: np.ndarray = field(default_factory=lambda: np.zeros((0, 8), dtype=np.int32))   # [n,8] the two dihedrals
+    # CustomTorsionForce: per expression p its energy (a Lepton expression of theta, the per-torsion parameters
+    # custom_param_names[p] and the global parameters custom_global_names), and per term its expression, atoms and parameters.
+    # custom_prog_start / op / arg / imm are the compiled programs b200md_set_custom_torsions takes (program 2p = energy of
+    # expression p, 2p+1 = its dE/dtheta); they come from the plugin's translator (plugin/custom_translate.h).
+    custom_energy: tuple = ()
+    custom_param_names: tuple = ()                        # per expression: the names of its per-torsion parameters
+    custom_global_names: tuple = ()                       # global slot s <- name s
+    custom_global_values: np.ndarray = field(default_factory=_d)
+    custom_prog: np.ndarray = field(default_factory=_i)   # [n] expression of each term
+    custom_atoms: np.ndarray = field(default_factory=lambda: np.zeros((0, 4), dtype=np.int32))
+    custom_params: np.ndarray = field(default_factory=lambda: np.zeros((0, 0)))   # [n, param_stride]
+    custom_prog_start: np.ndarray = field(default_factory=_i)
+    custom_op: np.ndarray = field(default_factory=_i)
+    custom_arg: np.ndarray = field(default_factory=_i)
+    custom_imm: np.ndarray = field(default_factory=_d)
     con_i: np.ndarray = field(default_factory=_i)
     con_j: np.ndarray = field(default_factory=_i)
     con_d: np.ndarray = field(default_factory=_d)
@@ -130,7 +145,11 @@ class SystemDesc:
         return d
 
     def save(self, path):
-        d = {k: (np.asarray(v) if v is not None else np.zeros(0)) for k, v in self.__dict__.items() if not isinstance(v, str)}
+        d = {k: (np.asarray(v) if v is not None else np.zeros(0)) for k, v in self.__dict__.items()
+             if not isinstance(v, str) and k != "custom_param_names"}
+        width = max([len(p) for p in self.custom_param_names] + [0])
+        rows = [list(p) + [""]*(width - len(p)) for p in self.custom_param_names]
+        d["custom_param_names"] = np.array(rows, dtype=str).reshape(len(rows), width)
         d["name"] = np.array(self.name)
         np.savez_compressed(path, **d)
 
@@ -142,6 +161,10 @@ class SystemDesc:
             v = z[k]
             if k == "name":
                 kw[k] = str(v)
+            elif k in ("custom_energy", "custom_global_names"):
+                kw[k] = tuple(str(x) for x in v)
+            elif k == "custom_param_names":
+                kw[k] = tuple(tuple(str(y) for y in x if str(y)) for x in v)
             elif k == "box":
                 kw[k] = v if v.size == 9 else None
             elif k == "pme_grid":
@@ -174,6 +197,76 @@ def periodic_to_rb(desc):
     d.rb_c = c
     d.tor_i, d.tor_j, d.tor_k, d.tor_l, d.tor_n, d.tor_phase, d.tor_kk = _i(), _i(), _i(), _i(), _i(), _d(), _d()
     return d
+
+
+PERIODIC_CUSTOM = "k*(1+cos(n*theta-theta0))"
+# CharmmPsfFile.createSystem's improper energy (app/charmmpsffile.py): harmonic in the angle's distance from theta0 across the
+# +-pi seam; pi as that code writes it ('pi = %f')
+CHARMM_IMPROPER = "k*min(dtheta, 2*pi-dtheta)^2; dtheta = abs(theta-theta0); pi = %f;" % math.pi
+
+
+def _custom_only(desc, energy, param_names, prog, atoms, params, global_names=(), global_values=()):
+    """desc with exactly these custom torsions (expressions not compiled yet)"""
+    import copy
+    d = copy.copy(desc)
+    d.custom_energy, d.custom_param_names = tuple(energy), tuple(tuple(p) for p in param_names)
+    d.custom_global_names, d.custom_global_values = tuple(global_names), np.asarray(global_values, dtype=np.float64)
+    d.custom_prog = np.asarray(prog, dtype=np.int32)
+    d.custom_atoms = np.asarray(atoms, dtype=np.int32).reshape(-1, 4)
+    width = max([len(p) for p in d.custom_param_names] + [0])
+    d.custom_params = np.asarray(params, dtype=np.float64).reshape(len(d.custom_prog), -1) if len(d.custom_prog) else np.zeros((0, width))
+    d.custom_prog_start, d.custom_op, d.custom_arg, d.custom_imm = _i(), _i(), _i(), _d()
+    return d
+
+
+def periodic_to_custom(desc):
+    """The same System with every periodic torsion k (1 + cos(n theta - theta0)) written as the CustomTorsionForce
+    PERIODIC_CUSTOM with per-torsion parameters (k, n, theta0): the exact counterpart of periodic_to_rb."""
+    atoms = np.stack([desc.tor_i, desc.tor_j, desc.tor_k, desc.tor_l], axis=1) if len(desc.tor_i) else np.zeros((0, 4))
+    params = np.stack([desc.tor_kk, np.asarray(desc.tor_n, dtype=np.float64), desc.tor_phase], axis=1) if len(desc.tor_i) else np.zeros((0, 3))
+    d = _custom_only(desc, [PERIODIC_CUSTOM], [("k", "n", "theta0")], np.zeros(len(desc.tor_i)), atoms, params)
+    d.tor_i, d.tor_j, d.tor_k, d.tor_l, d.tor_n, d.tor_phase, d.tor_kk = _i(), _i(), _i(), _i(), _i(), _d(), _d()
+    return d
+
+
+def improper_centres(desc):
+    """[n,4] impropers (centre, a, b, c) on every atom with exactly three bonded neighbours (bonds and constraints), the
+    neighbours in ascending order; ordered by the centre."""
+    nbr = [set() for _ in range(desc.natoms)]
+    for i, j in zip(np.concatenate([desc.bond_i, desc.con_i]).tolist(), np.concatenate([desc.bond_j, desc.con_j]).tolist()):
+        nbr[i].add(j)
+        nbr[j].add(i)
+    return np.array([[a] + sorted(nbr[a]) for a in range(desc.natoms) if len(nbr[a]) == 3], dtype=np.int32).reshape(-1, 4)
+
+
+def with_charmm_impropers(desc, seed=1, k_range=(20.0, 800.0)):
+    """desc plus one CHARMM improper (CHARMM_IMPROPER, per-torsion parameters k, theta0) per improper_centres quadruple, k
+    uniform in k_range kJ/mol/rad^2 and theta0 at the current dihedral plus up to 0.3 rad, both from `seed`: the form
+    CharmmPsfFile writes, with parameters that keep the terms near their minimum as force-field impropers are."""
+    atoms = improper_centres(desc)
+    rng = np.random.default_rng(seed)
+    x = np.asarray(desc.positions, dtype=np.float64)
+    theta = dihedrals(x, atoms, desc.box)
+    k = rng.uniform(k_range[0], k_range[1], len(atoms))
+    theta0 = np.mod(theta + rng.uniform(-0.3, 0.3, len(atoms)) + math.pi, 2*math.pi) - math.pi
+    return _custom_only(desc, [CHARMM_IMPROPER], [("k", "theta0")], np.zeros(len(atoms)), atoms, np.stack([k, theta0], axis=1))
+
+
+def dihedrals(x, atoms, box=None):
+    """Dihedral angle in (-pi, pi] of every quadruple of atoms [n,4] at positions x, as ReferenceBondIxn measures it (the
+    sign of the first difference vector against the second normal); minimum-image difference vectors when box is given."""
+    def d(a, b):
+        v = x[a] - x[b]
+        if box is not None:
+            bx = np.asarray(box, dtype=np.float64)
+            for k in (2, 1, 0):
+                v -= np.round(v[:, k:k+1]/bx[k, k])*bx[k]
+        return v
+    v0, v1, v2 = d(atoms[:, 0], atoms[:, 1]), d(atoms[:, 2], atoms[:, 1]), d(atoms[:, 2], atoms[:, 3])
+    c0, c1 = np.cross(v0, v1), np.cross(v1, v2)
+    cosang = np.clip(np.einsum("ij,ij->i", c0, c1)/np.sqrt(np.einsum("ij,ij->i", c0, c0)*np.einsum("ij,ij->i", c1, c1)), -1, 1)
+    theta = np.arccos(cosang)
+    return np.where(np.einsum("ij,ij->i", v0, c1) < 0, -theta, theta)
 
 
 def backbone_cmap_atoms(desc):

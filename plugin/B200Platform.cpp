@@ -7,8 +7,9 @@
 // (CudaPlatform.cpp:59-61).  Compiled against the reference's headers where they lie; no reference source is copied.
 //
 // Supported: NonbondedForce (NoCutoff, CutoffNonPeriodic, CutoffPeriodic, PME; parameter offsets), HarmonicBondForce,
-// HarmonicAngleForce, PeriodicTorsionForce, RBTorsionForce, CMAPTorsionForce (any number of objects, each in its own force
-// group), CMMotionRemover;
+// HarmonicAngleForce, PeriodicTorsionForce, RBTorsionForce, CMAPTorsionForce, CustomTorsionForce (any number of objects, each
+// in its own force group; custom torsions without energy parameter derivatives, expressions within the limits of
+// custom_translate.h), CMMotionRemover;
 // Verlet / Langevin / LangevinMiddle integrators; SETTLE + X-H_n SHAKE constraints; MonteCarloBarostat and
 // MonteCarloAnisotropicBarostat (ApplyMonteCarloBarostatKernel; MonteCarloMembraneBarostat is refused).  A Force class without a kernel here
 // makes Platform::supportsKernels() false; an unsupported OPTION of a supported class is rejected in contextCreated()
@@ -32,6 +33,7 @@
 #include "openmm/PeriodicTorsionForce.h"
 #include "openmm/RBTorsionForce.h"
 #include "openmm/CMAPTorsionForce.h"
+#include "openmm/CustomTorsionForce.h"
 #include "openmm/CMMotionRemover.h"
 #include "openmm/VerletIntegrator.h"
 #include "openmm/LangevinIntegrator.h"
@@ -41,6 +43,7 @@
 #include "openmm/internal/NonbondedForceImpl.h"
 #include "openmm/internal/CMAPTorsionForceImpl.h"
 #include "../include/b200md.h"
+#include "custom_translate.h"
 #include <algorithm>
 #include <map>
 #include <string>
@@ -79,7 +82,7 @@ struct PlatformData {
     int cmFrequency = 0;
     bool cmRequested = false;       // RemoveCMMotionKernel::execute seen since the last integrator step
     bool useFusedStep = true;       // B200MD_PLUGIN_FUSED=0: always compute + integrate_only (debugging)
-    vector<int> bondG, angG, torG, rbG, cmapG;  // force group of every bonded element
+    vector<int> bondG, angG, torG, rbG, cmapG, customG;  // force group of every bonded element
     // bonded terms are gathered over all force objects of a kind and sent at finalize
     vector<int> bondI, bondJ; vector<double> bondR0, bondK;
     vector<int> angI, angJ, angK; vector<double> angT0, angKK;
@@ -88,6 +91,20 @@ struct PlatformData {
     // CMAP: the maps of all objects one after the other (a term's map index counts from the first map of all objects);
     // coefficients from CMAPTorsionForceImpl::calcMapDerivatives, [sum size^2][16]
     vector<int> cmapSize, cmapMap, cmapAtoms; vector<double> cmapCoeff;
+    // custom torsions: the programs of all objects one after the other (object f's expression is the pair 2f, 2f+1); the
+    // parameters of every term padded to B200MD_CUSTOM_MAX_PARAMS here, packed to the widest object's count when sent
+    vector<int> customProgStart = vector<int>(1, 0), customOp, customArg, customProg, customAtoms; vector<double> customImm, customParams;
+    int customStride = 0;
+    // the global parameters the expressions read: slot of every name (shared by all objects) and the value last sent
+    map<string, int> customGlobalSlot;
+    vector<double> customGlobals;
+    vector<double> packedCustomParams() const {
+        const size_t n = customProg.size();
+        vector<double> p(n*customStride);
+        for (size_t i = 0; i < n; i++)
+            for (int k = 0; k < customStride; k++) p[i*customStride + k] = customParams[i*B200MD_CUSTOM_MAX_PARAMS + k];
+        return p;
+    }
     map<string, string> props;
     // a box b200md_set_box refused (smaller than twice the cutoff): the reference raises that at the next force evaluation
     // (ReferenceKernels.cpp:983-985), not in setPeriodicBoxVectors; a later box that passes clears it
@@ -113,6 +130,13 @@ struct PlatformData {
         if (!torG.empty()) check(b200md_set_bonded_groups(ctx, 2, (int) torG.size(), torG.data()));
         if (!rbG.empty()) check(b200md_set_bonded_groups(ctx, 3, (int) rbG.size(), rbG.data()));
         if (!cmapG.empty()) check(b200md_set_bonded_groups(ctx, 4, (int) cmapG.size(), cmapG.data()));
+        if (!customProg.empty()) {
+            const vector<double> par = packedCustomParams();
+            check(b200md_set_custom_torsions(ctx, (int) customProgStart.size()/2, customProgStart.data(), customOp.data(), customArg.data(),
+                                             customImm.data(), customStride, (int) customProg.size(), customProg.data(), customAtoms.data(), par.data()));
+            check(b200md_set_bonded_groups(ctx, 5, (int) customG.size(), customG.data()));
+        }
+        if (!customGlobals.empty()) check(b200md_set_custom_globals(ctx, (int) customGlobals.size(), customGlobals.data()));
         check(b200md_finalize(ctx));
         finalized = true;
     }
@@ -577,6 +601,92 @@ private:
     size_t firstCoeff = 0;
 };
 
+// CustomTorsionForce: the expression becomes two instruction programs (custom_translate.h), which k_custom_torsion interprets.
+vector<string> perTorsionParameterNames(const CustomTorsionForce& force) {
+    vector<string> names;
+    for (int i = 0; i < force.getNumPerTorsionParameters(); i++) names.push_back(force.getPerTorsionParameterName(i));
+    return names;
+}
+vector<string> globalParameterNames(const CustomTorsionForce& force) {
+    vector<string> names;
+    for (int i = 0; i < force.getNumGlobalParameters(); i++) names.push_back(force.getGlobalParameterName(i));
+    return names;
+}
+
+class B200CalcCustomTorsionForceKernel : public CalcCustomTorsionForceKernel {
+public:
+    B200CalcCustomTorsionForceKernel(string name, const Platform& platform, ContextImpl& context) : CalcCustomTorsionForceKernel(name, platform), context(context) {}
+    void initialize(const System& system, const CustomTorsionForce& force) {
+        PlatformData& d = getData(context);
+        if (d.finalized) throw OpenMMException("B200 platform: CustomTorsionForce initialised after the Context was finalised");
+        b200md_custom::Program energy, deriv;
+        const vector<string> globals = globalParameterNames(force);
+        b200md_custom::translateExpression(force.getEnergyFunction(), perTorsionParameterNames(force), globals, d.customGlobalSlot, energy, deriv);
+        const int prog = (int) d.customProgStart.size()/2;
+        for (const b200md_custom::Program* p : {&energy, &deriv}) {
+            d.customOp.insert(d.customOp.end(), p->op.begin(), p->op.end());
+            d.customArg.insert(d.customArg.end(), p->arg.begin(), p->arg.end());
+            d.customImm.insert(d.customImm.end(), p->imm.begin(), p->imm.end());
+            d.customProgStart.push_back((int) d.customOp.size());
+        }
+        // the Context's parameter map does not exist yet (ContextImpl.cpp:120-131 fills it after the kernels are initialised):
+        // start from the defaults, execute() sends whatever differs
+        d.customGlobals.resize(d.customGlobalSlot.size(), 0.0);
+        for (int i = 0; i < force.getNumGlobalParameters(); i++) {
+            const map<string, int>::const_iterator it = d.customGlobalSlot.find(force.getGlobalParameterName(i));
+            if (it == d.customGlobalSlot.end()) continue;         // declared, but the expression does not read it
+            slots.push_back(make_pair(it->first, it->second));
+            d.customGlobals[it->second] = force.getGlobalParameterDefaultValue(i);
+        }
+        numParams = force.getNumPerTorsionParameters();
+        d.customStride = max(d.customStride, numParams);
+        first = (int) d.customProg.size(); count = force.getNumTorsions();
+        vector<double> par;
+        for (int i = 0; i < count; i++) {
+            int a, b, c, e;
+            force.getTorsionParameters(i, a, b, c, e, par);
+            d.customProg.push_back(prog);
+            for (int x : {a, b, c, e}) d.customAtoms.push_back(x);
+            par.resize(B200MD_CUSTOM_MAX_PARAMS, 0.0);
+            d.customParams.insert(d.customParams.end(), par.begin(), par.end());
+            d.customG.push_back(force.getForceGroup() | (force.usesPeriodicBoundaryConditions() ? 0x80 : 0));
+        }
+        d.systemTerms |= B200MD_TERM_CUSTOM_TORSIONS; d.bondedGroupsUsed |= 1u << force.getForceGroup();
+    }
+    double execute(ContextImpl& context, bool includeForces, bool includeEnergy) {
+        PlatformData& d = getData(context);
+        // a changed global value is a stream-ordered copy into the buffer the step graph reads (NonbondedForce offsets alike)
+        bool changed = false;
+        for (const pair<string, int>& s : slots) {
+            const double v = context.getParameter(s.first);
+            if (v != d.customGlobals[s.second]) { d.customGlobals[s.second] = v; changed = true; }
+        }
+        if (changed) d.check(b200md_set_custom_globals(d.ctx, (int) d.customGlobals.size(), d.customGlobals.data()));
+        d.pendingTerms |= B200MD_TERM_CUSTOM_TORSIONS;
+        return 0.0;
+    }
+    void copyParametersToContext(ContextImpl& context, const CustomTorsionForce& force) {
+        PlatformData& d = getData(context);
+        d.ensureFinalized();
+        d.dropForces();
+        if (force.getNumTorsions() != count) throw OpenMMException("updateParametersInContext: The number of torsions has changed");
+        vector<double> par;
+        for (int i = 0; i < count; i++) {
+            int a[4];
+            force.getTorsionParameters(i, a[0], a[1], a[2], a[3], par);
+            for (int k = 0; k < 4; k++)
+                if (a[k] != d.customAtoms[4*(size_t) (first+i) + k]) throw OpenMMException("updateParametersInContext: The set of particles in a torsion has changed");
+            for (int k = 0; k < numParams && k < (int) par.size(); k++) d.customParams[(size_t) (first+i)*B200MD_CUSTOM_MAX_PARAMS + k] = par[k];
+        }
+        const vector<double> packed = d.packedCustomParams();
+        d.check(b200md_update_custom_torsion_params(d.ctx, (int) d.customProg.size(), packed.data()));
+    }
+private:
+    ContextImpl& context;
+    int first = 0, count = 0, numParams = 0;
+    vector<pair<string, int> > slots;     // the global parameters this object's expression reads, and their slots
+};
+
 // RemoveCMMotionKernel::execute is called by CMMotionRemoverImpl::updateContextState in EVERY step; the frequency test is
 // the kernel's (ReferenceKernels.cpp:2712-2714).  The removal itself is deferred to the integrator step that follows (the
 // fused step graph removes the centre-of-mass motion itself) or to the next read of the velocities (PlatformData::flushCm).
@@ -704,6 +814,7 @@ public:
         if (name == CalcPeriodicTorsionForceKernel::Name()) return new B200CalcPeriodicTorsionForceKernel(name, platform, context);
         if (name == CalcRBTorsionForceKernel::Name()) return new B200CalcRBTorsionForceKernel(name, platform, context);
         if (name == CalcCMAPTorsionForceKernel::Name()) return new B200CalcCMAPTorsionForceKernel(name, platform, context);
+        if (name == CalcCustomTorsionForceKernel::Name()) return new B200CalcCustomTorsionForceKernel(name, platform, context);
         if (name == RemoveCMMotionKernel::Name()) return new B200RemoveCMMotionKernel(name, platform, context);
         if (name == IntegrateVerletStepKernel::Name()) return new B200IntegrateVerletStepKernel(name, platform);
         if (name == IntegrateLangevinStepKernel::Name()) return new B200IntegrateLangevinStepKernel(name, platform);
@@ -720,7 +831,7 @@ public:
         for (const string& n : {CalcForcesAndEnergyKernel::Name(), UpdateStateDataKernel::Name(), ApplyConstraintsKernel::Name(), VirtualSitesKernel::Name(),
                                 CalcNonbondedForceKernel::Name(), CalcHarmonicBondForceKernel::Name(), CalcHarmonicAngleForceKernel::Name(),
                                 CalcPeriodicTorsionForceKernel::Name(), CalcRBTorsionForceKernel::Name(), CalcCMAPTorsionForceKernel::Name(),
-                                RemoveCMMotionKernel::Name(), IntegrateVerletStepKernel::Name(),
+                                CalcCustomTorsionForceKernel::Name(), RemoveCMMotionKernel::Name(), IntegrateVerletStepKernel::Name(),
                                 IntegrateLangevinStepKernel::Name(), IntegrateLangevinMiddleStepKernel::Name(), ApplyMonteCarloBarostatKernel::Name()})
             registerKernelFactory(n, factory);
         platformProperties.push_back(DeviceIndex());
@@ -762,6 +873,17 @@ public:
             }
             if (force.getForceGroup() < 0 || force.getForceGroup() > 31) throw OpenMMException("B200 platform: force group out of range");
             if (dynamic_cast<const MonteCarloMembraneBarostat*>(&force)) throw OpenMMException("B200 platform: MonteCarloMembraneBarostat is not supported");
+            if (const CustomTorsionForce* ct = dynamic_cast<const CustomTorsionForce*>(&force)) {
+                // getEnergyParameterDerivatives returns nothing here
+                if (ct->getNumEnergyParameterDerivatives() > 0) throw OpenMMException("B200 platform: energy parameter derivatives of a CustomTorsionForce are not supported");
+                // beyond the interpreter's limits: refused here; an unknown variable is an error on every platform and is
+                // raised by the kernel's initialize, as the Reference platform does
+                map<string, int> slots;
+                b200md_custom::Program e, de;
+                try { b200md_custom::translateExpression(ct->getEnergyFunction(), perTorsionParameterNames(*ct), globalParameterNames(*ct), slots, e, de); }
+                catch (const b200md_custom::Unsupported&) { throw; }
+                catch (const OpenMMException&) {}
+            }
         }
         const int nc = system.getNumConstraints();
         if (nc > 0) {
