@@ -465,9 +465,11 @@ extern "C" int b200md_custom_program_probe(int nprog, const int* prog_start, con
 extern "C" int b200md_set_bonded_groups(b200md_ctx* ctx, int kind, int n, const int* group) {
     API_BEGIN(ctx)
     check_set(ctx, "set_bonded_groups", n);
-    require(kind >= 0 && kind <= 5, "set_bonded_groups: kind must be 0 (bonds), 1 (angles), 2 (torsions), 3 (RB torsions), 4 (CMAP) or 5 (custom torsions)");
-    std::vector<unsigned char>& g = kind == 0 ? ctx->bonds.group : kind == 1 ? ctx->angles.group : kind == 2 ? ctx->torsions.group :
-                                    kind == 3 ? ctx->rb.group : kind == 4 ? ctx->cmap.group : ctx->custom.group;
+    require(kind >= B200MD_BONDED_BONDS && kind <= B200MD_BONDED_CUSTOM_TORSIONS,
+            "set_bonded_groups: kind must be 0 (bonds), 1 (angles), 2 (torsions), 3 (RB torsions), 4 (CMAP) or 5 (custom torsions)");
+    std::vector<unsigned char>& g = kind == B200MD_BONDED_BONDS ? ctx->bonds.group : kind == B200MD_BONDED_ANGLES ? ctx->angles.group :
+                                    kind == B200MD_BONDED_TORSIONS ? ctx->torsions.group : kind == B200MD_BONDED_RB_TORSIONS ? ctx->rb.group :
+                                    kind == B200MD_BONDED_CMAP ? ctx->cmap.group : ctx->custom.group;
     g.resize(n);
     for (int i = 0; i < n; i++) { require(group[i] >= 0 && (group[i] & ~0x80) < 32, "force group out of range"); g[i] = (unsigned char) group[i]; }
     API_END(ctx)
@@ -1452,22 +1454,22 @@ extern "C" int b200md_update_nonbonded_params(b200md_ctx* ctx, const double* q, 
 }
 
 // Calc{HarmonicBond,HarmonicAngle,PeriodicTorsion}ForceKernel::copyParametersToContext (kernels.h:305,375,445):
-// same topology, new parameters.  kind: 0 bonds (a=length,b=k), 1 angles (a=angle,b=k), 2 torsions (a=phase,b=k,per)
+// same topology, new parameters.  kind: B200MD_BONDED_BONDS (a=length,b=k), _ANGLES (a=angle,b=k), _TORSIONS (a=phase,b=k,per)
 extern "C" int b200md_update_bonded_params(b200md_ctx* ctx, int kind, int n, const double* a, const double* b, const int* periodicity) {
     API_BEGIN(ctx)
     require(ctx->finalized, "update_bonded_params before finalize");
     CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-    if (kind == 0) {
+    if (kind == B200MD_BONDED_BONDS) {
         require(n == ctx->bonds.n, "the number of bonds cannot change");
         for (int i = 0; i < n; i++) ctx->bonds.params[i] = make_double2(a[i], b[i]);
         ctx->bonds.paramsDev.upload(ctx->bonds.params);
     }
-    else if (kind == 1) {
+    else if (kind == B200MD_BONDED_ANGLES) {
         require(n == ctx->angles.n, "the number of angles cannot change");
         for (int i = 0; i < n; i++) ctx->angles.params[i] = make_double2(a[i], b[i]);
         ctx->angles.paramsDev.upload(ctx->angles.params);
     }
-    else if (kind == 2) {
+    else if (kind == B200MD_BONDED_TORSIONS) {
         require(n == ctx->torsions.n, "the number of torsions cannot change");
         for (int i = 0; i < n; i++) ctx->torsions.params[i] = make_double4(b[i], a[i], (double) periodicity[i], 0);
         ctx->torsions.paramsDev.upload(ctx->torsions.params);

@@ -15,6 +15,11 @@
 // makes Platform::supportsKernels() false; an unsupported OPTION of a supported class is rejected in contextCreated()
 // (validateSystem), which is the only place from which ContextImpl falls back to the next platform (ContextImpl.cpp:152-166).
 //
+// Bonded classes.  Each keeps the terms of all its Force objects in one TermRecord of PlatformData, sent at finalize; what
+// their kernels share (ObjectTerms: the object's range of the record, group tags, updates) exists once.  Bond, angle,
+// periodic-torsion and RB-torsion kernels are one template, B200CalcBondedForceKernel; CMAP and custom torsions keep
+// their own kernels for their maps and expression programs.
+//
 // The hot loop.  Integrator::step(n) of the reference is, per step, updateContextState() -> calcForcesAndEnergy(true,
 // false, groups) -> Integrate*StepKernel::execute (LangevinIntegrator.cpp:74-82).  Here a forces-only evaluation is
 // LAZY: finishComputation records what was asked for and returns; when the integrator kernel's execute() follows and the
@@ -66,6 +71,71 @@ int fftFriendly(int n) {
     }
 }
 
+// The terms of one bonded class over all its Force objects, as the arrays its b200md_set_* call takes: one column per
+// array, each holding the same number of entries for every term (bonds: atoms p1, p2 and parameters length, k; CMAP: one
+// atom column of 8 per term).  ints are the integer parameters: torsion periodicity, CMAP map, custom-torsion program.
+struct TermRecord {
+    int kind;                       // B200MD_BONDED_*
+    vector<vector<int> > atoms, ints;
+    vector<vector<double> > params;
+    vector<int> group;              // the force group of the term's Force, | 0x80 if it uses periodic boundary conditions
+    TermRecord(int kind, int numAtoms, int numInts, int numParams) : kind(kind), atoms(numAtoms), ints(numInts), params(numParams) {}
+    int size() const { return (int) group.size(); }
+    // appends one term, each list split evenly over its columns
+    void add(const vector<int>& a, const vector<int>& n, const vector<double>& p) { split(a, atoms); split(n, ints); split(p, params); }
+    template<class T> static void split(const vector<T>& v, vector<vector<T> >& columns) {
+        const size_t w = columns.empty() ? 0 : v.size()/columns.size();
+        for (size_t c = 0; c < columns.size(); c++) columns[c].insert(columns[c].end(), v.begin() + c*w, v.begin() + (c+1)*w);
+    }
+};
+
+// What the bond, angle, periodic-torsion and RB-torsion kernels differ in (B200CalcBondedForceKernel below): the Force,
+// the term bit, the names in messages, how term i is read into the record, and the calls that send the record.
+struct Bonds {
+    typedef HarmonicBondForce Force; typedef CalcHarmonicBondForceKernel Kernel;
+    enum { bit = B200MD_TERM_BONDS };
+    static constexpr const char* name = "HarmonicBondForce", *terms = "bonds", *aTerm = "a bond";
+    static int count(const Force& f) { return f.getNumBonds(); }
+    static void read(const Force& f, int i, TermRecord& r) { int a, b; double r0, k; f.getBondParameters(i, a, b, r0, k); r.add({a, b}, {}, {r0, k}); }
+    static int set(b200md_ctx* c, const TermRecord& r) { return b200md_set_bonds(c, r.size(), r.atoms[0].data(), r.atoms[1].data(), r.params[0].data(), r.params[1].data()); }
+    static int update(b200md_ctx* c, const TermRecord& r) { return b200md_update_bonded_params(c, r.kind, r.size(), r.params[0].data(), r.params[1].data(), nullptr); }
+};
+struct Angles {
+    typedef HarmonicAngleForce Force; typedef CalcHarmonicAngleForceKernel Kernel;
+    enum { bit = B200MD_TERM_ANGLES };
+    static constexpr const char* name = "HarmonicAngleForce", *terms = "angles", *aTerm = "an angle";
+    static int count(const Force& f) { return f.getNumAngles(); }
+    static void read(const Force& f, int i, TermRecord& r) { int a, b, c; double t0, k; f.getAngleParameters(i, a, b, c, t0, k); r.add({a, b, c}, {}, {t0, k}); }
+    static int set(b200md_ctx* c, const TermRecord& r) {
+        return b200md_set_angles(c, r.size(), r.atoms[0].data(), r.atoms[1].data(), r.atoms[2].data(), r.params[0].data(), r.params[1].data());
+    }
+    static int update(b200md_ctx* c, const TermRecord& r) { return b200md_update_bonded_params(c, r.kind, r.size(), r.params[0].data(), r.params[1].data(), nullptr); }
+};
+struct Torsions {
+    typedef PeriodicTorsionForce Force; typedef CalcPeriodicTorsionForceKernel Kernel;
+    enum { bit = B200MD_TERM_TORSIONS };
+    static constexpr const char* name = "PeriodicTorsionForce", *terms = "torsions", *aTerm = "a torsion";
+    static int count(const Force& f) { return f.getNumTorsions(); }
+    static void read(const Force& f, int i, TermRecord& r) { int a, b, c, e, n; double ph, k; f.getTorsionParameters(i, a, b, c, e, n, ph, k); r.add({a, b, c, e}, {n}, {ph, k}); }
+    static int set(b200md_ctx* c, const TermRecord& r) {
+        return b200md_set_torsions(c, r.size(), r.atoms[0].data(), r.atoms[1].data(), r.atoms[2].data(), r.atoms[3].data(), r.ints[0].data(), r.params[0].data(), r.params[1].data());
+    }
+    static int update(b200md_ctx* c, const TermRecord& r) { return b200md_update_bonded_params(c, r.kind, r.size(), r.params[0].data(), r.params[1].data(), r.ints[0].data()); }
+};
+struct RBTorsions {
+    typedef RBTorsionForce Force; typedef CalcRBTorsionForceKernel Kernel;
+    enum { bit = B200MD_TERM_RB_TORSIONS };
+    static constexpr const char* name = "RBTorsionForce", *terms = "torsions", *aTerm = "a torsion";
+    static int count(const Force& f) { return f.getNumTorsions(); }
+    static void read(const Force& f, int i, TermRecord& r) {
+        int a, b, c, e; double c0, c1, c2, c3, c4, c5;
+        f.getTorsionParameters(i, a, b, c, e, c0, c1, c2, c3, c4, c5);
+        r.add({a, b, c, e}, {}, {c0, c1, c2, c3, c4, c5});
+    }
+    static int set(b200md_ctx* c, const TermRecord& r) { return b200md_set_rb_torsions(c, r.size(), r.atoms[0].data(), r.atoms[1].data(), r.atoms[2].data(), r.atoms[3].data(), r.params[0].data()); }
+    static int update(b200md_ctx* c, const TermRecord& r) { return b200md_update_rb_torsion_params(c, r.size(), r.params[0].data()); }
+};
+
 // per-Context state (ContextImpl::setPlatformData)
 struct PlatformData {
     b200md_ctx* ctx = nullptr;
@@ -82,27 +152,24 @@ struct PlatformData {
     int cmFrequency = 0;
     bool cmRequested = false;       // RemoveCMMotionKernel::execute seen since the last integrator step
     bool useFusedStep = true;       // B200MD_PLUGIN_FUSED=0: always compute + integrate_only (debugging)
-    vector<int> bondG, angG, torG, rbG, cmapG, customG;  // force group of every bonded element
-    // bonded terms are gathered over all force objects of a kind and sent at finalize
-    vector<int> bondI, bondJ; vector<double> bondR0, bondK;
-    vector<int> angI, angJ, angK; vector<double> angT0, angKK;
-    vector<int> torI, torJ, torK, torL, torN; vector<double> torPhase, torKK;
-    vector<int> rbI, rbJ, rbK, rbL; vector<double> rbC;                     // rbC [n][6]
+    // the bonded terms of every Force object, one record per class (columns: atoms, integer parameters, parameters), sent at finalize
+    TermRecord bonds{B200MD_BONDED_BONDS, 2, 0, 2}, angles{B200MD_BONDED_ANGLES, 3, 0, 2}, torsions{B200MD_BONDED_TORSIONS, 4, 1, 2},
+               rb{B200MD_BONDED_RB_TORSIONS, 4, 0, 1}, cmap{B200MD_BONDED_CMAP, 1, 1, 0}, custom{B200MD_BONDED_CUSTOM_TORSIONS, 1, 1, 1};
     // CMAP: the maps of all objects one after the other (a term's map index counts from the first map of all objects);
     // coefficients from CMAPTorsionForceImpl::calcMapDerivatives, [sum size^2][16]
-    vector<int> cmapSize, cmapMap, cmapAtoms; vector<double> cmapCoeff;
+    vector<int> cmapSize; vector<double> cmapCoeff;
     // custom torsions: the programs of all objects one after the other (object f's expression is the pair 2f, 2f+1); the
-    // parameters of every term padded to B200MD_CUSTOM_MAX_PARAMS here, packed to the widest object's count when sent
-    vector<int> customProgStart = vector<int>(1, 0), customOp, customArg, customProg, customAtoms; vector<double> customImm, customParams;
+    // parameters of every term padded to B200MD_CUSTOM_MAX_PARAMS in the record, packed to the widest object's count when sent
+    vector<int> customProgStart = vector<int>(1, 0), customOp, customArg; vector<double> customImm;
     int customStride = 0;
     // the global parameters the expressions read: slot of every name (shared by all objects) and the value last sent
     map<string, int> customGlobalSlot;
     vector<double> customGlobals;
     vector<double> packedCustomParams() const {
-        const size_t n = customProg.size();
+        const size_t n = custom.size();
         vector<double> p(n*customStride);
         for (size_t i = 0; i < n; i++)
-            for (int k = 0; k < customStride; k++) p[i*customStride + k] = customParams[i*B200MD_CUSTOM_MAX_PARAMS + k];
+            for (int k = 0; k < customStride; k++) p[i*customStride + k] = custom.params[0][i*B200MD_CUSTOM_MAX_PARAMS + k];
         return p;
     }
     map<string, string> props;
@@ -120,21 +187,18 @@ struct PlatformData {
     }
     void ensureFinalized() {
         if (finalized) return;
-        if (!bondI.empty()) check(b200md_set_bonds(ctx, (int) bondI.size(), bondI.data(), bondJ.data(), bondR0.data(), bondK.data()));
-        if (!angI.empty()) check(b200md_set_angles(ctx, (int) angI.size(), angI.data(), angJ.data(), angK.data(), angT0.data(), angKK.data()));
-        if (!torI.empty()) check(b200md_set_torsions(ctx, (int) torI.size(), torI.data(), torJ.data(), torK.data(), torL.data(), torN.data(), torPhase.data(), torKK.data()));
-        if (!rbI.empty()) check(b200md_set_rb_torsions(ctx, (int) rbI.size(), rbI.data(), rbJ.data(), rbK.data(), rbL.data(), rbC.data()));
-        if (!cmapMap.empty()) check(b200md_set_cmap(ctx, (int) cmapSize.size(), cmapSize.data(), cmapCoeff.data(), (int) cmapMap.size(), cmapMap.data(), cmapAtoms.data()));
-        if (!bondG.empty()) check(b200md_set_bonded_groups(ctx, 0, (int) bondG.size(), bondG.data()));
-        if (!angG.empty()) check(b200md_set_bonded_groups(ctx, 1, (int) angG.size(), angG.data()));
-        if (!torG.empty()) check(b200md_set_bonded_groups(ctx, 2, (int) torG.size(), torG.data()));
-        if (!rbG.empty()) check(b200md_set_bonded_groups(ctx, 3, (int) rbG.size(), rbG.data()));
-        if (!cmapG.empty()) check(b200md_set_bonded_groups(ctx, 4, (int) cmapG.size(), cmapG.data()));
-        if (!customProg.empty()) {
+        if (bonds.size()) check(Bonds::set(ctx, bonds));
+        if (angles.size()) check(Angles::set(ctx, angles));
+        if (torsions.size()) check(Torsions::set(ctx, torsions));
+        if (rb.size()) check(RBTorsions::set(ctx, rb));
+        if (cmap.size()) check(b200md_set_cmap(ctx, (int) cmapSize.size(), cmapSize.data(), cmapCoeff.data(), cmap.size(), cmap.ints[0].data(), cmap.atoms[0].data()));
+        for (const TermRecord* r : {&bonds, &angles, &torsions, &rb, &cmap})
+            if (r->size()) check(b200md_set_bonded_groups(ctx, r->kind, r->size(), r->group.data()));
+        if (custom.size()) {
             const vector<double> par = packedCustomParams();
             check(b200md_set_custom_torsions(ctx, (int) customProgStart.size()/2, customProgStart.data(), customOp.data(), customArg.data(),
-                                             customImm.data(), customStride, (int) customProg.size(), customProg.data(), customAtoms.data(), par.data()));
-            check(b200md_set_bonded_groups(ctx, 5, (int) customG.size(), customG.data()));
+                                             customImm.data(), customStride, custom.size(), custom.ints[0].data(), custom.atoms[0].data(), par.data()));
+            check(b200md_set_bonded_groups(ctx, custom.kind, custom.size(), custom.group.data()));
         }
         if (!customGlobals.empty()) check(b200md_set_custom_globals(ctx, (int) customGlobals.size(), customGlobals.data()));
         check(b200md_finalize(ctx));
@@ -406,142 +470,66 @@ private:
 };
 
 // Bonded forces: any number of Force objects per class.  Every object appends its terms (tagged with its force group) to
-// the per-Context arrays; the engine evaluates a term iff its class was executed in this evaluation AND its group is in
+// its class's TermRecord; the engine evaluates a term iff its class was executed in this evaluation AND its group is in
 // the `groups` mask of finishComputation (ForceImpl::calcForcesAndEnergy only calls execute for objects whose group is in it).
-class B200CalcHarmonicBondForceKernel : public CalcHarmonicBondForceKernel {
-public:
-    B200CalcHarmonicBondForceKernel(string name, const Platform& platform, ContextImpl& context) : CalcHarmonicBondForceKernel(name, platform), context(context) {}
-    void initialize(const System& system, const HarmonicBondForce& force) {
-        PlatformData& d = getData(context);
-        if (d.finalized) throw OpenMMException("B200 platform: HarmonicBondForce initialised after the Context was finalised");
-        first = (int) d.bondI.size(); count = force.getNumBonds();
-        for (int i = 0; i < count; i++) {
-            int a, b; double r0, k;
-            force.getBondParameters(i, a, b, r0, k);
-            d.bondI.push_back(a); d.bondJ.push_back(b); d.bondR0.push_back(r0); d.bondK.push_back(k); d.bondG.push_back(force.getForceGroup() | (force.usesPeriodicBoundaryConditions() ? 0x80 : 0));
-        }
-        d.systemTerms |= B200MD_TERM_BONDS; d.bondedGroupsUsed |= 1u << force.getForceGroup();
+// ObjectTerms is what every bonded kernel shares: this object's terms are [first, first+count) of the record.  read(i, r)
+// appends term i of the object to r; the same reader fills the record at initialize and re-reads the object on update.
+class ObjectTerms {
+protected:
+    int first = 0, count = 0;
+    template<class Read> void add(PlatformData& d, TermRecord& r, const Force& force, int numTerms, int bit, const char* name, Read read) {
+        if (d.finalized) throw OpenMMException(string("B200 platform: ") + name + " initialised after the Context was finalised");
+        first = r.size(); count = numTerms;
+        for (int i = 0; i < count; i++) read(i, r);
+        r.group.resize(first + count, force.getForceGroup() | (force.usesPeriodicBoundaryConditions() ? 0x80 : 0));
+        d.systemTerms |= bit; d.bondedGroupsUsed |= 1u << force.getForceGroup();
     }
-    double execute(ContextImpl& context, bool includeForces, bool includeEnergy) { getData(context).pendingTerms |= B200MD_TERM_BONDS; return 0.0; }
-    void copyParametersToContext(ContextImpl& context, const HarmonicBondForce& force) {
-        PlatformData& d = getData(context);
+    // copyParametersToContext: the object read again, refused if the number of its terms or the atoms of one changed
+    template<class Read> TermRecord reread(PlatformData& d, const TermRecord& r, int numTerms, const char* terms, const char* aTerm, Read read) const {
         d.ensureFinalized();
         d.dropForces();
-        if (force.getNumBonds() != count) throw OpenMMException("updateParametersInContext: The number of bonds has changed");
-        for (int i = 0; i < count; i++) {
-            int p, q;
-            force.getBondParameters(i, p, q, d.bondR0[first+i], d.bondK[first+i]);
-            if (p != d.bondI[first+i] || q != d.bondJ[first+i]) throw OpenMMException("updateParametersInContext: The set of particles in a bond has changed");
-        }
-        d.check(b200md_update_bonded_params(d.ctx, 0, (int) d.bondI.size(), d.bondR0.data(), d.bondK.data(), nullptr));
+        if (numTerms != count) throw OpenMMException(string("updateParametersInContext: The number of ") + terms + " has changed");
+        TermRecord fresh(r.kind, r.atoms.size(), r.ints.size(), r.params.size());
+        for (int i = 0; i < count; i++) read(i, fresh);
+        for (size_t c = 0; c < r.atoms.size(); c++)
+            if (!equal(fresh.atoms[c].begin(), fresh.atoms[c].end(), start(r.atoms[c], r)))
+                throw OpenMMException(string("updateParametersInContext: The set of particles in ") + aTerm + " has changed");
+        return fresh;
+    }
+    // the parameters of `fresh` (reread) into [first, first+count)
+    void store(TermRecord& r, const TermRecord& fresh) const {
+        for (size_t c = 0; c < r.ints.size(); c++) copy(fresh.ints[c].begin(), fresh.ints[c].end(), start(r.ints[c], r));
+        for (size_t c = 0; c < r.params.size(); c++) copy(fresh.params[c].begin(), fresh.params[c].end(), start(r.params[c], r));
     }
 private:
-    ContextImpl& context;
-    int first = 0, count = 0;
+    // where this object's terms start in a column of r
+    template<class V> auto start(V& column, const TermRecord& r) const -> decltype(column.begin()) {
+        return column.begin() + (count ? column.size()/r.size()*first : 0);
+    }
 };
 
-class B200CalcHarmonicAngleForceKernel : public CalcHarmonicAngleForceKernel {
+// HarmonicBondForce, HarmonicAngleForce, PeriodicTorsionForce and RBTorsionForce (T: Bonds, Angles, Torsions, RBTorsions)
+template<class T, TermRecord PlatformData::* record>
+class B200CalcBondedForceKernel : public T::Kernel, ObjectTerms {
 public:
-    B200CalcHarmonicAngleForceKernel(string name, const Platform& platform, ContextImpl& context) : CalcHarmonicAngleForceKernel(name, platform), context(context) {}
-    void initialize(const System& system, const HarmonicAngleForce& force) {
+    B200CalcBondedForceKernel(string name, const Platform& platform, ContextImpl& context) : T::Kernel(name, platform), context(context) {}
+    void initialize(const System& system, const typename T::Force& force) {
         PlatformData& d = getData(context);
-        if (d.finalized) throw OpenMMException("B200 platform: HarmonicAngleForce initialised after the Context was finalised");
-        first = (int) d.angI.size(); count = force.getNumAngles();
-        for (int i = 0; i < count; i++) {
-            int a, b, c; double t0, k;
-            force.getAngleParameters(i, a, b, c, t0, k);
-            d.angI.push_back(a); d.angJ.push_back(b); d.angK.push_back(c); d.angT0.push_back(t0); d.angKK.push_back(k); d.angG.push_back(force.getForceGroup() | (force.usesPeriodicBoundaryConditions() ? 0x80 : 0));
-        }
-        d.systemTerms |= B200MD_TERM_ANGLES; d.bondedGroupsUsed |= 1u << force.getForceGroup();
+        add(d, d.*record, force, T::count(force), T::bit, T::name, [&](int i, TermRecord& r) { T::read(force, i, r); });
     }
-    double execute(ContextImpl& context, bool includeForces, bool includeEnergy) { getData(context).pendingTerms |= B200MD_TERM_ANGLES; return 0.0; }
-    void copyParametersToContext(ContextImpl& context, const HarmonicAngleForce& force) {
+    double execute(ContextImpl& context, bool includeForces, bool includeEnergy) { getData(context).pendingTerms |= T::bit; return 0.0; }
+    void copyParametersToContext(ContextImpl& context, const typename T::Force& force) {
         PlatformData& d = getData(context);
-        d.ensureFinalized();
-        d.dropForces();
-        if (force.getNumAngles() != count) throw OpenMMException("updateParametersInContext: The number of angles has changed");
-        for (int i = 0; i < count; i++) {
-            int p, q, r;
-            force.getAngleParameters(i, p, q, r, d.angT0[first+i], d.angKK[first+i]);
-            if (p != d.angI[first+i] || q != d.angJ[first+i] || r != d.angK[first+i]) throw OpenMMException("updateParametersInContext: The set of particles in an angle has changed");
-        }
-        d.check(b200md_update_bonded_params(d.ctx, 1, (int) d.angI.size(), d.angT0.data(), d.angKK.data(), nullptr));
+        TermRecord& r = d.*record;
+        store(r, reread(d, r, T::count(force), T::terms, T::aTerm, [&](int i, TermRecord& f) { T::read(force, i, f); }));
+        d.check(T::update(d.ctx, r));
     }
 private:
     ContextImpl& context;
-    int first = 0, count = 0;
-};
-
-class B200CalcPeriodicTorsionForceKernel : public CalcPeriodicTorsionForceKernel {
-public:
-    B200CalcPeriodicTorsionForceKernel(string name, const Platform& platform, ContextImpl& context) : CalcPeriodicTorsionForceKernel(name, platform), context(context) {}
-    void initialize(const System& system, const PeriodicTorsionForce& force) {
-        PlatformData& d = getData(context);
-        if (d.finalized) throw OpenMMException("B200 platform: PeriodicTorsionForce initialised after the Context was finalised");
-        first = (int) d.torI.size(); count = force.getNumTorsions();
-        for (int i = 0; i < count; i++) {
-            int a, b, c, e, n; double phase, k;
-            force.getTorsionParameters(i, a, b, c, e, n, phase, k);
-            d.torI.push_back(a); d.torJ.push_back(b); d.torK.push_back(c); d.torL.push_back(e); d.torN.push_back(n); d.torPhase.push_back(phase); d.torKK.push_back(k);
-            d.torG.push_back(force.getForceGroup() | (force.usesPeriodicBoundaryConditions() ? 0x80 : 0));
-        }
-        d.systemTerms |= B200MD_TERM_TORSIONS; d.bondedGroupsUsed |= 1u << force.getForceGroup();
-    }
-    double execute(ContextImpl& context, bool includeForces, bool includeEnergy) { getData(context).pendingTerms |= B200MD_TERM_TORSIONS; return 0.0; }
-    void copyParametersToContext(ContextImpl& context, const PeriodicTorsionForce& force) {
-        PlatformData& d = getData(context);
-        d.ensureFinalized();
-        d.dropForces();
-        if (force.getNumTorsions() != count) throw OpenMMException("updateParametersInContext: The number of torsions has changed");
-        for (int i = 0; i < count; i++) {
-            int p, q, r, t;
-            force.getTorsionParameters(i, p, q, r, t, d.torN[first+i], d.torPhase[first+i], d.torKK[first+i]);
-            if (p != d.torI[first+i] || q != d.torJ[first+i] || r != d.torK[first+i] || t != d.torL[first+i]) throw OpenMMException("updateParametersInContext: The set of particles in a torsion has changed");
-        }
-        d.check(b200md_update_bonded_params(d.ctx, 2, (int) d.torI.size(), d.torPhase.data(), d.torKK.data(), d.torN.data()));
-    }
-private:
-    ContextImpl& context;
-    int first = 0, count = 0;
-};
-
-class B200CalcRBTorsionForceKernel : public CalcRBTorsionForceKernel {
-public:
-    B200CalcRBTorsionForceKernel(string name, const Platform& platform, ContextImpl& context) : CalcRBTorsionForceKernel(name, platform), context(context) {}
-    void initialize(const System& system, const RBTorsionForce& force) {
-        PlatformData& d = getData(context);
-        if (d.finalized) throw OpenMMException("B200 platform: RBTorsionForce initialised after the Context was finalised");
-        first = (int) d.rbI.size(); count = force.getNumTorsions();
-        for (int i = 0; i < count; i++) {
-            int a, b, c, e; double c0, c1, c2, c3, c4, c5;
-            force.getTorsionParameters(i, a, b, c, e, c0, c1, c2, c3, c4, c5);
-            d.rbI.push_back(a); d.rbJ.push_back(b); d.rbK.push_back(c); d.rbL.push_back(e);
-            for (double x : {c0, c1, c2, c3, c4, c5}) d.rbC.push_back(x);
-            d.rbG.push_back(force.getForceGroup() | (force.usesPeriodicBoundaryConditions() ? 0x80 : 0));
-        }
-        d.systemTerms |= B200MD_TERM_RB_TORSIONS; d.bondedGroupsUsed |= 1u << force.getForceGroup();
-    }
-    double execute(ContextImpl& context, bool includeForces, bool includeEnergy) { getData(context).pendingTerms |= B200MD_TERM_RB_TORSIONS; return 0.0; }
-    void copyParametersToContext(ContextImpl& context, const RBTorsionForce& force) {
-        PlatformData& d = getData(context);
-        d.ensureFinalized();
-        d.dropForces();
-        if (force.getNumTorsions() != count) throw OpenMMException("updateParametersInContext: The number of torsions has changed");
-        for (int i = 0; i < count; i++) {
-            int p, q, r, t;
-            double* c = &d.rbC[6*(size_t) (first+i)];
-            force.getTorsionParameters(i, p, q, r, t, c[0], c[1], c[2], c[3], c[4], c[5]);
-            if (p != d.rbI[first+i] || q != d.rbJ[first+i] || r != d.rbK[first+i] || t != d.rbL[first+i]) throw OpenMMException("updateParametersInContext: The set of particles in a torsion has changed");
-        }
-        d.check(b200md_update_rb_torsion_params(d.ctx, (int) d.rbI.size(), d.rbC.data()));
-    }
-private:
-    ContextImpl& context;
-    int first = 0, count = 0;
 };
 
 // The library takes spline coefficients: the reference's own platform-independent fitter makes them (call, don't rewrite).
-class B200CalcCMAPTorsionForceKernel : public CalcCMAPTorsionForceKernel {
+class B200CalcCMAPTorsionForceKernel : public CalcCMAPTorsionForceKernel, ObjectTerms {
 public:
     B200CalcCMAPTorsionForceKernel(string name, const Platform& platform, ContextImpl& context) : CalcCMAPTorsionForceKernel(name, platform), context(context) {}
     // the coefficients of the maps of `force`, appended to coeff; their sizes appended to size
@@ -556,48 +544,37 @@ public:
             for (const vector<double>& patch : c) coeff.insert(coeff.end(), patch.begin(), patch.end());
         }
     }
+    void read(const CMAPTorsionForce& force, int i, TermRecord& r) const {
+        int m, a[8];
+        force.getTorsionParameters(i, m, a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7]);
+        r.add(vector<int>(a, a + 8), {firstMap + m}, {});
+    }
     void initialize(const System& system, const CMAPTorsionForce& force) {
         PlatformData& d = getData(context);
-        if (d.finalized) throw OpenMMException("B200 platform: CMAPTorsionForce initialised after the Context was finalised");
         firstMap = (int) d.cmapSize.size(); numMaps = force.getNumMaps();
         firstCoeff = d.cmapCoeff.size();
+        add(d, d.cmap, force, force.getNumTorsions(), B200MD_TERM_CMAP, "CMAPTorsionForce", [&](int i, TermRecord& r) { read(force, i, r); });
         readMaps(force, d.cmapSize, d.cmapCoeff);
-        first = (int) d.cmapMap.size(); count = force.getNumTorsions();
-        for (int i = 0; i < count; i++) {
-            int m, a[8];
-            force.getTorsionParameters(i, m, a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7]);
-            d.cmapMap.push_back(firstMap + m);
-            d.cmapAtoms.insert(d.cmapAtoms.end(), a, a + 8);
-            d.cmapG.push_back(force.getForceGroup() | (force.usesPeriodicBoundaryConditions() ? 0x80 : 0));
-        }
-        d.systemTerms |= B200MD_TERM_CMAP; d.bondedGroupsUsed |= 1u << force.getForceGroup();
     }
     double execute(ContextImpl& context, bool includeForces, bool includeEnergy) { getData(context).pendingTerms |= B200MD_TERM_CMAP; return 0.0; }
     void copyParametersToContext(ContextImpl& context, const CMAPTorsionForce& force) {
         PlatformData& d = getData(context);
-        d.ensureFinalized();
-        d.dropForces();
         if (force.getNumMaps() != numMaps) throw OpenMMException("updateParametersInContext: The number of maps has changed");
-        if (force.getNumTorsions() != count) throw OpenMMException("updateParametersInContext: The number of CMAP torsions has changed");
+        const TermRecord fresh = reread(d, d.cmap, force.getNumTorsions(), "CMAP torsions", "a CMAP torsion", [&](int i, TermRecord& r) { read(force, i, r); });
         vector<int> size;
         vector<double> coeff;
         readMaps(force, size, coeff);
         for (int m = 0; m < numMaps; m++)
             if (size[m] != d.cmapSize[firstMap+m]) throw OpenMMException("updateParametersInContext: The size of a map has changed");
-        for (int i = 0; i < count; i++) {
-            int m, a[8];
-            force.getTorsionParameters(i, m, a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7]);
-            for (int k = 0; k < 8; k++)
-                if (a[k] != d.cmapAtoms[8*(size_t) (first+i) + k]) throw OpenMMException("updateParametersInContext: The set of particles in a CMAP torsion has changed");
-            if (m < 0 || m >= numMaps) throw OpenMMException("updateParametersInContext: CMAP torsion map index out of range");
-            d.cmapMap[first+i] = firstMap + m;
-        }
+        for (int m : fresh.ints[0])
+            if (m < firstMap || m >= firstMap + numMaps) throw OpenMMException("updateParametersInContext: CMAP torsion map index out of range");
+        store(d.cmap, fresh);
         copy(coeff.begin(), coeff.end(), d.cmapCoeff.begin() + firstCoeff);
-        d.check(b200md_update_cmap_params(d.ctx, (int) d.cmapSize.size(), d.cmapSize.data(), d.cmapCoeff.data(), (int) d.cmapMap.size(), d.cmapMap.data()));
+        d.check(b200md_update_cmap_params(d.ctx, (int) d.cmapSize.size(), d.cmapSize.data(), d.cmapCoeff.data(), d.cmap.size(), d.cmap.ints[0].data()));
     }
 private:
     ContextImpl& context;
-    int first = 0, count = 0, firstMap = 0, numMaps = 0;
+    int firstMap = 0, numMaps = 0;
     size_t firstCoeff = 0;
 };
 
@@ -613,16 +590,26 @@ vector<string> globalParameterNames(const CustomTorsionForce& force) {
     return names;
 }
 
-class B200CalcCustomTorsionForceKernel : public CalcCustomTorsionForceKernel {
+class B200CalcCustomTorsionForceKernel : public CalcCustomTorsionForceKernel, ObjectTerms {
 public:
     B200CalcCustomTorsionForceKernel(string name, const Platform& platform, ContextImpl& context) : CalcCustomTorsionForceKernel(name, platform), context(context) {}
+    // the term's parameters: as many as the force declares (the Reference platform reads as many), padded with zeros
+    void read(const CustomTorsionForce& force, int i, TermRecord& r) const {
+        int a, b, c, e;
+        vector<double> par;
+        force.getTorsionParameters(i, a, b, c, e, par);
+        par.resize(numParams);
+        par.resize(B200MD_CUSTOM_MAX_PARAMS, 0.0);
+        r.add({a, b, c, e}, {prog}, par);
+    }
     void initialize(const System& system, const CustomTorsionForce& force) {
         PlatformData& d = getData(context);
-        if (d.finalized) throw OpenMMException("B200 platform: CustomTorsionForce initialised after the Context was finalised");
+        prog = (int) d.customProgStart.size()/2;
+        numParams = force.getNumPerTorsionParameters();
+        add(d, d.custom, force, force.getNumTorsions(), B200MD_TERM_CUSTOM_TORSIONS, "CustomTorsionForce", [&](int i, TermRecord& r) { read(force, i, r); });
         b200md_custom::Program energy, deriv;
         const vector<string> globals = globalParameterNames(force);
         b200md_custom::translateExpression(force.getEnergyFunction(), perTorsionParameterNames(force), globals, d.customGlobalSlot, energy, deriv);
-        const int prog = (int) d.customProgStart.size()/2;
         for (const b200md_custom::Program* p : {&energy, &deriv}) {
             d.customOp.insert(d.customOp.end(), p->op.begin(), p->op.end());
             d.customArg.insert(d.customArg.end(), p->arg.begin(), p->arg.end());
@@ -638,20 +625,7 @@ public:
             slots.push_back(make_pair(it->first, it->second));
             d.customGlobals[it->second] = force.getGlobalParameterDefaultValue(i);
         }
-        numParams = force.getNumPerTorsionParameters();
         d.customStride = max(d.customStride, numParams);
-        first = (int) d.customProg.size(); count = force.getNumTorsions();
-        vector<double> par;
-        for (int i = 0; i < count; i++) {
-            int a, b, c, e;
-            force.getTorsionParameters(i, a, b, c, e, par);
-            d.customProg.push_back(prog);
-            for (int x : {a, b, c, e}) d.customAtoms.push_back(x);
-            par.resize(B200MD_CUSTOM_MAX_PARAMS, 0.0);
-            d.customParams.insert(d.customParams.end(), par.begin(), par.end());
-            d.customG.push_back(force.getForceGroup() | (force.usesPeriodicBoundaryConditions() ? 0x80 : 0));
-        }
-        d.systemTerms |= B200MD_TERM_CUSTOM_TORSIONS; d.bondedGroupsUsed |= 1u << force.getForceGroup();
     }
     double execute(ContextImpl& context, bool includeForces, bool includeEnergy) {
         PlatformData& d = getData(context);
@@ -667,23 +641,13 @@ public:
     }
     void copyParametersToContext(ContextImpl& context, const CustomTorsionForce& force) {
         PlatformData& d = getData(context);
-        d.ensureFinalized();
-        d.dropForces();
-        if (force.getNumTorsions() != count) throw OpenMMException("updateParametersInContext: The number of torsions has changed");
-        vector<double> par;
-        for (int i = 0; i < count; i++) {
-            int a[4];
-            force.getTorsionParameters(i, a[0], a[1], a[2], a[3], par);
-            for (int k = 0; k < 4; k++)
-                if (a[k] != d.customAtoms[4*(size_t) (first+i) + k]) throw OpenMMException("updateParametersInContext: The set of particles in a torsion has changed");
-            for (int k = 0; k < numParams && k < (int) par.size(); k++) d.customParams[(size_t) (first+i)*B200MD_CUSTOM_MAX_PARAMS + k] = par[k];
-        }
+        store(d.custom, reread(d, d.custom, force.getNumTorsions(), "torsions", "a torsion", [&](int i, TermRecord& r) { read(force, i, r); }));
         const vector<double> packed = d.packedCustomParams();
-        d.check(b200md_update_custom_torsion_params(d.ctx, (int) d.customProg.size(), packed.data()));
+        d.check(b200md_update_custom_torsion_params(d.ctx, d.custom.size(), packed.data()));
     }
 private:
     ContextImpl& context;
-    int first = 0, count = 0, numParams = 0;
+    int prog = 0, numParams = 0;          // this object's program pair; its number of per-torsion parameters
     vector<pair<string, int> > slots;     // the global parameters this object's expression reads, and their slots
 };
 
@@ -809,10 +773,10 @@ public:
         if (name == ApplyConstraintsKernel::Name()) return new B200ApplyConstraintsKernel(name, platform);
         if (name == VirtualSitesKernel::Name()) return new B200VirtualSitesKernel(name, platform);
         if (name == CalcNonbondedForceKernel::Name()) return new B200CalcNonbondedForceKernel(name, platform, context);
-        if (name == CalcHarmonicBondForceKernel::Name()) return new B200CalcHarmonicBondForceKernel(name, platform, context);
-        if (name == CalcHarmonicAngleForceKernel::Name()) return new B200CalcHarmonicAngleForceKernel(name, platform, context);
-        if (name == CalcPeriodicTorsionForceKernel::Name()) return new B200CalcPeriodicTorsionForceKernel(name, platform, context);
-        if (name == CalcRBTorsionForceKernel::Name()) return new B200CalcRBTorsionForceKernel(name, platform, context);
+        if (name == CalcHarmonicBondForceKernel::Name()) return new B200CalcBondedForceKernel<Bonds, &PlatformData::bonds>(name, platform, context);
+        if (name == CalcHarmonicAngleForceKernel::Name()) return new B200CalcBondedForceKernel<Angles, &PlatformData::angles>(name, platform, context);
+        if (name == CalcPeriodicTorsionForceKernel::Name()) return new B200CalcBondedForceKernel<Torsions, &PlatformData::torsions>(name, platform, context);
+        if (name == CalcRBTorsionForceKernel::Name()) return new B200CalcBondedForceKernel<RBTorsions, &PlatformData::rb>(name, platform, context);
         if (name == CalcCMAPTorsionForceKernel::Name()) return new B200CalcCMAPTorsionForceKernel(name, platform, context);
         if (name == CalcCustomTorsionForceKernel::Name()) return new B200CalcCustomTorsionForceKernel(name, platform, context);
         if (name == RemoveCMMotionKernel::Name()) return new B200RemoveCMMotionKernel(name, platform, context);

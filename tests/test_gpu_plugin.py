@@ -119,6 +119,17 @@ def test_reference_own_test_bodies_pass_on_b200_platform(name):
     assert p.returncode == 0 and "Done" in p.stdout, p.stdout[-2000:] + p.stderr[-2000:]
 
 
+def test_two_objects_of_every_bonded_class_match_reference_platform():
+    """plugin/tests/bonded_objects.cpp: two Force objects of each bonded class in force groups 1 and 2 (the second periodic),
+    per-group and total forces and energies against the Reference platform, after updating the second object alone (its
+    terms do not start at 0 in the platform's arrays) and then the first; a changed atom of the second is refused."""
+    exe = os.path.join(REFTESTS, "bonded_objects")
+    if not os.path.exists(exe):
+        pytest.fail("%s not built (make -C plugin reftests where /root/reference exists)" % exe)
+    p = subprocess.run([exe], capture_output=True, text=True, timeout=600, env=dict(os.environ, B200_PLUGIN=PLUGIN))
+    assert p.returncode == 0 and "Done" in p.stdout, p.stdout[-2000:] + p.stderr[-2000:]
+
+
 _PME_HOOK_SCRIPT = r"""
 import sys, os, ctypes, numpy as np
 root = os.environ["B200MD_ROOT"]
