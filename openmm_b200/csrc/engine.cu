@@ -148,6 +148,14 @@ struct NcclApi {
 static NcclApi g_nccl;
 enum { NCCL_INT8 = 0, NCCL_INT64 = 4, NCCL_FLOAT32 = 7, NCCL_FLOAT64 = 8, NCCL_SUM = 0 };
 
+// The multi-GPU scheme of a context, decided once by b200md_finalize (MG_SINGLE before it):
+//   MG_SINGLE       world == 1
+//   MG_P2P          the peer-memory data plane (comm.cu, DESIGN.md section 5): B200MD_MGPU unset or not "nccl"
+//   MG_NCCL_SPLIT   B200MD_MGPU=nccl with PME: the last rank does reciprocal space for every atom and nothing else, the others
+//                   share the direct-space tiles and the bonded terms; an NCCL all-reduce of the force buffer joins them
+//   MG_NCCL_SHARED  B200MD_MGPU=nccl without PME: every rank takes a share of everything, joined the same way
+enum MultiGpu { MG_SINGLE, MG_P2P, MG_NCCL_SPLIT, MG_NCCL_SHARED };
+
 struct b200md_ctx {
     int device = 0;
     int natoms = 0, npad = 0, nblocks = 0;
@@ -241,14 +249,14 @@ struct b200md_ctx {
     // ---- multi-GPU ----
     void* comm = nullptr;
     int rank = 0, world = 1;
+    MultiGpu mg = MG_SINGLE;
     // peer-memory data plane (comm.cu): one window per rank, mapped by every other rank with CUDA IPC
-    bool p2p = false;                    // world > 1 and B200MD_MGPU != nccl
-    CommDev cd{};                        // world == 1 unless p2p
+    CommDev cd{};                        // world == 1 unless MG_P2P
     char* window = nullptr; size_t windowBytes = 0;
     void* peerMapped[B200MD_MAX_RANKS] = {nullptr};
     DevBuf<unsigned long long> commCounters;   // [0] epoch, [1] posNeed
     DevBuf<unsigned int> commDone;             // [CH_COUNT]
-    bool velStale = false;               // p2p: the velocities of foreign atoms are behind (only owners integrate)
+    bool velStale = false;               // MG_P2P: the velocities of foreign atoms are behind (only owners integrate)
     std::vector<float4> hbuf4, hcorr4;
     std::vector<int> hoffset;
     std::vector<long long> hforce;
@@ -972,7 +980,7 @@ static void build_ccma(b200md_ctx* c) {
     const int nc = (int) c->ccmaCons.size();
     c->ccma = CcmaDev{};
     if (nc == 0) return;
-    require(!c->p2p && c->world == 1, "general (CCMA) constraint networks are not supported in multi-GPU runs");
+    require(c->mg == MG_SINGLE, "general (CCMA) constraint networks are not supported in multi-GPU runs");
     const CcmaInput in{c->natoms, c->mass, c->ccmaCons, c->conI, c->conJ, c->conD, c->angles.atoms, c->angles.params};
     CcmaHost H;
     ccma_host_setup(&in, H);
@@ -1248,7 +1256,7 @@ static void alloc_tile_pools(b200md_ctx* c, int poolCap) {
 // The reciprocal-space chain runs beside a tile kernel that holds every SM: one GPU, two streams, no SM partition.  Its FFT
 // then runs as small CTAs that fit the slots retiring tile CTAs hand back (fft.cu); everywhere else it keeps the larger ones.
 static bool fft_beside_tiles(const b200md_ctx* c) {
-    return c->world == 1 && !c->pmeOnly && c->overlapPme && !c->nb.smPartition && c->nbdesc.method == B200MD_NB_PME;
+    return c->mg == MG_SINGLE && !c->pmeOnly && c->overlapPme && !c->nb.smPartition && c->nbdesc.method == B200MD_NB_PME;
 }
 
 // finalize: the custom torsions in the layout of k_custom_torsion (CustomTorsionDev): grouped by expression, each group padded
@@ -1263,7 +1271,7 @@ static void upload_custom_torsions(b200md_ctx* c) {
     t.globalsDev.alloc(std::max<size_t>(t.globals.size(), 1)); t.globalsDev.upload(t.globals);
     d.globals = t.globalsDev.p;
     if (t.n == 0) return;
-    require(c->world == 1, "custom torsions are not supported in multi-GPU runs");
+    require(c->mg == MG_SINGLE, "custom torsions are not supported in multi-GPU runs");
     require(t.group.empty() || (int) t.group.size() == t.n, "set_bonded_groups: group array length differs from the number of terms");
     for (int q = 0; q < 2*t.nprog; q++) {
         const char* why = custom_check_program(t.code.data(), t.progStart[q], t.progStart[q+1], t.stride, (int) t.globals.size());
@@ -1298,10 +1306,18 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     NbDev& nb = c->nb;
     nb.natoms = N; nb.npad = NP; nb.nblocks = c->nblocks;
     nb.method = c->nbdesc.method;
+    const bool nccl = getenv("B200MD_MGPU") && std::string(getenv("B200MD_MGPU")) == "nccl";
+    // b200md_comm_init sets world and comm together
+    c->mg = c->world == 1 ? MG_SINGLE : !nccl ? MG_P2P : (nb.method == B200MD_NB_PME && c->haveNb) ? MG_NCCL_SPLIT : MG_NCCL_SHARED;
+    // this rank's share of the sharded kernels (k_bonded, k_build_tiles, k_pair, the user-order k_pme_spread and
+    // k_pme_gather): in the NCCL role split the PME rank takes every atom, the direct ranks deal the rest among world-1
     nb.rank = c->rank; nb.world = c->world;
+    if (c->mg == MG_NCCL_SPLIT) {
+        if (c->rank == c->world - 1) { nb.rank = 0; nb.world = 1; }
+        else nb.world = c->world - 1;
+    }
     c->cd = CommDev{}; c->cd.world = 1;
-    c->p2p = c->world > 1 && c->comm && !(getenv("B200MD_MGPU") && std::string(getenv("B200MD_MGPU")) == "nccl");
-    if (c->p2p) setup_window(c);
+    if (c->mg == MG_P2P) setup_window(c);
     { const double cc = getenv("B200MD_CLOSE_NM") ? atof(getenv("B200MD_CLOSE_NM")) : 0.36; nb.closeCut2 = (float) (cc*cc); }
     // SM partition between the tile kernel and the reciprocal-space chain (B200MD_PME_SMS=k reserves k SMs; 0 = off)
     for (int w = 0; w < 4; w++) nb.pmeSmMask[w] = 0ull;
@@ -1314,7 +1330,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
         int want = 0;
         // at least one SM per x plane of this rank; the more ranks, the shorter the tile kernel and the longer (relatively)
         // the chain of exchanges: 44 / 40 / 64 SMs at 2 / 4 / 8 ranks for an 88^3 grid
-        if (c->p2p) want = std::min(74, std::max((c->nbdesc.grid[0] + c->world - 1)/c->world, 16 + 6*c->world));
+        if (c->mg == MG_P2P) want = std::min(74, std::max((c->nbdesc.grid[0] + c->world - 1)/c->world, 16 + 6*c->world));
         if (getenv("B200MD_PME_SMS")) want = atoi(getenv("B200MD_PME_SMS"));
         const int got = want > 0 ? choose_pme_sms(want, nb.pmeSmMask) : 0;
         if (got > 0) {
@@ -1391,7 +1407,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     upload_params(c);
     build_units(c);
     build_ccma(c);
-    if (c->p2p) {
+    if (c->mg == MG_P2P) {
         setup_ownership(c);
         if (nb.method == B200MD_NB_PME) {
             PmeDev probe{}; probe.nx = c->nbdesc.grid[0]; probe.ny = c->nbdesc.grid[1]; probe.nz = c->nbdesc.grid[2]; probe.nzc = probe.nz/2 + 1;
@@ -1403,7 +1419,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     // and the reciprocal-space rank builds no list) ----
     c->cellOffset.alloc((size_t) 3*NP); c->cellOffset.zero();
     nb.cellOffset = c->cellOffset.p; nb.nmol = 0; nb.molStart = nullptr; nb.molAtoms = nullptr;
-    if ((nb.method == B200MD_NB_CUTOFF_PERIODIC || nb.method == B200MD_NB_PME) && c->world == 1 && !c->pmeOnly) {
+    if ((nb.method == B200MD_NB_CUTOFF_PERIODIC || nb.method == B200MD_NB_PME) && c->mg == MG_SINGLE && !c->pmeOnly) {
         std::vector<int> parent(N);
         for (int i = 0; i < N; i++) parent[i] = i;
         auto find = [&](int x) { while (parent[x] != x) { parent[x] = parent[parent[x]]; x = parent[x]; } return x; };
@@ -1519,15 +1535,15 @@ extern "C" int b200md_update_custom_torsion_params(b200md_ctx* ctx, int n, const
 // ---------------------------------------------------------------- state
 // Multi-GPU (peer-memory data plane): only the owner integrates an atom.  Positions reach every rank with the step itself;
 // velocities stay with the owner until somebody reads them from the host side.
-static void sync_positions(b200md_ctx* c) { if (c->p2p && c->finalized) launch_pos_wait(c->nb, c->cd, c->stream); }
+static void sync_positions(b200md_ctx* c) { if (c->mg == MG_P2P && c->finalized) launch_pos_wait(c->nb, c->cd, c->stream); }
 static void sync_velocities(b200md_ctx* c) {
-    if (!c->p2p || !c->velStale) return;
+    if (c->mg != MG_P2P || !c->velStale) return;
     launch_vel_push(c->nb, c->cd, c->stream);
     c->kernelLaunches += 2;
     c->velStale = false;
 }
 static void host_set_state(b200md_ctx* c) {       // the host wrote the full state on every rank: nothing to wait for
-    if (!c->p2p) return;
+    if (c->mg != MG_P2P) return;
     const unsigned long long zero = 0ull;
     CUDA_CHECK(cudaMemcpyAsync(c->cd.posNeed, &zero, sizeof(zero), cudaMemcpyHostToDevice, c->stream));
 }
@@ -1697,91 +1713,31 @@ extern "C" int b200md_checkpoint_load(b200md_ctx* ctx, const void* buf, int64_t 
     API_END(ctx)
 }
 
-// Multi-GPU role split (replicated atoms): with PME and world > 1 the LAST rank computes reciprocal space for all atoms and
-// nothing else; the other world-1 ranks share the direct-space tiles (by i-block: list construction AND tile kernel) and the
-// bonded terms.  Returns the rank's view of the sharding.
-static bool role_split(const b200md_ctx* c) { return c->world > 1 && c->comm && !c->p2p && c->nb.method == B200MD_NB_PME && c->haveNb; }
-static NbDev role_nb(const b200md_ctx* c) {
-    NbDev nb = c->nb;
-    if (role_split(c)) {
-        if (c->rank == c->world - 1) { nb.rank = 0; nb.world = 1; }
-        else nb.world = c->world - 1;
-    }
-    return nb;
-}
+// NCCL role split (replicated atoms): the LAST rank computes reciprocal space for all atoms and nothing else, so it keeps no
+// neighbour list; the other world-1 ranks share the direct-space tiles (by i-block: list construction AND tile kernel) and
+// the bonded terms
+static bool nccl_pme_rank(const b200md_ctx* c) { return c->mg == MG_NCCL_SPLIT && c->rank == c->world - 1; }
 
 // ---------------------------------------------------------------- force evaluation
 // PME parameters of the next spread launch: the brick path needs a list that covers every atom on this GPU
 static PmeDev pme_for_launch(const b200md_ctx* c) {
     PmeDev p = c->pme;
-    p.brickAtoms = (c->pmeBrick && c->world == 1 && !c->pmeOnly && c->listBuilt) ? c->brickAtoms : 0;
+    p.brickAtoms = (c->pmeBrick && c->mg == MG_SINGLE && !c->pmeOnly && c->listBuilt) ? c->brickAtoms : 0;
     p.brickPoints = c->brickPoints;
     return p;
 }
 
 // Enqueue one force evaluation on the stream (no host sync).  Returns the number of kernels launched.
 static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlreadyZero = false, bool inStep = false, unsigned int groupMask = 0xffffffffu) {
-    int launches = 0;
     cudaStream_t s = c->stream;
-    if (!forcesAlreadyZero) CUDA_CHECK(cudaMemsetAsync(c->force.p, 0, sizeof(long long)*3*c->npad, s));
-    if (energy) CUDA_CHECK(cudaMemsetAsync(c->energy.p, 0, sizeof(double)*B200MD_NUM_ENERGY, s));
-    bool direct = (terms & B200MD_TERM_NB_DIRECT) && c->haveNb;
-    bool recip = (terms & B200MD_TERM_NB_RECIP) && c->haveNb && c->nb.method == B200MD_NB_PME;
-    // Multi-GPU role split (replicated atoms): the LAST rank computes reciprocal space for all atoms and nothing else; the
-    // other world-1 ranks share the direct-space tiles (by i-block) and the bonded terms.  The two halves of the force
-    // field thus overlap on different GPUs, there is no charge-grid collective, and one int64 all-reduce of the force buffer
-    // per step joins them.  (With PME and world > 1 only; otherwise every rank takes a share of everything.)
-    const bool split = role_split(c);
-    const int pmeRank = c->world - 1;
-    NbDev nbSave = c->nb;
-    if (split) {
-        if (c->rank == pmeRank) direct = false; else recip = false;
-        c->nb = role_nb(c);
-    }
-    struct Restore { b200md_ctx* c; NbDev saved; ~Restore() { c->nb = saved; } } restore{c, nbSave};
-    // Reciprocal space (spread -> FFT/convolution -> gather, in USER atom order: independent of the neighbour list) and
-    // direct space (list check / rebuild, tile kernel, bonded terms) are independent until the integrator: fork them onto
-    // two streams (also inside the captured step graph).  Both accumulate into the same fixed-point force buffer, so the
-    // overlap cannot change the result.  Single-GPU only: with NCCL the collectives of one communicator stay on one stream.
-    const bool p2p = c->p2p;
-    const bool fork = direct && recip && c->overlapPme && !(c->world > 1 && c->comm && !p2p);
-    cudaStream_t sp = fork ? c->streamPme : s;
-    if (p2p && !direct) { launch_pos_wait(c->nb, c->cd, s); launches++; }       // nobody else on this stream waits for the owners' position stores
-    // The brick path of the spread walks the current list's sorted order, so when it runs beside direct space the
-    // fork comes after the list build: the list then cannot flip under it (a rebuild flips at the end of k_build_tiles).
-    // On one stream it runs before the build and reads the current list, which is complete even when stale.
-    const PmeDev pme = pme_for_launch(c);
-    const bool forkAfterList = fork && direct && pme.brickAtoms > 0;
-    auto launch_recip = [&]() {
-        if (fork) {
-            CUDA_CHECK(cudaEventRecord(c->evFork, s));
-            CUDA_CHECK(cudaStreamWaitEvent(sp, c->evFork, 0));
-        }
-        if (recip) {
-            launch_pme_spread(c->nb, pme, c->cd, sp, !forkAfterList); launches++;
-            if (p2p) { launch_grid_push(c->pme, c->cd, sp); launches++; }
-            else if (c->world > 1 && c->comm && !split) {
-                int rc = g_nccl.AllReduce(c->gridFixed.p, c->gridFixed.p, (size_t) c->pme.nx*c->pme.ny*c->pme.nz, NCCL_INT64, NCCL_SUM, c->comm, sp);
-                if (rc != 0) throw std::runtime_error("ncclAllReduce(grid) failed");
-            }
-            launch_pme_fft_conv(c->nb, c->pme, c->cd, energy && (split || p2p || c->rank == 0), fft_beside_tiles(c), sp); launches += pme_fft_launch_count(c->pme);
-            launch_pme_gather(c->nb, pme, c->cd, sp); launches++;
-        }
-        if (fork) CUDA_CHECK(cudaEventRecord(c->evJoin, sp));
-    };
-    if (!forkAfterList) launch_recip();
-    // When the chain forks after the list build, the charge grid is zeroed at the head of the step on the chain's stream,
-    // beside the list check and build: it needs nothing from them, and as the spread's first node it sat on the chain, which
-    // is the step's longest path (DHFR: memset 1.6 us plus a node gap before the spread).
-    if (forkAfterList && recip) {
-        CUDA_CHECK(cudaEventRecord(c->evForkGrid, s));
-        CUDA_CHECK(cudaStreamWaitEvent(sp, c->evForkGrid, 0));
-        CUDA_CHECK(cudaMemsetAsync(pme.gridFixed, 0, sizeof(long long)*(size_t) pme.nx*pme.ny*pme.nz, sp));
-    }
-    if (direct) {
-        launch_check_displacement(c->nb, c->cd, s); launches++;
-        launch_list_build(c->nb, s); launches += LIST_BUILD_LAUNCHES;
-    }
+    // ---- what this evaluation runs ----
+    // NCCL role split: the PME rank does reciprocal space only, the direct ranks everything else.  The two halves of the
+    // force field thus overlap on different GPUs, there is no charge-grid collective, and one int64 all-reduce of the force
+    // buffer per step joins them.  NCCL without PME has no reciprocal space: every rank takes a share of everything.
+    const bool p2p = c->mg == MG_P2P, nccl = c->mg == MG_NCCL_SPLIT || c->mg == MG_NCCL_SHARED;
+    const bool pmeRank = nccl_pme_rank(c), directRank = c->mg == MG_NCCL_SPLIT && !pmeRank;
+    const bool direct = (terms & B200MD_TERM_NB_DIRECT) && c->haveNb && !pmeRank;
+    const bool recip = (terms & B200MD_TERM_NB_RECIP) && c->haveNb && c->nb.method == B200MD_NB_PME && !directRank;
     int bterms = terms & (B200MD_TERM_BONDS | B200MD_TERM_ANGLES | B200MD_TERM_TORSIONS | B200MD_TERM_RB_TORSIONS | B200MD_TERM_CMAP |
                           B200MD_TERM_CUSTOM_TORSIONS);
     if (c->haveNb) bterms |= terms & B200MD_TERM_NB_DIRECT;
@@ -1790,16 +1746,65 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     // launch_bonded skips the kernel); k_custom_torsion is counted when it runs
     const bool classic = (bterms & ~B200MD_TERM_CUSTOM_TORSIONS) && nbonded > 0;
     const bool custom = (bterms & B200MD_TERM_CUSTOM_TORSIONS) && c->ctd.nslots > 0;
-    const bool bonded = (classic || custom) && !(split && c->rank == pmeRank);
+    const bool bonded = (classic || custom) && !pmeRank;
+    // Reciprocal space (spread -> FFT/convolution -> gather, in USER atom order: independent of the neighbour list) and
+    // direct space (list check / rebuild, tile kernel, bonded terms) are independent until the integrator: fork them onto
+    // two streams (also inside the captured step graph).  Both accumulate into the same fixed-point force buffer, so the
+    // overlap cannot change the result.  Never under NCCL, whose collectives of one communicator stay on one stream: there a
+    // rank runs at most one of the two halves.
+    const bool fork = direct && recip && c->overlapPme;
+    cudaStream_t sp = fork ? c->streamPme : s;
+    // The brick path of the spread walks the current list's sorted order, so when it runs beside direct space the
+    // fork comes after the list build: the list then cannot flip under it (a rebuild flips at the end of k_build_tiles).
+    // On one stream it runs before the build and reads the current list, which is complete even when stale.
+    const PmeDev pme = pme_for_launch(c);
+    const bool forkAfterList = fork && pme.brickAtoms > 0;
+    // The bonded terms need nothing from the tile kernel either: on one GPU they fork with the spread onto a stream of their
+    // own (not before the list build, whose wrap phase moves molecules in posq) and join before the integrator.
+    const bool forkBonded = forkAfterList && bonded;
+    // p2p: partial forces of the atoms this rank does not own -> the owners' inboxes.  Reciprocal space only ever touches the
+    // atoms this rank OWNS (k_pme_gather), so when it runs on its own stream the push does not have to wait for it: it goes
+    // out right behind the tile kernel and the bonded terms, beside the FFT chain.
+    const bool pushEarly = p2p && fork;
+
+    int launches = 0;
+    auto launch_recip = [&]() {
+        if (fork) {
+            CUDA_CHECK(cudaEventRecord(c->evFork, s));
+            CUDA_CHECK(cudaStreamWaitEvent(sp, c->evFork, 0));
+        }
+        if (recip) {
+            launch_pme_spread(c->nb, pme, c->cd, sp, !forkAfterList); launches++;
+            if (p2p) { launch_grid_push(c->pme, c->cd, sp); launches++; }
+            launch_pme_fft_conv(c->nb, c->pme, c->cd, energy, fft_beside_tiles(c), sp); launches += pme_fft_launch_count(c->pme);
+            launch_pme_gather(c->nb, pme, c->cd, sp); launches++;
+        }
+        if (fork) CUDA_CHECK(cudaEventRecord(c->evJoin, sp));
+    };
     auto launch_bonded_terms = [&](cudaStream_t sb) {
         BondedDev bd = c->bd; bd.groupMask = groupMask;
         CustomTorsionDev ct = c->ctd; ct.groupMask = groupMask;
         launch_bonded(c->nb, bd, ct, bterms, energy, sb);
         launches += (classic ? 1 : 0) + (custom ? 1 : 0);
     };
-    // The bonded terms need nothing from the tile kernel either: on one GPU they fork with the spread onto a stream of their
-    // own (not before the list build, whose wrap phase moves molecules in posq) and join before the integrator.
-    const bool forkBonded = forkAfterList && bonded;
+
+    // ---- the schedule, in stream order ----
+    if (!forcesAlreadyZero) CUDA_CHECK(cudaMemsetAsync(c->force.p, 0, sizeof(long long)*3*c->npad, s));
+    if (energy) CUDA_CHECK(cudaMemsetAsync(c->energy.p, 0, sizeof(double)*B200MD_NUM_ENERGY, s));
+    if (p2p && !direct) { launch_pos_wait(c->nb, c->cd, s); launches++; }       // nobody else on this stream waits for the owners' position stores
+    if (!forkAfterList) launch_recip();
+    else {
+        // the charge grid is zeroed at the head of the step on the chain's stream, beside the list check and build: it needs
+        // nothing from them, and as the spread's first node it sat on the chain, which is the step's longest path (DHFR:
+        // memset 1.6 us plus a node gap before the spread)
+        CUDA_CHECK(cudaEventRecord(c->evForkGrid, s));
+        CUDA_CHECK(cudaStreamWaitEvent(sp, c->evForkGrid, 0));
+        CUDA_CHECK(cudaMemsetAsync(pme.gridFixed, 0, sizeof(long long)*(size_t) pme.nx*pme.ny*pme.nz, sp));
+    }
+    if (direct) {
+        launch_check_displacement(c->nb, c->cd, s); launches++;
+        launch_list_build(c->nb, s); launches += LIST_BUILD_LAUNCHES;
+    }
     if (forkAfterList) launch_recip();
     if (forkBonded) {
         CUDA_CHECK(cudaStreamWaitEvent(c->streamBonded, c->evFork, 0));
@@ -1808,10 +1813,6 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     }
     if (direct) { launch_pair(c->nb, energy, s); launches += PAIR_LAUNCHES; }
     if (bonded && !forkBonded) launch_bonded_terms(s);
-    // p2p: partial forces of the atoms this rank does not own -> the owners' inboxes.  Reciprocal space only ever touches the
-    // atoms this rank OWNS (k_pme_gather), so when it runs on its own stream the push does not have to wait for it: it goes
-    // out right behind the tile kernel and the bonded terms, beside the FFT chain.
-    const bool pushEarly = p2p && fork;
     if (pushEarly) { launch_force_push(c->nb, c->cd, s); launches++; }
     if (fork) CUDA_CHECK(cudaStreamWaitEvent(s, c->evJoin, 0));
     if (forkBonded) CUDA_CHECK(cudaStreamWaitEvent(s, c->evJoinBonded, 0));
@@ -1821,15 +1822,11 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
         // so that every rank ends up with every force
         if (!inStep) { launch_force_total(c->nb, c->cd, s); launches += 2; }
     }
-    if (c->world > 1 && c->comm) {
-        int rc = 0;
-        if (!p2p) rc = g_nccl.AllReduce(c->force.p, c->force.p, (size_t) 3*c->npad, NCCL_INT64, NCCL_SUM, c->comm, s);
-        if (rc != 0) throw std::runtime_error("ncclAllReduce(force) failed");
-        if (energy) {
-            rc = g_nccl.AllReduce(c->energy.p, c->energy.p, B200MD_NUM_ENERGY, NCCL_FLOAT64, NCCL_SUM, c->comm, s);
-            if (rc != 0) throw std::runtime_error("ncclAllReduce(energy) failed");
-        }
-    }
+    if (nccl && g_nccl.AllReduce(c->force.p, c->force.p, (size_t) 3*c->npad, NCCL_INT64, NCCL_SUM, c->comm, s) != 0)
+        throw std::runtime_error("ncclAllReduce(force) failed");
+    // the energies are summed over the ranks in every multi-GPU mode, p2p included
+    if (c->mg != MG_SINGLE && energy && g_nccl.AllReduce(c->energy.p, c->energy.p, B200MD_NUM_ENERGY, NCCL_FLOAT64, NCCL_SUM, c->comm, s) != 0)
+        throw std::runtime_error("ncclAllReduce(energy) failed");
     CUDA_CHECK(cudaGetLastError());
     return launches;
 }
@@ -1866,11 +1863,10 @@ static void check_flags(b200md_ctx* c) {
 // and size the tile pools from what the build actually used.  The step graphs trust the current list and never grow it.
 static void prepare_list(b200md_ctx* c) {
     if (!c->listDirty || !c->haveNb) { c->listDirty = false; return; }
-    if (c->pmeOnly || (role_split(c) && c->rank == c->world - 1)) { c->listDirty = false; return; }    // keeps no list
+    if (c->pmeOnly || nccl_pme_rank(c)) { c->listDirty = false; return; }    // keeps no list
     for (int attempt = 0; attempt < 8; attempt++) {
-        const NbDev nb = role_nb(c);
-        launch_check_displacement(nb, c->cd, c->stream);
-        launch_list_build(nb, c->stream);
+        launch_check_displacement(c->nb, c->cd, c->stream);
+        launch_list_build(c->nb, c->stream);
         c->kernelLaunches += 1 + LIST_BUILD_LAUNCHES;
         const DevFlags f = read_flags(c, true);
         raise_timeouts(f);
@@ -1974,7 +1970,7 @@ extern "C" int b200md_integrate_only(b200md_ctx* ctx) {
     if (ctx->ccma.ncomp > 0) launch_ccma_step(ctx->nb, ctx->ccma, ctx->integ, ctx->stream);
     launch_integrate(ctx->nb, ctx->units, ctx->integ, ctx->cd, ctx->stream);
     ctx->kernelLaunches += 2;
-    ctx->velStale = ctx->p2p;
+    ctx->velStale = ctx->mg == MG_P2P;
     ctx->time += ctx->dt; ctx->stepCount++;
     CUDA_CHECK(cudaGetLastError());
     API_END(ctx)
@@ -1999,7 +1995,7 @@ static void capture_steps(b200md_ctx* c, int nsteps, cudaGraphExec_t* exec, int*
     // One GPU: the graph runs each kernel node at its own priority (launch_high), not at the priority of c->stream, so the
     // reciprocal-space chain and the bonded terms take the SM slots that the tile kernel's CTAs hand back.  An update in
     // place keeps the priorities: every capture gives the same nodes the same ones.
-    const cudaError_t e = cudaGraphInstantiate(exec, g, c->world == 1 ? cudaGraphInstantiateFlagUseNodePriority : 0);
+    const cudaError_t e = cudaGraphInstantiate(exec, g, c->mg == MG_SINGLE ? cudaGraphInstantiateFlagUseNodePriority : 0);
     cudaGraphDestroy(g);
     CUDA_CHECK(e);
     c->graphInstantiations++;
@@ -2041,7 +2037,7 @@ extern "C" int b200md_step(b200md_ctx* ctx, int nsteps) {
         }
         else
             c->kernelLaunches += enqueue_step(c);
-        c->velStale = c->p2p;
+        c->velStale = c->mg == MG_P2P;
         c->forceEvals += done;
         c->stepCount += done;
         c->time += c->dt*done;
@@ -2176,7 +2172,6 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
     prepare_list(c);
     c->stepStateValid = false;            // phases 0, 3, 6 accumulate into the force buffer, phase 5 flips the list
     cudaStream_t s = c->stream;
-    const NbDev nbv = role_nb(c);        // the sharding the step graphs use
     CommDev local{}; local.world = 1;   // phases are timed rank-locally (no peer traffic, no waits)
     cudaEvent_t e0, e1;
     CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
@@ -2196,14 +2191,14 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
         if (phase == 0) { CUDA_CHECK(cudaMemsetAsync(&c->counters.p[CT_CURSOR], 0, sizeof(int), s)); CUDA_CHECK(cudaMemsetAsync(&c->counters.p[CT_PAIRSTART], 0, sizeof(int), s)); }      // the SM-partitioned tile kernel's cursor starts from tile 0
         CUDA_CHECK(cudaEventRecord(e0, s));
         switch (phase) {
-            case 0: launch_pair(nbv, false, s); break;
-            case 1: launch_pme_spread(nbv, pme_for_launch(c), local, s); break;
-            case 2: launch_pme_fft_conv(nbv, c->pme, local, false, fft_beside_tiles(c), s); break;
-            case 3: launch_pme_gather(nbv, pme_for_launch(c), local, s); break;
-            case 4: launch_integrate(nbv, c->units, c->integ, local, s); break;
-            case 5: launch_list_build(nbv, s); break;
-            case 6: launch_bonded(nbv, c->bd, c->ctd, B200MD_TERM_ALL, false, s); break;
-            case 7: launch_custom_torsion(nbv, c->ctd, false, s); break;
+            case 0: launch_pair(c->nb, false, s); break;
+            case 1: launch_pme_spread(c->nb, pme_for_launch(c), local, s); break;
+            case 2: launch_pme_fft_conv(c->nb, c->pme, local, false, fft_beside_tiles(c), s); break;
+            case 3: launch_pme_gather(c->nb, pme_for_launch(c), local, s); break;
+            case 4: launch_integrate(c->nb, c->units, c->integ, local, s); break;
+            case 5: launch_list_build(c->nb, s); break;
+            case 6: launch_bonded(c->nb, c->bd, c->ctd, B200MD_TERM_ALL, false, s); break;
+            case 7: launch_custom_torsion(c->nb, c->ctd, false, s); break;
             default: throw std::runtime_error("unknown phase");
         }
         CUDA_CHECK(cudaEventRecord(e1, s));

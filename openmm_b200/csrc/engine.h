@@ -145,7 +145,8 @@ struct NbDev {
     const int* molAtoms;
     int* cellOffset;             // [3][npad] lattice vector counts to ADD when reporting positions
     float halfPad2;              // (padding/2)^2: beyond this displacement the current list is invalid
-    // multi-GPU sharding of the tile list / PME atoms
+    // multi-GPU sharding of the tile list, bonded terms and user-order PME atoms: this rank's share, set once by
+    // b200md_finalize (in the NCCL role split the PME rank is rank 0 of 1 and the direct ranks deal among world-1)
     int rank, world;
     // origin of the primary periodic cell used for binning (chosen at set_positions so that a structure centred anywhere,
     // e.g. a PDB centred on 0, is binned WITHOUT lattice shifts: a shift costs one fp32 rounding of the coordinate)

@@ -171,7 +171,7 @@ template <> __device__ __forceinline__ float4 unit_params<float>(const UnitDev& 
 template <> __device__ __forceinline__ double4 unit_params<double>(const UnitDev& un, int u) { return un.unitParamsD[u]; }
 
 template <class R>
-__device__ __forceinline__ bool load_unit(const NbDev& nb, const UnitDev& un, int u, Unit<R>& U, bool wantForce, const CommDev* cd = nullptr) {
+__device__ __forceinline__ void load_unit(const NbDev& nb, const UnitDev& un, int u, Unit<R>& U, bool wantForce) {
     const int4 at = un.unitAtoms[u];
     U.atom[0] = at.x; U.atom[1] = at.y; U.atom[2] = at.z; U.atom[3] = at.w;
     U.type = un.unitType[u];
@@ -189,19 +189,10 @@ __device__ __forceinline__ bool load_unit(const NbDev& nb, const UnitDev& un, in
         U.invM[k] = v.w;
         U.m[k] = (v.w > R(0)) ? R(1)/v.w : R(0);
         if (wantForce) {
-            long long fx = nb.force[a], fy = nb.force[a + nb.npad], fz = nb.force[a + 2*nb.npad];
-            if (cd != nullptr && cd->world > 1) {
-                // owner: total = own partial + what the other ranks pushed into the inboxes (exact int64 sums, any order)
-                const long long* in = (const long long*) (cd->peer[cd->rank] + cd->offFinbox);
-                for (int q = 0; q < cd->world; q++) if (q != cd->rank) {
-                    const long long* iq = in + (size_t) q*3*nb.npad;
-                    fx += iq[a]; fy += iq[a + nb.npad]; fz += iq[a + 2*nb.npad];
-                }
-            }
+            const long long fx = nb.force[a], fy = nb.force[a + nb.npad], fz = nb.force[a + 2*nb.npad];
             U.f[k] = {fixed_to_real<R>(fx), fixed_to_real<R>(fy), fixed_to_real<R>(fz)};
         }
     }
-    return true;
 }
 
 template <class R>

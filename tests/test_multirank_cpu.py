@@ -102,7 +102,7 @@ def test_round_robin_sharding_is_a_partition():
 
 def _role_worker(rank, world, port, out):
     """DESIGN.md section 5 at world 2: rank 0 = direct space + bonded terms + exclusion correction, rank 1 = reciprocal space
-    for all atoms (what engine.cu:role_split / role_nb arrange), joined by one int64 all-reduce of the force buffer."""
+    for all atoms (what engine.cu arranges for MG_NCCL_SPLIT), joined by one int64 all-reduce of the force buffer."""
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
     dist.init_process_group("gloo", rank=rank, world_size=world)
