@@ -41,7 +41,9 @@ typedef struct b200md_ctx b200md_ctx;
 #define B200MD_TERM_RB_TORSIONS 32
 #define B200MD_TERM_CMAP       64
 #define B200MD_TERM_CUSTOM_TORSIONS 128
-#define B200MD_TERM_ALL        255
+#define B200MD_TERM_CUSTOM_BONDS     256
+#define B200MD_TERM_CUSTOM_EXTERNALS 512
+#define B200MD_TERM_ALL        1023
 
 /* ---- the bonded classes: kind argument of b200md_set_bonded_groups and b200md_update_bonded_params ---- */
 #define B200MD_BONDED_BONDS           0
@@ -50,14 +52,24 @@ typedef struct b200md_ctx b200md_ctx;
 #define B200MD_BONDED_RB_TORSIONS     3
 #define B200MD_BONDED_CMAP            4
 #define B200MD_BONDED_CUSTOM_TORSIONS 5
+#define B200MD_BONDED_CUSTOM_BONDS    6
+#define B200MD_BONDED_CUSTOM_EXTERNALS 7
 
-/* ---- instructions of a custom-torsion expression program (b200md_set_custom_torsions) ----
+/* ---- the classes of custom terms: which variables a program may read (custom_check_program) ---- */
+#define B200MD_CUSTOM_TORSION  0      /* THETA                                   */
+#define B200MD_CUSTOM_BOND     1      /* VAR 0 = r                                */
+#define B200MD_CUSTOM_EXTERNAL 2      /* VAR 0, 1, 2 = x, y, z; PERIODIC_DIST      */
+
+/* ---- instructions of a custom-term expression program (b200md_set_custom_torsions / _bonds / _externals) ----
  * One instruction = (opcode, operand index, double immediate).  A program is the flat stack program of a Lepton
  * ExpressionProgram (lepton/ExpressionProgram.h), one instruction per Lepton::Operation, in the same order and with the same
  * argument order: an operation of k arguments reads them from the top of the stack, argument 0 being the value pushed LAST,
  * and replaces them with its result (ExpressionProgram::evaluate).  Each opcode computes exactly what the Operation of the
  * same name computes.  THETA pushes the dihedral in (-pi, pi], PARAM k the term's k-th parameter, GLOBAL s the context's
- * global value in slot s; CONST, ADD_CONST, MUL_CONST and POW_CONST take their constant from the immediate. */
+ * global value in slot s; CONST, ADD_CONST, MUL_CONST and POW_CONST take their constant from the immediate.  VAR k pushes
+ * variable k of the term (a bond: 0 = r; an external: 0, 1, 2 = x, y, z).  PERIODIC_DIST is Lepton's periodicdistance(x, y,
+ * z, x0, y0, z0) with argument k at st[sp+k] as for every operation: operand -1 gives the minimum-image distance, operand
+ * k in 0..5 its derivative by argument k (ReferencePointDistanceFunction, periodic), every one of them 0 at distance 0. */
 enum {
     B200MD_OP_CONST = 0, B200MD_OP_THETA, B200MD_OP_PARAM, B200MD_OP_GLOBAL,
     B200MD_OP_ADD, B200MD_OP_SUB, B200MD_OP_MUL, B200MD_OP_DIV, B200MD_OP_POW, B200MD_OP_NEG, B200MD_OP_SQRT, B200MD_OP_EXP,
@@ -65,10 +77,10 @@ enum {
     B200MD_OP_ACOS, B200MD_OP_ATAN, B200MD_OP_ATAN2, B200MD_OP_SINH, B200MD_OP_COSH, B200MD_OP_TANH, B200MD_OP_ERF,
     B200MD_OP_ERFC, B200MD_OP_STEP, B200MD_OP_DELTA, B200MD_OP_SQUARE, B200MD_OP_CUBE, B200MD_OP_RECIP, B200MD_OP_ADD_CONST,
     B200MD_OP_MUL_CONST, B200MD_OP_POW_CONST, B200MD_OP_MIN, B200MD_OP_MAX, B200MD_OP_ABS, B200MD_OP_FLOOR, B200MD_OP_CEIL,
-    B200MD_OP_SELECT,
+    B200MD_OP_SELECT, B200MD_OP_VAR, B200MD_OP_PERIODIC_DIST,
     B200MD_OP_COUNT
 };
-/* hard limits of a custom-torsion program: stack depth, instructions per program, parameters per term */
+/* hard limits of a custom-term program: stack depth, instructions per program, parameters per term */
 #define B200MD_CUSTOM_MAX_STACK  16
 #define B200MD_CUSTOM_MAX_CODE   256
 #define B200MD_CUSTOM_MAX_PARAMS 16
@@ -130,6 +142,16 @@ int b200md_set_cmap(b200md_ctx* ctx, int nmaps, const int* size, const double* c
  * of global values at finalize.  Single GPU only.                                                                        */
 int b200md_set_custom_torsions(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
                                int param_stride, int n, const int* prog, const int* atoms, const double* params);
+/* CalcCustomBondForceKernel::initialize (kernels.h): as b200md_set_custom_torsions, with programs 2p and 2p+1 the energy of
+ * expression p and its dE/dr (VAR 0 = r = |x_b - x_a|, the minimum image for a term whose group byte has 0x80); term i
+ * joins the atoms atoms[2i], atoms[2i+1].  The force is (dE/dr)/r (x_b - x_a) on a and its negative on b, 0 at r = 0.   */
+int b200md_set_custom_bonds(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                            int param_stride, int n, const int* prog, const int* atoms, const double* params);
+/* CalcCustomExternalForceKernel::initialize (kernels.h): programs 4p .. 4p+3 are the energy of expression p and its
+ * derivatives by x, y and z (VAR 0..2), the continuous coordinate of particle atoms[i] that b200md_get_positions reports;
+ * PERIODIC_DIST takes the current box.  The force is minus the gradient.                                                */
+int b200md_set_custom_externals(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                int param_stride, int n, const int* prog, const int* atoms, const double* params);
 /* The global parameter values the GLOBAL instructions read (slot s = values[s]).  Before finalize it sets the number of
  * slots; after it, a stream-ordered copy of n == that number of values into the same device buffer, so a captured step
  * graph keeps running with the new values and is never instantiated again.                                               */
@@ -186,12 +208,21 @@ int b200md_update_cmap_params(b200md_ctx* ctx, int nmaps, const int* size, const
 /* CalcCustomTorsionForceKernel::copyParametersToContext (kernels.h:544): same terms, same program per term, new parameters
  * params[n][param_stride], written into the same device buffers.                                                         */
 int b200md_update_custom_torsion_params(b200md_ctx* ctx, int n, const double* params);
+/* CalcCustom{Bond,External}ForceKernel::copyParametersToContext: the same for custom bonds and custom externals.          */
+int b200md_update_custom_bond_params(b200md_ctx* ctx, int n, const double* params);
+int b200md_update_custom_external_params(b200md_ctx* ctx, int n, const double* params);
 /* Test hook, no context and no device: program `which` of a b200md_set_custom_torsions program set, checked as that call
  * checks it (nglobals = the number of global slots), evaluated at (theta, params, globals) on the host by the interpreter
  * source the device kernel runs.  0 and *out on success, -1 with the reason in msg.                                       */
 int b200md_custom_program_probe(int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
                                 int param_stride, int nglobals, int which, double theta, const double* params,
                                 const double* globals, double* out, char* msg, int msglen);
+/* The same for any class (B200MD_CUSTOM_*): a program set of b200md_set_custom_torsions / _bonds / _externals (1 + the
+ * class's number of variables programs per expression), evaluated at the variables vars[] (theta; r; x, y, z) in the box
+ * whose vectors are box[0..2], box[3..5], box[6..8] (read by PERIODIC_DIST only).                                         */
+int b200md_custom_term_probe(int cls, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                             int param_stride, int nglobals, int which, const double* vars, const double* box,
+                             const double* params, const double* globals, double* out, char* msg, int msglen);
 
 /* ---------------------------------------------------------------------------------------------------
  * UpdateStateDataKernel (kernels.h:125-214).                                                         */
@@ -283,7 +314,7 @@ typedef struct b200md_stats {
 int b200md_get_stats(b200md_ctx* ctx, b200md_stats* out);
 /* mean device time (ms) of named phases measured with CUDA events on the engine's stream:
  * phase: 0 pair kernel, 1 pme spread, 2 fft+convolution, 3 pme gather, 4 integrate+constrain, 5 list build,
- * 6 bonded+exceptions (k_bonded and, with custom torsions, k_custom_torsion), 7 custom torsions alone (k_custom_torsion).
+ * 6 bonded+exceptions (k_bonded and, with custom terms, k_custom), 7 custom torsions, bonds and externals alone (k_custom).
  * Runs `reps` isolated launches of that phase on the current state.                                  */
 int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* ms_mean);
 /* stand-alone 3-D FFT entry (the bespoke FFT alone, for parity against fftpack / numpy):

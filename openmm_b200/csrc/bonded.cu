@@ -1,5 +1,6 @@
 // bonded.cu -- harmonic bonds, harmonic angles, periodic torsions, Ryckaert-Bellemans torsions, CMAP terms, 1-4
-// exceptions and the Ewald exclusion correction in ONE launch (sm_90a); custom torsions in a second launch behind it.
+// exceptions and the Ewald exclusion correction in ONE launch (sm_90a); custom torsions, bonds and externals in a second
+// launch behind it.
 // Double precision arithmetic on fp32 positions: these terms are a few thousand work items, far below any roofline, and
 // double removes them from the 1e-4 parity budget.
 //
@@ -227,23 +228,59 @@ __global__ void __launch_bounds__(128) k_bonded(NbDev nb, BondedDev bd, int term
     }
 }
 
-// One thread per custom torsion (CustomTorsionForce, restating ReferenceCustomTorsionIxn::calculateBondIxn): the dihedral as
-// for every other torsion, dE/dtheta from the term's derivative program, the forces through torsion_force, and the energy
-// program only when the energy is asked for.  A kernel of its own rather than a segment of k_bonded: the interpreter's stack
-// and registers would otherwise weigh on every bonded term of every System.
-__global__ void __launch_bounds__(128) k_custom_torsion(NbDev nb, CustomTorsionDev ct, int wantEnergy) {
+// One thread per custom term (restating ReferenceCustomTorsionIxn / ReferenceCustomBondIxn::calculateBondIxn and
+// ReferenceCustomExternalIxn::calculateForce).  A torsion: the dihedral as for every other torsion, dE/dtheta from the term's
+// derivative program, the forces through torsion_force.  A bond: r = |x_b - x_a|, dE/dr, (dE/dr)/r (x_b - x_a) on a and its
+// negative on b.  An external: the particle's continuous coordinate (posq plus cellOffset lattice vectors, what
+// b200md_get_positions reports: the molecule wrap of the list build must not move a restraint), minus the three derivatives.
+// The energy program runs only when the energy is asked for, and a class only when its bit is in `terms`.  A kernel of its
+// own rather than a segment of k_bonded: the interpreter's stack and registers would otherwise weigh on every bonded term of
+// every System.
+__global__ void __launch_bounds__(128) k_custom(NbDev nb, CustomDev ct, int terms, int wantEnergy) {
     const int i = blockIdx.x*blockDim.x + threadIdx.x;
     double e = 0;
     if (i < ct.nslots) {
-        const int p = ct.prog[i];          // uniform across the warp: the terms of one expression fill whole warps
+        const int p = ct.expr[i];          // uniform across the warp: the terms of one expression fill whole warps
         const unsigned char g = ct.group[i];
-        if (p >= 0 && ((ct.groupMask >> (g & 31)) & 1u)) {
+        const int cls = p >= 0 ? ct.exprClass[p] : 0;
+        const int bit = cls == B200MD_CUSTOM_TORSION ? B200MD_TERM_CUSTOM_TORSIONS :
+                        cls == B200MD_CUSTOM_BOND ? B200MD_TERM_CUSTOM_BONDS : B200MD_TERM_CUSTOM_EXTERNALS;
+        if (p >= 0 && (terms & bit) && ((ct.groupMask >> (g & 31)) & 1u)) {
             const int4 at = ct.atoms[i];
-            const Dihedral d = dihedral(nb, at, g & 0x80);
             const double* par = ct.params + (size_t) i*ct.paramStride;
-            const double dE = custom_run(ct.code, ct.imm, ct.progStart[2*p+1], ct.progStart[2*p+2], d.theta, par, ct.globals);
-            torsion_force(nb, at, d, dE);
-            if (wantEnergy) e = custom_run(ct.code, ct.imm, ct.progStart[2*p], ct.progStart[2*p+1], d.theta, par, ct.globals);
+            const int q = ct.exprProg[p];
+            // periodicdistance reduces by the box the pair terms use (a barostat's box reaches it the same way)
+            const CustomBox box = {nb.box.dax, nb.box.bx, nb.box.dby, nb.box.cx, nb.box.cy, nb.box.dcz};
+            double v[3];
+            if (cls == B200MD_CUSTOM_TORSION) {
+                const Dihedral d = dihedral(nb, at, g & 0x80);
+                v[0] = d.theta;
+                const double dE = custom_run(ct.code, ct.imm, ct.progStart[q+1], ct.progStart[q+2], v, par, ct.globals, box);
+                torsion_force(nb, at, d, dE);
+            }
+            else if (cls == B200MD_CUSTOM_BOND) {
+                D3 d = sub(nb.posq[at.y], nb.posq[at.x]);
+                if (g & 0x80) d = min_image_d(d, nb.box);
+                v[0] = sqrt(dot(d, d));
+                const double dE = custom_run(ct.code, ct.imm, ct.progStart[q+1], ct.progStart[q+2], v, par, ct.globals, box);
+                const double s = v[0] > 0 ? dE/v[0] : 0.0;
+                add_force(nb, at.x, scale(d, s));
+                add_force(nb, at.y, scale(d, -s));
+            }
+            else {
+                const float4 x = nb.posq[at.x];
+                v[0] = x.x; v[1] = x.y; v[2] = x.z;
+                const int kx = nb.cellOffset[at.x], ky = nb.cellOffset[at.x + nb.npad], kz = nb.cellOffset[at.x + 2*nb.npad];
+                v[0] += kx*nb.box.dax + ky*(double) nb.box.bx + kz*(double) nb.box.cx;
+                v[1] += ky*nb.box.dby + kz*(double) nb.box.cy;
+                v[2] += kz*nb.box.dcz;
+                D3 f;
+                f.x = -custom_run(ct.code, ct.imm, ct.progStart[q+1], ct.progStart[q+2], v, par, ct.globals, box);
+                f.y = -custom_run(ct.code, ct.imm, ct.progStart[q+2], ct.progStart[q+3], v, par, ct.globals, box);
+                f.z = -custom_run(ct.code, ct.imm, ct.progStart[q+3], ct.progStart[q+4], v, par, ct.globals, box);
+                add_force(nb, at.x, f);
+            }
+            if (wantEnergy) e = custom_run(ct.code, ct.imm, ct.progStart[q], ct.progStart[q+1], v, par, ct.globals, box);
         }
     }
     if (wantEnergy) {
@@ -253,16 +290,16 @@ __global__ void __launch_bounds__(128) k_custom_torsion(NbDev nb, CustomTorsionD
         __syncthreads();
         if (threadIdx.x == 0) {
             const double x = red[0] + red[1] + red[2] + red[3];
-            if (x != 0.0) atomicAdd(&nb.energy[EN_CUSTOM_TORSION], x);
+            if (x != 0.0) atomicAdd(&nb.energy[EN_CUSTOM], x);
         }
     }
 }
 
-void launch_custom_torsion(const NbDev& nb, const CustomTorsionDev& ct, bool energy, cudaStream_t s) {
-    launch_high(k_custom_torsion, (ct.nslots + 127)/128, 128, 0, s, nb, ct, energy ? 1 : 0);
+void launch_custom(const NbDev& nb, const CustomDev& ct, int terms, bool energy, cudaStream_t s) {
+    launch_high(k_custom, (ct.nslots + 127)/128, 128, 0, s, nb, ct, terms, energy ? 1 : 0);
 }
 
-void launch_bonded(const NbDev& nb, const BondedDev& bd, const CustomTorsionDev& ct, int terms, bool energy, cudaStream_t s) {
+void launch_bonded(const NbDev& nb, const BondedDev& bd, const CustomDev& ct, int terms, bool energy, cudaStream_t s) {
     int n = 0;
     if (terms & B200MD_TERM_BONDS) n += bd.nbonds;
     if (terms & B200MD_TERM_ANGLES) n += bd.nangles;
@@ -274,5 +311,5 @@ void launch_bonded(const NbDev& nb, const BondedDev& bd, const CustomTorsionDev&
         int per = (n + nb.world - 1)/nb.world;
         launch_high(k_bonded, (per + 127)/128, 128, 0, s, nb, bd, terms, energy ? 1 : 0);
     }
-    if ((terms & B200MD_TERM_CUSTOM_TORSIONS) && ct.nslots > 0) launch_custom_torsion(nb, ct, energy, s);
+    if (terms & ct.terms) launch_custom(nb, ct, terms, energy, s);
 }

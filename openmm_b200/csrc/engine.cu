@@ -81,18 +81,28 @@ struct CmapTable : TermTable<int4, double> {
     std::vector<int> map; std::vector<int2> maps;
     DevBuf<int> mapDev; DevBuf<int2> mapsDev;
 };
-// Custom torsions: atoms, params [n][stride] and groups in the caller's term order; besides, the programs (code = (opcode,
-// operand), imm, progStart), the expression of every term and the global values.  finalize lays the terms out as
-// k_custom_torsion reads them: grouped by expression, each group padded to whole warps; slot[i] is the slot of term i.
-struct CustomTorsionTable : TermTable<int4, double> {
-    int stride = 0, nprog = 0, nslots = 0;
+// One class of custom terms (B200MD_CUSTOM_*): atoms (a torsion's four, a bond's two, an external's one, zero-padded to an
+// int4), params [n][stride] and groups in the caller's term order; besides, the programs (code = (opcode, operand), imm,
+// progStart; 1 + the class's number of variables programs per expression) and the expression of every term.
+struct CustomClass : TermTable<int4, double> {
+    int stride = 0, nprog = 0;
     std::vector<int2> code; std::vector<double> imm; std::vector<int> progStart, prog, slot;
+};
+// The custom torsions, bonds and externals and the global values (one slot space for all three).  finalize lays the terms of
+// all three out as k_custom reads them (CustomDev): grouped by expression, each group padded to whole warps, with one
+// parameter stride (the widest class's); cls[k].slot[i] is the slot of term i of class k.
+struct CustomTable {
+    CustomClass cls[3];
+    int nslots = 0, stride = 0;
     std::vector<double> globals;
-    DevBuf<int2> codeDev; DevBuf<double> immDev, globalsDev; DevBuf<int> progStartDev, progDev;
+    DevBuf<int4> atomsDev; DevBuf<double> paramsDev, immDev, globalsDev; DevBuf<unsigned char> groupDev;
+    DevBuf<int2> codeDev; DevBuf<int> exprDev, exprClassDev, exprProgDev, progStartDev;
     // params in the slot layout (padding slots 0)
     std::vector<double> slot_params() const {
         std::vector<double> p((size_t) nslots*stride, 0.0);
-        for (int i = 0; i < n; i++) std::copy(params.begin() + (size_t) i*stride, params.begin() + (size_t) (i+1)*stride, p.begin() + (size_t) slot[i]*stride);
+        for (const CustomClass& t : cls)
+            for (int i = 0; i < t.n; i++)
+                std::copy(t.params.begin() + (size_t) i*t.stride, t.params.begin() + (size_t) (i+1)*t.stride, p.begin() + (size_t) t.slot[i]*stride);
         return p;
     }
 };
@@ -184,7 +194,7 @@ struct b200md_ctx {
     TermTable<int4, double4> torsions;      // (k, phase, n, 0)
     TermTable<int4, double> rb;             // [n][6] c0..c5
     CmapTable cmap;
-    CustomTorsionTable custom;
+    CustomTable custom;
     std::vector<int> conI, conJ; std::vector<double> conD;
     int cmFreq = 0;
     std::vector<int4> hUnitAtoms;        // host copy of the integration units (ownership cuts of the multi-GPU data plane)
@@ -224,7 +234,7 @@ struct b200md_ctx {
     NbDev nb{};
     PmeDev pme{};
     BondedDev bd{};
-    CustomTorsionDev ctd{};
+    CustomDev ctd{};
     UnitDev units{};
     IntegDev integ{};
     bool haveIntegrator = false;
@@ -414,41 +424,73 @@ extern "C" int b200md_set_cmap(b200md_ctx* ctx, int nmaps, const int* size, cons
     ctx->cmap.map.assign(map, map + n); ctx->cmap.maps.swap(maps);
     API_END(ctx)
 }
-// A custom-torsion program set (b200md_set_custom_torsions): prog_start well formed and every program passing
-// custom_check_program (nglobals < 0: GLOBAL operands are checked at finalize).  Returns the instructions as (opcode, operand).
-static std::vector<int2> check_programs(int nprog, const int* prog_start, const int* op, const int* arg, int stride, int nglobals) {
-    require(nprog >= 0, "set_custom_torsions: negative number of programs");
-    require(stride >= 0 && stride <= B200MD_CUSTOM_MAX_PARAMS, "set_custom_torsions: more than 16 parameters per torsion");
-    require(nprog == 0 || prog_start[0] == 0, "set_custom_torsions: prog_start[0] must be 0");
-    for (int q = 0; q < 2*nprog; q++) require(prog_start[q+1] >= prog_start[q], "set_custom_torsions: prog_start must not decrease");
-    const int total = nprog ? prog_start[2*nprog] : 0;
+// What the messages of a custom class's calls name it
+struct CustomNames { const char* call; const char* term; const char* per; };
+static const CustomNames CUSTOM_NAMES[3] = {{"set_custom_torsions", "custom torsion", "torsion"},
+                                            {"set_custom_bonds", "custom bond", "bond"},
+                                            {"set_custom_externals", "custom external", "particle"}};
+
+// A program set of class cls (b200md_set_custom_torsions / _bonds / _externals): prog_start well formed and every program
+// passing custom_check_program (nglobals < 0: GLOBAL operands are checked at finalize).  Returns the instructions as
+// (opcode, operand).
+static std::vector<int2> check_programs(int cls, int nprog, const int* prog_start, const int* op, const int* arg, int stride, int nglobals) {
+    const std::string call = CUSTOM_NAMES[cls].call;
+    require(nprog >= 0, (call + ": negative number of programs").c_str());
+    require(stride >= 0 && stride <= B200MD_CUSTOM_MAX_PARAMS, (call + ": more than 16 parameters per " + CUSTOM_NAMES[cls].per).c_str());
+    require(nprog == 0 || prog_start[0] == 0, (call + ": prog_start[0] must be 0").c_str());
+    const int nq = nprog*(1 + custom_num_vars(cls));
+    for (int q = 0; q < nq; q++) require(prog_start[q+1] >= prog_start[q], (call + ": prog_start must not decrease").c_str());
+    const int total = nprog ? prog_start[nq] : 0;
     std::vector<int2> code(total);
     for (int k = 0; k < total; k++) code[k] = make_int2(op[k], arg[k]);
-    for (int q = 0; q < 2*nprog; q++) {
-        const char* why = custom_check_program(code.data(), prog_start[q], prog_start[q+1], stride, nglobals);
+    for (int q = 0; q < nq; q++) {
+        const char* why = custom_check_program(cls, code.data(), prog_start[q], prog_start[q+1], stride, nglobals);
         if (why) throw std::runtime_error(std::string(why) + " (program " + std::to_string(q) + ")");
     }
     return code;
 }
+// The terms of class cls: term i evaluates expression prog[i] on the atoms atoms[w*i .. w*i+w-1] (w = 4, 2, 1)
+static void set_custom(b200md_ctx* ctx, int cls, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                       int stride, int n, const int* prog, const int* atoms, const double* params) {
+    const CustomNames& nm = CUSTOM_NAMES[cls];
+    check_set(ctx, nm.call, n);
+    require(ctx->world == 1, (std::string(nm.term) + "s are not supported in multi-GPU runs").c_str());
+    std::vector<int2> code = check_programs(cls, nprog, prog_start, op, arg, stride, -1);
+    for (int i = 0; i < n; i++) require(prog[i] >= 0 && prog[i] < nprog, (std::string(nm.term) + ": program index out of range").c_str());
+    const int w = cls == B200MD_CUSTOM_TORSION ? 4 : cls == B200MD_CUSTOM_BOND ? 2 : 1;
+    std::vector<int4> a(n, make_int4(0, 0, 0, 0)); std::vector<double> p(params, params + (size_t) n*stride);
+    for (int i = 0; i < n; i++) {
+        int* q = &a[i].x;
+        for (int k = 0; k < w; k++) q[k] = atoms[w*i + k];
+    }
+    CustomClass& t = ctx->custom.cls[cls];
+    t.set(ctx->natoms, nm.term, n, a, p);
+    t.stride = stride; t.nprog = nprog; t.code.swap(code);
+    t.imm.assign(imm, imm + t.code.size());
+    t.progStart.assign(prog_start, prog_start + (nprog ? nprog*(1 + custom_num_vars(cls)) + 1 : 0)); t.prog.assign(prog, prog + n);
+}
 extern "C" int b200md_set_custom_torsions(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
                                           int stride, int n, const int* prog, const int* atoms, const double* params) {
     API_BEGIN(ctx)
-    check_set(ctx, "set_custom_torsions", n);
-    require(ctx->world == 1, "custom torsions are not supported in multi-GPU runs");
-    std::vector<int2> code = check_programs(nprog, prog_start, op, arg, stride, -1);
-    for (int i = 0; i < n; i++) require(prog[i] >= 0 && prog[i] < nprog, "custom torsion: program index out of range");
-    std::vector<int4> a(n); std::vector<double> p(params, params + (size_t) n*stride);
-    for (int i = 0; i < n; i++) a[i] = make_int4(atoms[4*i], atoms[4*i+1], atoms[4*i+2], atoms[4*i+3]);
-    CustomTorsionTable& t = ctx->custom;
-    t.set(ctx->natoms, "custom torsion", n, a, p);
-    t.stride = stride; t.nprog = nprog; t.code.swap(code);
-    t.imm.assign(imm, imm + t.code.size()); t.progStart.assign(prog_start, prog_start + (nprog ? 2*nprog + 1 : 0)); t.prog.assign(prog, prog + n);
+    set_custom(ctx, B200MD_CUSTOM_TORSION, nprog, prog_start, op, arg, imm, stride, n, prog, atoms, params);
+    API_END(ctx)
+}
+extern "C" int b200md_set_custom_bonds(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                       int stride, int n, const int* prog, const int* atoms, const double* params) {
+    API_BEGIN(ctx)
+    set_custom(ctx, B200MD_CUSTOM_BOND, nprog, prog_start, op, arg, imm, stride, n, prog, atoms, params);
+    API_END(ctx)
+}
+extern "C" int b200md_set_custom_externals(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                           int stride, int n, const int* prog, const int* atoms, const double* params) {
+    API_BEGIN(ctx)
+    set_custom(ctx, B200MD_CUSTOM_EXTERNAL, nprog, prog_start, op, arg, imm, stride, n, prog, atoms, params);
     API_END(ctx)
 }
 extern "C" int b200md_set_custom_globals(b200md_ctx* ctx, int n, const double* values) {
     API_BEGIN(ctx)
     require(n >= 0, "set_custom_globals: negative count");
-    CustomTorsionTable& t = ctx->custom;
+    CustomTable& t = ctx->custom;
     if (!ctx->finalized) { t.globals.assign(values, values + n); return 0; }
     require(n == (int) t.globals.size(), "set_custom_globals: the number of global parameters cannot change after finalize");
     t.globals.assign(values, values + n);
@@ -456,28 +498,39 @@ extern "C" int b200md_set_custom_globals(b200md_ctx* ctx, int n, const double* v
     if (n) CUDA_CHECK(cudaMemcpyAsync(t.globalsDev.p, t.globals.data(), sizeof(double)*n, cudaMemcpyHostToDevice, ctx->stream));
     API_END(ctx)
 }
-extern "C" int b200md_custom_program_probe(int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
-                                           int stride, int nglobals, int which, double theta, const double* params,
-                                           const double* globals, double* out, char* msg, int msglen) {
+extern "C" int b200md_custom_term_probe(int cls, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                        int stride, int nglobals, int which, const double* vars, const double* box,
+                                        const double* params, const double* globals, double* out, char* msg, int msglen) {
     try {
+        require(cls >= B200MD_CUSTOM_TORSION && cls <= B200MD_CUSTOM_EXTERNAL, "custom_term_probe: unknown class");
         require(nglobals >= 0, "custom_program_probe: negative number of globals");
-        const std::vector<int2> code = check_programs(nprog, prog_start, op, arg, stride, nglobals);
-        require(which >= 0 && which < 2*nprog, "custom_program_probe: program index out of range");
-        *out = custom_run(code.data(), imm, prog_start[which], prog_start[which+1], theta, params, globals);
+        const std::vector<int2> code = check_programs(cls, nprog, prog_start, op, arg, stride, nglobals);
+        require(which >= 0 && which < nprog*(1 + custom_num_vars(cls)), "custom_program_probe: program index out of range");
+        CustomBox b = {1.0, 0.0, 1.0, 0.0, 0.0, 1.0};
+        if (box) b = CustomBox{box[0], box[3], box[4], box[6], box[7], box[8]};
+        *out = custom_run(code.data(), imm, prog_start[which], prog_start[which+1], vars, params, globals, b);
         return 0;
     } catch (std::exception& e) {
         if (msg && msglen > 0) { strncpy(msg, e.what(), msglen - 1); msg[msglen - 1] = 0; }
         return -1;
     }
 }
+extern "C" int b200md_custom_program_probe(int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                           int stride, int nglobals, int which, double theta, const double* params,
+                                           const double* globals, double* out, char* msg, int msglen) {
+    return b200md_custom_term_probe(B200MD_CUSTOM_TORSION, nprog, prog_start, op, arg, imm, stride, nglobals, which, &theta, nullptr,
+                                    params, globals, out, msg, msglen);
+}
 extern "C" int b200md_set_bonded_groups(b200md_ctx* ctx, int kind, int n, const int* group) {
     API_BEGIN(ctx)
     check_set(ctx, "set_bonded_groups", n);
-    require(kind >= B200MD_BONDED_BONDS && kind <= B200MD_BONDED_CUSTOM_TORSIONS,
-            "set_bonded_groups: kind must be 0 (bonds), 1 (angles), 2 (torsions), 3 (RB torsions), 4 (CMAP) or 5 (custom torsions)");
+    require(kind >= B200MD_BONDED_BONDS && kind <= B200MD_BONDED_CUSTOM_EXTERNALS,
+            "set_bonded_groups: kind must be 0 (bonds), 1 (angles), 2 (torsions), 3 (RB torsions), 4 (CMAP), 5 (custom torsions), "
+            "6 (custom bonds) or 7 (custom externals)");
     std::vector<unsigned char>& g = kind == B200MD_BONDED_BONDS ? ctx->bonds.group : kind == B200MD_BONDED_ANGLES ? ctx->angles.group :
                                     kind == B200MD_BONDED_TORSIONS ? ctx->torsions.group : kind == B200MD_BONDED_RB_TORSIONS ? ctx->rb.group :
-                                    kind == B200MD_BONDED_CMAP ? ctx->cmap.group : ctx->custom.group;
+                                    kind == B200MD_BONDED_CMAP ? ctx->cmap.group :
+                                    ctx->custom.cls[kind - B200MD_BONDED_CUSTOM_TORSIONS].group;
     g.resize(n);
     for (int i = 0; i < n; i++) { require(group[i] >= 0 && (group[i] & ~0x80) < 32, "force group out of range"); g[i] = (unsigned char) group[i]; }
     API_END(ctx)
@@ -1259,41 +1312,74 @@ static bool fft_beside_tiles(const b200md_ctx* c) {
     return c->mg == MG_SINGLE && !c->pmeOnly && c->overlapPme && !c->nb.smPartition && c->nbdesc.method == B200MD_NB_PME;
 }
 
-// finalize: the custom torsions in the layout of k_custom_torsion (CustomTorsionDev): grouped by expression, each group padded
-// to whole warps, and the programs, checked once more now that the number of global slots is final
-static void upload_custom_torsions(b200md_ctx* c) {
-    CustomTorsionTable& t = c->custom;
-    CustomTorsionDev& d = c->ctd;
-    d = CustomTorsionDev{};
+// finalize: the custom terms of all three classes in the layout of k_custom (CustomDev): grouped by expression, each group
+// padded to whole warps, and the programs, checked once more now that the number of global slots is final
+static void upload_custom(b200md_ctx* c) {
+    CustomTable& t = c->custom;
+    CustomDev& d = c->ctd;
+    d = CustomDev{};
     d.groupMask = 0xffffffffu;
-    // the global values get their buffer even without terms: a CustomTorsionForce with no torsions may still name globals, and
+    // the global values get their buffer even without terms: a custom force with no terms may still name globals, and
     // b200md_set_custom_globals copies into this buffer after finalize
     t.globalsDev.alloc(std::max<size_t>(t.globals.size(), 1)); t.globalsDev.upload(t.globals);
     d.globals = t.globalsDev.p;
-    if (t.n == 0) return;
-    require(c->mg == MG_SINGLE, "custom torsions are not supported in multi-GPU runs");
-    require(t.group.empty() || (int) t.group.size() == t.n, "set_bonded_groups: group array length differs from the number of terms");
-    for (int q = 0; q < 2*t.nprog; q++) {
-        const char* why = custom_check_program(t.code.data(), t.progStart[q], t.progStart[q+1], t.stride, (int) t.globals.size());
-        if (why) throw std::runtime_error(std::string(why) + " (program " + std::to_string(q) + ")");
+    const int bits[3] = {B200MD_TERM_CUSTOM_TORSIONS, B200MD_TERM_CUSTOM_BONDS, B200MD_TERM_CUSTOM_EXTERNALS};
+    // expressions of all classes one after the other (class k's expression p is expression exprBase[k] + p), their programs
+    // likewise, the code of class k shifted by the instructions of the classes before it
+    std::vector<int2> code; std::vector<double> imm; std::vector<int> progStart(1, 0), exprClass, exprProg;
+    std::vector<int> exprBase(3, 0);
+    t.stride = 0;
+    for (int k = 0; k < 3; k++) {
+        CustomClass& cl = t.cls[k];
+        exprBase[k] = (int) exprClass.size();
+        if (cl.n == 0) continue;
+        require(c->mg == MG_SINGLE, (std::string(CUSTOM_NAMES[k].term) + "s are not supported in multi-GPU runs").c_str());
+        require(cl.group.empty() || (int) cl.group.size() == cl.n, "set_bonded_groups: group array length differs from the number of terms");
+        const int nv = custom_num_vars(k);
+        for (int q = 0; q < cl.nprog*(1 + nv); q++) {
+            const char* why = custom_check_program(k, cl.code.data(), cl.progStart[q], cl.progStart[q+1], cl.stride, (int) t.globals.size());
+            if (why) throw std::runtime_error(std::string(why) + " (program " + std::to_string(q) + ")");
+        }
+        const int codeBase = (int) code.size();
+        for (int p = 0; p < cl.nprog; p++) {
+            exprClass.push_back(k);
+            exprProg.push_back((int) progStart.size() - 1 + p*(1 + nv));
+        }
+        for (int q = 0; q < cl.nprog*(1 + nv); q++) progStart.push_back(codeBase + cl.progStart[q+1]);
+        code.insert(code.end(), cl.code.begin(), cl.code.end());
+        imm.insert(imm.end(), cl.imm.begin(), cl.imm.end());
+        t.stride = std::max(t.stride, cl.stride);
+        d.terms |= bits[k];
     }
-    t.slot.assign(t.n, 0);
+    t.nslots = 0;
+    if (d.terms == 0) return;
     int cursor = 0;
-    for (int p = 0; p < t.nprog; p++) {
-        for (int i = 0; i < t.n; i++) if (t.prog[i] == p) t.slot[i] = cursor++;
-        cursor = (cursor + 31)/32*32;
+    for (int k = 0; k < 3; k++) {
+        CustomClass& cl = t.cls[k];
+        cl.slot.assign(cl.n, 0);
+        for (int p = 0; p < cl.nprog; p++) {
+            for (int i = 0; i < cl.n; i++) if (cl.prog[i] == p) cl.slot[i] = cursor++;
+            cursor = (cursor + 31)/32*32;
+        }
     }
     t.nslots = cursor;
     std::vector<int4> atoms(cursor, make_int4(0, 0, 0, 0));
     std::vector<unsigned char> group(cursor, 0);
-    std::vector<int> prog(cursor, -1);
-    for (int i = 0; i < t.n; i++) { atoms[t.slot[i]] = t.atoms[i]; group[t.slot[i]] = t.group.empty() ? 0 : t.group[i]; prog[t.slot[i]] = t.prog[i]; }
-    t.atomsDev.upload(atoms); t.groupDev.upload(group); t.progDev.upload(prog);
+    std::vector<int> expr(cursor, -1);
+    for (int k = 0; k < 3; k++) {
+        const CustomClass& cl = t.cls[k];
+        for (int i = 0; i < cl.n; i++) {
+            atoms[cl.slot[i]] = cl.atoms[i]; group[cl.slot[i]] = cl.group.empty() ? 0 : cl.group[i]; expr[cl.slot[i]] = exprBase[k] + cl.prog[i];
+        }
+    }
+    t.atomsDev.upload(atoms); t.groupDev.upload(group); t.exprDev.upload(expr);
     const std::vector<double> par = t.slot_params();
     t.paramsDev.alloc(std::max<size_t>(par.size(), 1)); t.paramsDev.upload(par);
-    t.codeDev.upload(t.code); t.immDev.upload(t.imm); t.progStartDev.upload(t.progStart);
+    t.codeDev.upload(code); t.immDev.upload(imm); t.progStartDev.upload(progStart);
+    t.exprClassDev.upload(exprClass); t.exprProgDev.upload(exprProg);
     d.nslots = t.nslots; d.paramStride = t.stride;
-    d.atoms = t.atomsDev.p; d.params = t.paramsDev.p; d.group = t.groupDev.p; d.prog = t.progDev.p;
+    d.atoms = t.atomsDev.p; d.params = t.paramsDev.p; d.group = t.groupDev.p; d.expr = t.exprDev.p;
+    d.exprClass = t.exprClassDev.p; d.exprProg = t.exprProgDev.p;
     d.code = t.codeDev.p; d.imm = t.immDev.p; d.progStart = t.progStartDev.p;
 }
 
@@ -1403,7 +1489,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     c->cmap.mapDev.upload(c->cmap.map); c->cmap.mapsDev.upload(c->cmap.maps); bd.cmapMap = c->cmap.mapDev.p; bd.cmapMaps = c->cmap.mapsDev.p;
     bd.excPeriodic = c->nbdesc.exceptions_periodic;
     bd.groupMask = 0xffffffffu;
-    upload_custom_torsions(c);
+    upload_custom(c);
     upload_params(c);
     build_units(c);
     build_ccma(c);
@@ -1414,7 +1500,8 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
             require(fft_slab_path(probe), "multi-GPU: the PME grid plane does not fit the slab FFT kernels (B200MD_MGPU=nccl selects the NCCL scheme)");
         }
     }
-    // ---- molecules (connected components of bonds, angles, torsions, RB torsions, CMAP terms, custom torsions, constraints and exceptions) for the wrap at list
+    // ---- molecules (connected components of bonds, angles, torsions, RB torsions, CMAP terms, custom torsions and bonds,
+    // constraints and exceptions; not custom externals, which act on one particle) for the wrap at list
     // builds; off for non-periodic systems and with more than one rank (every rank would have to wrap in the same step,
     // and the reciprocal-space rank builds no list) ----
     c->cellOffset.alloc((size_t) 3*NP); c->cellOffset.zero();
@@ -1426,7 +1513,8 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
         auto join = [&](int a, int b) { a = find(a); b = find(b); if (a != b) parent[std::max(a, b)] = std::min(a, b); };
         for (const int2& a : c->bonds.atoms) join(a.x, a.y);
         for (const int4& a : c->angles.atoms) { join(a.x, a.y); join(a.y, a.z); }
-        for (auto* t : {&c->torsions.atoms, &c->rb.atoms, &c->cmap.atoms, &c->custom.atoms}) for (const int4& a : *t) { join(a.x, a.y); join(a.y, a.z); join(a.z, a.w); }
+        for (auto* t : {&c->torsions.atoms, &c->rb.atoms, &c->cmap.atoms, &c->custom.cls[B200MD_CUSTOM_TORSION].atoms}) for (const int4& a : *t) { join(a.x, a.y); join(a.y, a.z); join(a.z, a.w); }
+        for (const int4& a : c->custom.cls[B200MD_CUSTOM_BOND].atoms) join(a.x, a.y);
         for (size_t d = 1; d < c->cmap.atoms.size(); d += 2) join(c->cmap.atoms[d-1].x, c->cmap.atoms[d].x);     // a CMAP term's two dihedrals
         for (size_t i = 0; i < c->conI.size(); i++) join(c->conI[i], c->conJ[i]);
         for (const int2& a : c->exc.atoms) join(a.x, a.y);
@@ -1519,16 +1607,30 @@ extern "C" int b200md_update_cmap_params(b200md_ctx* ctx, int nmaps, const int* 
     API_END(ctx)
 }
 
-// CalcCustomTorsionForceKernel::copyParametersToContext (kernels.h:544): same terms and programs, new parameters, into the
-// same device buffer.
+// CalcCustom{Torsion,Bond,External}ForceKernel::copyParametersToContext (kernels.h): same terms and programs, new
+// parameters, into the same device buffer.
+static void update_custom(b200md_ctx* ctx, int cls, const char* call, const char* terms, int n, const double* params) {
+    require(ctx->finalized, (std::string(call) + " before finalize").c_str());
+    CustomTable& t = ctx->custom;
+    CustomClass& cl = t.cls[cls];
+    require(n == cl.n, (std::string("updateParametersInContext: The number of ") + terms + " has changed").c_str());
+    CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+    cl.params.assign(params, params + (size_t) n*cl.stride);
+    if (n) t.paramsDev.upload(t.slot_params());
+}
 extern "C" int b200md_update_custom_torsion_params(b200md_ctx* ctx, int n, const double* params) {
     API_BEGIN(ctx)
-    require(ctx->finalized, "update_custom_torsion_params before finalize");
-    CustomTorsionTable& t = ctx->custom;
-    require(n == t.n, "updateParametersInContext: The number of torsions has changed");
-    CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-    t.params.assign(params, params + (size_t) n*t.stride);
-    if (n) t.paramsDev.upload(t.slot_params());
+    update_custom(ctx, B200MD_CUSTOM_TORSION, "update_custom_torsion_params", "torsions", n, params);
+    API_END(ctx)
+}
+extern "C" int b200md_update_custom_bond_params(b200md_ctx* ctx, int n, const double* params) {
+    API_BEGIN(ctx)
+    update_custom(ctx, B200MD_CUSTOM_BOND, "update_custom_bond_params", "bonds", n, params);
+    API_END(ctx)
+}
+extern "C" int b200md_update_custom_external_params(b200md_ctx* ctx, int n, const double* params) {
+    API_BEGIN(ctx)
+    update_custom(ctx, B200MD_CUSTOM_EXTERNAL, "update_custom_external_params", "particles", n, params);
     API_END(ctx)
 }
 
@@ -1738,14 +1840,15 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     const bool pmeRank = nccl_pme_rank(c), directRank = c->mg == MG_NCCL_SPLIT && !pmeRank;
     const bool direct = (terms & B200MD_TERM_NB_DIRECT) && c->haveNb && !pmeRank;
     const bool recip = (terms & B200MD_TERM_NB_RECIP) && c->haveNb && c->nb.method == B200MD_NB_PME && !directRank;
+    const int customBits = B200MD_TERM_CUSTOM_TORSIONS | B200MD_TERM_CUSTOM_BONDS | B200MD_TERM_CUSTOM_EXTERNALS;
     int bterms = terms & (B200MD_TERM_BONDS | B200MD_TERM_ANGLES | B200MD_TERM_TORSIONS | B200MD_TERM_RB_TORSIONS | B200MD_TERM_CMAP |
-                          B200MD_TERM_CUSTOM_TORSIONS);
+                          customBits);
     if (c->haveNb) bterms |= terms & B200MD_TERM_NB_DIRECT;
     const int nbonded = c->bd.nbonds + c->bd.nangles + c->bd.ntorsions + c->bd.nrb + c->bd.ncmap + c->bd.nexc;
     // the k_bonded branch is counted as one launch whenever it is taken (even when the selected classes have no terms and
-    // launch_bonded skips the kernel); k_custom_torsion is counted when it runs
-    const bool classic = (bterms & ~B200MD_TERM_CUSTOM_TORSIONS) && nbonded > 0;
-    const bool custom = (bterms & B200MD_TERM_CUSTOM_TORSIONS) && c->ctd.nslots > 0;
+    // launch_bonded skips the kernel); k_custom is counted once when it runs, for any number of custom classes
+    const bool classic = (bterms & ~customBits) && nbonded > 0;
+    const bool custom = (bterms & c->ctd.terms) != 0;
     const bool bonded = (classic || custom) && !pmeRank;
     // Reciprocal space (spread -> FFT/convolution -> gather, in USER atom order: independent of the neighbour list) and
     // direct space (list check / rebuild, tile kernel, bonded terms) are independent until the integrator: fork them onto
@@ -1783,7 +1886,7 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     };
     auto launch_bonded_terms = [&](cudaStream_t sb) {
         BondedDev bd = c->bd; bd.groupMask = groupMask;
-        CustomTorsionDev ct = c->ctd; ct.groupMask = groupMask;
+        CustomDev ct = c->ctd; ct.groupMask = groupMask;
         launch_bonded(c->nb, bd, ct, bterms, energy, sb);
         launches += (classic ? 1 : 0) + (custom ? 1 : 0);
     };
@@ -1911,7 +2014,7 @@ extern "C" int b200md_compute_groups(b200md_ctx* ctx, int terms, unsigned int bo
         if (terms & B200MD_TERM_TORSIONS) e += h[EN_TORSION];
         if (terms & B200MD_TERM_RB_TORSIONS) e += h[EN_RBTORSION];
         if (terms & B200MD_TERM_CMAP) e += h[EN_CMAP];
-        if (terms & B200MD_TERM_CUSTOM_TORSIONS) e += h[EN_CUSTOM_TORSION];
+        if (terms & (B200MD_TERM_CUSTOM_TORSIONS | B200MD_TERM_CUSTOM_BONDS | B200MD_TERM_CUSTOM_EXTERNALS)) e += h[EN_CUSTOM];
         if (ctx->haveNb) {
             if (terms & B200MD_TERM_NB_DIRECT) {
                 e += h[EN_NB] + h[EN_EXC];
@@ -2198,7 +2301,7 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
             case 4: launch_integrate(c->nb, c->units, c->integ, local, s); break;
             case 5: launch_list_build(c->nb, s); break;
             case 6: launch_bonded(c->nb, c->bd, c->ctd, B200MD_TERM_ALL, false, s); break;
-            case 7: launch_custom_torsion(c->nb, c->ctd, false, s); break;
+            case 7: launch_custom(c->nb, c->ctd, B200MD_TERM_ALL, false, s); break;
             default: throw std::runtime_error("unknown phase");
         }
         CUDA_CHECK(cudaEventRecord(e1, s));

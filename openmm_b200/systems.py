@@ -85,6 +85,28 @@ class SystemDesc:
     custom_op: np.ndarray = field(default_factory=_i)
     custom_arg: np.ndarray = field(default_factory=_i)
     custom_imm: np.ndarray = field(default_factory=_d)
+    # CustomBondForce (cbond_*) and CustomExternalForce (cext_*), laid out as the custom torsions: per expression its energy (of
+    # r; of x, y, z) and parameter names, per term its expression, atoms ([n,2]; [n]) and parameters; the compiled programs
+    # (a bond: 2p energy, 2p+1 dE/dr; an external: 4p energy, 4p+1..4p+3 its x, y, z derivatives).  The global parameters
+    # are custom_global_names / custom_global_values for all three classes.
+    cbond_energy: tuple = ()
+    cbond_param_names: tuple = ()
+    cbond_prog: np.ndarray = field(default_factory=_i)
+    cbond_atoms: np.ndarray = field(default_factory=lambda: np.zeros((0, 2), dtype=np.int32))
+    cbond_params: np.ndarray = field(default_factory=lambda: np.zeros((0, 0)))
+    cbond_prog_start: np.ndarray = field(default_factory=_i)
+    cbond_op: np.ndarray = field(default_factory=_i)
+    cbond_arg: np.ndarray = field(default_factory=_i)
+    cbond_imm: np.ndarray = field(default_factory=_d)
+    cext_energy: tuple = ()
+    cext_param_names: tuple = ()
+    cext_prog: np.ndarray = field(default_factory=_i)
+    cext_atoms: np.ndarray = field(default_factory=_i)
+    cext_params: np.ndarray = field(default_factory=lambda: np.zeros((0, 0)))
+    cext_prog_start: np.ndarray = field(default_factory=_i)
+    cext_op: np.ndarray = field(default_factory=_i)
+    cext_arg: np.ndarray = field(default_factory=_i)
+    cext_imm: np.ndarray = field(default_factory=_d)
     con_i: np.ndarray = field(default_factory=_i)
     con_j: np.ndarray = field(default_factory=_i)
     con_d: np.ndarray = field(default_factory=_d)
@@ -145,11 +167,13 @@ class SystemDesc:
         return d
 
     def save(self, path):
+        names = ("custom_param_names", "cbond_param_names", "cext_param_names")
         d = {k: (np.asarray(v) if v is not None else np.zeros(0)) for k, v in self.__dict__.items()
-             if not isinstance(v, str) and k != "custom_param_names"}
-        width = max([len(p) for p in self.custom_param_names] + [0])
-        rows = [list(p) + [""]*(width - len(p)) for p in self.custom_param_names]
-        d["custom_param_names"] = np.array(rows, dtype=str).reshape(len(rows), width)
+             if not isinstance(v, str) and k not in names}
+        for k in names:
+            width = max([len(p) for p in getattr(self, k)] + [0])
+            rows = [list(p) + [""]*(width - len(p)) for p in getattr(self, k)]
+            d[k] = np.array(rows, dtype=str).reshape(len(rows), width)
         d["name"] = np.array(self.name)
         np.savez_compressed(path, **d)
 
@@ -161,9 +185,9 @@ class SystemDesc:
             v = z[k]
             if k == "name":
                 kw[k] = str(v)
-            elif k in ("custom_energy", "custom_global_names"):
+            elif k in ("custom_energy", "custom_global_names", "cbond_energy", "cext_energy"):
                 kw[k] = tuple(str(x) for x in v)
-            elif k == "custom_param_names":
+            elif k in ("custom_param_names", "cbond_param_names", "cext_param_names"):
                 kw[k] = tuple(tuple(str(y) for y in x if str(y)) for x in v)
             elif k == "box":
                 kw[k] = v if v.size == 9 else None
@@ -227,6 +251,57 @@ def periodic_to_custom(desc):
     d = _custom_only(desc, [PERIODIC_CUSTOM], [("k", "n", "theta0")], np.zeros(len(desc.tor_i)), atoms, params)
     d.tor_i, d.tor_j, d.tor_k, d.tor_l, d.tor_n, d.tor_phase, d.tor_kk = _i(), _i(), _i(), _i(), _i(), _d(), _d()
     return d
+
+
+def _with_custom_class(desc, cls, energy, param_names, prog, atoms, params):
+    """desc with exactly these custom bonds (cls "cbond", atoms [n,2]) or custom externals (cls "cext", atoms [n]), expressions
+    not compiled yet"""
+    import copy
+    d = copy.copy(desc)
+    setattr(d, cls + "_energy", tuple(energy))
+    setattr(d, cls + "_param_names", tuple(tuple(p) for p in param_names))
+    setattr(d, cls + "_prog", np.asarray(prog, dtype=np.int32))
+    setattr(d, cls + "_atoms", np.asarray(atoms, dtype=np.int32).reshape((-1, 2) if cls == "cbond" else (-1,)))
+    width = max([len(p) for p in param_names] + [0])
+    setattr(d, cls + "_params", np.asarray(params, dtype=np.float64).reshape(len(prog), -1) if len(prog) else np.zeros((0, width)))
+    for k, v in (("_prog_start", _i()), ("_op", _i()), ("_arg", _i()), ("_imm", _d())):
+        setattr(d, cls + k, v)
+    return d
+
+
+HARMONIC_CUSTOM_BOND = "0.5*k*(r-r0)^2"
+# the position restraint of OpenMM's documentation, and the same without the minimum image
+POSITION_RESTRAINT_PERIODIC = "k*periodicdistance(x, y, z, x0, y0, z0)^2"
+POSITION_RESTRAINT_PLAIN = "k*((x-x0)^2+(y-y0)^2+(z-z0)^2)"
+# the reference point of with_position_restraints: the atom's position shifted by this much (nm), so that forces are not zero
+RESTRAINT_OFFSET = (0.011, -0.007, 0.005)
+
+
+def bonds_to_custom(desc):
+    """The same System with every HarmonicBondForce bond written as the CustomBondForce HARMONIC_CUSTOM_BOND with per-bond
+    parameters (k, r0)."""
+    atoms = np.stack([desc.bond_i, desc.bond_j], axis=1) if len(desc.bond_i) else np.zeros((0, 2))
+    params = np.stack([desc.bond_k, desc.bond_r0], axis=1) if len(desc.bond_i) else np.zeros((0, 2))
+    d = _with_custom_class(desc, "cbond", [HARMONIC_CUSTOM_BOND], [("k", "r0")], np.zeros(len(atoms)), atoms, params)
+    d.bond_i, d.bond_j, d.bond_r0, d.bond_k = _i(), _i(), _d(), _d()
+    return d
+
+
+def solute_heavy_atoms(desc):
+    """The atoms heavier than 1.5 amu of every molecule (desc.molecules()) of more than three atoms: DHFR's protein heavy atoms"""
+    m = np.asarray(desc.masses)
+    return np.array(sorted(a for mol in desc.molecules() if len(mol) > 3 for a in mol if m[a] > 1.5), dtype=np.int32)
+
+
+def with_position_restraints(desc, atoms, k, periodic=True):
+    """desc plus a CustomExternalForce position restraint of strength k (kJ/mol/nm^2) on each of `atoms`, towards the atom's
+    position shifted by RESTRAINT_OFFSET: POSITION_RESTRAINT_PERIODIC (periodic) or POSITION_RESTRAINT_PLAIN, with per-particle
+    parameters (k, x0, y0, z0)."""
+    atoms = np.asarray(atoms, dtype=np.int32)
+    ref = np.asarray(desc.positions, dtype=np.float64)[atoms] + np.array(RESTRAINT_OFFSET)
+    params = np.concatenate([np.full((len(atoms), 1), float(k)), ref], axis=1)
+    return _with_custom_class(desc, "cext", [POSITION_RESTRAINT_PERIODIC if periodic else POSITION_RESTRAINT_PLAIN],
+                              [("k", "x0", "y0", "z0")], np.zeros(len(atoms)), atoms, params)
 
 
 def improper_centres(desc):

@@ -7,9 +7,9 @@
 // (CudaPlatform.cpp:59-61).  Compiled against the reference's headers where they lie; no reference source is copied.
 //
 // Supported: NonbondedForce (NoCutoff, CutoffNonPeriodic, CutoffPeriodic, PME; parameter offsets), HarmonicBondForce,
-// HarmonicAngleForce, PeriodicTorsionForce, RBTorsionForce, CMAPTorsionForce, CustomTorsionForce (any number of objects, each
-// in its own force group; custom torsions without energy parameter derivatives, expressions within the limits of
-// custom_translate.h), CMMotionRemover;
+// HarmonicAngleForce, PeriodicTorsionForce, RBTorsionForce, CMAPTorsionForce, CustomTorsionForce, CustomBondForce,
+// CustomExternalForce (any number of objects, each in its own force group; custom forces without energy parameter
+// derivatives, expressions within the limits of custom_translate.h), CMMotionRemover;
 // Verlet / Langevin / LangevinMiddle integrators; SETTLE + X-H_n SHAKE constraints; MonteCarloBarostat and
 // MonteCarloAnisotropicBarostat (ApplyMonteCarloBarostatKernel; MonteCarloMembraneBarostat is refused).  A Force class without a kernel here
 // makes Platform::supportsKernels() false; an unsupported OPTION of a supported class is rejected in contextCreated()
@@ -17,8 +17,8 @@
 //
 // Bonded classes.  Each keeps the terms of all its Force objects in one TermRecord of PlatformData, sent at finalize; what
 // their kernels share (ObjectTerms: the object's range of the record, group tags, updates) exists once.  Bond, angle,
-// periodic-torsion and RB-torsion kernels are one template, B200CalcBondedForceKernel; CMAP and custom torsions keep
-// their own kernels for their maps and expression programs.
+// periodic-torsion and RB-torsion kernels are one template, B200CalcBondedForceKernel; the custom torsion, bond and
+// external kernels another, B200CalcCustomForceKernel, for their expression programs; CMAP keeps its own for its maps.
 //
 // The hot loop.  Integrator::step(n) of the reference is, per step, updateContextState() -> calcForcesAndEnergy(true,
 // false, groups) -> Integrate*StepKernel::execute (LangevinIntegrator.cpp:74-82).  Here a forces-only evaluation is
@@ -39,6 +39,8 @@
 #include "openmm/RBTorsionForce.h"
 #include "openmm/CMAPTorsionForce.h"
 #include "openmm/CustomTorsionForce.h"
+#include "openmm/CustomBondForce.h"
+#include "openmm/CustomExternalForce.h"
 #include "openmm/CMMotionRemover.h"
 #include "openmm/VerletIntegrator.h"
 #include "openmm/LangevinIntegrator.h"
@@ -136,6 +138,22 @@ struct RBTorsions {
     static int update(b200md_ctx* c, const TermRecord& r) { return b200md_update_rb_torsion_params(c, r.size(), r.params[0].data()); }
 };
 
+// The expression programs of one custom class over all its Force objects, one after the other (object f's expression is
+// programs (1 + number of variables)*f ..); the parameters of every term padded to B200MD_CUSTOM_MAX_PARAMS in the record,
+// packed to the widest object's count when sent
+struct CustomPrograms {
+    vector<int> progStart = vector<int>(1, 0), op, arg; vector<double> imm;
+    int stride = 0;
+    int numExpressions(int numVars) const { return (int) (progStart.size() - 1)/(1 + numVars); }
+    vector<double> packed(const TermRecord& r) const {
+        const size_t n = r.size();
+        vector<double> p(n*stride);
+        for (size_t i = 0; i < n; i++)
+            for (int k = 0; k < stride; k++) p[i*stride + k] = r.params[0][i*B200MD_CUSTOM_MAX_PARAMS + k];
+        return p;
+    }
+};
+
 // per-Context state (ContextImpl::setPlatformData)
 struct PlatformData {
     b200md_ctx* ctx = nullptr;
@@ -154,24 +172,17 @@ struct PlatformData {
     bool useFusedStep = true;       // B200MD_PLUGIN_FUSED=0: always compute + integrate_only (debugging)
     // the bonded terms of every Force object, one record per class (columns: atoms, integer parameters, parameters), sent at finalize
     TermRecord bonds{B200MD_BONDED_BONDS, 2, 0, 2}, angles{B200MD_BONDED_ANGLES, 3, 0, 2}, torsions{B200MD_BONDED_TORSIONS, 4, 1, 2},
-               rb{B200MD_BONDED_RB_TORSIONS, 4, 0, 1}, cmap{B200MD_BONDED_CMAP, 1, 1, 0}, custom{B200MD_BONDED_CUSTOM_TORSIONS, 1, 1, 1};
+               rb{B200MD_BONDED_RB_TORSIONS, 4, 0, 1}, cmap{B200MD_BONDED_CMAP, 1, 1, 0}, custom{B200MD_BONDED_CUSTOM_TORSIONS, 1, 1, 1},
+               customBonds{B200MD_BONDED_CUSTOM_BONDS, 1, 1, 1}, customExternals{B200MD_BONDED_CUSTOM_EXTERNALS, 1, 1, 1};
     // CMAP: the maps of all objects one after the other (a term's map index counts from the first map of all objects);
     // coefficients from CMAPTorsionForceImpl::calcMapDerivatives, [sum size^2][16]
     vector<int> cmapSize; vector<double> cmapCoeff;
-    // custom torsions: the programs of all objects one after the other (object f's expression is the pair 2f, 2f+1); the
-    // parameters of every term padded to B200MD_CUSTOM_MAX_PARAMS in the record, packed to the widest object's count when sent
-    vector<int> customProgStart = vector<int>(1, 0), customOp, customArg; vector<double> customImm;
-    int customStride = 0;
-    // the global parameters the expressions read: slot of every name (shared by all objects) and the value last sent
+    // custom torsions, bonds and externals: the programs of each class (B200MD_CUSTOM_*)
+    CustomPrograms customPrograms[3];
+    // the global parameters the expressions of all three classes read: slot of every name (shared by all objects) and the
+    // value last sent
     map<string, int> customGlobalSlot;
     vector<double> customGlobals;
-    vector<double> packedCustomParams() const {
-        const size_t n = custom.size();
-        vector<double> p(n*customStride);
-        for (size_t i = 0; i < n; i++)
-            for (int k = 0; k < customStride; k++) p[i*customStride + k] = custom.params[0][i*B200MD_CUSTOM_MAX_PARAMS + k];
-        return p;
-    }
     map<string, string> props;
     // a box b200md_set_box refused (smaller than twice the cutoff): the reference raises that at the next force evaluation
     // (ReferenceKernels.cpp:983-985), not in setPeriodicBoxVectors; a later box that passes clears it
@@ -194,11 +205,17 @@ struct PlatformData {
         if (cmap.size()) check(b200md_set_cmap(ctx, (int) cmapSize.size(), cmapSize.data(), cmapCoeff.data(), cmap.size(), cmap.ints[0].data(), cmap.atoms[0].data()));
         for (const TermRecord* r : {&bonds, &angles, &torsions, &rb, &cmap})
             if (r->size()) check(b200md_set_bonded_groups(ctx, r->kind, r->size(), r->group.data()));
-        if (custom.size()) {
-            const vector<double> par = packedCustomParams();
-            check(b200md_set_custom_torsions(ctx, (int) customProgStart.size()/2, customProgStart.data(), customOp.data(), customArg.data(),
-                                             customImm.data(), customStride, custom.size(), custom.ints[0].data(), custom.atoms[0].data(), par.data()));
-            check(b200md_set_bonded_groups(ctx, custom.kind, custom.size(), custom.group.data()));
+        typedef int (*SetCustom)(b200md_ctx*, int, const int*, const int*, const int*, const double*, int, int, const int*, const int*, const double*);
+        const SetCustom setCustom[3] = {b200md_set_custom_torsions, b200md_set_custom_bonds, b200md_set_custom_externals};
+        const TermRecord* customRecord[3] = {&custom, &customBonds, &customExternals};
+        for (int k = 0; k < 3; k++) {
+            const TermRecord& r = *customRecord[k];
+            if (!r.size()) continue;
+            const CustomPrograms& c = customPrograms[k];
+            const vector<double> par = c.packed(r);
+            check(setCustom[k](ctx, c.numExpressions(k == B200MD_CUSTOM_EXTERNAL ? 3 : 1), c.progStart.data(), c.op.data(), c.arg.data(),
+                               c.imm.data(), c.stride, r.size(), r.ints[0].data(), r.atoms[0].data(), par.data()));
+            check(b200md_set_bonded_groups(ctx, r.kind, r.size(), r.group.data()));
         }
         if (!customGlobals.empty()) check(b200md_set_custom_globals(ctx, (int) customGlobals.size(), customGlobals.data()));
         check(b200md_finalize(ctx));
@@ -485,7 +502,9 @@ protected:
         d.systemTerms |= bit; d.bondedGroupsUsed |= 1u << force.getForceGroup();
     }
     // copyParametersToContext: the object read again, refused if the number of its terms or the atoms of one changed
-    template<class Read> TermRecord reread(PlatformData& d, const TermRecord& r, int numTerms, const char* terms, const char* aTerm, Read read) const {
+    // changed: the message for a changed atom, if not "The set of particles in <aTerm> has changed"
+    template<class Read> TermRecord reread(PlatformData& d, const TermRecord& r, int numTerms, const char* terms, const char* aTerm, Read read,
+                                           const char* changed = nullptr) const {
         d.ensureFinalized();
         d.dropForces();
         if (numTerms != count) throw OpenMMException(string("updateParametersInContext: The number of ") + terms + " has changed");
@@ -493,7 +512,7 @@ protected:
         for (int i = 0; i < count; i++) read(i, fresh);
         for (size_t c = 0; c < r.atoms.size(); c++)
             if (!equal(fresh.atoms[c].begin(), fresh.atoms[c].end(), start(r.atoms[c], r)))
-                throw OpenMMException(string("updateParametersInContext: The set of particles in ") + aTerm + " has changed");
+                throw OpenMMException(string("updateParametersInContext: ") + (changed ? string(changed) : string("The set of particles in ") + aTerm + " has changed"));
         return fresh;
     }
     // the parameters of `fresh` (reread) into [first, first+count)
@@ -578,43 +597,92 @@ private:
     size_t firstCoeff = 0;
 };
 
-// CustomTorsionForce: the expression becomes two instruction programs (custom_translate.h), which k_custom_torsion interprets.
-vector<string> perTorsionParameterNames(const CustomTorsionForce& force) {
+// What the custom torsion, bond and external kernels differ in (B200CalcCustomForceKernel below): the Force, its class and
+// term bit, its variables, the names in messages, how term i is read, and the calls that send the parameters.
+struct CustomTorsions {
+    typedef CustomTorsionForce Force; typedef CalcCustomTorsionForceKernel Kernel;
+    enum { cls = B200MD_CUSTOM_TORSION, bit = B200MD_TERM_CUSTOM_TORSIONS };
+    static constexpr const char* name = "CustomTorsionForce", *terms = "torsions", *aTerm = "a torsion", *perTerm = "torsion", *changed = nullptr;
+    static vector<string> variables() { return {"theta"}; }
+    static TermRecord PlatformData::* record() { return &PlatformData::custom; }
+    static int count(const Force& f) { return f.getNumTorsions(); }
+    static int numParams(const Force& f) { return f.getNumPerTorsionParameters(); }
+    static string paramName(const Force& f, int i) { return f.getPerTorsionParameterName(i); }
+    static vector<int> read(const Force& f, int i, vector<double>& par) { int a, b, c, e; f.getTorsionParameters(i, a, b, c, e, par); return {a, b, c, e}; }
+    static int update(b200md_ctx* c, int n, const double* p) { return b200md_update_custom_torsion_params(c, n, p); }
+    static int numParamDerivatives(const Force& f) { return f.getNumEnergyParameterDerivatives(); }
+};
+struct CustomBonds {
+    typedef CustomBondForce Force; typedef CalcCustomBondForceKernel Kernel;
+    enum { cls = B200MD_CUSTOM_BOND, bit = B200MD_TERM_CUSTOM_BONDS };
+    static constexpr const char* name = "CustomBondForce", *terms = "bonds", *aTerm = "a bond", *perTerm = "bond", *changed = nullptr;
+    static vector<string> variables() { return {"r"}; }
+    static TermRecord PlatformData::* record() { return &PlatformData::customBonds; }
+    static int count(const Force& f) { return f.getNumBonds(); }
+    static int numParams(const Force& f) { return f.getNumPerBondParameters(); }
+    static string paramName(const Force& f, int i) { return f.getPerBondParameterName(i); }
+    static vector<int> read(const Force& f, int i, vector<double>& par) { int a, b; f.getBondParameters(i, a, b, par); return {a, b}; }
+    static int update(b200md_ctx* c, int n, const double* p) { return b200md_update_custom_bond_params(c, n, p); }
+    static int numParamDerivatives(const Force& f) { return f.getNumEnergyParameterDerivatives(); }
+};
+struct CustomExternals {
+    typedef CustomExternalForce Force; typedef CalcCustomExternalForceKernel Kernel;
+    enum { cls = B200MD_CUSTOM_EXTERNAL, bit = B200MD_TERM_CUSTOM_EXTERNALS };
+    static constexpr const char* name = "CustomExternalForce", *terms = "particles", *aTerm = "a particle", *perTerm = "particle",
+                                 *changed = "A particle index has changed";
+    static vector<string> variables() { return {"x", "y", "z"}; }
+    static TermRecord PlatformData::* record() { return &PlatformData::customExternals; }
+    static int count(const Force& f) { return f.getNumParticles(); }
+    static int numParams(const Force& f) { return f.getNumPerParticleParameters(); }
+    static string paramName(const Force& f, int i) { return f.getPerParticleParameterName(i); }
+    static vector<int> read(const Force& f, int i, vector<double>& par) { int a; f.getParticleParameters(i, a, par); return {a}; }
+    static int update(b200md_ctx* c, int n, const double* p) { return b200md_update_custom_external_params(c, n, p); }
+    static int numParamDerivatives(const Force&) { return 0; }        // CustomExternalForce has none
+};
+
+template<class T> vector<string> perTermParameterNames(const typename T::Force& force) {
     vector<string> names;
-    for (int i = 0; i < force.getNumPerTorsionParameters(); i++) names.push_back(force.getPerTorsionParameterName(i));
+    for (int i = 0; i < T::numParams(force); i++) names.push_back(T::paramName(force, i));
     return names;
 }
-vector<string> globalParameterNames(const CustomTorsionForce& force) {
+template<class F> vector<string> globalParameterNames(const F& force) {
     vector<string> names;
     for (int i = 0; i < force.getNumGlobalParameters(); i++) names.push_back(force.getGlobalParameterName(i));
     return names;
 }
+// The programs of one custom force's expression (custom_translate.h): the energy and one derivative per variable
+template<class T> void translate(const typename T::Force& force, map<string, int>& globalSlot, vector<b200md_custom::Program>& programs) {
+    b200md_custom::translateExpression(force.getEnergyFunction(), T::variables(), T::name, T::perTerm, T::cls == B200MD_CUSTOM_EXTERNAL,
+                                       perTermParameterNames<T>(force), globalParameterNames(force), globalSlot, programs);
+}
 
-class B200CalcCustomTorsionForceKernel : public CalcCustomTorsionForceKernel, ObjectTerms {
+// CustomTorsionForce, CustomBondForce and CustomExternalForce (T: CustomTorsions, CustomBonds, CustomExternals): the
+// expression becomes 1 + (number of variables) instruction programs, which k_custom interprets.
+template<class T>
+class B200CalcCustomForceKernel : public T::Kernel, ObjectTerms {
 public:
-    B200CalcCustomTorsionForceKernel(string name, const Platform& platform, ContextImpl& context) : CalcCustomTorsionForceKernel(name, platform), context(context) {}
+    B200CalcCustomForceKernel(string name, const Platform& platform, ContextImpl& context) : T::Kernel(name, platform), context(context) {}
     // the term's parameters: as many as the force declares (the Reference platform reads as many), padded with zeros
-    void read(const CustomTorsionForce& force, int i, TermRecord& r) const {
-        int a, b, c, e;
+    void read(const typename T::Force& force, int i, TermRecord& r) const {
         vector<double> par;
-        force.getTorsionParameters(i, a, b, c, e, par);
+        const vector<int> atoms = T::read(force, i, par);
         par.resize(numParams);
         par.resize(B200MD_CUSTOM_MAX_PARAMS, 0.0);
-        r.add({a, b, c, e}, {prog}, par);
+        r.add(atoms, {prog}, par);
     }
-    void initialize(const System& system, const CustomTorsionForce& force) {
+    void initialize(const System& system, const typename T::Force& force) {
         PlatformData& d = getData(context);
-        prog = (int) d.customProgStart.size()/2;
-        numParams = force.getNumPerTorsionParameters();
-        add(d, d.custom, force, force.getNumTorsions(), B200MD_TERM_CUSTOM_TORSIONS, "CustomTorsionForce", [&](int i, TermRecord& r) { read(force, i, r); });
-        b200md_custom::Program energy, deriv;
-        const vector<string> globals = globalParameterNames(force);
-        b200md_custom::translateExpression(force.getEnergyFunction(), perTorsionParameterNames(force), globals, d.customGlobalSlot, energy, deriv);
-        for (const b200md_custom::Program* p : {&energy, &deriv}) {
-            d.customOp.insert(d.customOp.end(), p->op.begin(), p->op.end());
-            d.customArg.insert(d.customArg.end(), p->arg.begin(), p->arg.end());
-            d.customImm.insert(d.customImm.end(), p->imm.begin(), p->imm.end());
-            d.customProgStart.push_back((int) d.customOp.size());
+        CustomPrograms& c = d.customPrograms[T::cls];
+        prog = c.numExpressions((int) T::variables().size());
+        numParams = T::numParams(force);
+        add(d, d.*T::record(), force, T::count(force), T::bit, T::name, [&](int i, TermRecord& r) { read(force, i, r); });
+        vector<b200md_custom::Program> programs;
+        translate<T>(force, d.customGlobalSlot, programs);
+        for (const b200md_custom::Program& p : programs) {
+            c.op.insert(c.op.end(), p.op.begin(), p.op.end());
+            c.arg.insert(c.arg.end(), p.arg.begin(), p.arg.end());
+            c.imm.insert(c.imm.end(), p.imm.begin(), p.imm.end());
+            c.progStart.push_back((int) c.op.size());
         }
         // the Context's parameter map does not exist yet (ContextImpl.cpp:120-131 fills it after the kernels are initialised):
         // start from the defaults, execute() sends whatever differs
@@ -625,7 +693,7 @@ public:
             slots.push_back(make_pair(it->first, it->second));
             d.customGlobals[it->second] = force.getGlobalParameterDefaultValue(i);
         }
-        d.customStride = max(d.customStride, numParams);
+        c.stride = max(c.stride, numParams);
     }
     double execute(ContextImpl& context, bool includeForces, bool includeEnergy) {
         PlatformData& d = getData(context);
@@ -636,18 +704,19 @@ public:
             if (v != d.customGlobals[s.second]) { d.customGlobals[s.second] = v; changed = true; }
         }
         if (changed) d.check(b200md_set_custom_globals(d.ctx, (int) d.customGlobals.size(), d.customGlobals.data()));
-        d.pendingTerms |= B200MD_TERM_CUSTOM_TORSIONS;
+        d.pendingTerms |= T::bit;
         return 0.0;
     }
-    void copyParametersToContext(ContextImpl& context, const CustomTorsionForce& force) {
+    void copyParametersToContext(ContextImpl& context, const typename T::Force& force) {
         PlatformData& d = getData(context);
-        store(d.custom, reread(d, d.custom, force.getNumTorsions(), "torsions", "a torsion", [&](int i, TermRecord& r) { read(force, i, r); }));
-        const vector<double> packed = d.packedCustomParams();
-        d.check(b200md_update_custom_torsion_params(d.ctx, d.custom.size(), packed.data()));
+        TermRecord& r = d.*T::record();
+        store(r, reread(d, r, T::count(force), T::terms, T::aTerm, [&](int i, TermRecord& f) { read(force, i, f); }, T::changed));
+        const vector<double> packed = d.customPrograms[T::cls].packed(r);
+        d.check(T::update(d.ctx, r.size(), packed.data()));
     }
 private:
     ContextImpl& context;
-    int prog = 0, numParams = 0;          // this object's program pair; its number of per-torsion parameters
+    int prog = 0, numParams = 0;          // this object's expression; its number of per-term parameters
     vector<pair<string, int> > slots;     // the global parameters this object's expression reads, and their slots
 };
 
@@ -778,7 +847,9 @@ public:
         if (name == CalcPeriodicTorsionForceKernel::Name()) return new B200CalcBondedForceKernel<Torsions, &PlatformData::torsions>(name, platform, context);
         if (name == CalcRBTorsionForceKernel::Name()) return new B200CalcBondedForceKernel<RBTorsions, &PlatformData::rb>(name, platform, context);
         if (name == CalcCMAPTorsionForceKernel::Name()) return new B200CalcCMAPTorsionForceKernel(name, platform, context);
-        if (name == CalcCustomTorsionForceKernel::Name()) return new B200CalcCustomTorsionForceKernel(name, platform, context);
+        if (name == CalcCustomTorsionForceKernel::Name()) return new B200CalcCustomForceKernel<CustomTorsions>(name, platform, context);
+        if (name == CalcCustomBondForceKernel::Name()) return new B200CalcCustomForceKernel<CustomBonds>(name, platform, context);
+        if (name == CalcCustomExternalForceKernel::Name()) return new B200CalcCustomForceKernel<CustomExternals>(name, platform, context);
         if (name == RemoveCMMotionKernel::Name()) return new B200RemoveCMMotionKernel(name, platform, context);
         if (name == IntegrateVerletStepKernel::Name()) return new B200IntegrateVerletStepKernel(name, platform);
         if (name == IntegrateLangevinStepKernel::Name()) return new B200IntegrateLangevinStepKernel(name, platform);
@@ -795,7 +866,8 @@ public:
         for (const string& n : {CalcForcesAndEnergyKernel::Name(), UpdateStateDataKernel::Name(), ApplyConstraintsKernel::Name(), VirtualSitesKernel::Name(),
                                 CalcNonbondedForceKernel::Name(), CalcHarmonicBondForceKernel::Name(), CalcHarmonicAngleForceKernel::Name(),
                                 CalcPeriodicTorsionForceKernel::Name(), CalcRBTorsionForceKernel::Name(), CalcCMAPTorsionForceKernel::Name(),
-                                CalcCustomTorsionForceKernel::Name(), RemoveCMMotionKernel::Name(), IntegrateVerletStepKernel::Name(),
+                                CalcCustomTorsionForceKernel::Name(), CalcCustomBondForceKernel::Name(), CalcCustomExternalForceKernel::Name(),
+                                RemoveCMMotionKernel::Name(), IntegrateVerletStepKernel::Name(),
                                 IntegrateLangevinStepKernel::Name(), IntegrateLangevinMiddleStepKernel::Name(), ApplyMonteCarloBarostatKernel::Name()})
             registerKernelFactory(n, factory);
         platformProperties.push_back(DeviceIndex());
@@ -822,6 +894,18 @@ public:
     // Everything the kernels would refuse LATER must be refused HERE: ContextImpl only falls back to the next platform
     // when contextCreated() throws (ContextImpl.cpp:152-166); a throw from Kernel::initialize or from the first
     // setPositions would instead make Context creation fail for a System that CUDA / CPU can run.
+    // A custom force: getEnergyParameterDerivatives returns nothing here; an expression beyond the interpreter's limits or with
+    // a tabulated function is refused; an unknown variable is an error on every platform and is raised by the kernel's
+    // initialize, as the Reference platform does
+    template<class T> static void validateCustom(const typename T::Force& force) {
+        if (T::numParamDerivatives(force) > 0)
+            throw OpenMMException(string("B200 platform: energy parameter derivatives of a ") + T::name + " are not supported");
+        map<string, int> slots;
+        vector<b200md_custom::Program> programs;
+        try { translate<T>(force, slots, programs); }
+        catch (const b200md_custom::Unsupported&) { throw; }
+        catch (const OpenMMException&) {}
+    }
     static void validateSystem(const System& system) {
         for (int i = 0; i < system.getNumParticles(); i++)
             if (system.isVirtualSite(i)) throw OpenMMException("B200 platform: virtual sites are not supported");
@@ -837,17 +921,9 @@ public:
             }
             if (force.getForceGroup() < 0 || force.getForceGroup() > 31) throw OpenMMException("B200 platform: force group out of range");
             if (dynamic_cast<const MonteCarloMembraneBarostat*>(&force)) throw OpenMMException("B200 platform: MonteCarloMembraneBarostat is not supported");
-            if (const CustomTorsionForce* ct = dynamic_cast<const CustomTorsionForce*>(&force)) {
-                // getEnergyParameterDerivatives returns nothing here
-                if (ct->getNumEnergyParameterDerivatives() > 0) throw OpenMMException("B200 platform: energy parameter derivatives of a CustomTorsionForce are not supported");
-                // beyond the interpreter's limits: refused here; an unknown variable is an error on every platform and is
-                // raised by the kernel's initialize, as the Reference platform does
-                map<string, int> slots;
-                b200md_custom::Program e, de;
-                try { b200md_custom::translateExpression(ct->getEnergyFunction(), perTorsionParameterNames(*ct), globalParameterNames(*ct), slots, e, de); }
-                catch (const b200md_custom::Unsupported&) { throw; }
-                catch (const OpenMMException&) {}
-            }
+            if (const CustomTorsionForce* f = dynamic_cast<const CustomTorsionForce*>(&force)) validateCustom<CustomTorsions>(*f);
+            if (const CustomBondForce* f = dynamic_cast<const CustomBondForce*>(&force)) validateCustom<CustomBonds>(*f);
+            if (const CustomExternalForce* f = dynamic_cast<const CustomExternalForce*>(&force)) validateCustom<CustomExternals>(*f);
         }
         const int nc = system.getNumConstraints();
         if (nc > 0) {

@@ -1,11 +1,13 @@
-// custom_translate.h -- CustomTorsionForce expression -> the instruction programs of b200md_set_custom_torsions (B200MD_OP_*,
-// include/b200md.h).  Lepton, part of the host's libOpenMM.so, parses, optimises and differentiates the expression exactly as
-// the Reference platform does (ReferenceCalcCustomTorsionForceKernel::initialize, ReferenceKernels.cpp:807-809) and makes
-// the stack program (ExpressionProgram); this file only maps every Lepton::Operation to one instruction.  Included by the
-// plugin (B200Platform.cpp) and by its test C API (tests/custom_torsion_capi.cpp), so that both make the same programs.
+// custom_translate.h -- CustomTorsionForce, CustomBondForce and CustomExternalForce expressions -> the instruction programs
+// of b200md_set_custom_torsions / _bonds / _externals (B200MD_OP_*, include/b200md.h).  Lepton, part of the host's
+// libOpenMM.so, parses, optimises and differentiates the expression exactly as the Reference platform does
+// (ReferenceCalcCustom{Torsion,Bond,External}ForceKernel::initialize) and makes the stack program (ExpressionProgram); this
+// file only maps every Lepton::Operation to one instruction.  Included by the plugin (B200Platform.cpp) and by its test C APIs
+// (tests/custom_torsion_capi.cpp, tests/custom_terms_capi.cpp), so that all make the same programs.
 #ifndef B200MD_CUSTOM_TRANSLATE_H_
 #define B200MD_CUSTOM_TRANSLATE_H_
 #include "openmm/OpenMMException.h"
+#include "lepton/CustomFunction.h"
 #include "lepton/ExpressionProgram.h"
 #include "lepton/Operation.h"
 #include "lepton/ParsedExpression.h"
@@ -29,16 +31,29 @@ struct Program {
     std::vector<double> imm;
 };
 
-// One Lepton program as instructions.  Variables: "theta" -> THETA, a per-torsion parameter -> PARAM (its index), a global
-// parameter -> GLOBAL (its slot in globalSlot, the per-Context map shared by every CustomTorsionForce; a name seen for the
-// first time gets the next slot).  Any other variable is an error, as on the Reference platform.
-inline Program translateProgram(const Lepton::ExpressionProgram& prog, const std::vector<std::string>& paramNames,
-                                const std::vector<std::string>& globalNames, std::map<std::string, int>& globalSlot) {
+// periodicdistance(x, y, z, x0, y0, z0) of a CustomExternalForce, for Lepton's parser: the programs compute it on the device
+// (PERIODIC_DIST), so it is never evaluated here.  An expression that would have it evaluated while optimising (all six
+// arguments constant) is refused.
+class PeriodicDistancePlaceholder : public Lepton::CustomFunction {
+public:
+    int getNumArguments() const { return 6; }
+    double evaluate(const double*) const { throw Unsupported("B200 platform: periodicdistance of constant arguments is not supported"); }
+    double evaluateDerivative(const double*, const int*) const { throw Unsupported("B200 platform: periodicdistance of constant arguments is not supported"); }
+    Lepton::CustomFunction* clone() const { return new PeriodicDistancePlaceholder(); }
+};
+
+// One Lepton program as instructions.  Variables: variables[k] -> VAR k, or THETA for a torsion's "theta"; a per-term
+// parameter -> PARAM (its index), a global parameter -> GLOBAL (its slot in globalSlot, the per-Context map shared by every
+// custom force; a name seen for the first time gets the next slot).  Any other variable is an error, as on the Reference
+// platform.  periodicdistance and its first derivatives -> PERIODIC_DIST.  forceName names the class in messages.
+inline Program translateProgram(const Lepton::ExpressionProgram& prog, const std::vector<std::string>& variables, const std::string& forceName,
+                                const std::vector<std::string>& paramNames, const std::vector<std::string>& globalNames,
+                                std::map<std::string, int>& globalSlot) {
     typedef Lepton::Operation Op;
     if (prog.getStackSize() > B200MD_CUSTOM_MAX_STACK)
-        throw Unsupported("B200 platform: a CustomTorsionForce expression needs a stack deeper than 16");
+        throw Unsupported("B200 platform: a " + forceName + " expression needs a stack deeper than 16");
     if (prog.getNumOperations() > B200MD_CUSTOM_MAX_CODE)
-        throw Unsupported("B200 platform: a CustomTorsionForce expression has more than 256 operations");
+        throw Unsupported("B200 platform: a " + forceName + " expression has more than 256 operations");
     Program out;
     for (int k = 0; k < prog.getNumOperations(); k++) {
         const Op& o = prog.getOperation(k);
@@ -48,7 +63,8 @@ inline Program translateProgram(const Lepton::ExpressionProgram& prog, const std
             case Op::CONSTANT: code = B200MD_OP_CONST; imm = dynamic_cast<const Op::Constant&>(o).getValue(); break;
             case Op::VARIABLE: {
                 const std::string& name = o.getName();
-                if (name == "theta") { code = B200MD_OP_THETA; break; }
+                for (size_t v = 0; v < variables.size() && code < 0; v++)
+                    if (variables[v] == name) { code = name == "theta" ? B200MD_OP_THETA : B200MD_OP_VAR; arg = (int) v; }
                 for (size_t p = 0; p < paramNames.size() && code < 0; p++)
                     if (paramNames[p] == name) { code = B200MD_OP_PARAM; arg = (int) p; }
                 for (size_t g = 0; g < globalNames.size() && code < 0; g++)
@@ -61,7 +77,17 @@ inline Program translateProgram(const Lepton::ExpressionProgram& prog, const std
                 if (code < 0) throw OpenMM::OpenMMException("Unknown variable in expression: " + name);
                 break;
             }
-            case Op::CUSTOM: throw Unsupported("B200 platform: tabulated functions in a CustomTorsionForce expression are not supported");
+            case Op::CUSTOM: {
+                if (o.getName() != "periodicdistance")
+                    throw Unsupported("B200 platform: tabulated functions in a " + forceName + " expression are not supported");
+                // getDerivOrder: all zero is the distance, a single 1 the first derivative by that argument
+                const std::vector<int>& order = dynamic_cast<const Op::Custom&>(o).getDerivOrder();
+                int which = -1, total = 0;
+                for (size_t k = 0; k < order.size(); k++) { total += order[k]; if (order[k] == 1) which = (int) k; }
+                if (total > 1) throw Unsupported("B200 platform: second derivatives of periodicdistance are not supported");
+                code = B200MD_OP_PERIODIC_DIST; arg = total ? which : -1;
+                break;
+            }
             case Op::ADD: code = B200MD_OP_ADD; break;
             case Op::SUBTRACT: code = B200MD_OP_SUB; break;
             case Op::MULTIPLY: code = B200MD_OP_MUL; break;
@@ -101,24 +127,41 @@ inline Program translateProgram(const Lepton::ExpressionProgram& prog, const std
             case Op::CEIL: code = B200MD_OP_CEIL; break;
             case Op::SELECT: code = B200MD_OP_SELECT; break;
         }
-        if (code < 0) throw Unsupported("B200 platform: operation '" + o.getName() + "' in a CustomTorsionForce expression is not supported");
+        if (code < 0) throw Unsupported("B200 platform: operation '" + o.getName() + "' in a " + forceName + " expression is not supported");
         out.op.push_back(code); out.arg.push_back(arg); out.imm.push_back(imm);
     }
     return out;
 }
 
-// The energy program and the dE/dtheta program of one expression: Parser::parse(energy).optimize(), and the same expression
-// .differentiate("theta").optimize().
+// The energy program and one derivative program per variable of one expression: Parser::parse(energy).optimize(), and the
+// same expression .differentiate(variable).optimize() for every variable in order.  periodic: periodicdistance is a function
+// of the expression (a CustomExternalForce).  perTerm names a term in messages ("torsion", "bond", "particle").
+inline void translateExpression(const std::string& energy, const std::vector<std::string>& variables, const std::string& forceName,
+                                const std::string& perTerm, bool periodic, const std::vector<std::string>& paramNames,
+                                const std::vector<std::string>& globalNames, std::map<std::string, int>& globalSlot,
+                                std::vector<Program>& programs) {
+    if ((int) paramNames.size() > B200MD_CUSTOM_MAX_PARAMS)
+        throw Unsupported("B200 platform: a " + forceName + " with more than 16 per-" + perTerm + " parameters is not supported");
+    PeriodicDistancePlaceholder pd;
+    std::map<std::string, Lepton::CustomFunction*> functions;
+    if (periodic) functions["periodicdistance"] = &pd;
+    const Lepton::ParsedExpression expr = Lepton::Parser::parse(energy, functions).optimize();
+    std::map<std::string, int> slots = globalSlot;      // committed only when every program translates
+    std::vector<Program> out(1, translateProgram(expr.createProgram(), variables, forceName, paramNames, globalNames, slots));
+    for (const std::string& v : variables)
+        out.push_back(translateProgram(expr.differentiate(v).optimize().createProgram(), variables, forceName, paramNames, globalNames, slots));
+    programs.swap(out);
+    globalSlot.swap(slots);
+}
+
+// A CustomTorsionForce expression: the energy program and the dE/dtheta program.
 inline void translateExpression(const std::string& energy, const std::vector<std::string>& paramNames,
                                 const std::vector<std::string>& globalNames, std::map<std::string, int>& globalSlot,
                                 Program& energyProgram, Program& derivProgram) {
-    if ((int) paramNames.size() > B200MD_CUSTOM_MAX_PARAMS)
-        throw Unsupported("B200 platform: a CustomTorsionForce with more than 16 per-torsion parameters is not supported");
-    const Lepton::ParsedExpression expr = Lepton::Parser::parse(energy).optimize();
-    std::map<std::string, int> slots = globalSlot;      // committed only when both programs translate
-    energyProgram = translateProgram(expr.createProgram(), paramNames, globalNames, slots);
-    derivProgram = translateProgram(expr.differentiate("theta").optimize().createProgram(), paramNames, globalNames, slots);
-    globalSlot.swap(slots);
+    std::vector<Program> programs;
+    translateExpression(energy, std::vector<std::string>(1, "theta"), "CustomTorsionForce", "torsion", false, paramNames, globalNames,
+                        globalSlot, programs);
+    energyProgram = programs[0]; derivProgram = programs[1];
 }
 
 } // namespace b200md_custom
