@@ -43,7 +43,9 @@ typedef struct b200md_ctx b200md_ctx;
 #define B200MD_TERM_CUSTOM_TORSIONS 128
 #define B200MD_TERM_CUSTOM_BONDS     256
 #define B200MD_TERM_CUSTOM_EXTERNALS 512
-#define B200MD_TERM_ALL        1023
+#define B200MD_TERM_CUSTOM_ANGLES    1024
+#define B200MD_TERM_CUSTOM_COMPOUND  2048
+#define B200MD_TERM_ALL        4095
 
 /* ---- the bonded classes: kind argument of b200md_set_bonded_groups and b200md_update_bonded_params ---- */
 #define B200MD_BONDED_BONDS           0
@@ -54,13 +56,19 @@ typedef struct b200md_ctx b200md_ctx;
 #define B200MD_BONDED_CUSTOM_TORSIONS 5
 #define B200MD_BONDED_CUSTOM_BONDS    6
 #define B200MD_BONDED_CUSTOM_EXTERNALS 7
+/* 8 is not a kind: b200md_set_bonded_groups has always refused it, and callers probe with it */
+#define B200MD_BONDED_CUSTOM_ANGLES   9
+#define B200MD_BONDED_CUSTOM_COMPOUND 10
 
 /* ---- the classes of custom terms: which variables a program may read (custom_check_program) ---- */
 #define B200MD_CUSTOM_TORSION  0      /* THETA                                   */
 #define B200MD_CUSTOM_BOND     1      /* VAR 0 = r                                */
 #define B200MD_CUSTOM_EXTERNAL 2      /* VAR 0, 1, 2 = x, y, z; PERIODIC_DIST      */
+#define B200MD_CUSTOM_ANGLE    3      /* THETA = the angle in [0, pi]             */
+#define B200MD_CUSTOM_COMPOUND 4      /* VAR 3i, 3i+1, 3i+2 = x, y, z of particle i; POINT_DIST, POINT_ANGLE, POINT_DIHEDRAL */
 
-/* ---- instructions of a custom-term expression program (b200md_set_custom_torsions / _bonds / _externals) ----
+/* ---- instructions of a custom-term expression program (b200md_set_custom_torsions / _bonds / _externals / _angles /
+ * _compound) ----
  * One instruction = (opcode, operand index, double immediate).  A program is the flat stack program of a Lepton
  * ExpressionProgram (lepton/ExpressionProgram.h), one instruction per Lepton::Operation, in the same order and with the same
  * argument order: an operation of k arguments reads them from the top of the stack, argument 0 being the value pushed LAST,
@@ -69,7 +77,10 @@ typedef struct b200md_ctx b200md_ctx;
  * global value in slot s; CONST, ADD_CONST, MUL_CONST and POW_CONST take their constant from the immediate.  VAR k pushes
  * variable k of the term (a bond: 0 = r; an external: 0, 1, 2 = x, y, z).  PERIODIC_DIST is Lepton's periodicdistance(x, y,
  * z, x0, y0, z0) with argument k at st[sp+k] as for every operation: operand -1 gives the minimum-image distance, operand
- * k in 0..5 its derivative by argument k (ReferencePointDistanceFunction, periodic), every one of them 0 at distance 0. */
+ * k in 0..5 its derivative by argument k (ReferencePointDistanceFunction, periodic), every one of them 0 at distance 0.
+ * POINT_DIST (6 arguments), POINT_ANGLE (9) and POINT_DIHEDRAL (12) are pointdistance, pointangle and pointdihedral of a
+ * CustomCompoundBondForce (ReferencePointFunctions.cpp) with the same operand convention: -1 the value, k >= 0 the first
+ * derivative by argument k.  They take the minimum image of every displacement iff their expression is periodic. */
 enum {
     B200MD_OP_CONST = 0, B200MD_OP_THETA, B200MD_OP_PARAM, B200MD_OP_GLOBAL,
     B200MD_OP_ADD, B200MD_OP_SUB, B200MD_OP_MUL, B200MD_OP_DIV, B200MD_OP_POW, B200MD_OP_NEG, B200MD_OP_SQRT, B200MD_OP_EXP,
@@ -77,11 +88,14 @@ enum {
     B200MD_OP_ACOS, B200MD_OP_ATAN, B200MD_OP_ATAN2, B200MD_OP_SINH, B200MD_OP_COSH, B200MD_OP_TANH, B200MD_OP_ERF,
     B200MD_OP_ERFC, B200MD_OP_STEP, B200MD_OP_DELTA, B200MD_OP_SQUARE, B200MD_OP_CUBE, B200MD_OP_RECIP, B200MD_OP_ADD_CONST,
     B200MD_OP_MUL_CONST, B200MD_OP_POW_CONST, B200MD_OP_MIN, B200MD_OP_MAX, B200MD_OP_ABS, B200MD_OP_FLOOR, B200MD_OP_CEIL,
-    B200MD_OP_SELECT, B200MD_OP_VAR, B200MD_OP_PERIODIC_DIST,
+    B200MD_OP_SELECT, B200MD_OP_VAR, B200MD_OP_PERIODIC_DIST, B200MD_OP_POINT_DIST, B200MD_OP_POINT_ANGLE, B200MD_OP_POINT_DIHEDRAL,
     B200MD_OP_COUNT
 };
-/* hard limits of a custom-term program: stack depth, instructions per program, parameters per term */
+/* hard limits of a custom-term program: stack depth (of a compound-bond program: B200MD_CUSTOM_COMPOUND_MAX_STACK, a
+ * dihedral call alone holds 12 values), instructions per program, parameters per term, particles per compound bond */
 #define B200MD_CUSTOM_MAX_STACK  16
+#define B200MD_CUSTOM_COMPOUND_MAX_STACK 32
+#define B200MD_CUSTOM_MAX_PARTICLES 8
 #define B200MD_CUSTOM_MAX_CODE   256
 #define B200MD_CUSTOM_MAX_PARAMS 16
 
@@ -152,6 +166,20 @@ int b200md_set_custom_bonds(b200md_ctx* ctx, int nprog, const int* prog_start, c
  * PERIODIC_DIST takes the current box.  The force is minus the gradient.                                                */
 int b200md_set_custom_externals(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
                                 int param_stride, int n, const int* prog, const int* atoms, const double* params);
+/* CalcCustomAngleForceKernel::initialize (kernels.h): as b200md_set_custom_bonds, with programs 2p and 2p+1 the energy of
+ * expression p and its dE/dtheta (THETA = the angle at atoms[3i+1] between atoms[3i] and atoms[3i+2], in [0, pi], of
+ * minimum-image vectors for a term whose group byte has 0x80); the forces are those of ReferenceAngleBondIxn.           */
+int b200md_set_custom_angles(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                             int param_stride, int n, const int* prog, const int* atoms, const double* params);
+/* CalcCustomCompoundBondForceKernel::initialize (kernels.h): nexpr expressions; expression p joins nparticles[p] <=
+ * B200MD_CUSTOM_MAX_PARTICLES particles, is periodic (its point functions take the minimum image) iff periodic[p], and has
+ * 1 + 3 nparticles[p] programs, one expression's after the other's: its energy, then the derivatives by x1, y1, z1, x2 ..
+ * (VAR 3i+k = coordinate k of particle i: the continuous coordinate b200md_get_positions reports).  n terms: term i
+ * evaluates expression expr[i] on the particles atoms[8i ..] (unused slots -1) with params[i*param_stride ..].  The force
+ * on a particle is minus the three derivatives.  Programs are checked as for the other classes.  Single GPU only.       */
+int b200md_set_custom_compound(b200md_ctx* ctx, int nexpr, const int* nparticles, const int* periodic, const int* prog_start,
+                               const int* op, const int* arg, const double* imm, int param_stride, int n, const int* expr,
+                               const int* atoms, const double* params);
 /* The global parameter values the GLOBAL instructions read (slot s = values[s]).  Before finalize it sets the number of
  * slots; after it, a stream-ordered copy of n == that number of values into the same device buffer, so a captured step
  * graph keeps running with the new values and is never instantiated again.                                               */
@@ -211,18 +239,26 @@ int b200md_update_custom_torsion_params(b200md_ctx* ctx, int n, const double* pa
 /* CalcCustom{Bond,External}ForceKernel::copyParametersToContext: the same for custom bonds and custom externals.          */
 int b200md_update_custom_bond_params(b200md_ctx* ctx, int n, const double* params);
 int b200md_update_custom_external_params(b200md_ctx* ctx, int n, const double* params);
+/* CalcCustom{Angle,CompoundBond}ForceKernel::copyParametersToContext: the same for custom angles and compound bonds.      */
+int b200md_update_custom_angle_params(b200md_ctx* ctx, int n, const double* params);
+int b200md_update_custom_compound_params(b200md_ctx* ctx, int n, const double* params);
 /* Test hook, no context and no device: program `which` of a b200md_set_custom_torsions program set, checked as that call
  * checks it (nglobals = the number of global slots), evaluated at (theta, params, globals) on the host by the interpreter
  * source the device kernel runs.  0 and *out on success, -1 with the reason in msg.                                       */
 int b200md_custom_program_probe(int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
                                 int param_stride, int nglobals, int which, double theta, const double* params,
                                 const double* globals, double* out, char* msg, int msglen);
-/* The same for any class (B200MD_CUSTOM_*): a program set of b200md_set_custom_torsions / _bonds / _externals (1 + the
- * class's number of variables programs per expression), evaluated at the variables vars[] (theta; r; x, y, z) in the box
- * whose vectors are box[0..2], box[3..5], box[6..8] (read by PERIODIC_DIST only).                                         */
+/* The same for any class (B200MD_CUSTOM_*): a program set of b200md_set_custom_torsions / _bonds / _externals / _angles (1 +
+ * the class's number of variables programs per expression), evaluated at the variables vars[] (theta; r; x, y, z) in the box
+ * whose vectors are box[0..2], box[3..5], box[6..8] (read by PERIODIC_DIST and the periodic point functions only).         */
 int b200md_custom_term_probe(int cls, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
                              int param_stride, int nglobals, int which, const double* vars, const double* box,
                              const double* params, const double* globals, double* out, char* msg, int msglen);
+/* The same for ONE compound-bond expression of nparticles particles (1 + 3 nparticles programs), periodic or not, at the 3
+ * nparticles coordinates vars[].                                                                                          */
+int b200md_custom_compound_probe(int nparticles, int periodic, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                 int param_stride, int nglobals, int which, const double* vars, const double* box,
+                                 const double* params, const double* globals, double* out, char* msg, int msglen);
 
 /* ---------------------------------------------------------------------------------------------------
  * UpdateStateDataKernel (kernels.h:125-214).                                                         */
@@ -314,7 +350,8 @@ typedef struct b200md_stats {
 int b200md_get_stats(b200md_ctx* ctx, b200md_stats* out);
 /* mean device time (ms) of named phases measured with CUDA events on the engine's stream:
  * phase: 0 pair kernel, 1 pme spread, 2 fft+convolution, 3 pme gather, 4 integrate+constrain, 5 list build,
- * 6 bonded+exceptions (k_bonded and, with custom terms, k_custom), 7 custom torsions, bonds and externals alone (k_custom).
+ * 6 bonded+exceptions (k_bonded and, with custom terms, k_custom and k_compound), 7 custom torsions, bonds, externals and
+ * angles alone (k_custom), 8 custom compound bonds alone (k_compound).
  * Runs `reps` isolated launches of that phase on the current state.                                  */
 int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* ms_mean);
 /* stand-alone 3-D FFT entry (the bespoke FFT alone, for parity against fftpack / numpy):

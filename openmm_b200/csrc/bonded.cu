@@ -1,6 +1,6 @@
 // bonded.cu -- harmonic bonds, harmonic angles, periodic torsions, Ryckaert-Bellemans torsions, CMAP terms, 1-4
-// exceptions and the Ewald exclusion correction in ONE launch (sm_90a); custom torsions, bonds and externals in a second
-// launch behind it.
+// exceptions and the Ewald exclusion correction in ONE launch (sm_90a); custom torsions, bonds, externals and angles in a
+// second launch behind it, custom compound bonds in a third.
 // Double precision arithmetic on fp32 positions: these terms are a few thousand work items, far below any roofline, and
 // double removes them from the 1e-4 parity budget.
 //
@@ -228,10 +228,11 @@ __global__ void __launch_bounds__(128) k_bonded(NbDev nb, BondedDev bd, int term
     }
 }
 
-// One thread per custom term (restating ReferenceCustomTorsionIxn / ReferenceCustomBondIxn::calculateBondIxn and
-// ReferenceCustomExternalIxn::calculateForce).  A torsion: the dihedral as for every other torsion, dE/dtheta from the term's
+// One thread per custom term (restating ReferenceCustomTorsionIxn / ReferenceCustomBondIxn / ReferenceCustomAngleIxn::
+// calculateBondIxn and ReferenceCustomExternalIxn::calculateForce).  A torsion: the dihedral as for every other torsion, dE/dtheta from the term's
 // derivative program, the forces through torsion_force.  A bond: r = |x_b - x_a|, dE/dr, (dE/dr)/r (x_b - x_a) on a and its
-// negative on b.  An external: the particle's continuous coordinate (posq plus cellOffset lattice vectors, what
+// negative on b.  An angle: the angle and its forces as the harmonic-angle segment of k_bonded computes them, with dE/dtheta
+// from the derivative program.  An external: the particle's continuous coordinate (posq plus cellOffset lattice vectors, what
 // b200md_get_positions reports: the molecule wrap of the list build must not move a restraint), minus the three derivatives.
 // The energy program runs only when the energy is asked for, and a class only when its bit is in `terms`.  A kernel of its
 // own rather than a segment of k_bonded: the interpreter's stack and registers would otherwise weigh on every bonded term of
@@ -244,7 +245,8 @@ __global__ void __launch_bounds__(128) k_custom(NbDev nb, CustomDev ct, int term
         const unsigned char g = ct.group[i];
         const int cls = p >= 0 ? ct.exprClass[p] : 0;
         const int bit = cls == B200MD_CUSTOM_TORSION ? B200MD_TERM_CUSTOM_TORSIONS :
-                        cls == B200MD_CUSTOM_BOND ? B200MD_TERM_CUSTOM_BONDS : B200MD_TERM_CUSTOM_EXTERNALS;
+                        cls == B200MD_CUSTOM_BOND ? B200MD_TERM_CUSTOM_BONDS :
+                        cls == B200MD_CUSTOM_ANGLE ? B200MD_TERM_CUSTOM_ANGLES : B200MD_TERM_CUSTOM_EXTERNALS;
         if (p >= 0 && (terms & bit) && ((ct.groupMask >> (g & 31)) & 1u)) {
             const int4 at = ct.atoms[i];
             const double* par = ct.params + (size_t) i*ct.paramStride;
@@ -255,17 +257,35 @@ __global__ void __launch_bounds__(128) k_custom(NbDev nb, CustomDev ct, int term
             if (cls == B200MD_CUSTOM_TORSION) {
                 const Dihedral d = dihedral(nb, at, g & 0x80);
                 v[0] = d.theta;
-                const double dE = custom_run(ct.code, ct.imm, ct.progStart[q+1], ct.progStart[q+2], v, par, ct.globals, box);
+                const double dE = custom_run<B200MD_CUSTOM_MAX_STACK, false>(ct.code, ct.imm, ct.progStart[q+1], ct.progStart[q+2], v, par, ct.globals, box);
                 torsion_force(nb, at, d, dE);
             }
             else if (cls == B200MD_CUSTOM_BOND) {
                 D3 d = sub(nb.posq[at.y], nb.posq[at.x]);
                 if (g & 0x80) d = min_image_d(d, nb.box);
                 v[0] = sqrt(dot(d, d));
-                const double dE = custom_run(ct.code, ct.imm, ct.progStart[q+1], ct.progStart[q+2], v, par, ct.globals, box);
+                const double dE = custom_run<B200MD_CUSTOM_MAX_STACK, false>(ct.code, ct.imm, ct.progStart[q+1], ct.progStart[q+2], v, par, ct.globals, box);
                 const double s = v[0] > 0 ? dE/v[0] : 0.0;
                 add_force(nb, at.x, scale(d, s));
                 add_force(nb, at.y, scale(d, -s));
+            }
+            else if (cls == B200MD_CUSTOM_ANGLE) {
+                D3 v0 = sub(nb.posq[at.y], nb.posq[at.x]);
+                D3 v1 = sub(nb.posq[at.y], nb.posq[at.z]);
+                if (g & 0x80) { v0 = min_image_d(v0, nb.box); v1 = min_image_d(v1, nb.box); }
+                D3 cp = cross(v0, v1);
+                double rp = sqrt(dot(cp, cp));
+                rp = fmax(rp, 1e-6);
+                const double r21 = dot(v0, v0), r23 = dot(v1, v1);
+                double c = dot(v0, v1)/sqrt(r21*r23);
+                c = fmin(1.0, fmax(-1.0, c));
+                v[0] = acos(c);
+                const double dE = custom_run<B200MD_CUSTOM_MAX_STACK, false>(ct.code, ct.imm, ct.progStart[q+1], ct.progStart[q+2], v, par, ct.globals, box);
+                D3 f1 = scale(cross(v0, cp), dE/(r21*rp));
+                D3 f3 = scale(cross(cp, v1), dE/(r23*rp));
+                add_force(nb, at.x, f1);
+                add_force(nb, at.z, f3);
+                add_force(nb, at.y, {-f1.x-f3.x, -f1.y-f3.y, -f1.z-f3.z});
             }
             else {
                 const float4 x = nb.posq[at.x];
@@ -275,12 +295,12 @@ __global__ void __launch_bounds__(128) k_custom(NbDev nb, CustomDev ct, int term
                 v[1] += ky*nb.box.dby + kz*(double) nb.box.cy;
                 v[2] += kz*nb.box.dcz;
                 D3 f;
-                f.x = -custom_run(ct.code, ct.imm, ct.progStart[q+1], ct.progStart[q+2], v, par, ct.globals, box);
-                f.y = -custom_run(ct.code, ct.imm, ct.progStart[q+2], ct.progStart[q+3], v, par, ct.globals, box);
-                f.z = -custom_run(ct.code, ct.imm, ct.progStart[q+3], ct.progStart[q+4], v, par, ct.globals, box);
+                f.x = -custom_run<B200MD_CUSTOM_MAX_STACK, false>(ct.code, ct.imm, ct.progStart[q+1], ct.progStart[q+2], v, par, ct.globals, box);
+                f.y = -custom_run<B200MD_CUSTOM_MAX_STACK, false>(ct.code, ct.imm, ct.progStart[q+2], ct.progStart[q+3], v, par, ct.globals, box);
+                f.z = -custom_run<B200MD_CUSTOM_MAX_STACK, false>(ct.code, ct.imm, ct.progStart[q+3], ct.progStart[q+4], v, par, ct.globals, box);
                 add_force(nb, at.x, f);
             }
-            if (wantEnergy) e = custom_run(ct.code, ct.imm, ct.progStart[q], ct.progStart[q+1], v, par, ct.globals, box);
+            if (wantEnergy) e = custom_run<B200MD_CUSTOM_MAX_STACK, false>(ct.code, ct.imm, ct.progStart[q], ct.progStart[q+1], v, par, ct.globals, box);
         }
     }
     if (wantEnergy) {
@@ -299,7 +319,64 @@ void launch_custom(const NbDev& nb, const CustomDev& ct, int terms, bool energy,
     launch_high(k_custom, (ct.nslots + 127)/128, 128, 0, s, nb, ct, terms, energy ? 1 : 0);
 }
 
-void launch_bonded(const NbDev& nb, const BondedDev& bd, const CustomDev& ct, int terms, bool energy, cudaStream_t s) {
+// Custom compound bonds (restating ReferenceCustomCompoundBondIxn::calculateOneIxn): the energy is a function of the 3 N
+// coordinates of the term's N particles, the force on particle k minus the derivatives by its three.  One thread per (term,
+// program): warp W runs program W % COMPOUND_PROGRAMS (0 the energy, 1 + 3 k + c the derivative by coordinate c of particle
+// k) for the 32 slots of group W / COMPOUND_PROGRAMS, so a warp still runs one program with uniform code loads, and the
+// programs of a term, which do not depend on each other, run side by side: a lone six-particle restraint takes the time of
+// its longest program, not of all 19.  The coordinates are the continuous ones (posq plus cellOffset lattice vectors, what
+// b200md_get_positions reports): an expression may read them directly, and a non-periodic restraint between two molecules
+// must not jump when the list build wraps one of them.  A derivative program that is the single instruction CONST 0 is not
+// run and adds nothing.  A kernel of its own: its interpreter holds a 32-deep stack and the three point functions, which
+// k_custom's terms never need.
+#define COMPOUND_PROGRAMS (1 + 3*B200MD_CUSTOM_MAX_PARTICLES)
+__global__ void __launch_bounds__(128) k_compound(NbDev nb, CompoundDev cd, int wantEnergy) {
+    const int warp = (blockIdx.x*blockDim.x + threadIdx.x) >> 5;
+    const int j = warp % COMPOUND_PROGRAMS, i = (warp/COMPOUND_PROGRAMS)*32 + (threadIdx.x & 31);
+    double e = 0;
+    if (i < cd.nslots && (j > 0 || wantEnergy)) {
+        const int p = cd.expr[i];          // uniform across the warp: the terms of one expression fill whole warps
+        if (p >= 0 && j <= 3*cd.exprParticles[p] && ((cd.groupMask >> (cd.group[i] & 31)) & 1u)) {
+            const int np = cd.exprParticles[p], q = cd.exprProg[p] + j;
+            const int begin = cd.progStart[q], end = cd.progStart[q+1];
+            if (j == 0 || !(end - begin == 1 && cd.code[begin].x == B200MD_OP_CONST && cd.imm[begin] == 0.0)) {
+                const int* at = cd.atoms + B200MD_CUSTOM_MAX_PARTICLES*(size_t) i;
+                const CustomBox box = {nb.box.dax, nb.box.bx, nb.box.dby, nb.box.cx, nb.box.cy, nb.box.dcz};
+                double v[3*B200MD_CUSTOM_MAX_PARTICLES];
+                for (int k = 0; k < np; k++) {
+                    const int a = at[k];
+                    const float4 x = nb.posq[a];
+                    const int kx = nb.cellOffset[a], ky = nb.cellOffset[a + nb.npad], kz = nb.cellOffset[a + 2*nb.npad];
+                    v[3*k] = x.x + (kx*nb.box.dax + ky*(double) nb.box.bx + kz*(double) nb.box.cx);
+                    v[3*k+1] = x.y + (ky*nb.box.dby + kz*(double) nb.box.cy);
+                    v[3*k+2] = x.z + kz*nb.box.dcz;
+                }
+                const double r = custom_run<B200MD_CUSTOM_COMPOUND_MAX_STACK, true>(cd.code, cd.imm, begin, end, v, cd.params + (size_t) i*cd.paramStride,
+                                                                                    cd.globals, box, cd.exprPeriodic[p] != 0);
+                if (j == 0) e = r;
+                else
+                    atomicAdd((unsigned long long*) &nb.force[at[(j-1)/3] + ((j-1) % 3)*nb.npad], (unsigned long long) __double2ll_rn(-r*B200MD_FORCE_SCALE));
+            }
+        }
+    }
+    if (wantEnergy) {
+        __shared__ double red[4];
+        for (int off = 16; off > 0; off >>= 1) e += __shfl_xor_sync(0xffffffffu, e, off);
+        if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = e;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            const double x = red[0] + red[1] + red[2] + red[3];
+            if (x != 0.0) atomicAdd(&nb.energy[EN_CUSTOM], x);
+        }
+    }
+}
+
+void launch_compound(const NbDev& nb, const CompoundDev& cd, bool energy, cudaStream_t s) {
+    const int warps = cd.nslots/32*COMPOUND_PROGRAMS;      // nslots is a whole number of warps
+    launch_high(k_compound, (warps + 3)/4, 128, 0, s, nb, cd, energy ? 1 : 0);
+}
+
+void launch_bonded(const NbDev& nb, const BondedDev& bd, const CustomDev& ct, const CompoundDev& cd, int terms, bool energy, cudaStream_t s) {
     int n = 0;
     if (terms & B200MD_TERM_BONDS) n += bd.nbonds;
     if (terms & B200MD_TERM_ANGLES) n += bd.nangles;
@@ -312,4 +389,5 @@ void launch_bonded(const NbDev& nb, const BondedDev& bd, const CustomDev& ct, in
         launch_high(k_bonded, (per + 127)/128, 128, 0, s, nb, bd, terms, energy ? 1 : 0);
     }
     if (terms & ct.terms) launch_custom(nb, ct, terms, energy, s);
+    if ((terms & B200MD_TERM_CUSTOM_COMPOUND) && cd.nslots > 0) launch_compound(nb, cd, energy, s);
 }

@@ -81,18 +81,18 @@ struct CmapTable : TermTable<int4, double> {
     std::vector<int> map; std::vector<int2> maps;
     DevBuf<int> mapDev; DevBuf<int2> mapsDev;
 };
-// One class of custom terms (B200MD_CUSTOM_*): atoms (a torsion's four, a bond's two, an external's one, zero-padded to an
+// One class of custom terms (B200MD_CUSTOM_* but the compound bonds): atoms (a torsion's four, a bond's two, an external's one, an angle's three, zero-padded to an
 // int4), params [n][stride] and groups in the caller's term order; besides, the programs (code = (opcode, operand), imm,
 // progStart; 1 + the class's number of variables programs per expression) and the expression of every term.
 struct CustomClass : TermTable<int4, double> {
     int stride = 0, nprog = 0;
     std::vector<int2> code; std::vector<double> imm; std::vector<int> progStart, prog, slot;
 };
-// The custom torsions, bonds and externals and the global values (one slot space for all three).  finalize lays the terms of
-// all three out as k_custom reads them (CustomDev): grouped by expression, each group padded to whole warps, with one
+// The custom torsions, bonds, externals and angles and the global values (one slot space for all, the compound bonds
+// included).  finalize lays the terms of all four out as k_custom reads them (CustomDev): grouped by expression, each group padded to whole warps, with one
 // parameter stride (the widest class's); cls[k].slot[i] is the slot of term i of class k.
 struct CustomTable {
-    CustomClass cls[3];
+    CustomClass cls[4];
     int nslots = 0, stride = 0;
     std::vector<double> globals;
     DevBuf<int4> atomsDev; DevBuf<double> paramsDev, immDev, globalsDev; DevBuf<unsigned char> groupDev;
@@ -103,6 +103,22 @@ struct CustomTable {
         for (const CustomClass& t : cls)
             for (int i = 0; i < t.n; i++)
                 std::copy(t.params.begin() + (size_t) i*t.stride, t.params.begin() + (size_t) (i+1)*t.stride, p.begin() + (size_t) t.slot[i]*stride);
+        return p;
+    }
+};
+
+// The custom compound bonds: per expression its number of particles, whether its point functions take the minimum image and
+// its 1 + 3 particles programs; per term its expression, 8 atom slots (unused -1), params [n][stride] and group, in the
+// caller's order.  finalize lays the terms out as k_compound reads them (CompoundDev); slot[i] is the slot of term i.
+struct CompoundTable {
+    int n = 0, stride = 0, nexpr = 0, nslots = 0;
+    std::vector<int> nparticles, periodic, exprProg, progStart, expr, atoms, slot;
+    std::vector<int2> code; std::vector<double> imm, params; std::vector<unsigned char> group;
+    DevBuf<int> atomsDev, exprDev, nparticlesDev, periodicDev, exprProgDev, progStartDev;
+    DevBuf<int2> codeDev; DevBuf<double> immDev, paramsDev; DevBuf<unsigned char> groupDev;
+    std::vector<double> slot_params() const {
+        std::vector<double> p((size_t) nslots*stride, 0.0);
+        for (int i = 0; i < n; i++) std::copy(params.begin() + (size_t) i*stride, params.begin() + (size_t) (i+1)*stride, p.begin() + (size_t) slot[i]*stride);
         return p;
     }
 };
@@ -195,6 +211,7 @@ struct b200md_ctx {
     TermTable<int4, double> rb;             // [n][6] c0..c5
     CmapTable cmap;
     CustomTable custom;
+    CompoundTable compound;
     std::vector<int> conI, conJ; std::vector<double> conD;
     int cmFreq = 0;
     std::vector<int4> hUnitAtoms;        // host copy of the integration units (ownership cuts of the multi-GPU data plane)
@@ -235,6 +252,7 @@ struct b200md_ctx {
     PmeDev pme{};
     BondedDev bd{};
     CustomDev ctd{};
+    CompoundDev cpd{};
     UnitDev units{};
     IntegDev integ{};
     bool haveIntegrator = false;
@@ -426,11 +444,12 @@ extern "C" int b200md_set_cmap(b200md_ctx* ctx, int nmaps, const int* size, cons
 }
 // What the messages of a custom class's calls name it
 struct CustomNames { const char* call; const char* term; const char* per; };
-static const CustomNames CUSTOM_NAMES[3] = {{"set_custom_torsions", "custom torsion", "torsion"},
+static const CustomNames CUSTOM_NAMES[4] = {{"set_custom_torsions", "custom torsion", "torsion"},
                                             {"set_custom_bonds", "custom bond", "bond"},
-                                            {"set_custom_externals", "custom external", "particle"}};
+                                            {"set_custom_externals", "custom external", "particle"},
+                                            {"set_custom_angles", "custom angle", "angle"}};
 
-// A program set of class cls (b200md_set_custom_torsions / _bonds / _externals): prog_start well formed and every program
+// A program set of class cls (b200md_set_custom_torsions / _bonds / _externals / _angles): prog_start well formed and every program
 // passing custom_check_program (nglobals < 0: GLOBAL operands are checked at finalize).  Returns the instructions as
 // (opcode, operand).
 static std::vector<int2> check_programs(int cls, int nprog, const int* prog_start, const int* op, const int* arg, int stride, int nglobals) {
@@ -449,7 +468,7 @@ static std::vector<int2> check_programs(int cls, int nprog, const int* prog_star
     }
     return code;
 }
-// The terms of class cls: term i evaluates expression prog[i] on the atoms atoms[w*i .. w*i+w-1] (w = 4, 2, 1)
+// The terms of class cls: term i evaluates expression prog[i] on the atoms atoms[w*i .. w*i+w-1] (w = 4, 2, 1, 3)
 static void set_custom(b200md_ctx* ctx, int cls, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
                        int stride, int n, const int* prog, const int* atoms, const double* params) {
     const CustomNames& nm = CUSTOM_NAMES[cls];
@@ -457,7 +476,7 @@ static void set_custom(b200md_ctx* ctx, int cls, int nprog, const int* prog_star
     require(ctx->world == 1, (std::string(nm.term) + "s are not supported in multi-GPU runs").c_str());
     std::vector<int2> code = check_programs(cls, nprog, prog_start, op, arg, stride, -1);
     for (int i = 0; i < n; i++) require(prog[i] >= 0 && prog[i] < nprog, (std::string(nm.term) + ": program index out of range").c_str());
-    const int w = cls == B200MD_CUSTOM_TORSION ? 4 : cls == B200MD_CUSTOM_BOND ? 2 : 1;
+    const int w = cls == B200MD_CUSTOM_TORSION ? 4 : cls == B200MD_CUSTOM_BOND ? 2 : cls == B200MD_CUSTOM_ANGLE ? 3 : 1;
     std::vector<int4> a(n, make_int4(0, 0, 0, 0)); std::vector<double> p(params, params + (size_t) n*stride);
     for (int i = 0; i < n; i++) {
         int* q = &a[i].x;
@@ -487,6 +506,64 @@ extern "C" int b200md_set_custom_externals(b200md_ctx* ctx, int nprog, const int
     set_custom(ctx, B200MD_CUSTOM_EXTERNAL, nprog, prog_start, op, arg, imm, stride, n, prog, atoms, params);
     API_END(ctx)
 }
+extern "C" int b200md_set_custom_angles(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                        int stride, int n, const int* prog, const int* atoms, const double* params) {
+    API_BEGIN(ctx)
+    set_custom(ctx, B200MD_CUSTOM_ANGLE, nprog, prog_start, op, arg, imm, stride, n, prog, atoms, params);
+    API_END(ctx)
+}
+// The programs of compound-bond expressions (1 + 3 nparticles[p] each, one expression's after the other's), checked as
+// check_programs checks the other classes'.  Returns the instructions and, in exprProg, every expression's first program.
+static std::vector<int2> check_compound_programs(int nexpr, const int* nparticles, const int* prog_start, const int* op, const int* arg,
+                                                 int stride, int nglobals, std::vector<int>& exprProg) {
+    const std::string call = "set_custom_compound";
+    require(nexpr >= 0, (call + ": negative number of expressions").c_str());
+    require(stride >= 0 && stride <= B200MD_CUSTOM_MAX_PARAMS, (call + ": more than 16 parameters per bond").c_str());
+    require(nexpr == 0 || prog_start[0] == 0, (call + ": prog_start[0] must be 0").c_str());
+    exprProg.assign(nexpr, 0);
+    int nq = 0;
+    for (int p = 0; p < nexpr; p++) {
+        require(nparticles[p] >= 1 && nparticles[p] <= B200MD_CUSTOM_MAX_PARTICLES, (call + ": an expression must join 1 to 8 particles").c_str());
+        exprProg[p] = nq;
+        nq += 1 + 3*nparticles[p];
+    }
+    for (int q = 0; q < nq; q++) require(prog_start[q+1] >= prog_start[q], (call + ": prog_start must not decrease").c_str());
+    const int total = nexpr ? prog_start[nq] : 0;
+    std::vector<int2> code(total);
+    for (int k = 0; k < total; k++) code[k] = make_int2(op[k], arg[k]);
+    for (int p = 0; p < nexpr; p++)
+        for (int q = exprProg[p]; q < exprProg[p] + 1 + 3*nparticles[p]; q++) {
+            const char* why = custom_check_program(B200MD_CUSTOM_COMPOUND, code.data(), prog_start[q], prog_start[q+1], stride, nglobals, nparticles[p]);
+            if (why) throw std::runtime_error(std::string(why) + " (program " + std::to_string(q) + ")");
+        }
+    return code;
+}
+extern "C" int b200md_set_custom_compound(b200md_ctx* ctx, int nexpr, const int* nparticles, const int* periodic, const int* prog_start,
+                                          const int* op, const int* arg, const double* imm, int stride, int n, const int* expr,
+                                          const int* atoms, const double* params) {
+    API_BEGIN(ctx)
+    check_set(ctx, "set_custom_compound", n);
+    require(ctx->world == 1, "custom compound bonds are not supported in multi-GPU runs");
+    std::vector<int> exprProg;
+    std::vector<int2> code = check_compound_programs(nexpr, nparticles, prog_start, op, arg, stride, -1, exprProg);
+    for (int i = 0; i < n; i++) {
+        require(expr[i] >= 0 && expr[i] < nexpr, "custom compound bond: expression index out of range");
+        for (int k = 0; k < B200MD_CUSTOM_MAX_PARTICLES; k++) {
+            const int a = atoms[B200MD_CUSTOM_MAX_PARTICLES*i + k];
+            if (k < nparticles[expr[i]]) require(a >= 0 && a < ctx->natoms, "custom compound bond: atom index out of range");
+            else require(a == -1, "custom compound bond: an unused atom slot must be -1");
+        }
+    }
+    CompoundTable& t = ctx->compound;            // its group stays: groups may come before the terms
+    t.n = n; t.stride = stride; t.nexpr = nexpr; t.code.swap(code); t.exprProg.swap(exprProg);
+    t.nparticles.assign(nparticles, nparticles + nexpr); t.periodic.assign(periodic, periodic + nexpr);
+    const int nq = nexpr ? t.exprProg[nexpr-1] + 1 + 3*nparticles[nexpr-1] : 0;
+    t.progStart.assign(prog_start, prog_start + (nexpr ? nq + 1 : 0));
+    t.imm.assign(imm, imm + t.code.size());
+    t.expr.assign(expr, expr + n); t.atoms.assign(atoms, atoms + (size_t) B200MD_CUSTOM_MAX_PARTICLES*n);
+    t.params.assign(params, params + (size_t) n*stride);
+    API_END(ctx)
+}
 extern "C" int b200md_set_custom_globals(b200md_ctx* ctx, int n, const double* values) {
     API_BEGIN(ctx)
     require(n >= 0, "set_custom_globals: negative count");
@@ -502,13 +579,31 @@ extern "C" int b200md_custom_term_probe(int cls, int nprog, const int* prog_star
                                         int stride, int nglobals, int which, const double* vars, const double* box,
                                         const double* params, const double* globals, double* out, char* msg, int msglen) {
     try {
-        require(cls >= B200MD_CUSTOM_TORSION && cls <= B200MD_CUSTOM_EXTERNAL, "custom_term_probe: unknown class");
+        require(cls >= B200MD_CUSTOM_TORSION && cls <= B200MD_CUSTOM_ANGLE, "custom_term_probe: unknown class");
         require(nglobals >= 0, "custom_program_probe: negative number of globals");
         const std::vector<int2> code = check_programs(cls, nprog, prog_start, op, arg, stride, nglobals);
         require(which >= 0 && which < nprog*(1 + custom_num_vars(cls)), "custom_program_probe: program index out of range");
         CustomBox b = {1.0, 0.0, 1.0, 0.0, 0.0, 1.0};
         if (box) b = CustomBox{box[0], box[3], box[4], box[6], box[7], box[8]};
-        *out = custom_run(code.data(), imm, prog_start[which], prog_start[which+1], vars, params, globals, b);
+        *out = custom_run<B200MD_CUSTOM_MAX_STACK, false>(code.data(), imm, prog_start[which], prog_start[which+1], vars, params, globals, b);
+        return 0;
+    } catch (std::exception& e) {
+        if (msg && msglen > 0) { strncpy(msg, e.what(), msglen - 1); msg[msglen - 1] = 0; }
+        return -1;
+    }
+}
+extern "C" int b200md_custom_compound_probe(int nparticles, int periodic, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                            int stride, int nglobals, int which, const double* vars, const double* box,
+                                            const double* params, const double* globals, double* out, char* msg, int msglen) {
+    try {
+        require(nglobals >= 0, "custom_compound_probe: negative number of globals");
+        std::vector<int> exprProg;
+        const std::vector<int2> code = check_compound_programs(1, &nparticles, prog_start, op, arg, stride, nglobals, exprProg);
+        require(which >= 0 && which < 1 + 3*nparticles, "custom_compound_probe: program index out of range");
+        CustomBox b = {1.0, 0.0, 1.0, 0.0, 0.0, 1.0};
+        if (box) b = CustomBox{box[0], box[3], box[4], box[6], box[7], box[8]};
+        *out = custom_run<B200MD_CUSTOM_COMPOUND_MAX_STACK, true>(code.data(), imm, prog_start[which], prog_start[which+1], vars, params, globals,
+                                                                    b, periodic != 0);
         return 0;
     } catch (std::exception& e) {
         if (msg && msglen > 0) { strncpy(msg, e.what(), msglen - 1); msg[msglen - 1] = 0; }
@@ -524,12 +619,15 @@ extern "C" int b200md_custom_program_probe(int nprog, const int* prog_start, con
 extern "C" int b200md_set_bonded_groups(b200md_ctx* ctx, int kind, int n, const int* group) {
     API_BEGIN(ctx)
     check_set(ctx, "set_bonded_groups", n);
-    require(kind >= B200MD_BONDED_BONDS && kind <= B200MD_BONDED_CUSTOM_EXTERNALS,
+    require((kind >= B200MD_BONDED_BONDS && kind <= B200MD_BONDED_CUSTOM_EXTERNALS) || kind == B200MD_BONDED_CUSTOM_ANGLES ||
+            kind == B200MD_BONDED_CUSTOM_COMPOUND,
             "set_bonded_groups: kind must be 0 (bonds), 1 (angles), 2 (torsions), 3 (RB torsions), 4 (CMAP), 5 (custom torsions), "
-            "6 (custom bonds) or 7 (custom externals)");
+            "6 (custom bonds), 7 (custom externals), 9 (custom angles) or 10 (custom compound bonds)");
     std::vector<unsigned char>& g = kind == B200MD_BONDED_BONDS ? ctx->bonds.group : kind == B200MD_BONDED_ANGLES ? ctx->angles.group :
                                     kind == B200MD_BONDED_TORSIONS ? ctx->torsions.group : kind == B200MD_BONDED_RB_TORSIONS ? ctx->rb.group :
                                     kind == B200MD_BONDED_CMAP ? ctx->cmap.group :
+                                    kind == B200MD_BONDED_CUSTOM_ANGLES ? ctx->custom.cls[B200MD_CUSTOM_ANGLE].group :
+                                    kind == B200MD_BONDED_CUSTOM_COMPOUND ? ctx->compound.group :
                                     ctx->custom.cls[kind - B200MD_BONDED_CUSTOM_TORSIONS].group;
     g.resize(n);
     for (int i = 0; i < n; i++) { require(group[i] >= 0 && (group[i] & ~0x80) < 32, "force group out of range"); g[i] = (unsigned char) group[i]; }
@@ -1312,7 +1410,7 @@ static bool fft_beside_tiles(const b200md_ctx* c) {
     return c->mg == MG_SINGLE && !c->pmeOnly && c->overlapPme && !c->nb.smPartition && c->nbdesc.method == B200MD_NB_PME;
 }
 
-// finalize: the custom terms of all three classes in the layout of k_custom (CustomDev): grouped by expression, each group
+// finalize: the custom terms of all four classes in the layout of k_custom (CustomDev): grouped by expression, each group
 // padded to whole warps, and the programs, checked once more now that the number of global slots is final
 static void upload_custom(b200md_ctx* c) {
     CustomTable& t = c->custom;
@@ -1323,13 +1421,13 @@ static void upload_custom(b200md_ctx* c) {
     // b200md_set_custom_globals copies into this buffer after finalize
     t.globalsDev.alloc(std::max<size_t>(t.globals.size(), 1)); t.globalsDev.upload(t.globals);
     d.globals = t.globalsDev.p;
-    const int bits[3] = {B200MD_TERM_CUSTOM_TORSIONS, B200MD_TERM_CUSTOM_BONDS, B200MD_TERM_CUSTOM_EXTERNALS};
+    const int bits[4] = {B200MD_TERM_CUSTOM_TORSIONS, B200MD_TERM_CUSTOM_BONDS, B200MD_TERM_CUSTOM_EXTERNALS, B200MD_TERM_CUSTOM_ANGLES};
     // expressions of all classes one after the other (class k's expression p is expression exprBase[k] + p), their programs
     // likewise, the code of class k shifted by the instructions of the classes before it
     std::vector<int2> code; std::vector<double> imm; std::vector<int> progStart(1, 0), exprClass, exprProg;
-    std::vector<int> exprBase(3, 0);
+    std::vector<int> exprBase(4, 0);
     t.stride = 0;
-    for (int k = 0; k < 3; k++) {
+    for (int k = 0; k < 4; k++) {
         CustomClass& cl = t.cls[k];
         exprBase[k] = (int) exprClass.size();
         if (cl.n == 0) continue;
@@ -1354,7 +1452,7 @@ static void upload_custom(b200md_ctx* c) {
     t.nslots = 0;
     if (d.terms == 0) return;
     int cursor = 0;
-    for (int k = 0; k < 3; k++) {
+    for (int k = 0; k < 4; k++) {
         CustomClass& cl = t.cls[k];
         cl.slot.assign(cl.n, 0);
         for (int p = 0; p < cl.nprog; p++) {
@@ -1366,7 +1464,7 @@ static void upload_custom(b200md_ctx* c) {
     std::vector<int4> atoms(cursor, make_int4(0, 0, 0, 0));
     std::vector<unsigned char> group(cursor, 0);
     std::vector<int> expr(cursor, -1);
-    for (int k = 0; k < 3; k++) {
+    for (int k = 0; k < 4; k++) {
         const CustomClass& cl = t.cls[k];
         for (int i = 0; i < cl.n; i++) {
             atoms[cl.slot[i]] = cl.atoms[i]; group[cl.slot[i]] = cl.group.empty() ? 0 : cl.group[i]; expr[cl.slot[i]] = exprBase[k] + cl.prog[i];
@@ -1380,6 +1478,48 @@ static void upload_custom(b200md_ctx* c) {
     d.nslots = t.nslots; d.paramStride = t.stride;
     d.atoms = t.atomsDev.p; d.params = t.paramsDev.p; d.group = t.groupDev.p; d.expr = t.exprDev.p;
     d.exprClass = t.exprClassDev.p; d.exprProg = t.exprProgDev.p;
+    d.code = t.codeDev.p; d.imm = t.immDev.p; d.progStart = t.progStartDev.p;
+}
+
+// finalize: the compound bonds in the layout of k_compound (CompoundDev), after upload_custom (the global values are its)
+static void upload_compound(b200md_ctx* c) {
+    CompoundTable& t = c->compound;
+    CompoundDev& d = c->cpd;
+    d = CompoundDev{};
+    d.groupMask = 0xffffffffu;
+    d.globals = c->ctd.globals;
+    t.nslots = 0;
+    if (t.n == 0) return;
+    require(c->mg == MG_SINGLE, "custom compound bonds are not supported in multi-GPU runs");
+    require(t.group.empty() || (int) t.group.size() == t.n, "set_bonded_groups: group array length differs from the number of terms");
+    for (int p = 0; p < t.nexpr; p++)
+        for (int q = t.exprProg[p]; q < t.exprProg[p] + 1 + 3*t.nparticles[p]; q++) {
+            const char* why = custom_check_program(B200MD_CUSTOM_COMPOUND, t.code.data(), t.progStart[q], t.progStart[q+1], t.stride,
+                                                   (int) c->custom.globals.size(), t.nparticles[p]);
+            if (why) throw std::runtime_error(std::string(why) + " (program " + std::to_string(q) + ")");
+        }
+    int cursor = 0;
+    t.slot.assign(t.n, 0);
+    for (int p = 0; p < t.nexpr; p++) {
+        for (int i = 0; i < t.n; i++) if (t.expr[i] == p) t.slot[i] = cursor++;
+        cursor = (cursor + 31)/32*32;
+    }
+    t.nslots = cursor;
+    std::vector<int> atoms((size_t) B200MD_CUSTOM_MAX_PARTICLES*cursor, -1), expr(cursor, -1);
+    std::vector<unsigned char> group(cursor, 0);
+    for (int i = 0; i < t.n; i++) {
+        std::copy(t.atoms.begin() + (size_t) B200MD_CUSTOM_MAX_PARTICLES*i, t.atoms.begin() + (size_t) B200MD_CUSTOM_MAX_PARTICLES*(i+1),
+                  atoms.begin() + (size_t) B200MD_CUSTOM_MAX_PARTICLES*t.slot[i]);
+        expr[t.slot[i]] = t.expr[i]; group[t.slot[i]] = t.group.empty() ? 0 : t.group[i];
+    }
+    t.atomsDev.upload(atoms); t.exprDev.upload(expr); t.groupDev.upload(group);
+    const std::vector<double> par = t.slot_params();
+    t.paramsDev.alloc(std::max<size_t>(par.size(), 1)); t.paramsDev.upload(par);
+    t.nparticlesDev.upload(t.nparticles); t.periodicDev.upload(t.periodic); t.exprProgDev.upload(t.exprProg);
+    t.codeDev.upload(t.code); t.immDev.upload(t.imm); t.progStartDev.upload(t.progStart);
+    d.nslots = t.nslots; d.paramStride = t.stride;
+    d.atoms = t.atomsDev.p; d.params = t.paramsDev.p; d.group = t.groupDev.p; d.expr = t.exprDev.p;
+    d.exprParticles = t.nparticlesDev.p; d.exprPeriodic = t.periodicDev.p; d.exprProg = t.exprProgDev.p;
     d.code = t.codeDev.p; d.imm = t.immDev.p; d.progStart = t.progStartDev.p;
 }
 
@@ -1490,6 +1630,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     bd.excPeriodic = c->nbdesc.exceptions_periodic;
     bd.groupMask = 0xffffffffu;
     upload_custom(c);
+    upload_compound(c);
     upload_params(c);
     build_units(c);
     build_ccma(c);
@@ -1500,8 +1641,9 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
             require(fft_slab_path(probe), "multi-GPU: the PME grid plane does not fit the slab FFT kernels (B200MD_MGPU=nccl selects the NCCL scheme)");
         }
     }
-    // ---- molecules (connected components of bonds, angles, torsions, RB torsions, CMAP terms, custom torsions and bonds,
-    // constraints and exceptions; not custom externals, which act on one particle) for the wrap at list
+    // ---- molecules (connected components of bonds, angles, torsions, RB torsions, CMAP terms, custom torsions, bonds and
+    // angles, constraints and exceptions; not custom externals, which act on one particle, nor custom compound bonds, which
+    // read continuous coordinates and may tie two molecules that must keep wrapping apart) for the wrap at list
     // builds; off for non-periodic systems and with more than one rank (every rank would have to wrap in the same step,
     // and the reciprocal-space rank builds no list) ----
     c->cellOffset.alloc((size_t) 3*NP); c->cellOffset.zero();
@@ -1515,6 +1657,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
         for (const int4& a : c->angles.atoms) { join(a.x, a.y); join(a.y, a.z); }
         for (auto* t : {&c->torsions.atoms, &c->rb.atoms, &c->cmap.atoms, &c->custom.cls[B200MD_CUSTOM_TORSION].atoms}) for (const int4& a : *t) { join(a.x, a.y); join(a.y, a.z); join(a.z, a.w); }
         for (const int4& a : c->custom.cls[B200MD_CUSTOM_BOND].atoms) join(a.x, a.y);
+        for (const int4& a : c->custom.cls[B200MD_CUSTOM_ANGLE].atoms) { join(a.x, a.y); join(a.y, a.z); }
         for (size_t d = 1; d < c->cmap.atoms.size(); d += 2) join(c->cmap.atoms[d-1].x, c->cmap.atoms[d].x);     // a CMAP term's two dihedrals
         for (size_t i = 0; i < c->conI.size(); i++) join(c->conI[i], c->conJ[i]);
         for (const int2& a : c->exc.atoms) join(a.x, a.y);
@@ -1607,7 +1750,7 @@ extern "C" int b200md_update_cmap_params(b200md_ctx* ctx, int nmaps, const int* 
     API_END(ctx)
 }
 
-// CalcCustom{Torsion,Bond,External}ForceKernel::copyParametersToContext (kernels.h): same terms and programs, new
+// CalcCustom{Torsion,Bond,External,Angle}ForceKernel::copyParametersToContext (kernels.h): same terms and programs, new
 // parameters, into the same device buffer.
 static void update_custom(b200md_ctx* ctx, int cls, const char* call, const char* terms, int n, const double* params) {
     require(ctx->finalized, (std::string(call) + " before finalize").c_str());
@@ -1631,6 +1774,21 @@ extern "C" int b200md_update_custom_bond_params(b200md_ctx* ctx, int n, const do
 extern "C" int b200md_update_custom_external_params(b200md_ctx* ctx, int n, const double* params) {
     API_BEGIN(ctx)
     update_custom(ctx, B200MD_CUSTOM_EXTERNAL, "update_custom_external_params", "particles", n, params);
+    API_END(ctx)
+}
+extern "C" int b200md_update_custom_angle_params(b200md_ctx* ctx, int n, const double* params) {
+    API_BEGIN(ctx)
+    update_custom(ctx, B200MD_CUSTOM_ANGLE, "update_custom_angle_params", "angles", n, params);
+    API_END(ctx)
+}
+extern "C" int b200md_update_custom_compound_params(b200md_ctx* ctx, int n, const double* params) {
+    API_BEGIN(ctx)
+    require(ctx->finalized, "update_custom_compound_params before finalize");
+    CompoundTable& t = ctx->compound;
+    require(n == t.n, "updateParametersInContext: The number of bonds has changed");
+    CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+    t.params.assign(params, params + (size_t) n*t.stride);
+    if (n) t.paramsDev.upload(t.slot_params());
     API_END(ctx)
 }
 
@@ -1840,16 +1998,19 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     const bool pmeRank = nccl_pme_rank(c), directRank = c->mg == MG_NCCL_SPLIT && !pmeRank;
     const bool direct = (terms & B200MD_TERM_NB_DIRECT) && c->haveNb && !pmeRank;
     const bool recip = (terms & B200MD_TERM_NB_RECIP) && c->haveNb && c->nb.method == B200MD_NB_PME && !directRank;
-    const int customBits = B200MD_TERM_CUSTOM_TORSIONS | B200MD_TERM_CUSTOM_BONDS | B200MD_TERM_CUSTOM_EXTERNALS;
+    const int customBits = B200MD_TERM_CUSTOM_TORSIONS | B200MD_TERM_CUSTOM_BONDS | B200MD_TERM_CUSTOM_EXTERNALS | B200MD_TERM_CUSTOM_ANGLES |
+                           B200MD_TERM_CUSTOM_COMPOUND;
     int bterms = terms & (B200MD_TERM_BONDS | B200MD_TERM_ANGLES | B200MD_TERM_TORSIONS | B200MD_TERM_RB_TORSIONS | B200MD_TERM_CMAP |
                           customBits);
     if (c->haveNb) bterms |= terms & B200MD_TERM_NB_DIRECT;
     const int nbonded = c->bd.nbonds + c->bd.nangles + c->bd.ntorsions + c->bd.nrb + c->bd.ncmap + c->bd.nexc;
     // the k_bonded branch is counted as one launch whenever it is taken (even when the selected classes have no terms and
-    // launch_bonded skips the kernel); k_custom is counted once when it runs, for any number of custom classes
+    // launch_bonded skips the kernel); k_custom is counted once when it runs, for any number of custom classes, k_compound
+    // once when it runs
     const bool classic = (bterms & ~customBits) && nbonded > 0;
     const bool custom = (bterms & c->ctd.terms) != 0;
-    const bool bonded = (classic || custom) && !pmeRank;
+    const bool compound = (bterms & B200MD_TERM_CUSTOM_COMPOUND) && c->cpd.nslots > 0;
+    const bool bonded = (classic || custom || compound) && !pmeRank;
     // Reciprocal space (spread -> FFT/convolution -> gather, in USER atom order: independent of the neighbour list) and
     // direct space (list check / rebuild, tile kernel, bonded terms) are independent until the integrator: fork them onto
     // two streams (also inside the captured step graph).  Both accumulate into the same fixed-point force buffer, so the
@@ -1887,8 +2048,9 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     auto launch_bonded_terms = [&](cudaStream_t sb) {
         BondedDev bd = c->bd; bd.groupMask = groupMask;
         CustomDev ct = c->ctd; ct.groupMask = groupMask;
-        launch_bonded(c->nb, bd, ct, bterms, energy, sb);
-        launches += (classic ? 1 : 0) + (custom ? 1 : 0);
+        CompoundDev cp = c->cpd; cp.groupMask = groupMask;
+        launch_bonded(c->nb, bd, ct, cp, bterms, energy, sb);
+        launches += (classic ? 1 : 0) + (custom ? 1 : 0) + (compound ? 1 : 0);
     };
 
     // ---- the schedule, in stream order ----
@@ -2014,7 +2176,8 @@ extern "C" int b200md_compute_groups(b200md_ctx* ctx, int terms, unsigned int bo
         if (terms & B200MD_TERM_TORSIONS) e += h[EN_TORSION];
         if (terms & B200MD_TERM_RB_TORSIONS) e += h[EN_RBTORSION];
         if (terms & B200MD_TERM_CMAP) e += h[EN_CMAP];
-        if (terms & (B200MD_TERM_CUSTOM_TORSIONS | B200MD_TERM_CUSTOM_BONDS | B200MD_TERM_CUSTOM_EXTERNALS)) e += h[EN_CUSTOM];
+        if (terms & (B200MD_TERM_CUSTOM_TORSIONS | B200MD_TERM_CUSTOM_BONDS | B200MD_TERM_CUSTOM_EXTERNALS | B200MD_TERM_CUSTOM_ANGLES |
+                     B200MD_TERM_CUSTOM_COMPOUND)) e += h[EN_CUSTOM];
         if (ctx->haveNb) {
             if (terms & B200MD_TERM_NB_DIRECT) {
                 e += h[EN_NB] + h[EN_EXC];
@@ -2283,6 +2446,7 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
     // counter (which each repetition advances, as a step does) once at the end
     Snapshot state, counter;
     require(phase != 7 || c->ctd.nslots > 0, "time_phase(custom torsions): the System has none");
+    require(phase != 8 || c->cpd.nslots > 0, "time_phase(custom compound bonds): the System has none");
     if (phase == 4) {
         require(c->haveIntegrator, "time_phase(integrate) before set_integrator");
         state.parts = state_spans(c, ST_POS | ST_VEL); state.save(s);
@@ -2300,8 +2464,9 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
             case 3: launch_pme_gather(c->nb, pme_for_launch(c), local, s); break;
             case 4: launch_integrate(c->nb, c->units, c->integ, local, s); break;
             case 5: launch_list_build(c->nb, s); break;
-            case 6: launch_bonded(c->nb, c->bd, c->ctd, B200MD_TERM_ALL, false, s); break;
+            case 6: launch_bonded(c->nb, c->bd, c->ctd, c->cpd, B200MD_TERM_ALL, false, s); break;
             case 7: launch_custom(c->nb, c->ctd, B200MD_TERM_ALL, false, s); break;
+            case 8: launch_compound(c->nb, c->cpd, false, s); break;
             default: throw std::runtime_error("unknown phase");
         }
         CUDA_CHECK(cudaEventRecord(e1, s));

@@ -196,12 +196,13 @@ struct BondedDev {
     unsigned int groupMask;
 };
 
-// Custom torsions, bonds and externals (k_custom, bonded.cu): one kernel and a parameter block of their own, so that
-// BondedDev and k_bonded stay as they are.  The terms of all three classes are stored grouped by expression, each group
+// Custom torsions, bonds, externals and angles (k_custom, bonded.cu): one kernel and a parameter block of their own, so that
+// BondedDev and k_bonded stay as they are.  The terms of all four classes are stored grouped by expression, each group
 // padded to whole warps (expr = -1 in a padding slot), so that every warp runs one class and one program and reads its code
 // with uniform loads.  Expression p is of class exprClass[p] (B200MD_CUSTOM_*); its energy is program exprProg[p] and its
 // derivatives by the class's variables (theta; r; x, y, z) the programs that follow: the instructions
-// [progStart[q], progStart[q+1]) of code (opcode, operand) and imm.  A torsion reads atoms x..w, a bond x, y, an external x.
+// [progStart[q], progStart[q+1]) of code (opcode, operand) and imm.  A torsion reads atoms x..w, a bond x, y, an external x,
+// an angle x, y, z.
 struct CustomDev {
     int nslots;                  // terms + padding
     int paramStride;             // parameters per slot
@@ -210,6 +211,20 @@ struct CustomDev {
     const int* exprClass; const int* exprProg;
     const int2* code; const double* imm; const int* progStart;
     const double* globals;       // the values of the global parameter slots (b200md_set_custom_globals)
+    unsigned int groupMask;
+};
+
+// Custom compound bonds (k_compound, bonded.cu), laid out as the terms of CustomDev: grouped by expression, each group padded
+// to whole warps (expr = -1 in a padding slot).  Expression p joins exprParticles[p] particles, takes the minimum image in
+// its point functions iff exprPeriodic[p], and has the programs exprProg[p] (energy) and the 3 exprParticles[p] that follow
+// (derivatives by x1, y1, z1, x2, ..).  A slot's particles are atoms[8 slot ..], unused ones -1.  globals is CustomDev's.
+struct CompoundDev {
+    int nslots;                  // terms + padding
+    int paramStride;
+    const int* atoms; const double* params; const unsigned char* group; const int* expr;
+    const int* exprParticles; const int* exprPeriodic; const int* exprProg;
+    const int2* code; const double* imm; const int* progStart;
+    const double* globals;
     unsigned int groupMask;
 };
 
@@ -491,10 +506,11 @@ void fft_set_compact(int on);                   // smaller FFT CTAs (the chain s
 size_t fft_cta_smem_bytes(const PmeDev& pme);  // largest shared memory of one single-GPU FFT CTA of this grid (dynamic + static)
 bool fft_slab_path(const PmeDev& pme);          // the 3-launch slab pipeline is usable for this grid (precondition of the multi-GPU FFT)
 
-// k_bonded (when the classes in `terms` have terms) and, when a custom class in `terms` has terms (CustomDev::terms),
-// k_custom behind it on the same stream
-void launch_bonded(const NbDev& nb, const BondedDev& bd, const CustomDev& ct, int terms, bool energy, cudaStream_t s);
+// k_bonded (when the classes in `terms` have terms), when a custom class in `terms` has terms (CustomDev::terms) k_custom
+// behind it on the same stream, and when there are compound bonds and their bit is in `terms`, k_compound behind that
+void launch_bonded(const NbDev& nb, const BondedDev& bd, const CustomDev& ct, const CompoundDev& cd, int terms, bool energy, cudaStream_t s);
 void launch_custom(const NbDev& nb, const CustomDev& ct, int terms, bool energy, cudaStream_t s);
+void launch_compound(const NbDev& nb, const CompoundDev& cd, bool energy, cudaStream_t s);
 
 void launch_integrate(const NbDev& nb, const UnitDev& units, const IntegDev& integ, const CommDev& cd, cudaStream_t s);
 void launch_force_push(const NbDev& nb, const CommDev& cd, cudaStream_t s);          // partial forces of foreign atoms -> owners' inboxes

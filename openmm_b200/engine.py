@@ -7,12 +7,12 @@ from .systems import SystemDesc, NB_PME
 
 TERM_BONDS, TERM_ANGLES, TERM_TORSIONS, TERM_NB_DIRECT, TERM_NB_RECIP = 1, 2, 4, 8, 16
 TERM_RB_TORSIONS, TERM_CMAP, TERM_CUSTOM_TORSIONS = 32, 64, 128
-TERM_CUSTOM_BONDS, TERM_CUSTOM_EXTERNALS, TERM_ALL = 256, 512, 1023
+TERM_CUSTOM_BONDS, TERM_CUSTOM_EXTERNALS, TERM_CUSTOM_ANGLES, TERM_CUSTOM_COMPOUND, TERM_ALL = 256, 512, 1024, 2048, 4095
 # kinds of b200md_set_bonded_groups
 BONDED_KINDS = {"bonds": 0, "angles": 1, "torsions": 2, "rb_torsions": 3, "cmap": 4, "custom_torsions": 5, "custom_bonds": 6,
-                "custom_externals": 7}
+                "custom_externals": 7, "custom_angles": 9, "custom_compound": 10}
 PHASES = {"pair": 0, "pme_spread": 1, "pme_fft_conv": 2, "pme_gather": 3, "integrate": 4, "list_build": 5, "bonded": 6,
-          "custom_torsions": 7}
+          "custom_torsions": 7, "custom_compound": 8}
 
 
 class EngineError(RuntimeError):
@@ -111,8 +111,10 @@ class Engine:
             self._ck(L.b200md_set_custom_torsions(self.h, len(d.custom_prog_start)//2, _ip(_i32(d.custom_prog_start)), _ip(_i32(d.custom_op)),
                                                   _ip(_i32(d.custom_arg)), _dp(_f64(d.custom_imm)), params.shape[1], len(d.custom_prog),
                                                   _ip(_i32(d.custom_prog)), _ip(_i32(d.custom_atoms)), _dp(params)))
-        # custom bonds (programs per expression: E, dE/dr) and custom externals (E, dE/dx, dE/dy, dE/dz)
-        for cls, nprog, call in (("cbond", 2, L.b200md_set_custom_bonds), ("cext", 4, L.b200md_set_custom_externals)):
+        # custom bonds (programs per expression: E, dE/dr), custom externals (E, dE/dx, dE/dy, dE/dz) and custom angles (E,
+        # dE/dtheta)
+        for cls, nprog, call in (("cbond", 2, L.b200md_set_custom_bonds), ("cext", 4, L.b200md_set_custom_externals),
+                                 ("cangle", 2, L.b200md_set_custom_angles)):
             prog = getattr(d, cls + "_prog")
             if not len(prog):
                 continue
@@ -123,6 +125,18 @@ class Engine:
             params = _f64(getattr(d, cls + "_params")).reshape(len(prog), -1)
             self._ck(call(self.h, (len(start) - 1)//nprog, _ip(_i32(start)), _ip(_i32(op)), _ip(_i32(arg)), _dp(_f64(imm)),
                           params.shape[1], len(prog), _ip(_i32(prog)), _ip(_i32(getattr(d, cls + "_atoms"))), _dp(params)))
+        # custom compound bonds: per expression its particles per bond, whether it is periodic, and 1 + 3 particles programs
+        if len(d.ccompound_expr):
+            if not len(d.ccompound_op):
+                raise EngineError("custom compound bonds without programs: compile desc.ccompound_energy into ccompound_op / "
+                                  "ccompound_arg / ccompound_imm / ccompound_prog_start first (the plugin's expression translator)")
+            n = len(d.ccompound_expr)
+            params = _f64(d.ccompound_params).reshape(n, -1)
+            atoms = _i32(d.ccompound_atoms).reshape(n, 8)
+            self._ck(L.b200md_set_custom_compound(self.h, len(d.ccompound_particles), _ip(_i32(d.ccompound_particles)),
+                                                  _ip(_i32(d.ccompound_periodic)), _ip(_i32(d.ccompound_prog_start)),
+                                                  _ip(_i32(d.ccompound_op)), _ip(_i32(d.ccompound_arg)), _dp(_f64(d.ccompound_imm)),
+                                                  params.shape[1], n, _ip(_i32(d.ccompound_expr)), _ip(atoms), _dp(params)))
         if len(d.custom_global_values):
             self._ck(L.b200md_set_custom_globals(self.h, len(d.custom_global_values), _dp(_f64(d.custom_global_values))))
         for kind, g in self._bonded_groups.items():
@@ -237,6 +251,17 @@ class Engine:
         """New per-particle parameters [n, param_stride] for the same custom externals and expressions."""
         p = _f64(params)
         self._ck(self.lib.b200md_update_custom_external_params(self.h, len(p), _dp(p)))
+
+    # ---- CalcCustom{Angle,CompoundBond}ForceKernel::copyParametersToContext ----
+    def update_custom_angle_params(self, params):
+        """New per-angle parameters [n, param_stride] for the same custom angles and expressions."""
+        p = _f64(params)
+        self._ck(self.lib.b200md_update_custom_angle_params(self.h, len(p), _dp(p)))
+
+    def update_custom_compound_params(self, params):
+        """New per-bond parameters [n, param_stride] for the same custom compound bonds and expressions."""
+        p = _f64(params)
+        self._ck(self.lib.b200md_update_custom_compound_params(self.h, len(p), _dp(p)))
 
     def set_custom_globals(self, values):
         """The values of the global parameter slots the expressions read (the number of slots is fixed at definition)."""

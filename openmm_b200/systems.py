@@ -107,6 +107,32 @@ class SystemDesc:
     cext_op: np.ndarray = field(default_factory=_i)
     cext_arg: np.ndarray = field(default_factory=_i)
     cext_imm: np.ndarray = field(default_factory=_d)
+    # CustomAngleForce (cangle_*), laid out as the custom bonds: expressions of theta, atoms [n,3], programs 2p energy and 2p+1
+    # dE/dtheta.
+    cangle_energy: tuple = ()
+    cangle_param_names: tuple = ()
+    cangle_prog: np.ndarray = field(default_factory=_i)
+    cangle_atoms: np.ndarray = field(default_factory=lambda: np.zeros((0, 3), dtype=np.int32))
+    cangle_params: np.ndarray = field(default_factory=lambda: np.zeros((0, 0)))
+    cangle_prog_start: np.ndarray = field(default_factory=_i)
+    cangle_op: np.ndarray = field(default_factory=_i)
+    cangle_arg: np.ndarray = field(default_factory=_i)
+    cangle_imm: np.ndarray = field(default_factory=_d)
+    # CustomCompoundBondForce (ccompound_*): per expression its energy (of p1.., x1, y1, z1, .., distance, angle, dihedral and
+    # the point functions), parameter names, particles per bond (at most 8) and whether it uses periodic boundary conditions;
+    # per term its expression, atoms ([n,8], unused slots -1) and parameters.  The compiled programs of b200md_set_custom_compound:
+    # per expression the energy, then its derivatives by x1, y1, z1, x2, .. (1 + 3 particles programs).
+    ccompound_energy: tuple = ()
+    ccompound_param_names: tuple = ()
+    ccompound_particles: np.ndarray = field(default_factory=_i)
+    ccompound_periodic: np.ndarray = field(default_factory=_i)
+    ccompound_expr: np.ndarray = field(default_factory=_i)
+    ccompound_atoms: np.ndarray = field(default_factory=lambda: np.full((0, 8), -1, dtype=np.int32))
+    ccompound_params: np.ndarray = field(default_factory=lambda: np.zeros((0, 0)))
+    ccompound_prog_start: np.ndarray = field(default_factory=_i)
+    ccompound_op: np.ndarray = field(default_factory=_i)
+    ccompound_arg: np.ndarray = field(default_factory=_i)
+    ccompound_imm: np.ndarray = field(default_factory=_d)
     con_i: np.ndarray = field(default_factory=_i)
     con_j: np.ndarray = field(default_factory=_i)
     con_d: np.ndarray = field(default_factory=_d)
@@ -167,7 +193,7 @@ class SystemDesc:
         return d
 
     def save(self, path):
-        names = ("custom_param_names", "cbond_param_names", "cext_param_names")
+        names = ("custom_param_names", "cbond_param_names", "cext_param_names", "cangle_param_names", "ccompound_param_names")
         d = {k: (np.asarray(v) if v is not None else np.zeros(0)) for k, v in self.__dict__.items()
              if not isinstance(v, str) and k not in names}
         for k in names:
@@ -185,9 +211,9 @@ class SystemDesc:
             v = z[k]
             if k == "name":
                 kw[k] = str(v)
-            elif k in ("custom_energy", "custom_global_names", "cbond_energy", "cext_energy"):
+            elif k in ("custom_energy", "custom_global_names", "cbond_energy", "cext_energy", "cangle_energy", "ccompound_energy"):
                 kw[k] = tuple(str(x) for x in v)
-            elif k in ("custom_param_names", "cbond_param_names", "cext_param_names"):
+            elif k in ("custom_param_names", "cbond_param_names", "cext_param_names", "cangle_param_names", "ccompound_param_names"):
                 kw[k] = tuple(tuple(str(y) for y in x if str(y)) for x in v)
             elif k == "box":
                 kw[k] = v if v.size == 9 else None
@@ -254,14 +280,14 @@ def periodic_to_custom(desc):
 
 
 def _with_custom_class(desc, cls, energy, param_names, prog, atoms, params):
-    """desc with exactly these custom bonds (cls "cbond", atoms [n,2]) or custom externals (cls "cext", atoms [n]), expressions
-    not compiled yet"""
+    """desc with exactly these custom bonds (cls "cbond", atoms [n,2]), custom externals (cls "cext", atoms [n]) or custom
+    angles (cls "cangle", atoms [n,3]), expressions not compiled yet"""
     import copy
     d = copy.copy(desc)
     setattr(d, cls + "_energy", tuple(energy))
     setattr(d, cls + "_param_names", tuple(tuple(p) for p in param_names))
     setattr(d, cls + "_prog", np.asarray(prog, dtype=np.int32))
-    setattr(d, cls + "_atoms", np.asarray(atoms, dtype=np.int32).reshape((-1, 2) if cls == "cbond" else (-1,)))
+    setattr(d, cls + "_atoms", np.asarray(atoms, dtype=np.int32).reshape({"cbond": (-1, 2), "cangle": (-1, 3)}.get(cls, (-1,))))
     width = max([len(p) for p in param_names] + [0])
     setattr(d, cls + "_params", np.asarray(params, dtype=np.float64).reshape(len(prog), -1) if len(prog) else np.zeros((0, width)))
     for k, v in (("_prog_start", _i()), ("_op", _i()), ("_arg", _i()), ("_imm", _d())):
@@ -302,6 +328,97 @@ def with_position_restraints(desc, atoms, k, periodic=True):
     params = np.concatenate([np.full((len(atoms), 1), float(k)), ref], axis=1)
     return _with_custom_class(desc, "cext", [POSITION_RESTRAINT_PERIODIC if periodic else POSITION_RESTRAINT_PLAIN],
                               [("k", "x0", "y0", "z0")], np.zeros(len(atoms)), atoms, params)
+
+
+HARMONIC_CUSTOM_ANGLE = "0.5*k*(theta-theta0)^2"
+HARMONIC_COMPOUND_ANGLE = "0.5*k*(angle(p1,p2,p3)-theta0)^2"
+PERIODIC_COMPOUND_TORSION = "k*(1+cos(n*dihedral(p1,p2,p3,p4)-theta0))"
+# the receptor-ligand restraint of absolute binding free energy calculations: one distance, two angles, three dihedrals over
+# six particles, harmonic in each (the dihedrals across the +-pi seam)
+ORIENTATIONAL_RESTRAINT = ("0.5*kr*(distance(p3,p4)-r0)^2 + 0.5*ka*((angle(p2,p3,p4)-a0)^2 + (angle(p3,p4,p5)-b0)^2)"
+                           " + 0.5*kd*(w1^2 + w2^2 + w3^2);"
+                           " w1 = t1 - twopi*floor(t1/twopi + 0.5); w2 = t2 - twopi*floor(t2/twopi + 0.5);"
+                           " w3 = t3 - twopi*floor(t3/twopi + 0.5); t1 = dihedral(p1,p2,p3,p4) - d0;"
+                           " t2 = dihedral(p2,p3,p4,p5) - e0; t3 = dihedral(p3,p4,p5,p6) - f0; twopi = 6.283185307179586")
+ORIENTATIONAL_PARAMS = ("kr", "ka", "kd", "r0", "a0", "b0", "d0", "e0", "f0")
+
+
+def angles_to_custom(desc):
+    """The same System with every HarmonicAngleForce angle written as the CustomAngleForce HARMONIC_CUSTOM_ANGLE with
+    per-angle parameters (k, theta0)."""
+    atoms = np.stack([desc.angle_i, desc.angle_j, desc.angle_k], axis=1) if len(desc.angle_i) else np.zeros((0, 3))
+    params = np.stack([desc.angle_kk, desc.angle_t0], axis=1) if len(desc.angle_i) else np.zeros((0, 2))
+    d = _with_custom_class(desc, "cangle", [HARMONIC_CUSTOM_ANGLE], [("k", "theta0")], np.zeros(len(atoms)), atoms, params)
+    d.angle_i, d.angle_j, d.angle_k, d.angle_t0, d.angle_kk = _i(), _i(), _i(), _d(), _d()
+    return d
+
+
+def _add_compound(desc, energy, param_names, particles, periodic, atoms, params):
+    """desc plus one CustomCompoundBondForce expression and its bonds (atoms [n, particles], params [n, len(param_names)]),
+    not compiled yet"""
+    import copy
+    d = copy.copy(desc)
+    atoms = np.asarray(atoms, dtype=np.int32).reshape(-1, particles)
+    n, old = len(atoms), len(desc.ccompound_expr)
+    width = max([len(p) for p in desc.ccompound_param_names] + [len(param_names)])
+    par = np.zeros((old + n, width))
+    if old:
+        par[:old, :np.asarray(desc.ccompound_params).shape[1]] = desc.ccompound_params
+    par[old:, :len(param_names)] = np.asarray(params, dtype=np.float64).reshape(n, len(param_names))
+    padded = np.full((n, 8), -1, dtype=np.int32)
+    padded[:, :particles] = atoms
+    d.ccompound_expr = np.concatenate([desc.ccompound_expr, np.full(n, len(desc.ccompound_energy))]).astype(np.int32)
+    d.ccompound_energy = tuple(desc.ccompound_energy) + (energy,)
+    d.ccompound_param_names = tuple(desc.ccompound_param_names) + (tuple(param_names),)
+    d.ccompound_particles = np.concatenate([desc.ccompound_particles, [particles]]).astype(np.int32)
+    d.ccompound_periodic = np.concatenate([desc.ccompound_periodic, [int(periodic)]]).astype(np.int32)
+    d.ccompound_atoms = np.concatenate([np.asarray(desc.ccompound_atoms, dtype=np.int32).reshape(-1, 8), padded])
+    d.ccompound_params = par
+    d.ccompound_prog_start, d.ccompound_op, d.ccompound_arg, d.ccompound_imm = _i(), _i(), _i(), _d()
+    return d
+
+
+def angles_to_compound(desc):
+    """The same System with every HarmonicAngleForce angle written as the three-particle CustomCompoundBondForce
+    HARMONIC_COMPOUND_ANGLE with per-bond parameters (k, theta0)."""
+    atoms = np.stack([desc.angle_i, desc.angle_j, desc.angle_k], axis=1) if len(desc.angle_i) else np.zeros((0, 3))
+    params = np.stack([desc.angle_kk, desc.angle_t0], axis=1) if len(desc.angle_i) else np.zeros((0, 2))
+    d = _add_compound(desc, HARMONIC_COMPOUND_ANGLE, ("k", "theta0"), 3, False, atoms, params)
+    d.angle_i, d.angle_j, d.angle_k, d.angle_t0, d.angle_kk = _i(), _i(), _i(), _d(), _d()
+    return d
+
+
+def torsions_to_compound(desc):
+    """The same System with every periodic torsion written as the four-particle CustomCompoundBondForce
+    PERIODIC_COMPOUND_TORSION with per-bond parameters (k, n, theta0)."""
+    atoms = np.stack([desc.tor_i, desc.tor_j, desc.tor_k, desc.tor_l], axis=1) if len(desc.tor_i) else np.zeros((0, 4))
+    params = np.stack([desc.tor_kk, np.asarray(desc.tor_n, dtype=np.float64), desc.tor_phase], axis=1) if len(desc.tor_i) else np.zeros((0, 3))
+    d = _add_compound(desc, PERIODIC_COMPOUND_TORSION, ("k", "n", "theta0"), 4, False, atoms, params)
+    d.tor_i, d.tor_j, d.tor_k, d.tor_l, d.tor_n, d.tor_phase, d.tor_kk = _i(), _i(), _i(), _i(), _i(), _d(), _d()
+    return d
+
+
+def restraint_atoms(desc):
+    """Six heavy atoms of the largest molecule, spread evenly over its sequence: stand-ins for the three receptor and three
+    ligand atoms of an orientational restraint"""
+    mol = max(desc.molecules(), key=len)
+    heavy = [a for a in mol if desc.masses[a] > 1.5]
+    return np.array([heavy[int(round(f*(len(heavy) - 1)))] for f in (0.05, 0.2, 0.35, 0.65, 0.8, 0.95)], dtype=np.int32)
+
+
+def with_orientational_restraint(desc, atoms6, kr=4000.0, ka=400.0, kd=400.0, offset=0.05, periodic=False):
+    """desc plus one six-particle ORIENTATIONAL_RESTRAINT term on atoms6, its reference distance (nm), angles and dihedrals
+    (rad) those of desc.positions plus `offset`, so that the forces are not zero"""
+    x = np.asarray(desc.positions, dtype=np.float64)[np.asarray(atoms6)]
+
+    def ang(a, b, c):
+        u, v = x[a] - x[b], x[c] - x[b]
+        return math.acos(np.dot(u, v)/np.linalg.norm(u)/np.linalg.norm(v))
+    local = np.arange(6)
+    dih = [float(dihedrals(x, local[k:k+4].reshape(1, 4))[0]) for k in range(3)]
+    ref = [np.linalg.norm(x[2] - x[3]) + offset, ang(1, 2, 3) + offset, ang(2, 3, 4) + offset] + [t + offset for t in dih]
+    return _add_compound(desc, ORIENTATIONAL_RESTRAINT, ORIENTATIONAL_PARAMS, 6, periodic, np.asarray(atoms6).reshape(1, 6),
+                         np.array([[kr, ka, kd] + ref]))
 
 
 def improper_centres(desc):

@@ -8,7 +8,7 @@
 //
 // Supported: NonbondedForce (NoCutoff, CutoffNonPeriodic, CutoffPeriodic, PME; parameter offsets), HarmonicBondForce,
 // HarmonicAngleForce, PeriodicTorsionForce, RBTorsionForce, CMAPTorsionForce, CustomTorsionForce, CustomBondForce,
-// CustomExternalForce (any number of objects, each in its own force group; custom forces without energy parameter
+// CustomExternalForce, CustomAngleForce, CustomCompoundBondForce (any number of objects, each in its own force group; custom forces without energy parameter
 // derivatives, expressions within the limits of custom_translate.h), CMMotionRemover;
 // Verlet / Langevin / LangevinMiddle integrators; SETTLE + X-H_n SHAKE constraints; MonteCarloBarostat and
 // MonteCarloAnisotropicBarostat (ApplyMonteCarloBarostatKernel; MonteCarloMembraneBarostat is refused).  A Force class without a kernel here
@@ -17,8 +17,9 @@
 //
 // Bonded classes.  Each keeps the terms of all its Force objects in one TermRecord of PlatformData, sent at finalize; what
 // their kernels share (ObjectTerms: the object's range of the record, group tags, updates) exists once.  Bond, angle,
-// periodic-torsion and RB-torsion kernels are one template, B200CalcBondedForceKernel; the custom torsion, bond and
-// external kernels another, B200CalcCustomForceKernel, for their expression programs; CMAP keeps its own for its maps.
+// periodic-torsion and RB-torsion kernels are one template, B200CalcBondedForceKernel; the custom torsion, bond, external
+// and angle kernels another, B200CalcCustomForceKernel, for their expression programs; CMAP keeps its own for its maps, the
+// custom compound bond its own for its per-expression particle count.
 //
 // The hot loop.  Integrator::step(n) of the reference is, per step, updateContextState() -> calcForcesAndEnergy(true,
 // false, groups) -> Integrate*StepKernel::execute (LangevinIntegrator.cpp:74-82).  Here a forces-only evaluation is
@@ -41,6 +42,8 @@
 #include "openmm/CustomTorsionForce.h"
 #include "openmm/CustomBondForce.h"
 #include "openmm/CustomExternalForce.h"
+#include "openmm/CustomAngleForce.h"
+#include "openmm/CustomCompoundBondForce.h"
 #include "openmm/CMMotionRemover.h"
 #include "openmm/VerletIntegrator.h"
 #include "openmm/LangevinIntegrator.h"
@@ -173,13 +176,18 @@ struct PlatformData {
     // the bonded terms of every Force object, one record per class (columns: atoms, integer parameters, parameters), sent at finalize
     TermRecord bonds{B200MD_BONDED_BONDS, 2, 0, 2}, angles{B200MD_BONDED_ANGLES, 3, 0, 2}, torsions{B200MD_BONDED_TORSIONS, 4, 1, 2},
                rb{B200MD_BONDED_RB_TORSIONS, 4, 0, 1}, cmap{B200MD_BONDED_CMAP, 1, 1, 0}, custom{B200MD_BONDED_CUSTOM_TORSIONS, 1, 1, 1},
-               customBonds{B200MD_BONDED_CUSTOM_BONDS, 1, 1, 1}, customExternals{B200MD_BONDED_CUSTOM_EXTERNALS, 1, 1, 1};
+               customBonds{B200MD_BONDED_CUSTOM_BONDS, 1, 1, 1}, customExternals{B200MD_BONDED_CUSTOM_EXTERNALS, 1, 1, 1},
+               customAngles{B200MD_BONDED_CUSTOM_ANGLES, 1, 1, 1}, customCompound{B200MD_BONDED_CUSTOM_COMPOUND, 1, 1, 1};
     // CMAP: the maps of all objects one after the other (a term's map index counts from the first map of all objects);
     // coefficients from CMAPTorsionForceImpl::calcMapDerivatives, [sum size^2][16]
     vector<int> cmapSize; vector<double> cmapCoeff;
-    // custom torsions, bonds and externals: the programs of each class (B200MD_CUSTOM_*)
-    CustomPrograms customPrograms[3];
-    // the global parameters the expressions of all three classes read: slot of every name (shared by all objects) and the
+    // custom torsions, bonds, externals and angles: the programs of each class (B200MD_CUSTOM_*)
+    CustomPrograms customPrograms[4];
+    // custom compound bonds: the programs of every object (1 + 3 particles per bond each), its particles per bond and whether
+    // it uses periodic boundary conditions; a term's atom column holds B200MD_CUSTOM_MAX_PARTICLES entries, unused ones -1
+    CustomPrograms compoundPrograms;
+    vector<int> compoundParticles, compoundPeriodic;
+    // the global parameters the expressions of all custom classes read: slot of every name (shared by all objects) and the
     // value last sent
     map<string, int> customGlobalSlot;
     vector<double> customGlobals;
@@ -206,15 +214,23 @@ struct PlatformData {
         for (const TermRecord* r : {&bonds, &angles, &torsions, &rb, &cmap})
             if (r->size()) check(b200md_set_bonded_groups(ctx, r->kind, r->size(), r->group.data()));
         typedef int (*SetCustom)(b200md_ctx*, int, const int*, const int*, const int*, const double*, int, int, const int*, const int*, const double*);
-        const SetCustom setCustom[3] = {b200md_set_custom_torsions, b200md_set_custom_bonds, b200md_set_custom_externals};
-        const TermRecord* customRecord[3] = {&custom, &customBonds, &customExternals};
-        for (int k = 0; k < 3; k++) {
+        const SetCustom setCustom[4] = {b200md_set_custom_torsions, b200md_set_custom_bonds, b200md_set_custom_externals, b200md_set_custom_angles};
+        const TermRecord* customRecord[4] = {&custom, &customBonds, &customExternals, &customAngles};
+        for (int k = 0; k < 4; k++) {
             const TermRecord& r = *customRecord[k];
             if (!r.size()) continue;
             const CustomPrograms& c = customPrograms[k];
             const vector<double> par = c.packed(r);
             check(setCustom[k](ctx, c.numExpressions(k == B200MD_CUSTOM_EXTERNAL ? 3 : 1), c.progStart.data(), c.op.data(), c.arg.data(),
                                c.imm.data(), c.stride, r.size(), r.ints[0].data(), r.atoms[0].data(), par.data()));
+            check(b200md_set_bonded_groups(ctx, r.kind, r.size(), r.group.data()));
+        }
+        if (customCompound.size()) {
+            const TermRecord& r = customCompound;
+            const CustomPrograms& c = compoundPrograms;
+            const vector<double> par = c.packed(r);
+            check(b200md_set_custom_compound(ctx, (int) compoundParticles.size(), compoundParticles.data(), compoundPeriodic.data(), c.progStart.data(),
+                                             c.op.data(), c.arg.data(), c.imm.data(), c.stride, r.size(), r.ints[0].data(), r.atoms[0].data(), par.data()));
             check(b200md_set_bonded_groups(ctx, r.kind, r.size(), r.group.data()));
         }
         if (!customGlobals.empty()) check(b200md_set_custom_globals(ctx, (int) customGlobals.size(), customGlobals.data()));
@@ -597,7 +613,7 @@ private:
     size_t firstCoeff = 0;
 };
 
-// What the custom torsion, bond and external kernels differ in (B200CalcCustomForceKernel below): the Force, its class and
+// What the custom torsion, bond, external and angle kernels differ in (B200CalcCustomForceKernel below): the Force, its class and
 // term bit, its variables, the names in messages, how term i is read, and the calls that send the parameters.
 struct CustomTorsions {
     typedef CustomTorsionForce Force; typedef CalcCustomTorsionForceKernel Kernel;
@@ -640,6 +656,20 @@ struct CustomExternals {
     static int numParamDerivatives(const Force&) { return 0; }        // CustomExternalForce has none
 };
 
+struct CustomAngles {
+    typedef CustomAngleForce Force; typedef CalcCustomAngleForceKernel Kernel;
+    enum { cls = B200MD_CUSTOM_ANGLE, bit = B200MD_TERM_CUSTOM_ANGLES };
+    static constexpr const char* name = "CustomAngleForce", *terms = "angles", *aTerm = "an angle", *perTerm = "angle", *changed = nullptr;
+    static vector<string> variables() { return {"theta"}; }
+    static TermRecord PlatformData::* record() { return &PlatformData::customAngles; }
+    static int count(const Force& f) { return f.getNumAngles(); }
+    static int numParams(const Force& f) { return f.getNumPerAngleParameters(); }
+    static string paramName(const Force& f, int i) { return f.getPerAngleParameterName(i); }
+    static vector<int> read(const Force& f, int i, vector<double>& par) { int a, b, c; f.getAngleParameters(i, a, b, c, par); return {a, b, c}; }
+    static int update(b200md_ctx* c, int n, const double* p) { return b200md_update_custom_angle_params(c, n, p); }
+    static int numParamDerivatives(const Force& f) { return f.getNumEnergyParameterDerivatives(); }
+};
+
 template<class T> vector<string> perTermParameterNames(const typename T::Force& force) {
     vector<string> names;
     for (int i = 0; i < T::numParams(force); i++) names.push_back(T::paramName(force, i));
@@ -656,8 +686,44 @@ template<class T> void translate(const typename T::Force& force, map<string, int
                                        perTermParameterNames<T>(force), globalParameterNames(force), globalSlot, programs);
 }
 
-// CustomTorsionForce, CustomBondForce and CustomExternalForce (T: CustomTorsions, CustomBonds, CustomExternals): the
-// expression becomes 1 + (number of variables) instruction programs, which k_custom interprets.
+// The programs of one force object appended to its class's
+inline void appendPrograms(CustomPrograms& c, const vector<b200md_custom::Program>& programs) {
+    for (const b200md_custom::Program& p : programs) {
+        c.op.insert(c.op.end(), p.op.begin(), p.op.end());
+        c.arg.insert(c.arg.end(), p.arg.begin(), p.arg.end());
+        c.imm.insert(c.imm.end(), p.imm.begin(), p.imm.end());
+        c.progStart.push_back((int) c.op.size());
+    }
+}
+
+// The global parameters one custom force object's expression reads, and their slots in the Context's shared map
+struct ObjectGlobals {
+    vector<pair<string, int> > slots;
+    // after the object's expression was translated.  The Context's parameter map does not exist yet (ContextImpl.cpp:120-131
+    // fills it after the kernels are initialised): start from the defaults, send() sends whatever differs
+    template<class F> void init(PlatformData& d, const F& force) {
+        d.customGlobals.resize(d.customGlobalSlot.size(), 0.0);
+        for (int i = 0; i < force.getNumGlobalParameters(); i++) {
+            const map<string, int>::const_iterator it = d.customGlobalSlot.find(force.getGlobalParameterName(i));
+            if (it == d.customGlobalSlot.end()) continue;         // declared, but the expression does not read it
+            slots.push_back(make_pair(it->first, it->second));
+            d.customGlobals[it->second] = force.getGlobalParameterDefaultValue(i);
+        }
+    }
+    // execute: a changed global value is a stream-ordered copy into the buffer the step graph reads (NonbondedForce offsets alike)
+    void send(PlatformData& d, ContextImpl& context) const {
+        bool changed = false;
+        for (const pair<string, int>& s : slots) {
+            const double v = context.getParameter(s.first);
+            if (v != d.customGlobals[s.second]) { d.customGlobals[s.second] = v; changed = true; }
+        }
+        if (changed) d.check(b200md_set_custom_globals(d.ctx, (int) d.customGlobals.size(), d.customGlobals.data()));
+    }
+};
+
+// CustomTorsionForce, CustomBondForce, CustomExternalForce and CustomAngleForce (T: CustomTorsions, CustomBonds,
+// CustomExternals, CustomAngles): the expression becomes 1 + (number of variables) instruction programs, which k_custom
+// interprets.
 template<class T>
 class B200CalcCustomForceKernel : public T::Kernel, ObjectTerms {
 public:
@@ -678,32 +744,13 @@ public:
         add(d, d.*T::record(), force, T::count(force), T::bit, T::name, [&](int i, TermRecord& r) { read(force, i, r); });
         vector<b200md_custom::Program> programs;
         translate<T>(force, d.customGlobalSlot, programs);
-        for (const b200md_custom::Program& p : programs) {
-            c.op.insert(c.op.end(), p.op.begin(), p.op.end());
-            c.arg.insert(c.arg.end(), p.arg.begin(), p.arg.end());
-            c.imm.insert(c.imm.end(), p.imm.begin(), p.imm.end());
-            c.progStart.push_back((int) c.op.size());
-        }
-        // the Context's parameter map does not exist yet (ContextImpl.cpp:120-131 fills it after the kernels are initialised):
-        // start from the defaults, execute() sends whatever differs
-        d.customGlobals.resize(d.customGlobalSlot.size(), 0.0);
-        for (int i = 0; i < force.getNumGlobalParameters(); i++) {
-            const map<string, int>::const_iterator it = d.customGlobalSlot.find(force.getGlobalParameterName(i));
-            if (it == d.customGlobalSlot.end()) continue;         // declared, but the expression does not read it
-            slots.push_back(make_pair(it->first, it->second));
-            d.customGlobals[it->second] = force.getGlobalParameterDefaultValue(i);
-        }
+        appendPrograms(c, programs);
+        globals.init(d, force);
         c.stride = max(c.stride, numParams);
     }
     double execute(ContextImpl& context, bool includeForces, bool includeEnergy) {
         PlatformData& d = getData(context);
-        // a changed global value is a stream-ordered copy into the buffer the step graph reads (NonbondedForce offsets alike)
-        bool changed = false;
-        for (const pair<string, int>& s : slots) {
-            const double v = context.getParameter(s.first);
-            if (v != d.customGlobals[s.second]) { d.customGlobals[s.second] = v; changed = true; }
-        }
-        if (changed) d.check(b200md_set_custom_globals(d.ctx, (int) d.customGlobals.size(), d.customGlobals.data()));
+        globals.send(d, context);
         d.pendingTerms |= T::bit;
         return 0.0;
     }
@@ -717,7 +764,54 @@ public:
 private:
     ContextImpl& context;
     int prog = 0, numParams = 0;          // this object's expression; its number of per-term parameters
-    vector<pair<string, int> > slots;     // the global parameters this object's expression reads, and their slots
+    ObjectGlobals globals;
+};
+
+// CustomCompoundBondForce: the expression becomes 1 + 3 (particles per bond) instruction programs (the energy and its
+// derivative by every coordinate), which k_compound interprets.
+class B200CalcCustomCompoundBondForceKernel : public CalcCustomCompoundBondForceKernel, ObjectTerms {
+public:
+    B200CalcCustomCompoundBondForceKernel(string name, const Platform& platform, ContextImpl& context) :
+        CalcCustomCompoundBondForceKernel(name, platform), context(context) {}
+    void read(const CustomCompoundBondForce& force, int i, TermRecord& r) const {
+        vector<int> atoms;
+        vector<double> par;
+        force.getBondParameters(i, atoms, par);
+        atoms.resize(B200MD_CUSTOM_MAX_PARTICLES, -1);
+        par.resize(force.getNumPerBondParameters());
+        par.resize(B200MD_CUSTOM_MAX_PARAMS, 0.0);
+        r.add(atoms, {expr}, par);
+    }
+    void initialize(const System& system, const CustomCompoundBondForce& force) {
+        PlatformData& d = getData(context);
+        expr = (int) d.compoundParticles.size();
+        vector<b200md_custom::Program> programs;
+        b200md_custom::translateCompound(force, d.customGlobalSlot, programs);
+        add(d, d.customCompound, force, force.getNumBonds(), B200MD_TERM_CUSTOM_COMPOUND, "CustomCompoundBondForce",
+            [&](int i, TermRecord& r) { read(force, i, r); });
+        appendPrograms(d.compoundPrograms, programs);
+        d.compoundParticles.push_back(force.getNumParticlesPerBond());
+        d.compoundPeriodic.push_back(force.usesPeriodicBoundaryConditions() ? 1 : 0);
+        globals.init(d, force);
+        d.compoundPrograms.stride = max(d.compoundPrograms.stride, force.getNumPerBondParameters());
+    }
+    double execute(ContextImpl& context, bool includeForces, bool includeEnergy) {
+        PlatformData& d = getData(context);
+        globals.send(d, context);
+        d.pendingTerms |= B200MD_TERM_CUSTOM_COMPOUND;
+        return 0.0;
+    }
+    void copyParametersToContext(ContextImpl& context, const CustomCompoundBondForce& force) {
+        PlatformData& d = getData(context);
+        TermRecord& r = d.customCompound;
+        store(r, reread(d, r, force.getNumBonds(), "bonds", "a bond", [&](int i, TermRecord& f) { read(force, i, f); }));
+        const vector<double> packed = d.compoundPrograms.packed(r);
+        d.check(b200md_update_custom_compound_params(d.ctx, r.size(), packed.data()));
+    }
+private:
+    ContextImpl& context;
+    int expr = 0;                         // this object's expression
+    ObjectGlobals globals;
 };
 
 // RemoveCMMotionKernel::execute is called by CMMotionRemoverImpl::updateContextState in EVERY step; the frequency test is
@@ -850,6 +944,8 @@ public:
         if (name == CalcCustomTorsionForceKernel::Name()) return new B200CalcCustomForceKernel<CustomTorsions>(name, platform, context);
         if (name == CalcCustomBondForceKernel::Name()) return new B200CalcCustomForceKernel<CustomBonds>(name, platform, context);
         if (name == CalcCustomExternalForceKernel::Name()) return new B200CalcCustomForceKernel<CustomExternals>(name, platform, context);
+        if (name == CalcCustomAngleForceKernel::Name()) return new B200CalcCustomForceKernel<CustomAngles>(name, platform, context);
+        if (name == CalcCustomCompoundBondForceKernel::Name()) return new B200CalcCustomCompoundBondForceKernel(name, platform, context);
         if (name == RemoveCMMotionKernel::Name()) return new B200RemoveCMMotionKernel(name, platform, context);
         if (name == IntegrateVerletStepKernel::Name()) return new B200IntegrateVerletStepKernel(name, platform);
         if (name == IntegrateLangevinStepKernel::Name()) return new B200IntegrateLangevinStepKernel(name, platform);
@@ -867,6 +963,7 @@ public:
                                 CalcNonbondedForceKernel::Name(), CalcHarmonicBondForceKernel::Name(), CalcHarmonicAngleForceKernel::Name(),
                                 CalcPeriodicTorsionForceKernel::Name(), CalcRBTorsionForceKernel::Name(), CalcCMAPTorsionForceKernel::Name(),
                                 CalcCustomTorsionForceKernel::Name(), CalcCustomBondForceKernel::Name(), CalcCustomExternalForceKernel::Name(),
+                                CalcCustomAngleForceKernel::Name(), CalcCustomCompoundBondForceKernel::Name(),
                                 RemoveCMMotionKernel::Name(), IntegrateVerletStepKernel::Name(),
                                 IntegrateLangevinStepKernel::Name(), IntegrateLangevinMiddleStepKernel::Name(), ApplyMonteCarloBarostatKernel::Name()})
             registerKernelFactory(n, factory);
@@ -906,6 +1003,16 @@ public:
         catch (const b200md_custom::Unsupported&) { throw; }
         catch (const OpenMMException&) {}
     }
+    // The same for a CustomCompoundBondForce, whose limits also cover the particles per bond
+    static void validateCompound(const CustomCompoundBondForce& force) {
+        if (force.getNumEnergyParameterDerivatives() > 0)
+            throw OpenMMException("B200 platform: energy parameter derivatives of a CustomCompoundBondForce are not supported");
+        map<string, int> slots;
+        vector<b200md_custom::Program> programs;
+        try { b200md_custom::translateCompound(force, slots, programs); }
+        catch (const b200md_custom::Unsupported&) { throw; }
+        catch (const OpenMMException&) {}
+    }
     static void validateSystem(const System& system) {
         for (int i = 0; i < system.getNumParticles(); i++)
             if (system.isVirtualSite(i)) throw OpenMMException("B200 platform: virtual sites are not supported");
@@ -924,6 +1031,8 @@ public:
             if (const CustomTorsionForce* f = dynamic_cast<const CustomTorsionForce*>(&force)) validateCustom<CustomTorsions>(*f);
             if (const CustomBondForce* f = dynamic_cast<const CustomBondForce*>(&force)) validateCustom<CustomBonds>(*f);
             if (const CustomExternalForce* f = dynamic_cast<const CustomExternalForce*>(&force)) validateCustom<CustomExternals>(*f);
+            if (const CustomAngleForce* f = dynamic_cast<const CustomAngleForce*>(&force)) validateCustom<CustomAngles>(*f);
+            if (const CustomCompoundBondForce* f = dynamic_cast<const CustomCompoundBondForce*>(&force)) validateCompound(*f);
         }
         const int nc = system.getNumConstraints();
         if (nc > 0) {

@@ -1,12 +1,16 @@
-// custom_translate.h -- CustomTorsionForce, CustomBondForce and CustomExternalForce expressions -> the instruction programs
-// of b200md_set_custom_torsions / _bonds / _externals (B200MD_OP_*, include/b200md.h).  Lepton, part of the host's
-// libOpenMM.so, parses, optimises and differentiates the expression exactly as the Reference platform does
-// (ReferenceCalcCustom{Torsion,Bond,External}ForceKernel::initialize) and makes the stack program (ExpressionProgram); this
-// file only maps every Lepton::Operation to one instruction.  Included by the plugin (B200Platform.cpp) and by its test C APIs
-// (tests/custom_torsion_capi.cpp, tests/custom_terms_capi.cpp), so that all make the same programs.
+// custom_translate.h -- CustomTorsionForce, CustomBondForce, CustomExternalForce, CustomAngleForce and
+// CustomCompoundBondForce expressions -> the instruction programs of b200md_set_custom_torsions / _bonds / _externals /
+// _angles / _compound (B200MD_OP_*, include/b200md.h).  Lepton, part of the host's libOpenMM.so, parses, optimises and
+// differentiates the expression exactly as the Reference platform does
+// (ReferenceCalcCustom{Torsion,Bond,External,Angle,CompoundBond}ForceKernel::initialize) and makes the stack program
+// (ExpressionProgram); this file only maps every Lepton::Operation to one instruction.  Included by the plugin
+// (B200Platform.cpp) and by its test C APIs (tests/custom_torsion_capi.cpp, tests/custom_terms_capi.cpp,
+// tests/custom_compound_capi.cpp), so that all make the same programs.
 #ifndef B200MD_CUSTOM_TRANSLATE_H_
 #define B200MD_CUSTOM_TRANSLATE_H_
 #include "openmm/OpenMMException.h"
+#include "openmm/CustomCompoundBondForce.h"
+#include "openmm/internal/CustomCompoundBondForceImpl.h"
 #include "lepton/CustomFunction.h"
 #include "lepton/ExpressionProgram.h"
 #include "lepton/Operation.h"
@@ -42,16 +46,31 @@ public:
     Lepton::CustomFunction* clone() const { return new PeriodicDistancePlaceholder(); }
 };
 
+// pointdistance, pointangle and pointdihedral of a CustomCompoundBondForce (6, 9 and 12 arguments), likewise: the device
+// computes them (POINT_DIST, POINT_ANGLE, POINT_DIHEDRAL).
+class PointFunctionPlaceholder : public Lepton::CustomFunction {
+public:
+    explicit PointFunctionPlaceholder(int numArguments) : numArguments(numArguments) {}
+    int getNumArguments() const { return numArguments; }
+    double evaluate(const double*) const { throw Unsupported("B200 platform: a point function of constant arguments is not supported"); }
+    double evaluateDerivative(const double*, const int*) const { throw Unsupported("B200 platform: a point function of constant arguments is not supported"); }
+    Lepton::CustomFunction* clone() const { return new PointFunctionPlaceholder(numArguments); }
+private:
+    int numArguments;
+};
+
 // One Lepton program as instructions.  Variables: variables[k] -> VAR k, or THETA for a torsion's "theta"; a per-term
 // parameter -> PARAM (its index), a global parameter -> GLOBAL (its slot in globalSlot, the per-Context map shared by every
 // custom force; a name seen for the first time gets the next slot).  Any other variable is an error, as on the Reference
-// platform.  periodicdistance and its first derivatives -> PERIODIC_DIST.  forceName names the class in messages.
+// platform.  periodicdistance and its first derivatives -> PERIODIC_DIST, pointdistance / pointangle / pointdihedral and
+// theirs -> POINT_DIST / POINT_ANGLE / POINT_DIHEDRAL (the parser knows these names only for the classes that have them).
+// forceName names the class in messages; maxStack is the stack capacity of the class's interpreter.
 inline Program translateProgram(const Lepton::ExpressionProgram& prog, const std::vector<std::string>& variables, const std::string& forceName,
                                 const std::vector<std::string>& paramNames, const std::vector<std::string>& globalNames,
-                                std::map<std::string, int>& globalSlot) {
+                                std::map<std::string, int>& globalSlot, int maxStack = B200MD_CUSTOM_MAX_STACK) {
     typedef Lepton::Operation Op;
-    if (prog.getStackSize() > B200MD_CUSTOM_MAX_STACK)
-        throw Unsupported("B200 platform: a " + forceName + " expression needs a stack deeper than 16");
+    if (prog.getStackSize() > maxStack)
+        throw Unsupported("B200 platform: a " + forceName + " expression needs a stack deeper than " + std::to_string(maxStack));
     if (prog.getNumOperations() > B200MD_CUSTOM_MAX_CODE)
         throw Unsupported("B200 platform: a " + forceName + " expression has more than 256 operations");
     Program out;
@@ -78,14 +97,17 @@ inline Program translateProgram(const Lepton::ExpressionProgram& prog, const std
                 break;
             }
             case Op::CUSTOM: {
-                if (o.getName() != "periodicdistance")
+                const std::string& fn = o.getName();
+                code = fn == "periodicdistance" ? B200MD_OP_PERIODIC_DIST : fn == "pointdistance" ? B200MD_OP_POINT_DIST :
+                       fn == "pointangle" ? B200MD_OP_POINT_ANGLE : fn == "pointdihedral" ? B200MD_OP_POINT_DIHEDRAL : -1;
+                if (code < 0)
                     throw Unsupported("B200 platform: tabulated functions in a " + forceName + " expression are not supported");
-                // getDerivOrder: all zero is the distance, a single 1 the first derivative by that argument
+                // getDerivOrder: all zero is the value, a single 1 the first derivative by that argument
                 const std::vector<int>& order = dynamic_cast<const Op::Custom&>(o).getDerivOrder();
                 int which = -1, total = 0;
                 for (size_t k = 0; k < order.size(); k++) { total += order[k]; if (order[k] == 1) which = (int) k; }
-                if (total > 1) throw Unsupported("B200 platform: second derivatives of periodicdistance are not supported");
-                code = B200MD_OP_PERIODIC_DIST; arg = total ? which : -1;
+                if (total > 1) throw Unsupported("B200 platform: second derivatives of " + fn + " are not supported");
+                arg = total ? which : -1;
                 break;
             }
             case Op::ADD: code = B200MD_OP_ADD; break;
@@ -150,6 +172,37 @@ inline void translateExpression(const std::string& energy, const std::vector<std
     std::vector<Program> out(1, translateProgram(expr.createProgram(), variables, forceName, paramNames, globalNames, slots));
     for (const std::string& v : variables)
         out.push_back(translateProgram(expr.differentiate(v).optimize().createProgram(), variables, forceName, paramNames, globalNames, slots));
+    programs.swap(out);
+    globalSlot.swap(slots);
+}
+
+// A CustomCompoundBondForce: its energy program and the derivative programs by x1, y1, z1, x2, .. (1 + 3 particles per bond).
+// CustomCompoundBondForceImpl::prepareExpression (libOpenMM.so) turns distance, angle and dihedral into the point functions, as
+// for the Reference platform; the expression is then an ordinary function of the coordinates.
+inline void translateCompound(const OpenMM::CustomCompoundBondForce& force, std::map<std::string, int>& globalSlot, std::vector<Program>& programs) {
+    const std::string forceName = "CustomCompoundBondForce";
+    const int numParticles = force.getNumParticlesPerBond();
+    if (numParticles > B200MD_CUSTOM_MAX_PARTICLES)
+        throw Unsupported("B200 platform: a CustomCompoundBondForce with more than 8 particles per bond is not supported");
+    if (force.getNumPerBondParameters() > B200MD_CUSTOM_MAX_PARAMS)
+        throw Unsupported("B200 platform: a CustomCompoundBondForce with more than 16 per-bond parameters is not supported");
+    if (force.getNumTabulatedFunctions() > 0)
+        throw Unsupported("B200 platform: tabulated functions in a CustomCompoundBondForce expression are not supported");
+    PointFunctionPlaceholder distance(6), angle(9), dihedral(12);
+    std::map<std::string, Lepton::CustomFunction*> functions;
+    functions["pointdistance"] = &distance; functions["pointangle"] = &angle; functions["pointdihedral"] = &dihedral;
+    const Lepton::ParsedExpression expr = OpenMM::CustomCompoundBondForceImpl::prepareExpression(force, functions);
+    std::vector<std::string> variables, paramNames, globalNames;
+    for (int i = 1; i <= numParticles; i++)
+        for (const char* axis : {"x", "y", "z"}) variables.push_back(axis + std::to_string(i));
+    for (int i = 0; i < force.getNumPerBondParameters(); i++) paramNames.push_back(force.getPerBondParameterName(i));
+    for (int i = 0; i < force.getNumGlobalParameters(); i++) globalNames.push_back(force.getGlobalParameterName(i));
+    std::map<std::string, int> slots = globalSlot;      // committed only when every program translates
+    std::vector<Program> out(1, translateProgram(expr.createProgram(), variables, forceName, paramNames, globalNames, slots,
+                                                 B200MD_CUSTOM_COMPOUND_MAX_STACK));
+    for (const std::string& v : variables)
+        out.push_back(translateProgram(expr.differentiate(v).optimize().createProgram(), variables, forceName, paramNames, globalNames, slots,
+                                       B200MD_CUSTOM_COMPOUND_MAX_STACK));
     programs.swap(out);
     globalSlot.swap(slots);
 }
