@@ -81,44 +81,40 @@ struct CmapTable : TermTable<int4, double> {
     std::vector<int> map; std::vector<int2> maps;
     DevBuf<int> mapDev; DevBuf<int2> mapsDev;
 };
-// One class of custom terms (B200MD_CUSTOM_* but the compound bonds): atoms (a torsion's four, a bond's two, an external's one, an angle's three, zero-padded to an
-// int4), params [n][stride] and groups in the caller's term order; besides, the programs (code = (opcode, operand), imm,
-// progStart; 1 + the class's number of variables programs per expression) and the expression of every term.
-struct CustomClass : TermTable<int4, double> {
-    int stride = 0, nprog = 0;
-    std::vector<int2> code; std::vector<double> imm; std::vector<int> progStart, prog, slot;
+// One class of custom terms (B200MD_CUSTOM_*), in the caller's order: per term its expression, its atoms at the class's
+// width (CUSTOM_NAMES: a torsion's four, a bond's two, an external's one, an angle's three, a compound bond's eight with the
+// unused ones -1), params [n][stride] and group; per expression its first program (exprProg[nexpr]: the number of programs,
+// 1 + the class's number of variables per expression, 1 + 3 particles for a compound bond), its particles per term and
+// whether its point functions take the minimum image (both 0 but for compound bonds); the programs (op, arg, imm,
+// progStart).  slot[i] is the slot of term i in its kernel's layout.
+struct CustomClass {
+    int n = 0, stride = 0, nexpr = 0;
+    std::vector<int> atoms, expr, exprProg, nparticles, periodic, progStart, op, arg, slot;
+    std::vector<double> imm, params; std::vector<unsigned char> group;
 };
-// The custom torsions, bonds, externals and angles and the global values (one slot space for all, the compound bonds
-// included).  finalize lays the terms of all four out as k_custom reads them (CustomDev): grouped by expression, each group padded to whole warps, with one
-// parameter stride (the widest class's); cls[k].slot[i] is the slot of term i of class k.
-struct CustomTable {
-    CustomClass cls[4];
+// The classes [first, last) one kernel runs, in its layout (finalize, layout_custom): k_custom the torsions, bonds, externals
+// and angles (CustomDev), k_compound the compound bonds (CompoundDev).
+struct CustomSlots {
+    int first, last;
     int nslots = 0, stride = 0;
-    std::vector<double> globals;
-    DevBuf<int4> atomsDev; DevBuf<double> paramsDev, immDev, globalsDev; DevBuf<unsigned char> groupDev;
-    DevBuf<int2> codeDev; DevBuf<int> exprDev, exprClassDev, exprProgDev, progStartDev;
-    // params in the slot layout (padding slots 0)
-    std::vector<double> slot_params() const {
-        std::vector<double> p((size_t) nslots*stride, 0.0);
-        for (const CustomClass& t : cls)
-            for (int i = 0; i < t.n; i++)
-                std::copy(t.params.begin() + (size_t) i*t.stride, t.params.begin() + (size_t) (i+1)*t.stride, p.begin() + (size_t) t.slot[i]*stride);
-        return p;
-    }
-};
-
-// The custom compound bonds: per expression its number of particles, whether its point functions take the minimum image and
-// its 1 + 3 particles programs; per term its expression, 8 atom slots (unused -1), params [n][stride] and group, in the
-// caller's order.  finalize lays the terms out as k_compound reads them (CompoundDev); slot[i] is the slot of term i.
-struct CompoundTable {
-    int n = 0, stride = 0, nexpr = 0, nslots = 0;
-    std::vector<int> nparticles, periodic, exprProg, progStart, expr, atoms, slot;
-    std::vector<int2> code; std::vector<double> imm, params; std::vector<unsigned char> group;
-    DevBuf<int> atomsDev, exprDev, nparticlesDev, periodicDev, exprProgDev, progStartDev;
+    DevBuf<int> atomsDev, exprDev, exprClassDev, exprParticlesDev, exprPeriodicDev, exprProgDev, progStartDev;
     DevBuf<int2> codeDev; DevBuf<double> immDev, paramsDev; DevBuf<unsigned char> groupDev;
-    std::vector<double> slot_params() const {
-        std::vector<double> p((size_t) nslots*stride, 0.0);
-        for (int i = 0; i < n; i++) std::copy(params.begin() + (size_t) i*stride, params.begin() + (size_t) (i+1)*stride, p.begin() + (size_t) slot[i]*stride);
+};
+// Every custom class and the global values (one slot space for all classes)
+struct CustomTable {
+    CustomClass cls[5];
+    CustomSlots kernel[2] = {{B200MD_CUSTOM_TORSION, B200MD_CUSTOM_COMPOUND}, {B200MD_CUSTOM_COMPOUND, B200MD_CUSTOM_COMPOUND + 1}};
+    std::vector<double> globals;
+    DevBuf<double> globalsDev;
+    CustomSlots& kernel_of(int cls) { return kernel[cls == B200MD_CUSTOM_COMPOUND ? 1 : 0]; }
+    // the params of the classes of s in its slot layout (padding slots 0)
+    std::vector<double> slot_params(const CustomSlots& s) const {
+        std::vector<double> p((size_t) s.nslots*s.stride, 0.0);
+        for (int k = s.first; k < s.last; k++) {
+            const CustomClass& t = cls[k];
+            for (int i = 0; i < t.n; i++)
+                std::copy(t.params.begin() + (size_t) i*t.stride, t.params.begin() + (size_t) (i+1)*t.stride, p.begin() + (size_t) t.slot[i]*s.stride);
+        }
         return p;
     }
 };
@@ -211,7 +207,6 @@ struct b200md_ctx {
     TermTable<int4, double> rb;             // [n][6] c0..c5
     CmapTable cmap;
     CustomTable custom;
-    CompoundTable compound;
     std::vector<int> conI, conJ; std::vector<double> conD;
     int cmFreq = 0;
     std::vector<int4> hUnitAtoms;        // host copy of the integration units (ownership cuts of the multi-GPU data plane)
@@ -442,126 +437,115 @@ extern "C" int b200md_set_cmap(b200md_ctx* ctx, int nmaps, const int* size, cons
     ctx->cmap.map.assign(map, map + n); ctx->cmap.maps.swap(maps);
     API_END(ctx)
 }
-// What the messages of a custom class's calls name it
-struct CustomNames { const char* call; const char* term; const char* per; };
-static const CustomNames CUSTOM_NAMES[4] = {{"set_custom_torsions", "custom torsion", "torsion"},
-                                            {"set_custom_bonds", "custom bond", "bond"},
-                                            {"set_custom_externals", "custom external", "particle"},
-                                            {"set_custom_angles", "custom angle", "angle"}};
+// What the custom classes differ in on the host: the names in the messages of their calls (what the set call counts: programs,
+// or expressions for compound bonds), the atoms per term, whether a term's atoms join the molecules that wrap together (not an
+// external's, which acts on one particle, nor a compound bond's, which reads continuous coordinates and may tie two molecules
+// that must keep wrapping apart), the term bit and the bonded kind.
+struct CustomNames {
+    const char* call; const char* term; const char* per; const char* unit; const char* update; const char* terms;
+    int width; bool joins; int bit; int kind;
+};
+static const CustomNames CUSTOM_NAMES[5] = {
+    {"set_custom_torsions", "custom torsion", "torsion", "program", "update_custom_torsion_params", "torsions", 4, true,
+     B200MD_TERM_CUSTOM_TORSIONS, B200MD_BONDED_CUSTOM_TORSIONS},
+    {"set_custom_bonds", "custom bond", "bond", "program", "update_custom_bond_params", "bonds", 2, true,
+     B200MD_TERM_CUSTOM_BONDS, B200MD_BONDED_CUSTOM_BONDS},
+    {"set_custom_externals", "custom external", "particle", "program", "update_custom_external_params", "particles", 1, false,
+     B200MD_TERM_CUSTOM_EXTERNALS, B200MD_BONDED_CUSTOM_EXTERNALS},
+    {"set_custom_angles", "custom angle", "angle", "program", "update_custom_angle_params", "angles", 3, true,
+     B200MD_TERM_CUSTOM_ANGLES, B200MD_BONDED_CUSTOM_ANGLES},
+    {"set_custom_compound", "custom compound bond", "bond", "expression", "update_custom_compound_params", "bonds", B200MD_CUSTOM_MAX_PARTICLES, false,
+     B200MD_TERM_CUSTOM_COMPOUND, B200MD_BONDED_CUSTOM_COMPOUND}};
 
-// A program set of class cls (b200md_set_custom_torsions / _bonds / _externals / _angles): prog_start well formed and every program
-// passing custom_check_program (nglobals < 0: GLOBAL operands are checked at finalize).  Returns the instructions as
-// (opcode, operand).
-static std::vector<int2> check_programs(int cls, int nprog, const int* prog_start, const int* op, const int* arg, int stride, int nglobals) {
+// A program set of class cls (b200md_set_custom_torsions / _bonds / _externals / _angles / _compound): nexpr expressions, the
+// programs of one after the other's (1 + the class's number of variables each; 1 + 3 nparticles[p] for compound bonds),
+// prog_start well formed and every program passing custom_check_program (nglobals < 0: GLOBAL operands are checked at
+// finalize).  Returns the instructions as (opcode, operand) and, in exprProg, every expression's first program and, last,
+// the number of programs.
+static std::vector<int2> check_programs(int cls, int nexpr, const int* nparticles, const int* prog_start, const int* op, const int* arg,
+                                        int stride, int nglobals, std::vector<int>& exprProg) {
+    const bool compound = cls == B200MD_CUSTOM_COMPOUND;
     const std::string call = CUSTOM_NAMES[cls].call;
-    require(nprog >= 0, (call + ": negative number of programs").c_str());
+    require(nexpr >= 0, (call + ": negative number of " + CUSTOM_NAMES[cls].unit + "s").c_str());
     require(stride >= 0 && stride <= B200MD_CUSTOM_MAX_PARAMS, (call + ": more than 16 parameters per " + CUSTOM_NAMES[cls].per).c_str());
-    require(nprog == 0 || prog_start[0] == 0, (call + ": prog_start[0] must be 0").c_str());
-    const int nq = nprog*(1 + custom_num_vars(cls));
-    for (int q = 0; q < nq; q++) require(prog_start[q+1] >= prog_start[q], (call + ": prog_start must not decrease").c_str());
-    const int total = nprog ? prog_start[nq] : 0;
-    std::vector<int2> code(total);
-    for (int k = 0; k < total; k++) code[k] = make_int2(op[k], arg[k]);
-    for (int q = 0; q < nq; q++) {
-        const char* why = custom_check_program(cls, code.data(), prog_start[q], prog_start[q+1], stride, nglobals);
-        if (why) throw std::runtime_error(std::string(why) + " (program " + std::to_string(q) + ")");
-    }
-    return code;
-}
-// The terms of class cls: term i evaluates expression prog[i] on the atoms atoms[w*i .. w*i+w-1] (w = 4, 2, 1, 3)
-static void set_custom(b200md_ctx* ctx, int cls, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
-                       int stride, int n, const int* prog, const int* atoms, const double* params) {
-    const CustomNames& nm = CUSTOM_NAMES[cls];
-    check_set(ctx, nm.call, n);
-    require(ctx->world == 1, (std::string(nm.term) + "s are not supported in multi-GPU runs").c_str());
-    std::vector<int2> code = check_programs(cls, nprog, prog_start, op, arg, stride, -1);
-    for (int i = 0; i < n; i++) require(prog[i] >= 0 && prog[i] < nprog, (std::string(nm.term) + ": program index out of range").c_str());
-    const int w = cls == B200MD_CUSTOM_TORSION ? 4 : cls == B200MD_CUSTOM_BOND ? 2 : cls == B200MD_CUSTOM_ANGLE ? 3 : 1;
-    std::vector<int4> a(n, make_int4(0, 0, 0, 0)); std::vector<double> p(params, params + (size_t) n*stride);
-    for (int i = 0; i < n; i++) {
-        int* q = &a[i].x;
-        for (int k = 0; k < w; k++) q[k] = atoms[w*i + k];
-    }
-    CustomClass& t = ctx->custom.cls[cls];
-    t.set(ctx->natoms, nm.term, n, a, p);
-    t.stride = stride; t.nprog = nprog; t.code.swap(code);
-    t.imm.assign(imm, imm + t.code.size());
-    t.progStart.assign(prog_start, prog_start + (nprog ? nprog*(1 + custom_num_vars(cls)) + 1 : 0)); t.prog.assign(prog, prog + n);
-}
-extern "C" int b200md_set_custom_torsions(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
-                                          int stride, int n, const int* prog, const int* atoms, const double* params) {
-    API_BEGIN(ctx)
-    set_custom(ctx, B200MD_CUSTOM_TORSION, nprog, prog_start, op, arg, imm, stride, n, prog, atoms, params);
-    API_END(ctx)
-}
-extern "C" int b200md_set_custom_bonds(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
-                                       int stride, int n, const int* prog, const int* atoms, const double* params) {
-    API_BEGIN(ctx)
-    set_custom(ctx, B200MD_CUSTOM_BOND, nprog, prog_start, op, arg, imm, stride, n, prog, atoms, params);
-    API_END(ctx)
-}
-extern "C" int b200md_set_custom_externals(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
-                                           int stride, int n, const int* prog, const int* atoms, const double* params) {
-    API_BEGIN(ctx)
-    set_custom(ctx, B200MD_CUSTOM_EXTERNAL, nprog, prog_start, op, arg, imm, stride, n, prog, atoms, params);
-    API_END(ctx)
-}
-extern "C" int b200md_set_custom_angles(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
-                                        int stride, int n, const int* prog, const int* atoms, const double* params) {
-    API_BEGIN(ctx)
-    set_custom(ctx, B200MD_CUSTOM_ANGLE, nprog, prog_start, op, arg, imm, stride, n, prog, atoms, params);
-    API_END(ctx)
-}
-// The programs of compound-bond expressions (1 + 3 nparticles[p] each, one expression's after the other's), checked as
-// check_programs checks the other classes'.  Returns the instructions and, in exprProg, every expression's first program.
-static std::vector<int2> check_compound_programs(int nexpr, const int* nparticles, const int* prog_start, const int* op, const int* arg,
-                                                 int stride, int nglobals, std::vector<int>& exprProg) {
-    const std::string call = "set_custom_compound";
-    require(nexpr >= 0, (call + ": negative number of expressions").c_str());
-    require(stride >= 0 && stride <= B200MD_CUSTOM_MAX_PARAMS, (call + ": more than 16 parameters per bond").c_str());
     require(nexpr == 0 || prog_start[0] == 0, (call + ": prog_start[0] must be 0").c_str());
-    exprProg.assign(nexpr, 0);
-    int nq = 0;
+    exprProg.assign(nexpr + 1, 0);
     for (int p = 0; p < nexpr; p++) {
-        require(nparticles[p] >= 1 && nparticles[p] <= B200MD_CUSTOM_MAX_PARTICLES, (call + ": an expression must join 1 to 8 particles").c_str());
-        exprProg[p] = nq;
-        nq += 1 + 3*nparticles[p];
+        if (compound)
+            require(nparticles[p] >= 1 && nparticles[p] <= B200MD_CUSTOM_MAX_PARTICLES, (call + ": an expression must join 1 to 8 particles").c_str());
+        exprProg[p+1] = exprProg[p] + 1 + (compound ? 3*nparticles[p] : custom_num_vars(cls));
     }
+    const int nq = exprProg[nexpr];
     for (int q = 0; q < nq; q++) require(prog_start[q+1] >= prog_start[q], (call + ": prog_start must not decrease").c_str());
     const int total = nexpr ? prog_start[nq] : 0;
     std::vector<int2> code(total);
     for (int k = 0; k < total; k++) code[k] = make_int2(op[k], arg[k]);
     for (int p = 0; p < nexpr; p++)
-        for (int q = exprProg[p]; q < exprProg[p] + 1 + 3*nparticles[p]; q++) {
-            const char* why = custom_check_program(B200MD_CUSTOM_COMPOUND, code.data(), prog_start[q], prog_start[q+1], stride, nglobals, nparticles[p]);
+        for (int q = exprProg[p]; q < exprProg[p+1]; q++) {
+            const char* why = custom_check_program(cls, code.data(), prog_start[q], prog_start[q+1], stride, nglobals, compound ? nparticles[p] : 0);
             if (why) throw std::runtime_error(std::string(why) + " (program " + std::to_string(q) + ")");
         }
     return code;
+}
+// The terms of class cls: term i evaluates expression expr[i] on the atoms atoms[w*i .. w*i+w-1] (w = the class's width; a
+// compound bond's unused slots -1).  nparticles and periodic (per expression) are read for compound bonds only.
+static void set_custom(b200md_ctx* ctx, int cls, int nexpr, const int* nparticles, const int* periodic, const int* prog_start, const int* op,
+                       const int* arg, const double* imm, int stride, int n, const int* expr, const int* atoms, const double* params) {
+    const CustomNames& nm = CUSTOM_NAMES[cls];
+    const bool compound = cls == B200MD_CUSTOM_COMPOUND;
+    check_set(ctx, nm.call, n);
+    require(ctx->world == 1, (std::string(nm.term) + "s are not supported in multi-GPU runs").c_str());
+    std::vector<int> exprProg;
+    check_programs(cls, nexpr, nparticles, prog_start, op, arg, stride, -1, exprProg);
+    const int w = nm.width;
+    for (int i = 0; i < n; i++) {
+        require(expr[i] >= 0 && expr[i] < nexpr, (std::string(nm.term) + ": " + nm.unit + " index out of range").c_str());
+        for (int k = 0; k < w; k++) {
+            const int a = atoms[w*i + k];
+            if (!compound || k < nparticles[expr[i]]) require(a >= 0 && a < ctx->natoms, (std::string(nm.term) + ": atom index out of range").c_str());
+            else require(a == -1, "custom compound bond: an unused atom slot must be -1");
+        }
+    }
+    CustomClass& t = ctx->custom.cls[cls];            // its group stays: groups may come before the terms
+    const int nq = exprProg[nexpr];
+    t.n = n; t.stride = stride; t.nexpr = nexpr; t.exprProg.swap(exprProg);
+    t.nparticles.assign(nexpr, 0); t.periodic.assign(nexpr, 0);
+    if (compound) { t.nparticles.assign(nparticles, nparticles + nexpr); t.periodic.assign(periodic, periodic + nexpr); }
+    t.progStart.assign(prog_start, prog_start + (nexpr ? nq + 1 : 0));
+    const int total = nexpr ? prog_start[nq] : 0;
+    t.op.assign(op, op + total); t.arg.assign(arg, arg + total); t.imm.assign(imm, imm + total);
+    t.expr.assign(expr, expr + n); t.atoms.assign(atoms, atoms + (size_t) w*n);
+    t.params.assign(params, params + (size_t) n*stride);
+}
+extern "C" int b200md_set_custom_torsions(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                          int stride, int n, const int* prog, const int* atoms, const double* params) {
+    API_BEGIN(ctx)
+    set_custom(ctx, B200MD_CUSTOM_TORSION, nprog, nullptr, nullptr, prog_start, op, arg, imm, stride, n, prog, atoms, params);
+    API_END(ctx)
+}
+extern "C" int b200md_set_custom_bonds(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                       int stride, int n, const int* prog, const int* atoms, const double* params) {
+    API_BEGIN(ctx)
+    set_custom(ctx, B200MD_CUSTOM_BOND, nprog, nullptr, nullptr, prog_start, op, arg, imm, stride, n, prog, atoms, params);
+    API_END(ctx)
+}
+extern "C" int b200md_set_custom_externals(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                           int stride, int n, const int* prog, const int* atoms, const double* params) {
+    API_BEGIN(ctx)
+    set_custom(ctx, B200MD_CUSTOM_EXTERNAL, nprog, nullptr, nullptr, prog_start, op, arg, imm, stride, n, prog, atoms, params);
+    API_END(ctx)
+}
+extern "C" int b200md_set_custom_angles(b200md_ctx* ctx, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                        int stride, int n, const int* prog, const int* atoms, const double* params) {
+    API_BEGIN(ctx)
+    set_custom(ctx, B200MD_CUSTOM_ANGLE, nprog, nullptr, nullptr, prog_start, op, arg, imm, stride, n, prog, atoms, params);
+    API_END(ctx)
 }
 extern "C" int b200md_set_custom_compound(b200md_ctx* ctx, int nexpr, const int* nparticles, const int* periodic, const int* prog_start,
                                           const int* op, const int* arg, const double* imm, int stride, int n, const int* expr,
                                           const int* atoms, const double* params) {
     API_BEGIN(ctx)
-    check_set(ctx, "set_custom_compound", n);
-    require(ctx->world == 1, "custom compound bonds are not supported in multi-GPU runs");
-    std::vector<int> exprProg;
-    std::vector<int2> code = check_compound_programs(nexpr, nparticles, prog_start, op, arg, stride, -1, exprProg);
-    for (int i = 0; i < n; i++) {
-        require(expr[i] >= 0 && expr[i] < nexpr, "custom compound bond: expression index out of range");
-        for (int k = 0; k < B200MD_CUSTOM_MAX_PARTICLES; k++) {
-            const int a = atoms[B200MD_CUSTOM_MAX_PARTICLES*i + k];
-            if (k < nparticles[expr[i]]) require(a >= 0 && a < ctx->natoms, "custom compound bond: atom index out of range");
-            else require(a == -1, "custom compound bond: an unused atom slot must be -1");
-        }
-    }
-    CompoundTable& t = ctx->compound;            // its group stays: groups may come before the terms
-    t.n = n; t.stride = stride; t.nexpr = nexpr; t.code.swap(code); t.exprProg.swap(exprProg);
-    t.nparticles.assign(nparticles, nparticles + nexpr); t.periodic.assign(periodic, periodic + nexpr);
-    const int nq = nexpr ? t.exprProg[nexpr-1] + 1 + 3*nparticles[nexpr-1] : 0;
-    t.progStart.assign(prog_start, prog_start + (nexpr ? nq + 1 : 0));
-    t.imm.assign(imm, imm + t.code.size());
-    t.expr.assign(expr, expr + n); t.atoms.assign(atoms, atoms + (size_t) B200MD_CUSTOM_MAX_PARTICLES*n);
-    t.params.assign(params, params + (size_t) n*stride);
+    set_custom(ctx, B200MD_CUSTOM_COMPOUND, nexpr, nparticles, periodic, prog_start, op, arg, imm, stride, n, expr, atoms, params);
     API_END(ctx)
 }
 extern "C" int b200md_set_custom_globals(b200md_ctx* ctx, int n, const double* values) {
@@ -575,40 +559,44 @@ extern "C" int b200md_set_custom_globals(b200md_ctx* ctx, int n, const double* v
     if (n) CUDA_CHECK(cudaMemcpyAsync(t.globalsDev.p, t.globals.data(), sizeof(double)*n, cudaMemcpyHostToDevice, ctx->stream));
     API_END(ctx)
 }
-extern "C" int b200md_custom_term_probe(int cls, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
-                                        int stride, int nglobals, int which, const double* vars, const double* box,
-                                        const double* params, const double* globals, double* out, char* msg, int msglen) {
+// The probes: program `which` of a program set of class cls, checked as the set call checks it (nglobals = the number of
+// global slots) and run on the host by the interpreter source the device kernels run.  name begins the probe's own messages.
+static int custom_probe(const char* name, int cls, int nexpr, const int* nparticles, int periodic, const int* prog_start, const int* op,
+                        const int* arg, const double* imm, int stride, int nglobals, int which, const double* vars, const double* box,
+                        const double* params, const double* globals, double* out, char* msg, int msglen) {
     try {
-        require(cls >= B200MD_CUSTOM_TORSION && cls <= B200MD_CUSTOM_ANGLE, "custom_term_probe: unknown class");
-        require(nglobals >= 0, "custom_program_probe: negative number of globals");
-        const std::vector<int2> code = check_programs(cls, nprog, prog_start, op, arg, stride, nglobals);
-        require(which >= 0 && which < nprog*(1 + custom_num_vars(cls)), "custom_program_probe: program index out of range");
+        require(nglobals >= 0, (std::string(name) + ": negative number of globals").c_str());
+        std::vector<int> exprProg;
+        const std::vector<int2> code = check_programs(cls, nexpr, nparticles, prog_start, op, arg, stride, nglobals, exprProg);
+        require(which >= 0 && which < exprProg[nexpr], (std::string(name) + ": program index out of range").c_str());
         CustomBox b = {1.0, 0.0, 1.0, 0.0, 0.0, 1.0};
         if (box) b = CustomBox{box[0], box[3], box[4], box[6], box[7], box[8]};
-        *out = custom_run<B200MD_CUSTOM_MAX_STACK, false>(code.data(), imm, prog_start[which], prog_start[which+1], vars, params, globals, b);
+        *out = cls == B200MD_CUSTOM_COMPOUND
+            ? custom_run<B200MD_CUSTOM_COMPOUND_MAX_STACK, true>(code.data(), imm, prog_start[which], prog_start[which+1], vars, params, globals, b,
+                                                                  periodic != 0)
+            : custom_run<B200MD_CUSTOM_MAX_STACK, false>(code.data(), imm, prog_start[which], prog_start[which+1], vars, params, globals, b);
         return 0;
     } catch (std::exception& e) {
         if (msg && msglen > 0) { strncpy(msg, e.what(), msglen - 1); msg[msglen - 1] = 0; }
         return -1;
     }
 }
+extern "C" int b200md_custom_term_probe(int cls, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
+                                        int stride, int nglobals, int which, const double* vars, const double* box,
+                                        const double* params, const double* globals, double* out, char* msg, int msglen) {
+    // compound bonds have particle counts: b200md_custom_compound_probe
+    if (cls < B200MD_CUSTOM_TORSION || cls > B200MD_CUSTOM_ANGLE) {
+        if (msg && msglen > 0) { strncpy(msg, "custom_term_probe: unknown class", msglen - 1); msg[msglen - 1] = 0; }
+        return -1;
+    }
+    return custom_probe("custom_program_probe", cls, nprog, nullptr, 0, prog_start, op, arg, imm, stride, nglobals, which, vars, box, params,
+                        globals, out, msg, msglen);
+}
 extern "C" int b200md_custom_compound_probe(int nparticles, int periodic, const int* prog_start, const int* op, const int* arg, const double* imm,
                                             int stride, int nglobals, int which, const double* vars, const double* box,
                                             const double* params, const double* globals, double* out, char* msg, int msglen) {
-    try {
-        require(nglobals >= 0, "custom_compound_probe: negative number of globals");
-        std::vector<int> exprProg;
-        const std::vector<int2> code = check_compound_programs(1, &nparticles, prog_start, op, arg, stride, nglobals, exprProg);
-        require(which >= 0 && which < 1 + 3*nparticles, "custom_compound_probe: program index out of range");
-        CustomBox b = {1.0, 0.0, 1.0, 0.0, 0.0, 1.0};
-        if (box) b = CustomBox{box[0], box[3], box[4], box[6], box[7], box[8]};
-        *out = custom_run<B200MD_CUSTOM_COMPOUND_MAX_STACK, true>(code.data(), imm, prog_start[which], prog_start[which+1], vars, params, globals,
-                                                                    b, periodic != 0);
-        return 0;
-    } catch (std::exception& e) {
-        if (msg && msglen > 0) { strncpy(msg, e.what(), msglen - 1); msg[msglen - 1] = 0; }
-        return -1;
-    }
+    return custom_probe("custom_compound_probe", B200MD_CUSTOM_COMPOUND, 1, &nparticles, periodic, prog_start, op, arg, imm, stride, nglobals,
+                        which, vars, box, params, globals, out, msg, msglen);
 }
 extern "C" int b200md_custom_program_probe(int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
                                            int stride, int nglobals, int which, double theta, const double* params,
@@ -623,14 +611,12 @@ extern "C" int b200md_set_bonded_groups(b200md_ctx* ctx, int kind, int n, const 
             kind == B200MD_BONDED_CUSTOM_COMPOUND,
             "set_bonded_groups: kind must be 0 (bonds), 1 (angles), 2 (torsions), 3 (RB torsions), 4 (CMAP), 5 (custom torsions), "
             "6 (custom bonds), 7 (custom externals), 9 (custom angles) or 10 (custom compound bonds)");
-    std::vector<unsigned char>& g = kind == B200MD_BONDED_BONDS ? ctx->bonds.group : kind == B200MD_BONDED_ANGLES ? ctx->angles.group :
-                                    kind == B200MD_BONDED_TORSIONS ? ctx->torsions.group : kind == B200MD_BONDED_RB_TORSIONS ? ctx->rb.group :
-                                    kind == B200MD_BONDED_CMAP ? ctx->cmap.group :
-                                    kind == B200MD_BONDED_CUSTOM_ANGLES ? ctx->custom.cls[B200MD_CUSTOM_ANGLE].group :
-                                    kind == B200MD_BONDED_CUSTOM_COMPOUND ? ctx->compound.group :
-                                    ctx->custom.cls[kind - B200MD_BONDED_CUSTOM_TORSIONS].group;
-    g.resize(n);
-    for (int i = 0; i < n; i++) { require(group[i] >= 0 && (group[i] & ~0x80) < 32, "force group out of range"); g[i] = (unsigned char) group[i]; }
+    std::vector<unsigned char>* g = kind == B200MD_BONDED_BONDS ? &ctx->bonds.group : kind == B200MD_BONDED_ANGLES ? &ctx->angles.group :
+                                    kind == B200MD_BONDED_TORSIONS ? &ctx->torsions.group : kind == B200MD_BONDED_RB_TORSIONS ? &ctx->rb.group :
+                                    &ctx->cmap.group;
+    for (int k = 0; k < 5; k++) if (kind == CUSTOM_NAMES[k].kind) g = &ctx->custom.cls[k].group;
+    g->resize(n);
+    for (int i = 0; i < n; i++) { require(group[i] >= 0 && (group[i] & ~0x80) < 32, "force group out of range"); (*g)[i] = (unsigned char) group[i]; }
     API_END(ctx)
 }
 extern "C" int b200md_set_constraints(b200md_ctx* ctx, int n, const int* p1, const int* p2, const double* d) {
@@ -1410,117 +1396,93 @@ static bool fft_beside_tiles(const b200md_ctx* c) {
     return c->mg == MG_SINGLE && !c->pmeOnly && c->overlapPme && !c->nb.smPartition && c->nbdesc.method == B200MD_NB_PME;
 }
 
-// finalize: the custom terms of all four classes in the layout of k_custom (CustomDev): grouped by expression, each group
-// padded to whole warps, and the programs, checked once more now that the number of global slots is final
-static void upload_custom(b200md_ctx* c) {
+// finalize: the classes of one kernel in its layout: the terms grouped by expression, each group padded to whole warps (a
+// padding slot has expression -1 and the atoms `pad`), `width` atoms per slot, the parameters at one stride (the widest
+// class's); the expressions and programs of all its classes one after the other (class k's expression p is expression
+// exprBase[k] + p), the programs checked once more now that the number of global slots is final.  Returns the term bits of
+// the classes that have terms.
+static int layout_custom(b200md_ctx* c, CustomSlots& s, int width, int pad) {
     CustomTable& t = c->custom;
-    CustomDev& d = c->ctd;
-    d = CustomDev{};
-    d.groupMask = 0xffffffffu;
-    // the global values get their buffer even without terms: a custom force with no terms may still name globals, and
-    // b200md_set_custom_globals copies into this buffer after finalize
-    t.globalsDev.alloc(std::max<size_t>(t.globals.size(), 1)); t.globalsDev.upload(t.globals);
-    d.globals = t.globalsDev.p;
-    const int bits[4] = {B200MD_TERM_CUSTOM_TORSIONS, B200MD_TERM_CUSTOM_BONDS, B200MD_TERM_CUSTOM_EXTERNALS, B200MD_TERM_CUSTOM_ANGLES};
-    // expressions of all classes one after the other (class k's expression p is expression exprBase[k] + p), their programs
-    // likewise, the code of class k shifted by the instructions of the classes before it
-    std::vector<int2> code; std::vector<double> imm; std::vector<int> progStart(1, 0), exprClass, exprProg;
-    std::vector<int> exprBase(4, 0);
-    t.stride = 0;
-    for (int k = 0; k < 4; k++) {
-        CustomClass& cl = t.cls[k];
+    std::vector<int2> code; std::vector<double> imm;
+    std::vector<int> progStart(1, 0), exprClass, exprParticles, exprPeriodic, exprProg, exprBase(5, 0);
+    int terms = 0;
+    s.nslots = 0; s.stride = 0;
+    for (int k = s.first; k < s.last; k++) {
+        const CustomClass& cl = t.cls[k];
         exprBase[k] = (int) exprClass.size();
         if (cl.n == 0) continue;
         require(c->mg == MG_SINGLE, (std::string(CUSTOM_NAMES[k].term) + "s are not supported in multi-GPU runs").c_str());
         require(cl.group.empty() || (int) cl.group.size() == cl.n, "set_bonded_groups: group array length differs from the number of terms");
-        const int nv = custom_num_vars(k);
-        for (int q = 0; q < cl.nprog*(1 + nv); q++) {
-            const char* why = custom_check_program(k, cl.code.data(), cl.progStart[q], cl.progStart[q+1], cl.stride, (int) t.globals.size());
-            if (why) throw std::runtime_error(std::string(why) + " (program " + std::to_string(q) + ")");
+        std::vector<int> unused;
+        const std::vector<int2> cc = check_programs(k, cl.nexpr, cl.nparticles.data(), cl.progStart.data(), cl.op.data(), cl.arg.data(), cl.stride,
+                                                    (int) t.globals.size(), unused);
+        const int progBase = (int) progStart.size() - 1, codeBase = (int) code.size();
+        for (int p = 0; p < cl.nexpr; p++) {
+            exprClass.push_back(k); exprParticles.push_back(cl.nparticles[p]); exprPeriodic.push_back(cl.periodic[p]);
+            exprProg.push_back(progBase + cl.exprProg[p]);
         }
-        const int codeBase = (int) code.size();
-        for (int p = 0; p < cl.nprog; p++) {
-            exprClass.push_back(k);
-            exprProg.push_back((int) progStart.size() - 1 + p*(1 + nv));
-        }
-        for (int q = 0; q < cl.nprog*(1 + nv); q++) progStart.push_back(codeBase + cl.progStart[q+1]);
-        code.insert(code.end(), cl.code.begin(), cl.code.end());
+        for (int q = 0; q < cl.exprProg[cl.nexpr]; q++) progStart.push_back(codeBase + cl.progStart[q+1]);
+        code.insert(code.end(), cc.begin(), cc.end());
         imm.insert(imm.end(), cl.imm.begin(), cl.imm.end());
-        t.stride = std::max(t.stride, cl.stride);
-        d.terms |= bits[k];
+        s.stride = std::max(s.stride, cl.stride);
+        terms |= CUSTOM_NAMES[k].bit;
     }
-    t.nslots = 0;
-    if (d.terms == 0) return;
+    if (terms == 0) return 0;
     int cursor = 0;
-    for (int k = 0; k < 4; k++) {
+    for (int k = s.first; k < s.last; k++) {
         CustomClass& cl = t.cls[k];
         cl.slot.assign(cl.n, 0);
-        for (int p = 0; p < cl.nprog; p++) {
-            for (int i = 0; i < cl.n; i++) if (cl.prog[i] == p) cl.slot[i] = cursor++;
+        for (int p = 0; p < cl.nexpr; p++) {
+            for (int i = 0; i < cl.n; i++) if (cl.expr[i] == p) cl.slot[i] = cursor++;
             cursor = (cursor + 31)/32*32;
         }
     }
-    t.nslots = cursor;
-    std::vector<int4> atoms(cursor, make_int4(0, 0, 0, 0));
+    s.nslots = cursor;
+    std::vector<int> atoms((size_t) width*cursor, pad), expr(cursor, -1);
     std::vector<unsigned char> group(cursor, 0);
-    std::vector<int> expr(cursor, -1);
-    for (int k = 0; k < 4; k++) {
+    for (int k = s.first; k < s.last; k++) {
         const CustomClass& cl = t.cls[k];
+        const int w = CUSTOM_NAMES[k].width;
         for (int i = 0; i < cl.n; i++) {
-            atoms[cl.slot[i]] = cl.atoms[i]; group[cl.slot[i]] = cl.group.empty() ? 0 : cl.group[i]; expr[cl.slot[i]] = exprBase[k] + cl.prog[i];
+            std::copy(cl.atoms.begin() + (size_t) w*i, cl.atoms.begin() + (size_t) w*(i+1), atoms.begin() + (size_t) width*cl.slot[i]);
+            group[cl.slot[i]] = cl.group.empty() ? 0 : cl.group[i]; expr[cl.slot[i]] = exprBase[k] + cl.expr[i];
         }
     }
-    t.atomsDev.upload(atoms); t.groupDev.upload(group); t.exprDev.upload(expr);
-    const std::vector<double> par = t.slot_params();
-    t.paramsDev.alloc(std::max<size_t>(par.size(), 1)); t.paramsDev.upload(par);
-    t.codeDev.upload(code); t.immDev.upload(imm); t.progStartDev.upload(progStart);
-    t.exprClassDev.upload(exprClass); t.exprProgDev.upload(exprProg);
-    d.nslots = t.nslots; d.paramStride = t.stride;
-    d.atoms = t.atomsDev.p; d.params = t.paramsDev.p; d.group = t.groupDev.p; d.expr = t.exprDev.p;
-    d.exprClass = t.exprClassDev.p; d.exprProg = t.exprProgDev.p;
-    d.code = t.codeDev.p; d.imm = t.immDev.p; d.progStart = t.progStartDev.p;
+    s.atomsDev.upload(atoms); s.groupDev.upload(group); s.exprDev.upload(expr);
+    const std::vector<double> par = t.slot_params(s);
+    s.paramsDev.alloc(std::max<size_t>(par.size(), 1)); s.paramsDev.upload(par);
+    s.codeDev.upload(code); s.immDev.upload(imm); s.progStartDev.upload(progStart);
+    s.exprClassDev.upload(exprClass); s.exprParticlesDev.upload(exprParticles); s.exprPeriodicDev.upload(exprPeriodic); s.exprProgDev.upload(exprProg);
+    return terms;
 }
 
-// finalize: the compound bonds in the layout of k_compound (CompoundDev), after upload_custom (the global values are its)
-static void upload_compound(b200md_ctx* c) {
-    CompoundTable& t = c->compound;
-    CompoundDev& d = c->cpd;
-    d = CompoundDev{};
+// finalize: the custom terms in the layouts of k_custom (CustomDev: int4 atoms, zero-padded) and k_compound (CompoundDev: 8
+// atoms per slot, unused -1), and the global values both read
+static void upload_custom(b200md_ctx* c) {
+    CustomTable& t = c->custom;
+    // the global values get their buffer even without terms: a custom force with no terms may still name globals, and
+    // b200md_set_custom_globals copies into this buffer after finalize
+    t.globalsDev.alloc(std::max<size_t>(t.globals.size(), 1)); t.globalsDev.upload(t.globals);
+    CustomSlots& s = t.kernel[0];
+    CustomDev& d = c->ctd;
+    d = CustomDev{};
     d.groupMask = 0xffffffffu;
-    d.globals = c->ctd.globals;
-    t.nslots = 0;
-    if (t.n == 0) return;
-    require(c->mg == MG_SINGLE, "custom compound bonds are not supported in multi-GPU runs");
-    require(t.group.empty() || (int) t.group.size() == t.n, "set_bonded_groups: group array length differs from the number of terms");
-    for (int p = 0; p < t.nexpr; p++)
-        for (int q = t.exprProg[p]; q < t.exprProg[p] + 1 + 3*t.nparticles[p]; q++) {
-            const char* why = custom_check_program(B200MD_CUSTOM_COMPOUND, t.code.data(), t.progStart[q], t.progStart[q+1], t.stride,
-                                                   (int) c->custom.globals.size(), t.nparticles[p]);
-            if (why) throw std::runtime_error(std::string(why) + " (program " + std::to_string(q) + ")");
-        }
-    int cursor = 0;
-    t.slot.assign(t.n, 0);
-    for (int p = 0; p < t.nexpr; p++) {
-        for (int i = 0; i < t.n; i++) if (t.expr[i] == p) t.slot[i] = cursor++;
-        cursor = (cursor + 31)/32*32;
-    }
-    t.nslots = cursor;
-    std::vector<int> atoms((size_t) B200MD_CUSTOM_MAX_PARTICLES*cursor, -1), expr(cursor, -1);
-    std::vector<unsigned char> group(cursor, 0);
-    for (int i = 0; i < t.n; i++) {
-        std::copy(t.atoms.begin() + (size_t) B200MD_CUSTOM_MAX_PARTICLES*i, t.atoms.begin() + (size_t) B200MD_CUSTOM_MAX_PARTICLES*(i+1),
-                  atoms.begin() + (size_t) B200MD_CUSTOM_MAX_PARTICLES*t.slot[i]);
-        expr[t.slot[i]] = t.expr[i]; group[t.slot[i]] = t.group.empty() ? 0 : t.group[i];
-    }
-    t.atomsDev.upload(atoms); t.exprDev.upload(expr); t.groupDev.upload(group);
-    const std::vector<double> par = t.slot_params();
-    t.paramsDev.alloc(std::max<size_t>(par.size(), 1)); t.paramsDev.upload(par);
-    t.nparticlesDev.upload(t.nparticles); t.periodicDev.upload(t.periodic); t.exprProgDev.upload(t.exprProg);
-    t.codeDev.upload(t.code); t.immDev.upload(t.imm); t.progStartDev.upload(t.progStart);
-    d.nslots = t.nslots; d.paramStride = t.stride;
-    d.atoms = t.atomsDev.p; d.params = t.paramsDev.p; d.group = t.groupDev.p; d.expr = t.exprDev.p;
-    d.exprParticles = t.nparticlesDev.p; d.exprPeriodic = t.periodicDev.p; d.exprProg = t.exprProgDev.p;
-    d.code = t.codeDev.p; d.imm = t.immDev.p; d.progStart = t.progStartDev.p;
+    d.globals = t.globalsDev.p;
+    d.terms = layout_custom(c, s, 4, 0);
+    d.nslots = s.nslots; d.paramStride = s.stride;
+    d.atoms = (const int4*) s.atomsDev.p; d.params = s.paramsDev.p; d.group = s.groupDev.p; d.expr = s.exprDev.p;
+    d.exprClass = s.exprClassDev.p; d.exprProg = s.exprProgDev.p;
+    d.code = s.codeDev.p; d.imm = s.immDev.p; d.progStart = s.progStartDev.p;
+    CustomSlots& u = t.kernel[1];
+    CompoundDev& e = c->cpd;
+    e = CompoundDev{};
+    e.groupMask = 0xffffffffu;
+    e.globals = t.globalsDev.p;
+    layout_custom(c, u, B200MD_CUSTOM_MAX_PARTICLES, -1);
+    e.nslots = u.nslots; e.paramStride = u.stride;
+    e.atoms = u.atomsDev.p; e.params = u.paramsDev.p; e.group = u.groupDev.p; e.expr = u.exprDev.p;
+    e.exprParticles = u.exprParticlesDev.p; e.exprPeriodic = u.exprPeriodicDev.p; e.exprProg = u.exprProgDev.p;
+    e.code = u.codeDev.p; e.imm = u.immDev.p; e.progStart = u.progStartDev.p;
 }
 
 extern "C" int b200md_finalize(b200md_ctx* ctx) {
@@ -1630,7 +1592,6 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     bd.excPeriodic = c->nbdesc.exceptions_periodic;
     bd.groupMask = 0xffffffffu;
     upload_custom(c);
-    upload_compound(c);
     upload_params(c);
     build_units(c);
     build_ccma(c);
@@ -1655,9 +1616,13 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
         auto join = [&](int a, int b) { a = find(a); b = find(b); if (a != b) parent[std::max(a, b)] = std::min(a, b); };
         for (const int2& a : c->bonds.atoms) join(a.x, a.y);
         for (const int4& a : c->angles.atoms) { join(a.x, a.y); join(a.y, a.z); }
-        for (auto* t : {&c->torsions.atoms, &c->rb.atoms, &c->cmap.atoms, &c->custom.cls[B200MD_CUSTOM_TORSION].atoms}) for (const int4& a : *t) { join(a.x, a.y); join(a.y, a.z); join(a.z, a.w); }
-        for (const int4& a : c->custom.cls[B200MD_CUSTOM_BOND].atoms) join(a.x, a.y);
-        for (const int4& a : c->custom.cls[B200MD_CUSTOM_ANGLE].atoms) { join(a.x, a.y); join(a.y, a.z); }
+        for (auto* t : {&c->torsions.atoms, &c->rb.atoms, &c->cmap.atoms}) for (const int4& a : *t) { join(a.x, a.y); join(a.y, a.z); join(a.z, a.w); }
+        for (int k = 0; k < 5; k++) {
+            const CustomClass& cl = c->custom.cls[k];
+            const int w = CUSTOM_NAMES[k].width;
+            if (CUSTOM_NAMES[k].joins)
+                for (int i = 0; i < cl.n; i++) for (int j = 1; j < w; j++) join(cl.atoms[w*i + j - 1], cl.atoms[w*i + j]);
+        }
         for (size_t d = 1; d < c->cmap.atoms.size(); d += 2) join(c->cmap.atoms[d-1].x, c->cmap.atoms[d].x);     // a CMAP term's two dihedrals
         for (size_t i = 0; i < c->conI.size(); i++) join(c->conI[i], c->conJ[i]);
         for (const int2& a : c->exc.atoms) join(a.x, a.y);
@@ -1750,45 +1715,42 @@ extern "C" int b200md_update_cmap_params(b200md_ctx* ctx, int nmaps, const int* 
     API_END(ctx)
 }
 
-// CalcCustom{Torsion,Bond,External,Angle}ForceKernel::copyParametersToContext (kernels.h): same terms and programs, new
-// parameters, into the same device buffer.
-static void update_custom(b200md_ctx* ctx, int cls, const char* call, const char* terms, int n, const double* params) {
-    require(ctx->finalized, (std::string(call) + " before finalize").c_str());
+// CalcCustom{Torsion,Bond,External,Angle,CompoundBond}ForceKernel::copyParametersToContext (kernels.h): same terms and
+// programs, new parameters, into the same device buffer.
+static void update_custom(b200md_ctx* ctx, int cls, int n, const double* params) {
+    const CustomNames& nm = CUSTOM_NAMES[cls];
+    require(ctx->finalized, (std::string(nm.update) + " before finalize").c_str());
     CustomTable& t = ctx->custom;
     CustomClass& cl = t.cls[cls];
-    require(n == cl.n, (std::string("updateParametersInContext: The number of ") + terms + " has changed").c_str());
+    require(n == cl.n, (std::string("updateParametersInContext: The number of ") + nm.terms + " has changed").c_str());
     CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
     cl.params.assign(params, params + (size_t) n*cl.stride);
-    if (n) t.paramsDev.upload(t.slot_params());
+    CustomSlots& s = t.kernel_of(cls);
+    if (n) s.paramsDev.upload(t.slot_params(s));
 }
 extern "C" int b200md_update_custom_torsion_params(b200md_ctx* ctx, int n, const double* params) {
     API_BEGIN(ctx)
-    update_custom(ctx, B200MD_CUSTOM_TORSION, "update_custom_torsion_params", "torsions", n, params);
+    update_custom(ctx, B200MD_CUSTOM_TORSION, n, params);
     API_END(ctx)
 }
 extern "C" int b200md_update_custom_bond_params(b200md_ctx* ctx, int n, const double* params) {
     API_BEGIN(ctx)
-    update_custom(ctx, B200MD_CUSTOM_BOND, "update_custom_bond_params", "bonds", n, params);
+    update_custom(ctx, B200MD_CUSTOM_BOND, n, params);
     API_END(ctx)
 }
 extern "C" int b200md_update_custom_external_params(b200md_ctx* ctx, int n, const double* params) {
     API_BEGIN(ctx)
-    update_custom(ctx, B200MD_CUSTOM_EXTERNAL, "update_custom_external_params", "particles", n, params);
+    update_custom(ctx, B200MD_CUSTOM_EXTERNAL, n, params);
     API_END(ctx)
 }
 extern "C" int b200md_update_custom_angle_params(b200md_ctx* ctx, int n, const double* params) {
     API_BEGIN(ctx)
-    update_custom(ctx, B200MD_CUSTOM_ANGLE, "update_custom_angle_params", "angles", n, params);
+    update_custom(ctx, B200MD_CUSTOM_ANGLE, n, params);
     API_END(ctx)
 }
 extern "C" int b200md_update_custom_compound_params(b200md_ctx* ctx, int n, const double* params) {
     API_BEGIN(ctx)
-    require(ctx->finalized, "update_custom_compound_params before finalize");
-    CompoundTable& t = ctx->compound;
-    require(n == t.n, "updateParametersInContext: The number of bonds has changed");
-    CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-    t.params.assign(params, params + (size_t) n*t.stride);
-    if (n) t.paramsDev.upload(t.slot_params());
+    update_custom(ctx, B200MD_CUSTOM_COMPOUND, n, params);
     API_END(ctx)
 }
 

@@ -103,40 +103,30 @@ class Engine:
         if len(d.cmap_map):
             self._ck(L.b200md_set_cmap(self.h, len(d.cmap_size), _ip(_i32(d.cmap_size)), _dp(_f64(d.cmap_coeff)), len(d.cmap_map),
                                        _ip(_i32(d.cmap_map)), _ip(_i32(d.cmap_atoms))))
-        if len(d.custom_prog):
-            if not len(d.custom_op):
-                raise EngineError("custom torsions without programs: compile desc.custom_energy into custom_op / custom_arg / "
-                                  "custom_imm / custom_prog_start first (the plugin's expression translator)")
-            params = _f64(d.custom_params).reshape(len(d.custom_prog), -1)
-            self._ck(L.b200md_set_custom_torsions(self.h, len(d.custom_prog_start)//2, _ip(_i32(d.custom_prog_start)), _ip(_i32(d.custom_op)),
-                                                  _ip(_i32(d.custom_arg)), _dp(_f64(d.custom_imm)), params.shape[1], len(d.custom_prog),
-                                                  _ip(_i32(d.custom_prog)), _ip(_i32(d.custom_atoms)), _dp(params)))
-        # custom bonds (programs per expression: E, dE/dr), custom externals (E, dE/dx, dE/dy, dE/dz) and custom angles (E,
-        # dE/dtheta)
-        for cls, nprog, call in (("cbond", 2, L.b200md_set_custom_bonds), ("cext", 4, L.b200md_set_custom_externals),
-                                 ("cangle", 2, L.b200md_set_custom_angles)):
-            prog = getattr(d, cls + "_prog")
-            if not len(prog):
+        # the custom classes: field prefix, field of each term's expression, programs per expression (E and dE/dtheta, E and
+        # dE/dr, E and dE/dx, dE/dy, dE/dz, E and dE/dtheta; a compound bond's E and its derivatives by every coordinate of its
+        # particles, whose number and periodic flag per expression its call also takes), what messages call the terms
+        for prefix, expr_field, nprog, name, call in (
+                ("custom", "_prog", 2, "custom torsions", L.b200md_set_custom_torsions),
+                ("cbond", "_prog", 2, "custom bonds", L.b200md_set_custom_bonds),
+                ("cext", "_prog", 4, "custom externals", L.b200md_set_custom_externals),
+                ("cangle", "_prog", 2, "custom angles", L.b200md_set_custom_angles),
+                ("ccompound", "_expr", None, "custom compound bonds", L.b200md_set_custom_compound)):
+            expr = getattr(d, prefix + expr_field)
+            if not len(expr):
                 continue
-            start, op, arg, imm = (getattr(d, cls + k) for k in ("_prog_start", "_op", "_arg", "_imm"))
+            start, op, arg, imm = (getattr(d, prefix + k) for k in ("_prog_start", "_op", "_arg", "_imm"))
             if not len(op):
-                raise EngineError("custom %s without programs: compile desc.%s_energy into %s_op / %s_arg / %s_imm / %s_prog_start "
-                                  "first (the plugin's expression translator)" % (cls, cls, cls, cls, cls, cls))
-            params = _f64(getattr(d, cls + "_params")).reshape(len(prog), -1)
-            self._ck(call(self.h, (len(start) - 1)//nprog, _ip(_i32(start)), _ip(_i32(op)), _ip(_i32(arg)), _dp(_f64(imm)),
-                          params.shape[1], len(prog), _ip(_i32(prog)), _ip(_i32(getattr(d, cls + "_atoms"))), _dp(params)))
-        # custom compound bonds: per expression its particles per bond, whether it is periodic, and 1 + 3 particles programs
-        if len(d.ccompound_expr):
-            if not len(d.ccompound_op):
-                raise EngineError("custom compound bonds without programs: compile desc.ccompound_energy into ccompound_op / "
-                                  "ccompound_arg / ccompound_imm / ccompound_prog_start first (the plugin's expression translator)")
-            n = len(d.ccompound_expr)
-            params = _f64(d.ccompound_params).reshape(n, -1)
-            atoms = _i32(d.ccompound_atoms).reshape(n, 8)
-            self._ck(L.b200md_set_custom_compound(self.h, len(d.ccompound_particles), _ip(_i32(d.ccompound_particles)),
-                                                  _ip(_i32(d.ccompound_periodic)), _ip(_i32(d.ccompound_prog_start)),
-                                                  _ip(_i32(d.ccompound_op)), _ip(_i32(d.ccompound_arg)), _dp(_f64(d.ccompound_imm)),
-                                                  params.shape[1], n, _ip(_i32(d.ccompound_expr)), _ip(atoms), _dp(params)))
+                raise EngineError("%s without programs: compile desc.%s_energy into %s_op / %s_arg / %s_imm / %s_prog_start first (the "
+                                  "plugin's expression translator)" % (name, prefix, prefix, prefix, prefix, prefix))
+            params = _f64(getattr(d, prefix + "_params")).reshape(len(expr), -1)
+            atoms = _i32(getattr(d, prefix + "_atoms")).reshape(len(expr), -1)
+            if nprog is None:
+                head = (len(d.ccompound_particles), _ip(_i32(d.ccompound_particles)), _ip(_i32(d.ccompound_periodic)))
+            else:
+                head = ((len(start) - 1)//nprog,)
+            self._ck(call(self.h, *head, _ip(_i32(start)), _ip(_i32(op)), _ip(_i32(arg)), _dp(_f64(imm)), params.shape[1], len(expr),
+                          _ip(_i32(expr)), _ip(atoms), _dp(params)))
         if len(d.custom_global_values):
             self._ck(L.b200md_set_custom_globals(self.h, len(d.custom_global_values), _dp(_f64(d.custom_global_values))))
         for kind, g in self._bonded_groups.items():
@@ -235,33 +225,30 @@ class Engine:
         size, coeff, cmap_map = _i32(size), _f64(coeff), _i32(cmap_map)
         self._ck(self.lib.b200md_update_cmap_params(self.h, len(size), _ip(size), _dp(coeff), len(cmap_map), _ip(cmap_map)))
 
-    # ---- CalcCustomTorsionForceKernel::copyParametersToContext and the global parameters of its expressions ----
+    # ---- CalcCustom{Torsion,Bond,External,Angle,CompoundBond}ForceKernel::copyParametersToContext and the global parameters ----
+    def _update_custom(self, call, params):
+        p = _f64(params)
+        self._ck(call(self.h, len(p), _dp(p)))
+
     def update_custom_torsion_params(self, params):
         """New per-torsion parameters [n, param_stride] for the same torsions and expressions."""
-        p = _f64(params)
-        self._ck(self.lib.b200md_update_custom_torsion_params(self.h, len(p), _dp(p)))
+        self._update_custom(self.lib.b200md_update_custom_torsion_params, params)
 
-    # ---- CalcCustom{Bond,External}ForceKernel::copyParametersToContext ----
     def update_custom_bond_params(self, params):
         """New per-bond parameters [n, param_stride] for the same custom bonds and expressions."""
-        p = _f64(params)
-        self._ck(self.lib.b200md_update_custom_bond_params(self.h, len(p), _dp(p)))
+        self._update_custom(self.lib.b200md_update_custom_bond_params, params)
 
     def update_custom_external_params(self, params):
         """New per-particle parameters [n, param_stride] for the same custom externals and expressions."""
-        p = _f64(params)
-        self._ck(self.lib.b200md_update_custom_external_params(self.h, len(p), _dp(p)))
+        self._update_custom(self.lib.b200md_update_custom_external_params, params)
 
-    # ---- CalcCustom{Angle,CompoundBond}ForceKernel::copyParametersToContext ----
     def update_custom_angle_params(self, params):
         """New per-angle parameters [n, param_stride] for the same custom angles and expressions."""
-        p = _f64(params)
-        self._ck(self.lib.b200md_update_custom_angle_params(self.h, len(p), _dp(p)))
+        self._update_custom(self.lib.b200md_update_custom_angle_params, params)
 
     def update_custom_compound_params(self, params):
         """New per-bond parameters [n, param_stride] for the same custom compound bonds and expressions."""
-        p = _f64(params)
-        self._ck(self.lib.b200md_update_custom_compound_params(self.h, len(p), _dp(p)))
+        self._update_custom(self.lib.b200md_update_custom_compound_params, params)
 
     def set_custom_globals(self, values):
         """The values of the global parameter slots the expressions read (the number of slots is fixed at definition)."""

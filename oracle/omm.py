@@ -164,12 +164,16 @@ class Simulation:
             L.omm_system_add_force(self.sys, f)
         if desc.cm_frequency:
             L.omm_system_add_force(self.sys, L.omm_cmmotion_create(desc.cm_frequency))
+        self.add_forces()
         kind, T, fric, dt = integrator
         self.integ = L.omm_integrator_create(kind, T, fric, dt, seed, constraint_tol)
         self.ctx = L.omm_context_create(self.sys, self.integ, platform.encode(), props.encode())
         if not self.ctx:
             raise RuntimeError("Context creation failed: " + L.omm_last_error().decode())
         self.set_positions(desc.positions)
+
+    def add_forces(self):
+        """Subclasses add more forces to self.sys here: the Context is made after it."""
 
     def set_parameter(self, name, value):
         self._ck(self.L.omm_context_set_parameter(self.ctx, name.encode(), value))

@@ -17,9 +17,9 @@
 //
 // Bonded classes.  Each keeps the terms of all its Force objects in one TermRecord of PlatformData, sent at finalize; what
 // their kernels share (ObjectTerms: the object's range of the record, group tags, updates) exists once.  Bond, angle,
-// periodic-torsion and RB-torsion kernels are one template, B200CalcBondedForceKernel; the custom torsion, bond, external
-// and angle kernels another, B200CalcCustomForceKernel, for their expression programs; CMAP keeps its own for its maps, the
-// custom compound bond its own for its per-expression particle count.
+// periodic-torsion and RB-torsion kernels are one template, B200CalcBondedForceKernel; the custom torsion, bond, external,
+// angle and compound-bond kernels another, B200CalcCustomForceKernel, for their expression programs; CMAP keeps its own for
+// its maps.
 //
 // The hot loop.  Integrator::step(n) of the reference is, per step, updateContextState() -> calcForcesAndEnergy(true,
 // false, groups) -> Integrate*StepKernel::execute (LangevinIntegrator.cpp:74-82).  Here a forces-only evaluation is
@@ -142,12 +142,26 @@ struct RBTorsions {
 };
 
 // The expression programs of one custom class over all its Force objects, one after the other (object f's expression is
-// programs (1 + number of variables)*f ..); the parameters of every term padded to B200MD_CUSTOM_MAX_PARAMS in the record,
+// expression f); per expression its first program, its particles per term and whether its point functions take the minimum
+// image (both 0 but for compound bonds); the parameters of every term padded to B200MD_CUSTOM_MAX_PARAMS in the record,
 // packed to the widest object's count when sent
 struct CustomPrograms {
     vector<int> progStart = vector<int>(1, 0), op, arg; vector<double> imm;
+    vector<int> exprProg, particles, periodic;
     int stride = 0;
-    int numExpressions(int numVars) const { return (int) (progStart.size() - 1)/(1 + numVars); }
+    int numExpressions() const { return (int) exprProg.size(); }
+    // the programs of one more expression
+    void add(const vector<b200md_custom::Program>& programs, int numParticles, bool usesPeriodic) {
+        exprProg.push_back((int) progStart.size() - 1);
+        particles.push_back(numParticles);
+        periodic.push_back(usesPeriodic ? 1 : 0);
+        for (const b200md_custom::Program& p : programs) {
+            op.insert(op.end(), p.op.begin(), p.op.end());
+            arg.insert(arg.end(), p.arg.begin(), p.arg.end());
+            imm.insert(imm.end(), p.imm.begin(), p.imm.end());
+            progStart.push_back((int) op.size());
+        }
+    }
     vector<double> packed(const TermRecord& r) const {
         const size_t n = r.size();
         vector<double> p(n*stride);
@@ -175,18 +189,17 @@ struct PlatformData {
     bool useFusedStep = true;       // B200MD_PLUGIN_FUSED=0: always compute + integrate_only (debugging)
     // the bonded terms of every Force object, one record per class (columns: atoms, integer parameters, parameters), sent at finalize
     TermRecord bonds{B200MD_BONDED_BONDS, 2, 0, 2}, angles{B200MD_BONDED_ANGLES, 3, 0, 2}, torsions{B200MD_BONDED_TORSIONS, 4, 1, 2},
-               rb{B200MD_BONDED_RB_TORSIONS, 4, 0, 1}, cmap{B200MD_BONDED_CMAP, 1, 1, 0}, custom{B200MD_BONDED_CUSTOM_TORSIONS, 1, 1, 1},
-               customBonds{B200MD_BONDED_CUSTOM_BONDS, 1, 1, 1}, customExternals{B200MD_BONDED_CUSTOM_EXTERNALS, 1, 1, 1},
-               customAngles{B200MD_BONDED_CUSTOM_ANGLES, 1, 1, 1}, customCompound{B200MD_BONDED_CUSTOM_COMPOUND, 1, 1, 1};
+               rb{B200MD_BONDED_RB_TORSIONS, 4, 0, 1}, cmap{B200MD_BONDED_CMAP, 1, 1, 0};
+    // the custom terms of each class (B200MD_CUSTOM_*): one atom column (a compound bond's B200MD_CUSTOM_MAX_PARTICLES
+    // entries, unused ones -1), the expression, the parameters
+    TermRecord customTerms[5] = {{B200MD_BONDED_CUSTOM_TORSIONS, 1, 1, 1}, {B200MD_BONDED_CUSTOM_BONDS, 1, 1, 1},
+                                 {B200MD_BONDED_CUSTOM_EXTERNALS, 1, 1, 1}, {B200MD_BONDED_CUSTOM_ANGLES, 1, 1, 1},
+                                 {B200MD_BONDED_CUSTOM_COMPOUND, 1, 1, 1}};
     // CMAP: the maps of all objects one after the other (a term's map index counts from the first map of all objects);
     // coefficients from CMAPTorsionForceImpl::calcMapDerivatives, [sum size^2][16]
     vector<int> cmapSize; vector<double> cmapCoeff;
-    // custom torsions, bonds, externals and angles: the programs of each class (B200MD_CUSTOM_*)
-    CustomPrograms customPrograms[4];
-    // custom compound bonds: the programs of every object (1 + 3 particles per bond each), its particles per bond and whether
-    // it uses periodic boundary conditions; a term's atom column holds B200MD_CUSTOM_MAX_PARTICLES entries, unused ones -1
-    CustomPrograms compoundPrograms;
-    vector<int> compoundParticles, compoundPeriodic;
+    // the programs of each custom class
+    CustomPrograms customPrograms[5];
     // the global parameters the expressions of all custom classes read: slot of every name (shared by all objects) and the
     // value last sent
     map<string, int> customGlobalSlot;
@@ -215,22 +228,17 @@ struct PlatformData {
             if (r->size()) check(b200md_set_bonded_groups(ctx, r->kind, r->size(), r->group.data()));
         typedef int (*SetCustom)(b200md_ctx*, int, const int*, const int*, const int*, const double*, int, int, const int*, const int*, const double*);
         const SetCustom setCustom[4] = {b200md_set_custom_torsions, b200md_set_custom_bonds, b200md_set_custom_externals, b200md_set_custom_angles};
-        const TermRecord* customRecord[4] = {&custom, &customBonds, &customExternals, &customAngles};
-        for (int k = 0; k < 4; k++) {
-            const TermRecord& r = *customRecord[k];
+        for (int k = 0; k < 5; k++) {
+            const TermRecord& r = customTerms[k];
             if (!r.size()) continue;
             const CustomPrograms& c = customPrograms[k];
             const vector<double> par = c.packed(r);
-            check(setCustom[k](ctx, c.numExpressions(k == B200MD_CUSTOM_EXTERNAL ? 3 : 1), c.progStart.data(), c.op.data(), c.arg.data(),
-                               c.imm.data(), c.stride, r.size(), r.ints[0].data(), r.atoms[0].data(), par.data()));
-            check(b200md_set_bonded_groups(ctx, r.kind, r.size(), r.group.data()));
-        }
-        if (customCompound.size()) {
-            const TermRecord& r = customCompound;
-            const CustomPrograms& c = compoundPrograms;
-            const vector<double> par = c.packed(r);
-            check(b200md_set_custom_compound(ctx, (int) compoundParticles.size(), compoundParticles.data(), compoundPeriodic.data(), c.progStart.data(),
-                                             c.op.data(), c.arg.data(), c.imm.data(), c.stride, r.size(), r.ints[0].data(), r.atoms[0].data(), par.data()));
+            if (k == B200MD_CUSTOM_COMPOUND)
+                check(b200md_set_custom_compound(ctx, c.numExpressions(), c.particles.data(), c.periodic.data(), c.progStart.data(), c.op.data(),
+                                                 c.arg.data(), c.imm.data(), c.stride, r.size(), r.ints[0].data(), r.atoms[0].data(), par.data()));
+            else
+                check(setCustom[k](ctx, c.numExpressions(), c.progStart.data(), c.op.data(), c.arg.data(), c.imm.data(), c.stride, r.size(),
+                                   r.ints[0].data(), r.atoms[0].data(), par.data()));
             check(b200md_set_bonded_groups(ctx, r.kind, r.size(), r.group.data()));
         }
         if (!customGlobals.empty()) check(b200md_set_custom_globals(ctx, (int) customGlobals.size(), customGlobals.data()));
@@ -613,14 +621,26 @@ private:
     size_t firstCoeff = 0;
 };
 
-// What the custom torsion, bond, external and angle kernels differ in (B200CalcCustomForceKernel below): the Force, its class and
-// term bit, its variables, the names in messages, how term i is read, and the calls that send the parameters.
-struct CustomTorsions {
+// What the custom kernels differ in (B200CalcCustomForceKernel below): the Force, its class and term bit, the names in
+// messages, how its expression is translated, its particles per term and whether its point functions take the minimum image
+// (compound bonds only), how term i is read, and the call that sends new parameters.  CustomTerms is what the torsion, bond,
+// external and angle classes share: an expression of the class's variables, translated by translateExpression.
+template<class T> struct CustomTerms {
+    template<class F> static void translate(const F& force, map<string, int>& globalSlot, vector<b200md_custom::Program>& programs) {
+        vector<string> params, globals;
+        for (int i = 0; i < T::numParams(force); i++) params.push_back(T::paramName(force, i));
+        for (int i = 0; i < force.getNumGlobalParameters(); i++) globals.push_back(force.getGlobalParameterName(i));
+        b200md_custom::translateExpression(force.getEnergyFunction(), T::variables(), T::name, T::perTerm, T::cls == B200MD_CUSTOM_EXTERNAL,
+                                           params, globals, globalSlot, programs);
+    }
+    template<class F> static int particles(const F&) { return 0; }
+    template<class F> static bool periodic(const F&) { return false; }
+};
+struct CustomTorsions : CustomTerms<CustomTorsions> {
     typedef CustomTorsionForce Force; typedef CalcCustomTorsionForceKernel Kernel;
     enum { cls = B200MD_CUSTOM_TORSION, bit = B200MD_TERM_CUSTOM_TORSIONS };
     static constexpr const char* name = "CustomTorsionForce", *terms = "torsions", *aTerm = "a torsion", *perTerm = "torsion", *changed = nullptr;
     static vector<string> variables() { return {"theta"}; }
-    static TermRecord PlatformData::* record() { return &PlatformData::custom; }
     static int count(const Force& f) { return f.getNumTorsions(); }
     static int numParams(const Force& f) { return f.getNumPerTorsionParameters(); }
     static string paramName(const Force& f, int i) { return f.getPerTorsionParameterName(i); }
@@ -628,12 +648,11 @@ struct CustomTorsions {
     static int update(b200md_ctx* c, int n, const double* p) { return b200md_update_custom_torsion_params(c, n, p); }
     static int numParamDerivatives(const Force& f) { return f.getNumEnergyParameterDerivatives(); }
 };
-struct CustomBonds {
+struct CustomBonds : CustomTerms<CustomBonds> {
     typedef CustomBondForce Force; typedef CalcCustomBondForceKernel Kernel;
     enum { cls = B200MD_CUSTOM_BOND, bit = B200MD_TERM_CUSTOM_BONDS };
     static constexpr const char* name = "CustomBondForce", *terms = "bonds", *aTerm = "a bond", *perTerm = "bond", *changed = nullptr;
     static vector<string> variables() { return {"r"}; }
-    static TermRecord PlatformData::* record() { return &PlatformData::customBonds; }
     static int count(const Force& f) { return f.getNumBonds(); }
     static int numParams(const Force& f) { return f.getNumPerBondParameters(); }
     static string paramName(const Force& f, int i) { return f.getPerBondParameterName(i); }
@@ -641,13 +660,12 @@ struct CustomBonds {
     static int update(b200md_ctx* c, int n, const double* p) { return b200md_update_custom_bond_params(c, n, p); }
     static int numParamDerivatives(const Force& f) { return f.getNumEnergyParameterDerivatives(); }
 };
-struct CustomExternals {
+struct CustomExternals : CustomTerms<CustomExternals> {
     typedef CustomExternalForce Force; typedef CalcCustomExternalForceKernel Kernel;
     enum { cls = B200MD_CUSTOM_EXTERNAL, bit = B200MD_TERM_CUSTOM_EXTERNALS };
     static constexpr const char* name = "CustomExternalForce", *terms = "particles", *aTerm = "a particle", *perTerm = "particle",
                                  *changed = "A particle index has changed";
     static vector<string> variables() { return {"x", "y", "z"}; }
-    static TermRecord PlatformData::* record() { return &PlatformData::customExternals; }
     static int count(const Force& f) { return f.getNumParticles(); }
     static int numParams(const Force& f) { return f.getNumPerParticleParameters(); }
     static string paramName(const Force& f, int i) { return f.getPerParticleParameterName(i); }
@@ -655,13 +673,11 @@ struct CustomExternals {
     static int update(b200md_ctx* c, int n, const double* p) { return b200md_update_custom_external_params(c, n, p); }
     static int numParamDerivatives(const Force&) { return 0; }        // CustomExternalForce has none
 };
-
-struct CustomAngles {
+struct CustomAngles : CustomTerms<CustomAngles> {
     typedef CustomAngleForce Force; typedef CalcCustomAngleForceKernel Kernel;
     enum { cls = B200MD_CUSTOM_ANGLE, bit = B200MD_TERM_CUSTOM_ANGLES };
     static constexpr const char* name = "CustomAngleForce", *terms = "angles", *aTerm = "an angle", *perTerm = "angle", *changed = nullptr;
     static vector<string> variables() { return {"theta"}; }
-    static TermRecord PlatformData::* record() { return &PlatformData::customAngles; }
     static int count(const Force& f) { return f.getNumAngles(); }
     static int numParams(const Force& f) { return f.getNumPerAngleParameters(); }
     static string paramName(const Force& f, int i) { return f.getPerAngleParameterName(i); }
@@ -669,32 +685,28 @@ struct CustomAngles {
     static int update(b200md_ctx* c, int n, const double* p) { return b200md_update_custom_angle_params(c, n, p); }
     static int numParamDerivatives(const Force& f) { return f.getNumEnergyParameterDerivatives(); }
 };
-
-template<class T> vector<string> perTermParameterNames(const typename T::Force& force) {
-    vector<string> names;
-    for (int i = 0; i < T::numParams(force); i++) names.push_back(T::paramName(force, i));
-    return names;
-}
-template<class F> vector<string> globalParameterNames(const F& force) {
-    vector<string> names;
-    for (int i = 0; i < force.getNumGlobalParameters(); i++) names.push_back(force.getGlobalParameterName(i));
-    return names;
-}
-// The programs of one custom force's expression (custom_translate.h): the energy and one derivative per variable
-template<class T> void translate(const typename T::Force& force, map<string, int>& globalSlot, vector<b200md_custom::Program>& programs) {
-    b200md_custom::translateExpression(force.getEnergyFunction(), T::variables(), T::name, T::perTerm, T::cls == B200MD_CUSTOM_EXTERNAL,
-                                       perTermParameterNames<T>(force), globalParameterNames(force), globalSlot, programs);
-}
-
-// The programs of one force object appended to its class's
-inline void appendPrograms(CustomPrograms& c, const vector<b200md_custom::Program>& programs) {
-    for (const b200md_custom::Program& p : programs) {
-        c.op.insert(c.op.end(), p.op.begin(), p.op.end());
-        c.arg.insert(c.arg.end(), p.arg.begin(), p.arg.end());
-        c.imm.insert(c.imm.end(), p.imm.begin(), p.imm.end());
-        c.progStart.push_back((int) c.op.size());
+// A compound bond's expression is of the coordinates of its particles: 1 + 3 (particles per bond) programs, which k_compound
+// interprets.  Its atoms are padded to B200MD_CUSTOM_MAX_PARTICLES with -1.
+struct CustomCompounds {
+    typedef CustomCompoundBondForce Force; typedef CalcCustomCompoundBondForceKernel Kernel;
+    enum { cls = B200MD_CUSTOM_COMPOUND, bit = B200MD_TERM_CUSTOM_COMPOUND };
+    static constexpr const char* name = "CustomCompoundBondForce", *terms = "bonds", *aTerm = "a bond", *changed = nullptr;
+    static int count(const Force& f) { return f.getNumBonds(); }
+    static int numParams(const Force& f) { return f.getNumPerBondParameters(); }
+    static vector<int> read(const Force& f, int i, vector<double>& par) {
+        vector<int> atoms;
+        f.getBondParameters(i, atoms, par);
+        atoms.resize(B200MD_CUSTOM_MAX_PARTICLES, -1);
+        return atoms;
     }
-}
+    static int update(b200md_ctx* c, int n, const double* p) { return b200md_update_custom_compound_params(c, n, p); }
+    static int numParamDerivatives(const Force& f) { return f.getNumEnergyParameterDerivatives(); }
+    static void translate(const Force& f, map<string, int>& globalSlot, vector<b200md_custom::Program>& programs) {
+        b200md_custom::translateCompound(f, globalSlot, programs);
+    }
+    static int particles(const Force& f) { return f.getNumParticlesPerBond(); }
+    static bool periodic(const Force& f) { return f.usesPeriodicBoundaryConditions(); }
+};
 
 // The global parameters one custom force object's expression reads, and their slots in the Context's shared map
 struct ObjectGlobals {
@@ -721,9 +733,9 @@ struct ObjectGlobals {
     }
 };
 
-// CustomTorsionForce, CustomBondForce, CustomExternalForce and CustomAngleForce (T: CustomTorsions, CustomBonds,
-// CustomExternals, CustomAngles): the expression becomes 1 + (number of variables) instruction programs, which k_custom
-// interprets.
+// CustomTorsionForce, CustomBondForce, CustomExternalForce, CustomAngleForce and CustomCompoundBondForce (T: CustomTorsions,
+// CustomBonds, CustomExternals, CustomAngles, CustomCompounds): the expression becomes 1 + (number of variables) instruction
+// programs, which k_custom interprets (k_compound for compound bonds).
 template<class T>
 class B200CalcCustomForceKernel : public T::Kernel, ObjectTerms {
 public:
@@ -734,17 +746,17 @@ public:
         const vector<int> atoms = T::read(force, i, par);
         par.resize(numParams);
         par.resize(B200MD_CUSTOM_MAX_PARAMS, 0.0);
-        r.add(atoms, {prog}, par);
+        r.add(atoms, {expr}, par);
     }
     void initialize(const System& system, const typename T::Force& force) {
         PlatformData& d = getData(context);
         CustomPrograms& c = d.customPrograms[T::cls];
-        prog = c.numExpressions((int) T::variables().size());
+        expr = c.numExpressions();
         numParams = T::numParams(force);
-        add(d, d.*T::record(), force, T::count(force), T::bit, T::name, [&](int i, TermRecord& r) { read(force, i, r); });
+        add(d, d.customTerms[T::cls], force, T::count(force), T::bit, T::name, [&](int i, TermRecord& r) { read(force, i, r); });
         vector<b200md_custom::Program> programs;
-        translate<T>(force, d.customGlobalSlot, programs);
-        appendPrograms(c, programs);
+        T::translate(force, d.customGlobalSlot, programs);
+        c.add(programs, T::particles(force), T::periodic(force));
         globals.init(d, force);
         c.stride = max(c.stride, numParams);
     }
@@ -756,61 +768,14 @@ public:
     }
     void copyParametersToContext(ContextImpl& context, const typename T::Force& force) {
         PlatformData& d = getData(context);
-        TermRecord& r = d.*T::record();
+        TermRecord& r = d.customTerms[T::cls];
         store(r, reread(d, r, T::count(force), T::terms, T::aTerm, [&](int i, TermRecord& f) { read(force, i, f); }, T::changed));
         const vector<double> packed = d.customPrograms[T::cls].packed(r);
         d.check(T::update(d.ctx, r.size(), packed.data()));
     }
 private:
     ContextImpl& context;
-    int prog = 0, numParams = 0;          // this object's expression; its number of per-term parameters
-    ObjectGlobals globals;
-};
-
-// CustomCompoundBondForce: the expression becomes 1 + 3 (particles per bond) instruction programs (the energy and its
-// derivative by every coordinate), which k_compound interprets.
-class B200CalcCustomCompoundBondForceKernel : public CalcCustomCompoundBondForceKernel, ObjectTerms {
-public:
-    B200CalcCustomCompoundBondForceKernel(string name, const Platform& platform, ContextImpl& context) :
-        CalcCustomCompoundBondForceKernel(name, platform), context(context) {}
-    void read(const CustomCompoundBondForce& force, int i, TermRecord& r) const {
-        vector<int> atoms;
-        vector<double> par;
-        force.getBondParameters(i, atoms, par);
-        atoms.resize(B200MD_CUSTOM_MAX_PARTICLES, -1);
-        par.resize(force.getNumPerBondParameters());
-        par.resize(B200MD_CUSTOM_MAX_PARAMS, 0.0);
-        r.add(atoms, {expr}, par);
-    }
-    void initialize(const System& system, const CustomCompoundBondForce& force) {
-        PlatformData& d = getData(context);
-        expr = (int) d.compoundParticles.size();
-        vector<b200md_custom::Program> programs;
-        b200md_custom::translateCompound(force, d.customGlobalSlot, programs);
-        add(d, d.customCompound, force, force.getNumBonds(), B200MD_TERM_CUSTOM_COMPOUND, "CustomCompoundBondForce",
-            [&](int i, TermRecord& r) { read(force, i, r); });
-        appendPrograms(d.compoundPrograms, programs);
-        d.compoundParticles.push_back(force.getNumParticlesPerBond());
-        d.compoundPeriodic.push_back(force.usesPeriodicBoundaryConditions() ? 1 : 0);
-        globals.init(d, force);
-        d.compoundPrograms.stride = max(d.compoundPrograms.stride, force.getNumPerBondParameters());
-    }
-    double execute(ContextImpl& context, bool includeForces, bool includeEnergy) {
-        PlatformData& d = getData(context);
-        globals.send(d, context);
-        d.pendingTerms |= B200MD_TERM_CUSTOM_COMPOUND;
-        return 0.0;
-    }
-    void copyParametersToContext(ContextImpl& context, const CustomCompoundBondForce& force) {
-        PlatformData& d = getData(context);
-        TermRecord& r = d.customCompound;
-        store(r, reread(d, r, force.getNumBonds(), "bonds", "a bond", [&](int i, TermRecord& f) { read(force, i, f); }));
-        const vector<double> packed = d.compoundPrograms.packed(r);
-        d.check(b200md_update_custom_compound_params(d.ctx, r.size(), packed.data()));
-    }
-private:
-    ContextImpl& context;
-    int expr = 0;                         // this object's expression
+    int expr = 0, numParams = 0;          // this object's expression; its number of per-term parameters
     ObjectGlobals globals;
 };
 
@@ -945,7 +910,7 @@ public:
         if (name == CalcCustomBondForceKernel::Name()) return new B200CalcCustomForceKernel<CustomBonds>(name, platform, context);
         if (name == CalcCustomExternalForceKernel::Name()) return new B200CalcCustomForceKernel<CustomExternals>(name, platform, context);
         if (name == CalcCustomAngleForceKernel::Name()) return new B200CalcCustomForceKernel<CustomAngles>(name, platform, context);
-        if (name == CalcCustomCompoundBondForceKernel::Name()) return new B200CalcCustomCompoundBondForceKernel(name, platform, context);
+        if (name == CalcCustomCompoundBondForceKernel::Name()) return new B200CalcCustomForceKernel<CustomCompounds>(name, platform, context);
         if (name == RemoveCMMotionKernel::Name()) return new B200RemoveCMMotionKernel(name, platform, context);
         if (name == IntegrateVerletStepKernel::Name()) return new B200IntegrateVerletStepKernel(name, platform);
         if (name == IntegrateLangevinStepKernel::Name()) return new B200IntegrateLangevinStepKernel(name, platform);
@@ -999,17 +964,7 @@ public:
             throw OpenMMException(string("B200 platform: energy parameter derivatives of a ") + T::name + " are not supported");
         map<string, int> slots;
         vector<b200md_custom::Program> programs;
-        try { translate<T>(force, slots, programs); }
-        catch (const b200md_custom::Unsupported&) { throw; }
-        catch (const OpenMMException&) {}
-    }
-    // The same for a CustomCompoundBondForce, whose limits also cover the particles per bond
-    static void validateCompound(const CustomCompoundBondForce& force) {
-        if (force.getNumEnergyParameterDerivatives() > 0)
-            throw OpenMMException("B200 platform: energy parameter derivatives of a CustomCompoundBondForce are not supported");
-        map<string, int> slots;
-        vector<b200md_custom::Program> programs;
-        try { b200md_custom::translateCompound(force, slots, programs); }
+        try { T::translate(force, slots, programs); }
         catch (const b200md_custom::Unsupported&) { throw; }
         catch (const OpenMMException&) {}
     }
@@ -1032,7 +987,7 @@ public:
             if (const CustomBondForce* f = dynamic_cast<const CustomBondForce*>(&force)) validateCustom<CustomBonds>(*f);
             if (const CustomExternalForce* f = dynamic_cast<const CustomExternalForce*>(&force)) validateCustom<CustomExternals>(*f);
             if (const CustomAngleForce* f = dynamic_cast<const CustomAngleForce*>(&force)) validateCustom<CustomAngles>(*f);
-            if (const CustomCompoundBondForce* f = dynamic_cast<const CustomCompoundBondForce*>(&force)) validateCompound(*f);
+            if (const CustomCompoundBondForce* f = dynamic_cast<const CustomCompoundBondForce*>(&force)) validateCustom<CustomCompounds>(*f);
         }
         const int nc = system.getNumConstraints();
         if (nc > 0) {

@@ -4,8 +4,7 @@
 // differentiates the expression exactly as the Reference platform does
 // (ReferenceCalcCustom{Torsion,Bond,External,Angle,CompoundBond}ForceKernel::initialize) and makes the stack program
 // (ExpressionProgram); this file only maps every Lepton::Operation to one instruction.  Included by the plugin
-// (B200Platform.cpp) and by its test C APIs (tests/custom_torsion_capi.cpp, tests/custom_terms_capi.cpp,
-// tests/custom_compound_capi.cpp), so that all make the same programs.
+// (B200Platform.cpp) and by its test C API (tests/custom_capi.cpp), so that both make the same programs.
 #ifndef B200MD_CUSTOM_TRANSLATE_H_
 #define B200MD_CUSTOM_TRANSLATE_H_
 #include "openmm/OpenMMException.h"
@@ -155,6 +154,22 @@ inline Program translateProgram(const Lepton::ExpressionProgram& prog, const std
     return out;
 }
 
+namespace detail {
+// The energy program of a parsed expression and one derivative program per variable, in order (expr.differentiate(variable)
+// .optimize()).  The global slots new names take are committed to globalSlot only when every program translates.
+inline void translatePrograms(const Lepton::ParsedExpression& expr, const std::vector<std::string>& variables, const std::string& forceName,
+                              int maxStack, const std::vector<std::string>& paramNames, const std::vector<std::string>& globalNames,
+                              std::map<std::string, int>& globalSlot, std::vector<Program>& programs) {
+    std::map<std::string, int> slots = globalSlot;
+    std::vector<Program> out(1, translateProgram(expr.createProgram(), variables, forceName, paramNames, globalNames, slots, maxStack));
+    for (const std::string& v : variables)
+        out.push_back(translateProgram(expr.differentiate(v).optimize().createProgram(), variables, forceName, paramNames, globalNames, slots,
+                                       maxStack));
+    programs.swap(out);
+    globalSlot.swap(slots);
+}
+} // namespace detail
+
 // The energy program and one derivative program per variable of one expression: Parser::parse(energy).optimize(), and the
 // same expression .differentiate(variable).optimize() for every variable in order.  periodic: periodicdistance is a function
 // of the expression (a CustomExternalForce).  perTerm names a term in messages ("torsion", "bond", "particle").
@@ -167,20 +182,14 @@ inline void translateExpression(const std::string& energy, const std::vector<std
     PeriodicDistancePlaceholder pd;
     std::map<std::string, Lepton::CustomFunction*> functions;
     if (periodic) functions["periodicdistance"] = &pd;
-    const Lepton::ParsedExpression expr = Lepton::Parser::parse(energy, functions).optimize();
-    std::map<std::string, int> slots = globalSlot;      // committed only when every program translates
-    std::vector<Program> out(1, translateProgram(expr.createProgram(), variables, forceName, paramNames, globalNames, slots));
-    for (const std::string& v : variables)
-        out.push_back(translateProgram(expr.differentiate(v).optimize().createProgram(), variables, forceName, paramNames, globalNames, slots));
-    programs.swap(out);
-    globalSlot.swap(slots);
+    detail::translatePrograms(Lepton::Parser::parse(energy, functions).optimize(), variables, forceName, B200MD_CUSTOM_MAX_STACK, paramNames,
+                              globalNames, globalSlot, programs);
 }
 
 // A CustomCompoundBondForce: its energy program and the derivative programs by x1, y1, z1, x2, .. (1 + 3 particles per bond).
 // CustomCompoundBondForceImpl::prepareExpression (libOpenMM.so) turns distance, angle and dihedral into the point functions, as
 // for the Reference platform; the expression is then an ordinary function of the coordinates.
 inline void translateCompound(const OpenMM::CustomCompoundBondForce& force, std::map<std::string, int>& globalSlot, std::vector<Program>& programs) {
-    const std::string forceName = "CustomCompoundBondForce";
     const int numParticles = force.getNumParticlesPerBond();
     if (numParticles > B200MD_CUSTOM_MAX_PARTICLES)
         throw Unsupported("B200 platform: a CustomCompoundBondForce with more than 8 particles per bond is not supported");
@@ -191,30 +200,13 @@ inline void translateCompound(const OpenMM::CustomCompoundBondForce& force, std:
     PointFunctionPlaceholder distance(6), angle(9), dihedral(12);
     std::map<std::string, Lepton::CustomFunction*> functions;
     functions["pointdistance"] = &distance; functions["pointangle"] = &angle; functions["pointdihedral"] = &dihedral;
-    const Lepton::ParsedExpression expr = OpenMM::CustomCompoundBondForceImpl::prepareExpression(force, functions);
     std::vector<std::string> variables, paramNames, globalNames;
     for (int i = 1; i <= numParticles; i++)
         for (const char* axis : {"x", "y", "z"}) variables.push_back(axis + std::to_string(i));
     for (int i = 0; i < force.getNumPerBondParameters(); i++) paramNames.push_back(force.getPerBondParameterName(i));
     for (int i = 0; i < force.getNumGlobalParameters(); i++) globalNames.push_back(force.getGlobalParameterName(i));
-    std::map<std::string, int> slots = globalSlot;      // committed only when every program translates
-    std::vector<Program> out(1, translateProgram(expr.createProgram(), variables, forceName, paramNames, globalNames, slots,
-                                                 B200MD_CUSTOM_COMPOUND_MAX_STACK));
-    for (const std::string& v : variables)
-        out.push_back(translateProgram(expr.differentiate(v).optimize().createProgram(), variables, forceName, paramNames, globalNames, slots,
-                                       B200MD_CUSTOM_COMPOUND_MAX_STACK));
-    programs.swap(out);
-    globalSlot.swap(slots);
-}
-
-// A CustomTorsionForce expression: the energy program and the dE/dtheta program.
-inline void translateExpression(const std::string& energy, const std::vector<std::string>& paramNames,
-                                const std::vector<std::string>& globalNames, std::map<std::string, int>& globalSlot,
-                                Program& energyProgram, Program& derivProgram) {
-    std::vector<Program> programs;
-    translateExpression(energy, std::vector<std::string>(1, "theta"), "CustomTorsionForce", "torsion", false, paramNames, globalNames,
-                        globalSlot, programs);
-    energyProgram = programs[0]; derivProgram = programs[1];
+    detail::translatePrograms(OpenMM::CustomCompoundBondForceImpl::prepareExpression(force, functions), variables, "CustomCompoundBondForce",
+                              B200MD_CUSTOM_COMPOUND_MAX_STACK, paramNames, globalNames, globalSlot, programs);
 }
 
 } // namespace b200md_custom

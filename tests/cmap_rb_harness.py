@@ -51,28 +51,17 @@ class Simulation(omm.Simulation):
 
     def __init__(self, desc, platform="Reference", integrator=(0, 0.0, 0.0, 0.001), seed=7, constraint_tol=1e-5,
                  force_groups=None, bonded_periodic=False, **kw):
+        self.force_groups, self.bonded_periodic = force_groups or {}, bonded_periodic
         super().__init__(desc, platform, integrator=integrator, seed=seed, constraint_tol=constraint_tol,
                          bonded_periodic=bonded_periodic, **kw)
-        if not len(desc.rb_i) and not len(desc.cmap_map):
-            return
-        # the forces join the System after the base class made its Context: make that Context again, with a new
-        # Integrator (an Integrator stays bound to the first Context it served)
-        self.L.omm_context_destroy(self.ctx)
-        self.ctx = None
-        self.L.omm_integrator_destroy(self.integ)
-        kind, T, fric, dt = integrator
-        self.integ = self.L.omm_integrator_create(kind, T, fric, dt, seed, constraint_tol)
-        L, groups, per = lib(), force_groups or {}, int(bonded_periodic)
+
+    def add_forces(self):
+        desc, groups, per = self.desc, self.force_groups, int(self.bonded_periodic)
         i32 = lambda a: np.ascontiguousarray(a, dtype=np.int32)
         f64 = lambda a: np.ascontiguousarray(a, dtype=np.float64)
         if len(desc.rb_i):
-            L.cmap_rb_add_rb_torsions(self.sys, len(desc.rb_i), _ip(i32(desc.rb_i)), _ip(i32(desc.rb_j)), _ip(i32(desc.rb_k)),
-                                      _ip(i32(desc.rb_l)), _dp(f64(desc.rb_c)), per, groups.get("rb_torsions", 0))
+            lib().cmap_rb_add_rb_torsions(self.sys, len(desc.rb_i), _ip(i32(desc.rb_i)), _ip(i32(desc.rb_j)), _ip(i32(desc.rb_k)),
+                                          _ip(i32(desc.rb_l)), _dp(f64(desc.rb_c)), per, groups.get("rb_torsions", 0))
         if len(desc.cmap_map):
-            L.cmap_rb_add_cmap(self.sys, len(desc.cmap_size), _ip(i32(desc.cmap_size)), _dp(f64(desc.cmap_energy)), len(desc.cmap_map),
-                               _ip(i32(desc.cmap_map)), _ip(i32(desc.cmap_atoms)), per, groups.get("cmap", 0))
-        props = kw.get("props", "")
-        self.ctx = self.L.omm_context_create(self.sys, self.integ, platform.encode(), props.encode())
-        if not self.ctx:
-            raise RuntimeError("Context creation failed: " + self.L.omm_last_error().decode())
-        self.set_positions(desc.positions)
+            lib().cmap_rb_add_cmap(self.sys, len(desc.cmap_size), _ip(i32(desc.cmap_size)), _dp(f64(desc.cmap_energy)), len(desc.cmap_map),
+                                   _ip(i32(desc.cmap_map)), _ip(i32(desc.cmap_atoms)), per, groups.get("cmap", 0))

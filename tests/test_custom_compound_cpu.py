@@ -5,8 +5,7 @@ the limits validateSystem refuses."""
 import math
 import numpy as np
 import pytest
-import custom_compound_harness as H
-import custom_terms_harness
+import custom_harness as H
 
 pytestmark = pytest.mark.skipif(not H.available(), reason="oracle/_ref (the built reference and the test C APIs) is absent")
 
@@ -21,15 +20,21 @@ def _close(a, b, tol=1e-12):
     return abs(a - b) <= tol*max(1.0, abs(b)) or (math.isnan(a) and math.isnan(b))
 
 
+def _probe(nparticles, periodic, *rest):
+    """b200md_custom_compound_probe (nparticles > 0) or b200md_custom_term_probe of the angle class"""
+    return H.compound_probe(nparticles, periodic, *rest) if nparticles > 0 else H.term_probe(H.ANGLE, *rest)
+
+
 def _check(nparticles, energy, x, box=np.eye(3), periodic=False, params=(), pvals=(), globals_=(), gvals=()):
     """every program of the expression through the probe against Lepton"""
-    op, arg, imm, start = H.translate(nparticles, energy, params, globals_)
+    cls = H.COMPOUND if nparticles else H.ANGLE
+    op, arg, imm, start = H.translate(cls, energy, params, globals_, nparticles)
     nprog = 1 + 3*nparticles if nparticles else 2
     assert len(start) == nprog + 1
     for which in range(nprog):
-        got, msg = H.probe(nparticles, periodic, start, op, arg, imm, len(params), len(globals_), which, x, box, pvals, gvals)
+        got, msg = _probe(nparticles, periodic, start, op, arg, imm, len(params), len(globals_), which, x, box, pvals, gvals)
         assert msg is None, msg
-        want = H.lepton(nparticles, energy, which, x, box, periodic, params, pvals, globals_, gvals)
+        want = H.lepton(cls, energy, which, x, box, params, pvals, globals_, gvals, nparticles, periodic)
         assert _close(got, want), (energy, which, got, want)
     return op, arg, imm, start
 
@@ -66,8 +71,8 @@ def test_dihedral_sign_convention():
     op, arg, imm, start = _check(4, "dihedral(p1,p2,p3,p4)", x)
     mirrored = list(x)
     mirrored[11] = -0.4
-    v, _ = H.probe(4, False, start, op, arg, imm, 0, 0, 0, x, np.eye(3), (), ())
-    w, _ = H.probe(4, False, start, op, arg, imm, 0, 0, 0, mirrored, np.eye(3), (), ())
+    v, _ = H.compound_probe(4, False, start, op, arg, imm, 0, 0, 0, x, np.eye(3), (), ())
+    w, _ = H.compound_probe(4, False, start, op, arg, imm, 0, 0, 0, mirrored, np.eye(3), (), ())
     assert v == -w and v != 0.0
 
 
@@ -95,7 +100,7 @@ def test_realistic_expressions():
 
 
 def test_a_derivative_that_is_identically_zero_is_one_const():
-    op, arg, imm, start = H.translate(3, "distance(p1,p2)^2")
+    op, arg, imm, start = H.translate(H.COMPOUND, "distance(p1,p2)^2", nparticles=3)
     for q in range(7, 10):         # the programs of x3, y3, z3
         assert start[q+1] - start[q] == 1 and op[start[q]] == OP["CONST"] and imm[start[q]] == 0.0
 
@@ -121,7 +126,7 @@ def _one(nparticles, op, arg):
 ])
 def test_malformed_programs_are_refused(nparticles, op, arg, match):
     start, ops, args, imm = _one(nparticles, op, arg)
-    got, msg = H.probe(nparticles, False, start, ops, args, imm, 0, 0, 0, np.zeros(max(1, 3*nparticles)), np.eye(3), (), ())
+    got, msg = _probe(nparticles, False, start, ops, args, imm, 0, 0, 0, np.zeros(max(1, 3*nparticles)), np.eye(3), (), ())
     assert got is None and match in msg, msg
 
 
@@ -131,24 +136,24 @@ def test_point_opcodes_are_unknown_to_the_other_classes(cls, prefix):
     var = OP["THETA"] if cls == 0 else OP["VAR"]
     ops = [var]*6 + [OP["POINT_DIST"]] + [OP["CONST"]]*nvars
     start = [0, 7] + [8 + k for k in range(nvars)]
-    got, msg = custom_terms_harness.probe(cls, start, ops, [0]*len(ops), [0.0]*len(ops), 0, 0, 0, np.zeros(3), np.eye(3), (), ())
+    got, msg = H.term_probe(cls, start, ops, [0]*len(ops), [0.0]*len(ops), 0, 0, 0, np.zeros(3), np.eye(3), (), ())
     assert got is None and msg.startswith(prefix + " program: unknown opcode"), msg
 
 
 def test_limits_are_refused_as_unsupported():
     nine = "+".join("x%d" % i for i in range(1, 10))
     with pytest.raises(H.Refused, match="more than 8 particles per bond"):
-        H.translate(9, nine)
+        H.translate(H.COMPOUND, nine, nparticles=9)
     names = tuple("c%d" % i for i in range(17))
     with pytest.raises(H.Refused, match="more than 16 per-bond parameters"):
-        H.translate(2, "distance(p1,p2)*(" + "+".join(names) + ")", names)
+        H.translate(H.COMPOUND, "distance(p1,p2)*(" + "+".join(names) + ")", names, nparticles=2)
     with pytest.raises(H.Refused, match="tabulated functions"):
-        H.translate(2, "fn(distance(p1,p2))", tabulated=True)
+        H.translate(H.COMPOUND, "fn(distance(p1,p2))", nparticles=2, tabulated=True)
     # 13 values under a dihedral call, each pair of parentheses one more: deeper than 32
     deep = "dihedral(p1,p2,p3,p4)"
     for k in range(24):
         deep = "x1*(y1+" + deep + ")"
     with pytest.raises(H.Refused, match="deeper than 32"):
-        H.translate(4, deep)
+        H.translate(H.COMPOUND, deep, nparticles=4)
     with pytest.raises(ValueError, match="Unknown variable"):
-        H.translate(2, "1+none")
+        H.translate(H.COMPOUND, "1+none", nparticles=2)

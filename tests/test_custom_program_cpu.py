@@ -2,12 +2,12 @@
 the device kernel runs (openmm_b200/csrc/custom_interp.h), reached without a device through b200md_custom_program_probe,
 against Lepton's own ExpressionProgram::evaluate of the same expressions; and the checks b200md_set_custom_torsions makes of
 a program set, which the probe makes too."""
-import ctypes as C
 import math
 import zlib
 import numpy as np
 import pytest
-from openmm_b200 import _lib, systems
+from openmm_b200 import systems
+from custom_harness import program_probe as probe
 
 OP = dict(CONST=0, THETA=1, PARAM=2, GLOBAL=3, ADD=4, SUB=5, MUL=6, DIV=7, POW=8, NEG=9, SQRT=10, EXP=11, LOG=12, SIN=13,
           COS=14, SEC=15, CSC=16, TAN=17, COT=18, ASIN=19, ACOS=20, ATAN=21, ATAN2=22, SINH=23, COSH=24, TANH=25, ERF=26,
@@ -34,36 +34,15 @@ EXPRESSIONS = [
 
 @pytest.fixture(scope="module")
 def harness():
-    import custom_torsion_harness
-    if not custom_torsion_harness.available():
+    import custom_harness
+    if not custom_harness.available():
         pytest.fail("oracle/_ref is not built: run __graft_entry__.build() where /root/reference exists")
-    return custom_torsion_harness
-
-
-def _ints(a):
-    a = np.ascontiguousarray(a, dtype=np.int32)
-    return a, a.ctypes.data_as(C.POINTER(C.c_int))
-
-
-def _dbls(a):
-    a = np.ascontiguousarray(a, dtype=np.float64).reshape(-1)
-    if not len(a):
-        a = np.zeros(1)
-    return a, a.ctypes.data_as(C.POINTER(C.c_double))
-
-
-def probe(start, op, arg, imm, stride, nglobals, which, theta, params, globals_):
-    """b200md_custom_program_probe: (value, None) or (None, message)"""
-    keep = [_ints(start), _ints(op), _ints(arg), _dbls(imm), _dbls(params), _dbls(globals_)]
-    out, msg = C.c_double(), C.create_string_buffer(256)
-    rc = _lib.load().b200md_custom_program_probe(len(start)//2, keep[0][1], keep[1][1], keep[2][1], keep[3][1], stride, nglobals,
-                                                 which, theta, keep[4][1], keep[5][1], C.byref(out), msg, 256)
-    return (out.value, None) if rc == 0 else (None, msg.value.decode())
+    return custom_harness
 
 
 def run(harness, expr, deriv, theta, pv, gv, params=PARAMS, globals_=GLOBALS):
-    op, arg, imm, ne = harness.translate(expr, params, globals_)
-    value, err = probe([0, ne, len(op)], op, arg, imm, len(params), len(globals_), int(deriv), theta, pv, gv)
+    op, arg, imm, start = harness.translate(harness.TORSION, expr, params, globals_)
+    value, err = probe(start, op, arg, imm, len(params), len(globals_), int(deriv), theta, pv, gv)
     assert err is None, err
     return value
 
@@ -74,7 +53,7 @@ def _close(x, y):
 
 @pytest.mark.parametrize("expr,opname", EXPRESSIONS, ids=[e[0] for e in EXPRESSIONS])
 def test_every_opcode_matches_lepton(harness, expr, opname):
-    op, _, _, _ = harness.translate(expr, PARAMS, GLOBALS)
+    op, _, _, _ = harness.translate(harness.TORSION, expr, PARAMS, GLOBALS)
     assert OP[opname] in op.tolist(), (opname, op)
     rng = np.random.default_rng(zlib.crc32(expr.encode()))
     for _ in range(40):
@@ -82,7 +61,7 @@ def test_every_opcode_matches_lepton(harness, expr, opname):
         pv, gv = rng.uniform(0.3, 1.8, 2), rng.uniform(-2.0, 2.0, 1)
         for deriv in (False, True):
             ours = run(harness, expr, deriv, theta, pv, gv)
-            ref = harness.lepton(expr, deriv, theta, PARAMS, pv, GLOBALS, gv)
+            ref = harness.lepton(harness.TORSION, expr, deriv, [theta], params=PARAMS, pvals=pv, globals_=GLOBALS, gvals=gv)
             assert _close(ours, ref), (expr, deriv, theta, ours, ref)
 
 
@@ -96,7 +75,7 @@ def test_derivative_program_is_leptons_derivative(harness):
     pv, gv = np.array([1.3, 0.4]), np.array([0.7])
     for theta in np.linspace(-3.1, 3.1, 23):
         de = run(harness, expr, True, theta, pv, gv)
-        assert _close(de, harness.lepton(expr, True, theta, PARAMS, pv, GLOBALS, gv))
+        assert _close(de, harness.lepton(harness.TORSION, expr, True, [theta], params=PARAMS, pvals=pv, globals_=GLOBALS, gvals=gv))
         h = 1e-6
         fd = (run(harness, expr, False, theta + h, pv, gv) - run(harness, expr, False, theta - h, pv, gv))/(2*h)
         assert abs(fd - de) < 1e-7*max(1.0, abs(de))
@@ -110,8 +89,8 @@ def test_charmm_improper_across_the_seam(harness):
         for theta in np.concatenate([np.linspace(-math.pi, -math.pi + 0.05, 6), np.linspace(math.pi - 0.05, math.pi, 6), [0.0, 1.0]]):
             pv = np.array([250.0, theta0])
             e, de = (run(harness, expr, d, theta, pv, [], names, ()) for d in (False, True))
-            assert _close(e, harness.lepton(expr, False, theta, names, pv))
-            assert _close(de, harness.lepton(expr, True, theta, names, pv))
+            assert _close(e, harness.lepton(harness.TORSION, expr, False, [theta], params=names, pvals=pv))
+            assert _close(de, harness.lepton(harness.TORSION, expr, True, [theta], params=names, pvals=pv))
             dt = abs(theta - theta0)
             short = min(dt, 2*pi6 - dt)
             assert abs(e - 250.0*short**2) <= 1e-12*max(1.0, e)
@@ -121,7 +100,7 @@ def test_charmm_improper_across_the_seam(harness):
 
 def test_unknown_variable_is_an_error_not_a_refusal(harness):
     with pytest.raises(ValueError, match="Unknown variable"):
-        harness.translate("theta+none", (), ())
+        harness.translate(harness.TORSION, "theta+none", (), ())
 
 
 def test_limits_are_refusals(harness):
@@ -132,7 +111,7 @@ def test_limits_are_refusals(harness):
     long_expr = "+".join("sin(%d*theta)" % k for k in range(1, 120))
     for expr, params in ((deep, ()), (long_expr, ()), ("theta", tuple("p%d" % k for k in range(17)))):
         try:
-            op, _, _, ne = harness.translate(expr, params, ())
+            op, _, _, _ = harness.translate(harness.TORSION, expr, params, ())
         except harness.Refused:
             continue
         pytest.fail("not refused: %s (%d instructions)" % (expr[:40], len(op)))

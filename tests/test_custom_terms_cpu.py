@@ -12,15 +12,15 @@ BOX_TRICLINIC = np.array([[3.0, 0.0, 0.0], [0.9, 2.8, 0.0], [-0.7, 1.1, 3.3]])
 
 @pytest.fixture(scope="module")
 def harness():
-    import custom_terms_harness
-    if not custom_terms_harness.available():
+    import custom_harness
+    if not custom_harness.available():
         pytest.fail("oracle/_ref is not built: run __graft_entry__.build() where /root/reference exists")
-    return custom_terms_harness
+    return custom_harness
 
 
 def _run(h, cls, expr, which, variables, box=np.eye(3), params=(), pv=(), globals_=(), gv=()):
     op, arg, imm, starts = h.translate(cls, expr, params, globals_)
-    value, err = h.probe(cls, starts, op, arg, imm, len(params), len(globals_), which, variables, box, pv, gv)
+    value, err = h.term_probe(cls, starts, op, arg, imm, len(params), len(globals_), which, variables, box, pv, gv)
     assert err is None, err
     return value
 
@@ -83,7 +83,7 @@ def test_periodic_distance_opcode_derivatives(harness):
         arg = [2, 1, 0, 2, 1, 0, k, 0, 1, 2]
         x, p = np.array([2.9, -3.3, 7.1]), np.array([0.2, 1.4, -0.6])
         for box in (BOX_ORTHO, BOX_TRICLINIC):
-            value, err = h.probe(h.EXTERNAL, start, op, arg, [0.0]*10, 3, 0, 0, x, box, p, [])
+            value, err = h.term_probe(h.EXTERNAL, start, op, arg, [0.0]*10, 3, 0, 0, x, box, p, [])
             assert err is None, err
             if k < 3:
                 ref = h.lepton(h.EXTERNAL, expr, k + 1, x, box, ("x0", "y0", "z0"), p)
@@ -139,5 +139,5 @@ def test_malformed_programs_are_refused(harness, cls, op, arg, match):
     good = OP_THETA if cls == 0 else OP_VAR
     ops, args = op + [good]*nv, arg + [0]*nv
     start = [0, len(op)] + [len(op) + k + 1 for k in range(nv)]
-    value, err = harness.probe(cls, start, ops, args, [0.0]*len(ops), 0, 0, 0, [0.1, 0.2, 0.3], np.eye(3), [], [])
+    value, err = harness.term_probe(cls, start, ops, args, [0.0]*len(ops), 0, 0, 0, [0.1, 0.2, 0.3], np.eye(3), [], [])
     assert value is None and match in err, err

@@ -16,11 +16,11 @@ REFTESTS = os.path.join(ROOT, "oracle", "_ref", "tests")
 
 @pytest.fixture(scope="module")
 def harness():
-    import custom_compound_harness
-    if not custom_compound_harness.available() or not os.path.exists(PLUGIN):
+    import custom_harness
+    if not custom_harness.available() or not os.path.exists(PLUGIN):
         pytest.fail("oracle/_ref or the plugin is not built: run __graft_entry__.build() where /root/reference exists")
-    custom_compound_harness.omm.load_plugin(PLUGIN)
-    return custom_compound_harness
+    custom_harness.omm.load_plugin(PLUGIN)
+    return custom_harness
 
 
 def _dhfr():
@@ -86,7 +86,7 @@ def _probe_gradient(harness, r, x):
     """energy and gradient [6,3] of the one restraint term at the positions x [6,3], in double, through the host interpreter"""
     from openmm_b200 import systems
     start, par = r.ccompound_prog_start, r.ccompound_params[0]
-    vals = [harness.probe(6, bool(r.ccompound_periodic[0]), start, r.ccompound_op, r.ccompound_arg, r.ccompound_imm, len(par), 0, q,
+    vals = [harness.compound_probe(6, bool(r.ccompound_periodic[0]), start, r.ccompound_op, r.ccompound_arg, r.ccompound_imm, len(par), 0, q,
                           x.reshape(-1), np.asarray(r.box), par, ())[0] for q in range(19)]
     return vals[0], np.array(vals[1:]).reshape(6, 3)
 
@@ -312,7 +312,7 @@ def test_unsupported_compound_forces_move_the_context_elsewhere(harness, case, m
     else:
         d = _small("lam*distance(p1,p2)", 2)
         d.custom_global_names, d.custom_global_values = ("lam",), np.array([1.0])
-        kw = dict(compound_deriv_param="lam")
+        kw = dict(deriv_params={"custom_compound": "lam"})
     s = harness.Simulation(d, "Reference", **kw)
     assert s.default_platform() not in ("", "B200")
     with pytest.raises(RuntimeError, match=match):

@@ -18,12 +18,12 @@ RESTRAINT_K = 400.0          # kJ/mol/nm^2
 
 @pytest.fixture(scope="module")
 def harness():
-    """the translator, Lepton and the reference's custom forces (tests/custom_terms_harness.py), with the plugin loaded"""
-    import custom_terms_harness
-    if not custom_terms_harness.available() or not os.path.exists(PLUGIN):
+    """the translator, Lepton and the reference's custom forces (tests/custom_harness.py), with the plugin loaded"""
+    import custom_harness
+    if not custom_harness.available() or not os.path.exists(PLUGIN):
         pytest.fail("oracle/_ref or the plugin is not built: run __graft_entry__.build() where /root/reference exists")
-    custom_terms_harness.omm.load_plugin(PLUGIN)
-    return custom_terms_harness
+    custom_harness.omm.load_plugin(PLUGIN)
+    return custom_harness
 
 
 def _dhfr():
@@ -233,10 +233,10 @@ def test_update_parameters_in_context(harness):
 
 def test_energy_parameter_derivatives_move_the_context_elsewhere(harness):
     d = _three_classes(harness)
-    s = harness.Simulation(d, "Reference", deriv_param="lam")
+    s = harness.Simulation(d, "Reference", deriv_params={"custom_bonds": "lam"})
     assert s.default_platform() not in ("", "B200")
     with pytest.raises(RuntimeError, match="energy parameter derivatives of a CustomBondForce"):
-        harness.Simulation(d, "B200", deriv_param="lam")
+        harness.Simulation(d, "B200", deriv_params={"custom_bonds": "lam"})
 
 
 def _step_launches(eng):

@@ -16,12 +16,12 @@ REFTESTS = os.path.join(ROOT, "oracle", "_ref", "tests")
 
 @pytest.fixture(scope="module")
 def harness():
-    """the translator, Lepton and the reference's CustomTorsionForce (tests/custom_torsion_harness.py), with the plugin loaded"""
-    import custom_torsion_harness
-    if not custom_torsion_harness.available() or not os.path.exists(PLUGIN):
+    """the translator, Lepton and the reference's CustomTorsionForce (tests/custom_harness.py), with the plugin loaded"""
+    import custom_harness
+    if not custom_harness.available() or not os.path.exists(PLUGIN):
         pytest.fail("oracle/_ref or the plugin is not built: run __graft_entry__.build() where /root/reference exists")
-    custom_torsion_harness.omm.load_plugin(PLUGIN)
-    return custom_torsion_harness
+    custom_harness.omm.load_plugin(PLUGIN)
+    return custom_harness
 
 
 def _dhfr():
@@ -75,10 +75,10 @@ def test_energy_parameter_derivatives_move_the_context_elsewhere(harness):
     d = _tiny(harness)
     plain = harness.Simulation(d, "Reference")
     assert plain.default_platform() == "B200"
-    s = harness.Simulation(d, "Reference", deriv_param="lam")
-    assert s.default_platform() not in ("", "B200"), harness.lib().ct_last_error()
+    s = harness.Simulation(d, "Reference", deriv_params={"custom_torsions": "lam"})
+    assert s.default_platform() not in ("", "B200"), harness.lib().cc_last_error()
     with pytest.raises(RuntimeError, match="energy parameter derivatives"):
-        harness.Simulation(d, "B200", deriv_param="lam")
+        harness.Simulation(d, "B200", deriv_params={"custom_torsions": "lam"})
 
 
 # ---------------------------------------------------------------------------------------------------- engine
@@ -214,7 +214,7 @@ def test_update_parameters_in_context(harness, dhfr_charmm):
     rng = np.random.default_rng(9)
     new = np.stack([rng.uniform(50, 900, len(d.custom_prog)), rng.uniform(-np.pi, np.pi, len(d.custom_prog))], axis=1)
     for s in sims.values():
-        s.update_custom_torsions(0, d.custom_atoms, new)
+        s.update("custom", 0, d.custom_atoms, new)
     (f, e), (fr, er) = sims["B200"].forces_energy(1 << 5), sims["Reference"].forces_energy(1 << 5)
     _group_close(f, e, fr, er)
     b200 = sims["B200"]
@@ -222,9 +222,9 @@ def test_update_parameters_in_context(harness, dhfr_charmm):
     with pytest.raises(RuntimeError, match="set of particles in a torsion has changed"):
         atoms = d.custom_atoms.copy()
         atoms[3] = atoms[3][::-1]
-        b200.update_custom_torsions(0, atoms, new)
+        b200.update("custom", 0, atoms, new)
     with pytest.raises(RuntimeError, match="number of torsions has changed"):
-        b200.update_custom_torsions(0, np.concatenate([d.custom_atoms, d.custom_atoms[:1]]), np.concatenate([new, new[:1]]))
+        b200.update("custom", 0, np.concatenate([d.custom_atoms, d.custom_atoms[:1]]), np.concatenate([new, new[:1]]))
 
 
 def _plugin_run(harness, d, fused, steps=30):

@@ -76,7 +76,7 @@ def compute_counts():
 
 
 def custom_torsion_counts():
-    import custom_torsion_harness as harness
+    import custom_harness as harness
     from openmm_b200 import systems
     if not harness.available():
         pytest.fail("oracle/_ref is not built: run __graft_entry__.build() where /root/reference exists")

@@ -8,7 +8,7 @@
   anybody would write a force field.
 - The bonded kernels alone (b200md_time_phase): k_bonded of DHFR (phase 6), k_custom of the custom-angle variant (phase 7),
   k_compound of the restraint and of the stress case (phase 8).
-The programs come from the plugin's translator (tests/custom_compound_harness.py).  The card name, power limit and max SM clock
+The programs come from the plugin's translator (tests/custom_harness.py).  The card name, power limit and max SM clock
 come from a read-only nvidia-smi query in the same call.  Prints one JSON line.
 
     python tools/gpu_custom_compound_bench.py [--rounds 3] [--steps 10] [--warmup 2] [--md-steps 500]
@@ -34,7 +34,7 @@ def main():
     ap.add_argument("--phase-reps", type=int, default=500)
     args = ap.parse_args()
     import torch
-    import custom_compound_harness as harness
+    import custom_harness as harness
     from openmm_b200 import systems, Engine
     if not torch.cuda.is_available():
         raise SystemExit("gpu_custom_compound_bench.py: no CUDA device")

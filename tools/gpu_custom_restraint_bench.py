@@ -7,7 +7,7 @@
 - Device-timed ns/day of the step path (LangevinMiddle 2 fs, CUDA events on the engine's stream) for DHFR, DHFR plus
   position restraints on its 1,268 solute heavy atoms (k*periodicdistance(x, y, z, x0, y0, z0)^2), DHFR-CHARMM (DHFR plus the
   CHARMM36 CMAP maps and CharmmPsfFile-form impropers) and DHFR-CHARMM plus the same restraints, alternating.
-The programs come from the plugin's translator (tests/custom_terms_harness.py).  The card name, power limit and max SM clock
+The programs come from the plugin's translator (tests/custom_harness.py).  The card name, power limit and max SM clock
 come from a read-only nvidia-smi query in the same call.  Prints one JSON line.
 
     python tools/gpu_custom_restraint_bench.py [--parent DIR] [--rounds 3] [--steps 10] [--warmup 2] [--md-steps 500]
@@ -53,7 +53,7 @@ def main():
     args = ap.parse_args()
     import numpy as np
     import torch
-    import custom_terms_harness as harness
+    import custom_harness as harness
     from openmm_b200 import systems, Engine
     if not torch.cuda.is_available():
         raise SystemExit("gpu_custom_restraint_bench.py: no CUDA device")

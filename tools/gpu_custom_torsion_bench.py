@@ -7,7 +7,7 @@
   DHFR-CHARMM: DHFR plus the CHARMM36 CMAP maps on its backbone and CharmmPsfFile-form impropers (systems.with_cmap,
   systems.with_charmm_impropers).
 The configurations alternate for --rounds rounds.  The programs come from the plugin's translator (tests/
-custom_torsion_harness.py over oracle/_ref/tests/libcustom_torsion_capi.so).  The card name, power limit and max SM clock come
+custom_harness.py over oracle/_ref/tests/libcustom_capi.so).  The card name, power limit and max SM clock come
 from a read-only nvidia-smi query in the same call.  Prints one JSON line.
 
     python tools/gpu_custom_torsion_bench.py [--rounds 3] [--steps 10] [--warmup 2] [--md-steps 500]
@@ -34,7 +34,7 @@ def main():
     args = ap.parse_args()
     import numpy as np
     import torch
-    import custom_torsion_harness as harness
+    import custom_harness as harness
     from openmm_b200 import systems, Engine
     if not torch.cuda.is_available():
         raise SystemExit("gpu_custom_torsion_bench.py: no CUDA device")
