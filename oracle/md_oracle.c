@@ -525,45 +525,117 @@ void orc_settle_velocities(int nw, const int* a0, const int* a1, const int* a2, 
     }
 }
 
-/* One deterministic step (no random force: temperature 0).  kind 0: leapfrog Verlet (ReferenceVerletDynamics.cpp), 1: Langevin
- * (ReferenceStochasticDynamics.cpp:89-194), 2: LangevinMiddle (ReferenceLangevinMiddleDynamics.cpp:54-127: kick, velocity
- * constraints, half drift, friction, half drift, position constraints, velocity correction by the constraint displacement). */
-void orc_step(int kind, int n, double dt, double friction, const double* mass, const double* forces, double* x, double* v,
-              int nw, const int* a0, const int* a1, const int* a2, const double* d1, const double* d2) {
+int orc_ccma(int ncon, const int* ai, const int* aj, const double* dist, const double* invm, const double* x, double* xp,
+             const int* row_start, const int* col, const double* val, int constrain_velocities, double tol, int maxit);
+
+/* ---- the engine's random numbers ----
+ * Philox4x32-10 (Salmon et al., SC'11) and the Box-Muller transform exactly as the engine defines its noise
+ * (openmm_b200/csrc/engine.h: philox, gauss3): counter (atom, step_lo, step_hi, 0x5eed5eed), key (seed, 0xb200b200).  This
+ * restates the engine's OWN definition: the Reference platform draws its normals from a different generator, so it cannot
+ * be the oracle for these bits.  The integer-to-uniform conversion is the engine's, exact in any precision; the transform
+ * is done in double (the engine's fp32 transform agrees to a few 1e-7 relative). */
+void orc_philox4x32_10(const unsigned int ctr[4], const unsigned int key[2], unsigned int out[4]) {
+    unsigned int c0 = ctr[0], c1 = ctr[1], c2 = ctr[2], c3 = ctr[3], k0 = key[0], k1 = key[1];
+    for (int r = 0; r < 10; r++) {
+        const unsigned long long p0 = 0xD2511F53ull*c0, p1 = 0xCD9E8D57ull*c2;
+        const unsigned int hi0 = (unsigned int) (p0 >> 32), lo0 = (unsigned int) p0;
+        const unsigned int hi1 = (unsigned int) (p1 >> 32), lo1 = (unsigned int) p1;
+        c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
+        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
+    }
+    out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
+}
+
+void orc_gauss3(unsigned int seed, int atom, unsigned long long step, double g[3]) {
+    const unsigned int ctr[4] = {(unsigned int) atom, (unsigned int) step, (unsigned int) (step >> 32), 0x5eed5eedu};
+    const unsigned int key[2] = {seed, 0xb200b200u};
+    unsigned int r[4];
+    orc_philox4x32_10(ctr, key, r);
+    const double u1 = ((r[0] >> 8) + 1u)/16777216.0, u2 = (r[1] >> 8)/16777216.0;         /* (0,1], [0,1) */
+    const double u3 = ((r[2] >> 8) + 1u)/16777216.0, u4 = (r[3] >> 8)/16777216.0;
+    const double m1 = sqrt(-2.0*log(u1)), m2 = sqrt(-2.0*log(u3));
+    g[0] = m1*cos(2.0*M_PI*u2); g[1] = m1*sin(2.0*M_PI*u2); g[2] = m2*cos(2.0*M_PI*u4);
+}
+
+/* orc_gauss3 for the atoms atoms[0..n) at one step: g[3*i..] */
+void orc_gauss3_atoms(unsigned int seed, int n, const int* atoms, unsigned long long step, double* g) {
+    for (int i = 0; i < n; i++) orc_gauss3(seed, atoms[i], step, g + 3*i);
+}
+
+/* One Verlet / Langevin / LangevinMiddle step with its random force.  kind 0: leapfrog Verlet (ReferenceVerletDynamics.cpp),
+ * 1: Langevin (ReferenceStochasticDynamics.cpp:89-194), 2: LangevinMiddle (ReferenceLangevinMiddleDynamics.cpp:54-127: kick,
+ * velocity constraints, half drift, friction + noise, half drift, position constraints, velocity correction by the constraint
+ * displacement).  The noise of atom i is gauss[3*i..3*i+2] (NULL: none, the zero-temperature step), scaled as the reference
+ * scales it: sqrt(kT (1 - vscale^2)/m) g (Langevin), sqrt(1 - vscale^2) sqrt(kT/m) g (LangevinMiddle); massless atoms neither
+ * move nor change velocity.  Constraints: the nw SETTLE clusters as in orc_settle, and every other constraint (ncon of them,
+ * SHAKE clusters included) by orc_ccma in double with an identity coupling matrix to `tol` -- the Reference platform treats
+ * every non-water constraint as one CCMA system.  Returns the most CCMA iterations one solve used, -1 if a solve did not
+ * converge. */
+int orc_langevin_step(int kind, int n, double dt, double friction, double kT, const double* mass, const double* forces,
+                      const double* gauss, double* x, double* v, int nw, const int* a0, const int* a1, const int* a2,
+                      const double* d1, const double* d2, int ncon, const int* ai, const int* aj, const double* dist, double tol) {
+    const int maxit = 100000;
     double* xn = (double*) malloc(sizeof(double)*3*n);
+    double* invm = NULL;
+    int* rs = NULL; int* col = NULL; double* val = NULL;
+    int iters = 0;
+    if (ncon > 0) {
+        invm = (double*) malloc(sizeof(double)*n);
+        for (int i = 0; i < n; i++) invm[i] = mass[i] > 0 ? 1.0/mass[i] : 0.0;
+        rs = (int*) malloc(sizeof(int)*(ncon+1)); col = (int*) malloc(sizeof(int)*ncon); val = (double*) malloc(sizeof(double)*ncon);
+        for (int k = 0; k <= ncon; k++) rs[k] = k;
+        for (int k = 0; k < ncon; k++) { col[k] = k; val[k] = 1.0; }
+    }
+#define CCMA_SOLVE(target, vel) do { \
+        const int it = orc_ccma(ncon, ai, aj, dist, invm, x, target, rs, col, val, vel, tol, maxit); \
+        if (it >= maxit) iters = -1; else if (iters >= 0 && it > iters) iters = it; } while (0)
     const double vscale = exp(-dt*friction), fscale = (friction == 0 ? dt : (1-vscale)/friction);
     if (kind == 2) {
         double* xu = (double*) malloc(sizeof(double)*3*n);
         for (int i = 0; i < n; i++) if (mass[i] > 0) for (int k = 0; k < 3; k++) v[3*i+k] += dt*forces[3*i+k]/mass[i];
         if (nw > 0) orc_settle_velocities(nw, a0, a1, a2, mass, x, v);
+        if (ncon > 0) CCMA_SOLVE(v, 1);
         for (int i = 0; i < n; i++) for (int k = 0; k < 3; k++) {
             if (mass[i] > 0) {
                 xn[3*i+k] = x[3*i+k] + 0.5*dt*v[3*i+k];
                 v[3*i+k] *= vscale;
+                if (gauss) v[3*i+k] += sqrt(1-vscale*vscale)*sqrt(kT/mass[i])*gauss[3*i+k];
                 xn[3*i+k] += 0.5*dt*v[3*i+k];
             }
             else xn[3*i+k] = x[3*i+k];
             xu[3*i+k] = xn[3*i+k];
         }
         if (nw > 0) orc_settle(nw, a0, a1, a2, d1, d2, mass, x, xn);
+        if (ncon > 0) CCMA_SOLVE(xn, 0);
         for (int i = 0; i < n; i++) if (mass[i] > 0) for (int k = 0; k < 3; k++) { v[3*i+k] += (xn[3*i+k]-xu[3*i+k])/dt; x[3*i+k] = xn[3*i+k]; }
-        free(xu); free(xn);
-        return;
+        free(xu);
     }
-    for (int i = 0; i < n; i++) {
-        const double im = mass[i] > 0 ? 1.0/mass[i] : 0.0;
-        for (int k = 0; k < 3; k++) {
-            double vn = (kind == 1) ? vscale*v[3*i+k] + fscale*im*forces[3*i+k] : v[3*i+k] + dt*im*forces[3*i+k];
-            if (im == 0) vn = v[3*i+k];
-            v[3*i+k] = vn;
-            xn[3*i+k] = x[3*i+k] + (im == 0 ? 0.0 : vn*dt);
+    else {
+        for (int i = 0; i < n; i++) {
+            const double im = mass[i] > 0 ? 1.0/mass[i] : 0.0;
+            for (int k = 0; k < 3; k++) {
+                double vn = (kind == 1) ? vscale*v[3*i+k] + fscale*im*forces[3*i+k] : v[3*i+k] + dt*im*forces[3*i+k];
+                if (kind == 1 && gauss) vn += sqrt(kT*(1-vscale*vscale)*im)*gauss[3*i+k];
+                if (im == 0) vn = v[3*i+k];
+                v[3*i+k] = vn;
+                xn[3*i+k] = x[3*i+k] + (im == 0 ? 0.0 : vn*dt);
+            }
+        }
+        if (nw > 0) orc_settle(nw, a0, a1, a2, d1, d2, mass, x, xn);
+        if (ncon > 0) CCMA_SOLVE(xn, 0);
+        for (int i = 0; i < n; i++) {
+            if (mass[i] > 0) for (int k = 0; k < 3; k++) { v[3*i+k] = (xn[3*i+k]-x[3*i+k])/dt; x[3*i+k] = xn[3*i+k]; }
         }
     }
-    if (nw > 0) orc_settle(nw, a0, a1, a2, d1, d2, mass, x, xn);
-    for (int i = 0; i < n; i++) {
-        if (mass[i] > 0) for (int k = 0; k < 3; k++) { v[3*i+k] = (xn[3*i+k]-x[3*i+k])/dt; x[3*i+k] = xn[3*i+k]; }
-    }
-    free(xn);
+#undef CCMA_SOLVE
+    free(xn); free(invm); free(rs); free(col); free(val);
+    return iters;
+}
+
+/* One deterministic step (no random force: temperature 0), SETTLE the only constraints: orc_langevin_step without noise. */
+void orc_step(int kind, int n, double dt, double friction, const double* mass, const double* forces, double* x, double* v,
+              int nw, const int* a0, const int* a1, const int* a2, const double* d1, const double* d2) {
+    orc_langevin_step(kind, n, dt, friction, 0.0, mass, forces, NULL, x, v, nw, a0, a1, a2, d1, d2, 0, NULL, NULL, NULL, 0.0);
 }
 
 /* ---- CCMA: ReferenceCCMAAlgorithm::applyConstraints (ReferenceCCMAAlgorithm.cpp:235-316), positions or velocities ----

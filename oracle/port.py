@@ -1,23 +1,27 @@
 """oracle/port.py -- TEST INFRASTRUCTURE, not product code.
 
-ctypes binding of oracle/_ref/liboracle.so (md_oracle.c, the plain-C restatement of the reference algorithm).
+ctypes binding of oracle/_ref/liboracle-<sha1 of md_oracle.c>.so (md_oracle.c, the plain-C restatement of the reference algorithm).
 forces_energy(desc) evaluates a SystemDesc exactly the way ReferenceCalcNonbondedForceKernel::execute
 (ReferenceKernels.cpp:967-1014) + the bonded kernels do.  Only tests/, smoke() and bench.py's cpu_baseline may use it.
 """
 import ctypes as C
+import hashlib
 import os
 import subprocess
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = os.path.join(_HERE, "_ref", "liboracle.so")
+with open(os.path.join(_HERE, "md_oracle.c"), "rb") as _src:
+    _TAG = hashlib.sha1(_src.read()).hexdigest()[:16]
+# named after the source's content (oracle/Makefile `port`): a library built from another version is never loaded
+_LIB = os.path.join(_HERE, "_ref", "liboracle-%s.so" % _TAG)
 _lib = None
 D = C.POINTER(C.c_double)
 I = C.POINTER(C.c_int)
 
 
 def build():
-    subprocess.check_call(["make", "-s", "-C", _HERE, "port"])
+    subprocess.check_call(["make", "-s", "-C", _HERE, "port", "ORC_TAG=" + _TAG])
 
 
 def lib():
@@ -52,6 +56,16 @@ def lib():
         L.orc_fft3d_forward.argtypes = [C.c_int, C.c_int, C.c_int, D, D]
         L.orc_ccma.restype = C.c_int
         L.orc_ccma.argtypes = [C.c_int, I, I, D, D, D, D, I, I, D, C.c_int, C.c_double, C.c_int]
+        U = C.POINTER(C.c_uint32)
+        L.orc_philox4x32_10.restype = None
+        L.orc_philox4x32_10.argtypes = [U, U, U]
+        L.orc_gauss3.restype = None
+        L.orc_gauss3.argtypes = [C.c_uint32, C.c_int, C.c_uint64, D]
+        L.orc_gauss3_atoms.restype = None
+        L.orc_gauss3_atoms.argtypes = [C.c_uint32, C.c_int, I, C.c_uint64, D]
+        L.orc_langevin_step.restype = C.c_int
+        L.orc_langevin_step.argtypes = [C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, D, D, D, D, D, C.c_int, I, I, I, D, D,
+                                        C.c_int, I, I, D, C.c_double]
         L.orc_num_threads.restype = C.c_int
         _lib = L
     return _lib
@@ -184,6 +198,50 @@ def step(desc, kind, dt, friction, x, v, forces, clusters):
     L = lib()
     a0, a1, a2, d1, d2 = clusters
     L.orc_step(kind, desc.natoms, dt, friction, _dp(_d(desc.masses)), _dp(_d(forces)), _dp(x), _dp(v), len(a0), _ip(a0), _ip(a1), _ip(a2), _dp(d1), _dp(d2))
+
+
+BOLTZ = 0.00831446261815324          # kJ/mol/K, as md_oracle.c and the engine
+
+
+def philox4x32_10(ctr, key):
+    """Philox4x32-10 of a 4-word counter and a 2-word key (orc_philox4x32_10), as 4 uint32."""
+    c, k, out = (np.ascontiguousarray(np.asarray(a, dtype=np.uint64) & 0xffffffff, dtype=np.uint32) for a in (ctr, key, np.zeros(4)))
+    U = C.POINTER(C.c_uint32)
+    lib().orc_philox4x32_10(c.ctypes.data_as(U), k.ctypes.data_as(U), out.ctypes.data_as(U))
+    return out
+
+
+def gauss3(seed, atoms, step):
+    """[n, 3]: the three normals the engine draws for each of `atoms` in the step that starts with counter `step`
+    (engine.h gauss3, restated by orc_gauss3).  The seed is taken as the engine takes it, cast to 32-bit unsigned."""
+    a = _i(np.atleast_1d(atoms))
+    g = np.empty((len(a), 3))
+    lib().orc_gauss3_atoms(int(seed) & 0xffffffff, len(a), _ip(a), int(step), _dp(g))
+    return g
+
+
+def constraint_split(desc):
+    """(SETTLE clusters as settle_clusters(desc), (ai, aj, dist) of every other constraint): the Reference platform's split
+    of a System's constraints into rigid waters and one CCMA system (ReferenceConstraints.cpp:69-184)."""
+    cl = settle_clusters(desc)
+    settled = np.zeros(desc.natoms, bool)
+    for a in cl[:3]:
+        settled[a] = True
+    rest = ~(settled[desc.con_i] & settled[desc.con_j])
+    return cl, (_i(desc.con_i[rest]), _i(desc.con_j[rest]), _d(desc.con_d[rest]))
+
+
+def langevin_step(desc, kind, dt, friction, temperature, x, v, forces, gauss=None, split=None, tol=1e-12):
+    """One Verlet (0) / Langevin (1) / LangevinMiddle (2) step with the random force `gauss` [n, 3] (None: none) at
+    `temperature`; SETTLE for the rigid waters, CCMA in double to `tol` for every other constraint (split: constraint_split(desc),
+    computed when not given).  x, v modified in place; returns the most CCMA iterations a solve used (-1: no convergence)."""
+    L = lib()
+    (a0, a1, a2, d1, d2), (ai, aj, dist) = split or constraint_split(desc)
+    assert x.dtype == np.float64 and v.dtype == np.float64 and x.flags.c_contiguous and v.flags.c_contiguous
+    g = None if gauss is None else _d(gauss)
+    return L.orc_langevin_step(kind, desc.natoms, dt, friction, BOLTZ*temperature, _dp(_d(desc.masses)), _dp(_d(forces)),
+                               None if g is None else _dp(g), _dp(x), _dp(v), len(a0), _ip(a0), _ip(a1), _ip(a2), _dp(d1), _dp(d2),
+                               len(ai), _ip(ai), _ip(aj), _dp(dist), tol)
 
 
 def fft3d_forward(x):
