@@ -45,7 +45,8 @@ typedef struct b200md_ctx b200md_ctx;
 #define B200MD_TERM_CUSTOM_EXTERNALS 512
 #define B200MD_TERM_CUSTOM_ANGLES    1024
 #define B200MD_TERM_CUSTOM_COMPOUND  2048
-#define B200MD_TERM_ALL        4095
+#define B200MD_TERM_CUSTOM_CENTROID  4096
+#define B200MD_TERM_ALL        8191
 
 /* ---- the bonded classes: kind argument of b200md_set_bonded_groups and b200md_update_bonded_params ---- */
 #define B200MD_BONDED_BONDS           0
@@ -59,6 +60,7 @@ typedef struct b200md_ctx b200md_ctx;
 /* 8 is not a kind: b200md_set_bonded_groups has always refused it, and callers probe with it */
 #define B200MD_BONDED_CUSTOM_ANGLES   9
 #define B200MD_BONDED_CUSTOM_COMPOUND 10
+#define B200MD_BONDED_CUSTOM_CENTROID 11
 
 /* ---- the classes of custom terms: which variables a program may read (custom_check_program) ---- */
 #define B200MD_CUSTOM_TORSION  0      /* THETA                                   */
@@ -66,6 +68,7 @@ typedef struct b200md_ctx b200md_ctx;
 #define B200MD_CUSTOM_EXTERNAL 2      /* VAR 0, 1, 2 = x, y, z; PERIODIC_DIST      */
 #define B200MD_CUSTOM_ANGLE    3      /* THETA = the angle in [0, pi]             */
 #define B200MD_CUSTOM_COMPOUND 4      /* VAR 3i, 3i+1, 3i+2 = x, y, z of particle i; POINT_DIST, POINT_ANGLE, POINT_DIHEDRAL */
+#define B200MD_CUSTOM_CENTROID 5      /* as COMPOUND, with the centre of group i for particle i */
 
 /* ---- instructions of a custom-term expression program (b200md_set_custom_torsions / _bonds / _externals / _angles /
  * _compound) ----
@@ -180,6 +183,17 @@ int b200md_set_custom_angles(b200md_ctx* ctx, int nprog, const int* prog_start, 
 int b200md_set_custom_compound(b200md_ctx* ctx, int nexpr, const int* nparticles, const int* periodic, const int* prog_start,
                                const int* op, const int* arg, const double* imm, int param_stride, int n, const int* expr,
                                const int* atoms, const double* params);
+/* CalcCustomCentroidBondForceKernel::initialize (kernels.h): as b200md_set_custom_compound, with groups of atoms for
+ * particles.  ngroups groups: group g is the atoms group_atoms[group_start[g] .. group_start[g+1]-1] (at least one) with
+ * the weights group_weights[..] (finite; normalised, as CustomCentroidBondForceImpl::computeNormalizedWeights makes them:
+ * the centre of a group is the weighted sum of the continuous coordinates of its atoms).  Expression p joins
+ * ngroups_per_bond[p] <= B200MD_CUSTOM_MAX_PARTICLES groups (VAR 3i+k = coordinate k of the centre of group i of the bond);
+ * term i evaluates expression expr[i] on the groups groups[8i ..] (unused slots -1).  The force on atom a of group g of a
+ * bond is -w_a times the derivatives by the centre of g, summed over every bond and group a belongs to.  Single GPU only. */
+int b200md_set_custom_centroid(b200md_ctx* ctx, int nexpr, const int* ngroups_per_bond, const int* periodic, const int* prog_start,
+                               const int* op, const int* arg, const double* imm, int param_stride, int n, const int* expr,
+                               const int* groups, const double* params, int ngroups, const int* group_start,
+                               const int* group_atoms, const double* group_weights);
 /* The global parameter values the GLOBAL instructions read (slot s = values[s]).  Before finalize it sets the number of
  * slots; after it, a stream-ordered copy of n == that number of values into the same device buffer, so a captured step
  * graph keeps running with the new values and is never instantiated again.                                               */
@@ -242,6 +256,8 @@ int b200md_update_custom_external_params(b200md_ctx* ctx, int n, const double* p
 /* CalcCustom{Angle,CompoundBond}ForceKernel::copyParametersToContext: the same for custom angles and compound bonds.      */
 int b200md_update_custom_angle_params(b200md_ctx* ctx, int n, const double* params);
 int b200md_update_custom_compound_params(b200md_ctx* ctx, int n, const double* params);
+/* CalcCustomCentroidBondForceKernel::copyParametersToContext: the same for centroid bonds (groups and weights stay).       */
+int b200md_update_custom_centroid_params(b200md_ctx* ctx, int n, const double* params);
 /* Test hook, no context and no device: program `which` of a b200md_set_custom_torsions program set, checked as that call
  * checks it (nglobals = the number of global slots), evaluated at (theta, params, globals) on the host by the interpreter
  * source the device kernel runs.  0 and *out on success, -1 with the reason in msg.                                       */
@@ -351,7 +367,8 @@ int b200md_get_stats(b200md_ctx* ctx, b200md_stats* out);
 /* mean device time (ms) of named phases measured with CUDA events on the engine's stream:
  * phase: 0 pair kernel, 1 pme spread, 2 fft+convolution, 3 pme gather, 4 integrate+constrain, 5 list build,
  * 6 bonded+exceptions (k_bonded and, with custom terms, k_custom and k_compound), 7 custom torsions, bonds, externals and
- * angles alone (k_custom), 8 custom compound bonds alone (k_compound).
+ * angles alone (k_custom), 8 custom compound bonds alone (k_compound), 9 custom centroid bonds alone (k_centroid_centers,
+ * the k_compound instantiation that reads the centres, k_centroid_scatter).
  * Runs `reps` isolated launches of that phase on the current state.                                  */
 int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* ms_mean);
 /* stand-alone 3-D FFT entry (the bespoke FFT alone, for parity against fftpack / numpy):

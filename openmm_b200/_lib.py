@@ -44,6 +44,7 @@ SIGNATURES = {
     "b200md_set_custom_externals": (C.c_int, [_P, C.c_int, _I, _I, _I, _D, C.c_int, C.c_int, _I, _I, _D]),
     "b200md_set_custom_angles": (C.c_int, [_P, C.c_int, _I, _I, _I, _D, C.c_int, C.c_int, _I, _I, _D]),
     "b200md_set_custom_compound": (C.c_int, [_P, C.c_int, _I, _I, _I, _I, _I, _D, C.c_int, C.c_int, _I, _I, _D]),
+    "b200md_set_custom_centroid": (C.c_int, [_P, C.c_int, _I, _I, _I, _I, _I, _D, C.c_int, C.c_int, _I, _I, _D, C.c_int, _I, _I, _D]),
     "b200md_set_custom_globals": (C.c_int, [_P, C.c_int, _D]),
     "b200md_set_bonded_groups": (C.c_int, [_P, C.c_int, C.c_int, _I]),
     "b200md_set_constraints": (C.c_int, [_P, C.c_int, _I, _I, _D]),
@@ -63,6 +64,7 @@ SIGNATURES = {
     "b200md_update_custom_external_params": (C.c_int, [_P, C.c_int, _D]),
     "b200md_update_custom_angle_params": (C.c_int, [_P, C.c_int, _D]),
     "b200md_update_custom_compound_params": (C.c_int, [_P, C.c_int, _D]),
+    "b200md_update_custom_centroid_params": (C.c_int, [_P, C.c_int, _D]),
     "b200md_custom_program_probe": (C.c_int, [C.c_int, _I, _I, _I, _D, C.c_int, C.c_int, C.c_int, C.c_double, _D, _D, _D,
                                               C.c_char_p, C.c_int]),
     "b200md_custom_term_probe": (C.c_int, [C.c_int, C.c_int, _I, _I, _I, _D, C.c_int, C.c_int, C.c_int, _D, _D, _D, _D, _D,

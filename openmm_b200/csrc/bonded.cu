@@ -1,6 +1,6 @@
 // bonded.cu -- harmonic bonds, harmonic angles, periodic torsions, Ryckaert-Bellemans torsions, CMAP terms, 1-4
 // exceptions and the Ewald exclusion correction in ONE launch (sm_90a); custom torsions, bonds, externals and angles in a
-// second launch behind it, custom compound bonds in a third.
+// second launch behind it, custom compound bonds in a third, custom centroid bonds in three more.
 // Double precision arithmetic on fp32 positions: these terms are a few thousand work items, far below any roofline, and
 // double removes them from the 1e-4 parity budget.
 //
@@ -12,6 +12,7 @@
 #include "engine.h"
 #include "custom_interp.h"
 #include "../../include/b200md.h"
+#include <algorithm>
 
 struct D3 { double x, y, z; };
 __device__ __forceinline__ D3 sub(const float4& a, const float4& b) { return {(double) a.x - b.x, (double) a.y - b.y, (double) a.z - b.z}; }
@@ -319,6 +320,35 @@ void launch_custom(const NbDev& nb, const CustomDev& ct, int terms, bool energy,
     launch_high(k_custom, (ct.nslots + 127)/128, 128, 0, s, nb, ct, terms, energy ? 1 : 0);
 }
 
+// Where k_compound's particles come from and where a derivative program's value goes.  CompoundAtoms: a particle is an
+// atom, read at its continuous coordinate (posq plus cellOffset lattice vectors, what b200md_get_positions reports), and minus
+// the derivative is added to its force at once.  CentroidCenters: a particle is a group centre of k_centroid_centers, and
+// derivative j of slot i is stored to deriv[i][j-1] for k_centroid_scatter, every one of them in every evaluation (a CONST 0
+// program stores 0), so that the scatter never reads a value of an earlier evaluation.
+struct CompoundAtoms {
+    static constexpr bool STORE_ALL = false;
+    __device__ __forceinline__ void coords(const NbDev& nb, int a, double* v) const {
+        const float4 x = nb.posq[a];
+        const int kx = nb.cellOffset[a], ky = nb.cellOffset[a + nb.npad], kz = nb.cellOffset[a + 2*nb.npad];
+        v[0] = x.x + (kx*nb.box.dax + ky*(double) nb.box.bx + kz*(double) nb.box.cx);
+        v[1] = x.y + (ky*nb.box.dby + kz*(double) nb.box.cy);
+        v[2] = x.z + kz*nb.box.dcz;
+    }
+    __device__ __forceinline__ void store(const NbDev& nb, const int* at, int i, int j, double r) const {
+        atomicAdd((unsigned long long*) &nb.force[at[(j-1)/3] + ((j-1) % 3)*nb.npad], (unsigned long long) __double2ll_rn(-r*B200MD_FORCE_SCALE));
+    }
+};
+struct CentroidCenters {
+    static constexpr bool STORE_ALL = true;
+    const double* center; double* deriv;
+    __device__ __forceinline__ void coords(const NbDev&, int g, double* v) const {
+        v[0] = center[3*g]; v[1] = center[3*g+1]; v[2] = center[3*g+2];
+    }
+    __device__ __forceinline__ void store(const NbDev&, const int*, int i, int j, double r) const {
+        deriv[(size_t) i*CENTROID_DERIVS + j - 1] = r;
+    }
+};
+
 // Custom compound bonds (restating ReferenceCustomCompoundBondIxn::calculateOneIxn): the energy is a function of the 3 N
 // coordinates of the term's N particles, the force on particle k minus the derivatives by its three.  One thread per (term,
 // program): warp W runs program W % COMPOUND_PROGRAMS (0 the energy, 1 + 3 k + c the derivative by coordinate c of particle
@@ -328,9 +358,11 @@ void launch_custom(const NbDev& nb, const CustomDev& ct, int terms, bool energy,
 // b200md_get_positions reports): an expression may read them directly, and a non-periodic restraint between two molecules
 // must not jump when the list build wraps one of them.  A derivative program that is the single instruction CONST 0 is not
 // run and adds nothing.  A kernel of its own: its interpreter holds a 32-deep stack and the three point functions, which
-// k_custom's terms never need.
+// k_custom's terms never need.  Src (CompoundAtoms, CentroidCenters above) says what a particle is: custom centroid bonds
+// run the same programs at group centres.
 #define COMPOUND_PROGRAMS (1 + 3*B200MD_CUSTOM_MAX_PARTICLES)
-__global__ void __launch_bounds__(128) k_compound(NbDev nb, CompoundDev cd, int wantEnergy) {
+template <class Src>
+__global__ void __launch_bounds__(128) k_compound(NbDev nb, CompoundDev cd, int wantEnergy, Src src) {
     const int warp = (blockIdx.x*blockDim.x + threadIdx.x) >> 5;
     const int j = warp % COMPOUND_PROGRAMS, i = (warp/COMPOUND_PROGRAMS)*32 + (threadIdx.x & 31);
     double e = 0;
@@ -343,20 +375,13 @@ __global__ void __launch_bounds__(128) k_compound(NbDev nb, CompoundDev cd, int 
                 const int* at = cd.atoms + B200MD_CUSTOM_MAX_PARTICLES*(size_t) i;
                 const CustomBox box = {nb.box.dax, nb.box.bx, nb.box.dby, nb.box.cx, nb.box.cy, nb.box.dcz};
                 double v[3*B200MD_CUSTOM_MAX_PARTICLES];
-                for (int k = 0; k < np; k++) {
-                    const int a = at[k];
-                    const float4 x = nb.posq[a];
-                    const int kx = nb.cellOffset[a], ky = nb.cellOffset[a + nb.npad], kz = nb.cellOffset[a + 2*nb.npad];
-                    v[3*k] = x.x + (kx*nb.box.dax + ky*(double) nb.box.bx + kz*(double) nb.box.cx);
-                    v[3*k+1] = x.y + (ky*nb.box.dby + kz*(double) nb.box.cy);
-                    v[3*k+2] = x.z + kz*nb.box.dcz;
-                }
+                for (int k = 0; k < np; k++) src.coords(nb, at[k], v + 3*k);
                 const double r = custom_run<B200MD_CUSTOM_COMPOUND_MAX_STACK, true>(cd.code, cd.imm, begin, end, v, cd.params + (size_t) i*cd.paramStride,
                                                                                     cd.globals, box, cd.exprPeriodic[p] != 0);
                 if (j == 0) e = r;
-                else
-                    atomicAdd((unsigned long long*) &nb.force[at[(j-1)/3] + ((j-1) % 3)*nb.npad], (unsigned long long) __double2ll_rn(-r*B200MD_FORCE_SCALE));
+                else src.store(nb, at, i, j, r);
             }
+            else if (Src::STORE_ALL) src.store(nb, nullptr, i, j, 0.0);
         }
     }
     if (wantEnergy) {
@@ -373,10 +398,51 @@ __global__ void __launch_bounds__(128) k_compound(NbDev nb, CompoundDev cd, int 
 
 void launch_compound(const NbDev& nb, const CompoundDev& cd, bool energy, cudaStream_t s) {
     const int warps = cd.nslots/32*COMPOUND_PROGRAMS;      // nslots is a whole number of warps
-    launch_high(k_compound, (warps + 3)/4, 128, 0, s, nb, cd, energy ? 1 : 0);
+    launch_high(k_compound<CompoundAtoms>, (warps + 3)/4, 128, 0, s, nb, cd, energy ? 1 : 0, CompoundAtoms{});
 }
 
-void launch_bonded(const NbDev& nb, const BondedDev& bd, const CustomDev& ct, const CompoundDev& cd, int terms, bool energy, cudaStream_t s) {
+// Custom centroid bonds (restating ReferenceCustomCentroidBondIxn::calculateIxn), in three kernels.  k_centroid_centers:
+// one warp per group, its lanes striding over the group's atoms, each summing w x of their continuous coordinates (those of
+// CompoundAtoms, so that a single-atom group of weight 1 is exactly its atom's coordinate), then a fixed xor-shuffle tree:
+// the centres do not depend on timing, bit for bit.  The programs: k_compound<CentroidCenters>.  k_centroid_scatter: one
+// thread per scatter entry (slot, position k of the group in the bond, atom, weight w; in slot order, weight-0 entries dropped
+// on the host), adding -w times the three derivatives by the centre of group k to the atom's force through the fixed-point
+// atomics, whose integer sums do not depend on their order.
+__global__ void __launch_bounds__(128) k_centroid_centers(NbDev nb, CentroidDev cn) {
+    const int g = (blockIdx.x*blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (g >= cn.ngroups) return;           // whole warps
+    double c[3] = {0.0, 0.0, 0.0};
+    for (int k = cn.groupStart[g] + lane; k < cn.groupStart[g+1]; k += 32) {
+        double x[3];
+        CompoundAtoms().coords(nb, cn.groupAtoms[k], x);
+        const double w = cn.groupWeight[k];
+        c[0] += w*x[0]; c[1] += w*x[1]; c[2] += w*x[2];
+    }
+    for (int off = 16; off > 0; off >>= 1)
+        for (int d = 0; d < 3; d++) c[d] += __shfl_xor_sync(0xffffffffu, c[d], off);
+    if (lane == 0) { cn.center[3*g] = c[0]; cn.center[3*g+1] = c[1]; cn.center[3*g+2] = c[2]; }
+}
+
+__global__ void __launch_bounds__(128) k_centroid_scatter(NbDev nb, CompoundDev cd, CentroidDev cn) {
+    const int t = blockIdx.x*blockDim.x + threadIdx.x;
+    if (t >= cn.nscatter) return;
+    const int4 s = cn.scatter[t];          // (slot, group position k, atom, 0)
+    if (!((cd.groupMask >> (cd.group[s.x] & 31)) & 1u)) return;
+    const double w = cn.scatterWeight[t];
+    const double* d = cn.deriv + (size_t) s.x*CENTROID_DERIVS + 3*s.y;
+    for (int c = 0; c < 3; c++)
+        atomicAdd((unsigned long long*) &nb.force[s.z + c*nb.npad], (unsigned long long) __double2ll_rn(-(w*d[c])*B200MD_FORCE_SCALE));
+}
+
+void launch_centroid(const NbDev& nb, const CompoundDev& cd, const CentroidDev& cn, bool energy, cudaStream_t s) {
+    launch_high(k_centroid_centers, (cn.ngroups + 3)/4, 128, 0, s, nb, cn);
+    const int warps = cd.nslots/32*COMPOUND_PROGRAMS;
+    launch_high(k_compound<CentroidCenters>, (warps + 3)/4, 128, 0, s, nb, cd, energy ? 1 : 0, CentroidCenters{cn.center, cn.deriv});
+    launch_high(k_centroid_scatter, std::max(1, (cn.nscatter + 127)/128), 128, 0, s, nb, cd, cn);
+}
+
+void launch_bonded(const NbDev& nb, const BondedDev& bd, const CustomDev& ct, const CompoundDev& cd, const CompoundDev& cc, const CentroidDev& cn,
+                   int terms, bool energy, cudaStream_t s) {
     int n = 0;
     if (terms & B200MD_TERM_BONDS) n += bd.nbonds;
     if (terms & B200MD_TERM_ANGLES) n += bd.nangles;
@@ -390,4 +456,5 @@ void launch_bonded(const NbDev& nb, const BondedDev& bd, const CustomDev& ct, co
     }
     if (terms & ct.terms) launch_custom(nb, ct, terms, energy, s);
     if ((terms & B200MD_TERM_CUSTOM_COMPOUND) && cd.nslots > 0) launch_compound(nb, cd, energy, s);
+    if ((terms & B200MD_TERM_CUSTOM_CENTROID) && cc.nslots > 0) launch_centroid(nb, cc, cn, energy, s);
 }

@@ -213,12 +213,14 @@ CUSTOM_HD double custom_run(const int2* code, const double* imm, int begin, int 
 // from -1 to their number of arguments - 1), PARAM operands < param_stride, GLOBAL operands < nglobals (nglobals < 0: not
 // checked yet), no stack underflow, depth <= the class's stack capacity, exactly one value left, at most
 // B200MD_CUSTOM_MAX_CODE instructions.  nullptr if the program passes, else the reason.  An opcode of another class's is an
-// unknown opcode for a torsion or an angle program, as is a POINT_* opcode for every class but the compound bond.
+// unknown opcode for a torsion or an angle program, as is a POINT_* opcode for every class but the compound bond.  A centroid
+// bond's program (of nparticles group centres) is checked as a compound bond's.
 inline const char* custom_check_program(int cls, const int2* code, int begin, int end, int param_stride, int nglobals, int nparticles = 0) {
     const bool torsion = cls == B200MD_CUSTOM_TORSION, bond = cls == B200MD_CUSTOM_BOND, angle = cls == B200MD_CUSTOM_ANGLE,
-               compound = cls == B200MD_CUSTOM_COMPOUND;
+               centroid = cls == B200MD_CUSTOM_CENTROID, compound = cls == B200MD_CUSTOM_COMPOUND || centroid;
 #define CUSTOM_WHY(what) (torsion ? "custom torsion program: " what : bond ? "custom bond program: " what : \
-                          angle ? "custom angle program: " what : compound ? "custom compound program: " what : "custom external program: " what)
+                          angle ? "custom angle program: " what : centroid ? "custom centroid program: " what : \
+                          compound ? "custom compound program: " what : "custom external program: " what)
     if (end <= begin) return CUSTOM_WHY("empty program");
     if (end - begin > B200MD_CUSTOM_MAX_CODE) return CUSTOM_WHY("more than 256 instructions");
     const int numVars = compound ? 3*nparticles : custom_num_vars(cls);

@@ -93,20 +93,30 @@ struct CustomClass {
     std::vector<double> imm, params; std::vector<unsigned char> group;
 };
 // The classes [first, last) one kernel runs, in its layout (finalize, layout_custom): k_custom the torsions, bonds, externals
-// and angles (CustomDev), k_compound the compound bonds (CompoundDev).
+// and angles (CustomDev), k_compound the compound bonds (CompoundDev), its centroid instantiation the centroid bonds (a second
+// CompoundDev).
 struct CustomSlots {
     int first, last;
     int nslots = 0, stride = 0;
     DevBuf<int> atomsDev, exprDev, exprClassDev, exprParticlesDev, exprPeriodicDev, exprProgDev, progStartDev;
     DevBuf<int2> codeDev; DevBuf<double> immDev, paramsDev; DevBuf<unsigned char> groupDev;
 };
+// The groups of the centroid bonds (CentroidDev): CSR over atoms with their normalised weights, as the set call got them; on the
+// device besides the centres, the derivatives per slot and the scatter entries (finalize, upload_custom)
+struct CentroidGroups {
+    std::vector<int> start, atoms; std::vector<double> weight;
+    DevBuf<int> startDev, atomsDev; DevBuf<double> weightDev, centerDev, derivDev, scatterWeightDev; DevBuf<int4> scatterDev;
+};
+enum { CUSTOM_CLASSES = 6 };
 // Every custom class and the global values (one slot space for all classes)
 struct CustomTable {
-    CustomClass cls[5];
-    CustomSlots kernel[2] = {{B200MD_CUSTOM_TORSION, B200MD_CUSTOM_COMPOUND}, {B200MD_CUSTOM_COMPOUND, B200MD_CUSTOM_COMPOUND + 1}};
+    CustomClass cls[CUSTOM_CLASSES];
+    CustomSlots kernel[3] = {{B200MD_CUSTOM_TORSION, B200MD_CUSTOM_COMPOUND}, {B200MD_CUSTOM_COMPOUND, B200MD_CUSTOM_COMPOUND + 1},
+                             {B200MD_CUSTOM_CENTROID, B200MD_CUSTOM_CENTROID + 1}};
+    CentroidGroups groups;
     std::vector<double> globals;
     DevBuf<double> globalsDev;
-    CustomSlots& kernel_of(int cls) { return kernel[cls == B200MD_CUSTOM_COMPOUND ? 1 : 0]; }
+    CustomSlots& kernel_of(int cls) { return kernel[cls == B200MD_CUSTOM_COMPOUND ? 1 : cls == B200MD_CUSTOM_CENTROID ? 2 : 0]; }
     // the params of the classes of s in its slot layout (padding slots 0)
     std::vector<double> slot_params(const CustomSlots& s) const {
         std::vector<double> p((size_t) s.nslots*s.stride, 0.0);
@@ -248,6 +258,8 @@ struct b200md_ctx {
     BondedDev bd{};
     CustomDev ctd{};
     CompoundDev cpd{};
+    CompoundDev ccd{};          // the centroid bonds' programs and slots
+    CentroidDev cen{};
     UnitDev units{};
     IntegDev integ{};
     bool haveIntegrator = false;
@@ -438,14 +450,15 @@ extern "C" int b200md_set_cmap(b200md_ctx* ctx, int nmaps, const int* size, cons
     API_END(ctx)
 }
 // What the custom classes differ in on the host: the names in the messages of their calls (what the set call counts: programs,
-// or expressions for compound bonds), the atoms per term, whether a term's atoms join the molecules that wrap together (not an
-// external's, which acts on one particle, nor a compound bond's, which reads continuous coordinates and may tie two molecules
-// that must keep wrapping apart), the term bit and the bonded kind.
+// or expressions for compound and centroid bonds), the atoms per term (a centroid bond's are groups), whether a term's atoms
+// join the molecules that wrap together (not an external's, which acts on one particle, nor a compound bond's, which reads
+// continuous coordinates and may tie two molecules that must keep wrapping apart, nor a centroid bond's, whose groups would
+// otherwise tie a protein to every water near it), the term bit and the bonded kind.
 struct CustomNames {
     const char* call; const char* term; const char* per; const char* unit; const char* update; const char* terms;
     int width; bool joins; int bit; int kind;
 };
-static const CustomNames CUSTOM_NAMES[5] = {
+static const CustomNames CUSTOM_NAMES[CUSTOM_CLASSES] = {
     {"set_custom_torsions", "custom torsion", "torsion", "program", "update_custom_torsion_params", "torsions", 4, true,
      B200MD_TERM_CUSTOM_TORSIONS, B200MD_BONDED_CUSTOM_TORSIONS},
     {"set_custom_bonds", "custom bond", "bond", "program", "update_custom_bond_params", "bonds", 2, true,
@@ -455,16 +468,20 @@ static const CustomNames CUSTOM_NAMES[5] = {
     {"set_custom_angles", "custom angle", "angle", "program", "update_custom_angle_params", "angles", 3, true,
      B200MD_TERM_CUSTOM_ANGLES, B200MD_BONDED_CUSTOM_ANGLES},
     {"set_custom_compound", "custom compound bond", "bond", "expression", "update_custom_compound_params", "bonds", B200MD_CUSTOM_MAX_PARTICLES, false,
-     B200MD_TERM_CUSTOM_COMPOUND, B200MD_BONDED_CUSTOM_COMPOUND}};
+     B200MD_TERM_CUSTOM_COMPOUND, B200MD_BONDED_CUSTOM_COMPOUND},
+    {"set_custom_centroid", "custom centroid bond", "bond", "expression", "update_custom_centroid_params", "bonds", B200MD_CUSTOM_MAX_PARTICLES, false,
+     B200MD_TERM_CUSTOM_CENTROID, B200MD_BONDED_CUSTOM_CENTROID}};
+// compound and centroid bonds: expressions of the coordinates of up to 8 particles (atoms or group centres) per term
+static bool custom_points(int cls) { return cls == B200MD_CUSTOM_COMPOUND || cls == B200MD_CUSTOM_CENTROID; }
 
-// A program set of class cls (b200md_set_custom_torsions / _bonds / _externals / _angles / _compound): nexpr expressions, the
-// programs of one after the other's (1 + the class's number of variables each; 1 + 3 nparticles[p] for compound bonds),
-// prog_start well formed and every program passing custom_check_program (nglobals < 0: GLOBAL operands are checked at
-// finalize).  Returns the instructions as (opcode, operand) and, in exprProg, every expression's first program and, last,
+// A program set of class cls (b200md_set_custom_torsions / _bonds / _externals / _angles / _compound / _centroid): nexpr
+// expressions, the programs of one after the other's (1 + the class's number of variables each; 1 + 3 nparticles[p] for
+// compound and centroid bonds), prog_start well formed and every program passing custom_check_program (nglobals < 0: GLOBAL
+// operands are checked at finalize).  Returns the instructions as (opcode, operand) and, in exprProg, every expression's first program and, last,
 // the number of programs.
 static std::vector<int2> check_programs(int cls, int nexpr, const int* nparticles, const int* prog_start, const int* op, const int* arg,
                                         int stride, int nglobals, std::vector<int>& exprProg) {
-    const bool compound = cls == B200MD_CUSTOM_COMPOUND;
+    const bool compound = custom_points(cls);
     const std::string call = CUSTOM_NAMES[cls].call;
     require(nexpr >= 0, (call + ": negative number of " + CUSTOM_NAMES[cls].unit + "s").c_str());
     require(stride >= 0 && stride <= B200MD_CUSTOM_MAX_PARAMS, (call + ": more than 16 parameters per " + CUSTOM_NAMES[cls].per).c_str());
@@ -472,7 +489,8 @@ static std::vector<int2> check_programs(int cls, int nexpr, const int* nparticle
     exprProg.assign(nexpr + 1, 0);
     for (int p = 0; p < nexpr; p++) {
         if (compound)
-            require(nparticles[p] >= 1 && nparticles[p] <= B200MD_CUSTOM_MAX_PARTICLES, (call + ": an expression must join 1 to 8 particles").c_str());
+            require(nparticles[p] >= 1 && nparticles[p] <= B200MD_CUSTOM_MAX_PARTICLES,
+                    (call + ": an expression must join 1 to 8 " + (cls == B200MD_CUSTOM_CENTROID ? "groups" : "particles")).c_str());
         exprProg[p+1] = exprProg[p] + 1 + (compound ? 3*nparticles[p] : custom_num_vars(cls));
     }
     const int nq = exprProg[nexpr];
@@ -488,11 +506,14 @@ static std::vector<int2> check_programs(int cls, int nexpr, const int* nparticle
     return code;
 }
 // The terms of class cls: term i evaluates expression expr[i] on the atoms atoms[w*i .. w*i+w-1] (w = the class's width; a
-// compound bond's unused slots -1).  nparticles and periodic (per expression) are read for compound bonds only.
+// compound bond's unused slots -1; a centroid bond's are groups, indices below nindex).  nparticles and periodic (per
+// expression) are read for compound and centroid bonds only.
 static void set_custom(b200md_ctx* ctx, int cls, int nexpr, const int* nparticles, const int* periodic, const int* prog_start, const int* op,
-                       const int* arg, const double* imm, int stride, int n, const int* expr, const int* atoms, const double* params) {
+                       const int* arg, const double* imm, int stride, int n, const int* expr, const int* atoms, const double* params,
+                       int nindex = -1) {
     const CustomNames& nm = CUSTOM_NAMES[cls];
-    const bool compound = cls == B200MD_CUSTOM_COMPOUND;
+    const bool compound = custom_points(cls), centroid = cls == B200MD_CUSTOM_CENTROID;
+    if (nindex < 0) nindex = ctx->natoms;
     check_set(ctx, nm.call, n);
     require(ctx->world == 1, (std::string(nm.term) + "s are not supported in multi-GPU runs").c_str());
     std::vector<int> exprProg;
@@ -502,8 +523,9 @@ static void set_custom(b200md_ctx* ctx, int cls, int nexpr, const int* nparticle
         require(expr[i] >= 0 && expr[i] < nexpr, (std::string(nm.term) + ": " + nm.unit + " index out of range").c_str());
         for (int k = 0; k < w; k++) {
             const int a = atoms[w*i + k];
-            if (!compound || k < nparticles[expr[i]]) require(a >= 0 && a < ctx->natoms, (std::string(nm.term) + ": atom index out of range").c_str());
-            else require(a == -1, "custom compound bond: an unused atom slot must be -1");
+            if (!compound || k < nparticles[expr[i]])
+                require(a >= 0 && a < nindex, (std::string(nm.term) + (centroid ? ": group" : ": atom") + " index out of range").c_str());
+            else require(a == -1, (std::string(nm.term) + (centroid ? ": an unused group" : ": an unused atom") + " slot must be -1").c_str());
         }
     }
     CustomClass& t = ctx->custom.cls[cls];            // its group stays: groups may come before the terms
@@ -548,6 +570,25 @@ extern "C" int b200md_set_custom_compound(b200md_ctx* ctx, int nexpr, const int*
     set_custom(ctx, B200MD_CUSTOM_COMPOUND, nexpr, nparticles, periodic, prog_start, op, arg, imm, stride, n, expr, atoms, params);
     API_END(ctx)
 }
+extern "C" int b200md_set_custom_centroid(b200md_ctx* ctx, int nexpr, const int* ngroups_per_bond, const int* periodic, const int* prog_start,
+                                          const int* op, const int* arg, const double* imm, int stride, int n, const int* expr,
+                                          const int* groups, const double* params, int ngroups, const int* group_start,
+                                          const int* group_atoms, const double* group_weights) {
+    API_BEGIN(ctx)
+    check_set(ctx, "set_custom_centroid", ngroups);
+    require(ngroups == 0 || group_start[0] == 0, "set_custom_centroid: group_start[0] must be 0");
+    for (int g = 0; g < ngroups; g++) require(group_start[g+1] > group_start[g], "custom centroid bond: a group must hold at least one atom");
+    const int total = ngroups ? group_start[ngroups] : 0;
+    for (int k = 0; k < total; k++) {
+        require(group_atoms[k] >= 0 && group_atoms[k] < ctx->natoms, "custom centroid bond: atom index of a group out of range");
+        require(std::isfinite(group_weights[k]), "custom centroid bond: a group weight is not finite");
+    }
+    set_custom(ctx, B200MD_CUSTOM_CENTROID, nexpr, ngroups_per_bond, periodic, prog_start, op, arg, imm, stride, n, expr, groups, params, ngroups);
+    CentroidGroups& g = ctx->custom.groups;
+    g.start.assign(group_start, group_start + (ngroups ? ngroups + 1 : 0));
+    g.atoms.assign(group_atoms, group_atoms + total); g.weight.assign(group_weights, group_weights + total);
+    API_END(ctx)
+}
 extern "C" int b200md_set_custom_globals(b200md_ctx* ctx, int n, const double* values) {
     API_BEGIN(ctx)
     require(n >= 0, "set_custom_globals: negative count");
@@ -571,7 +612,7 @@ static int custom_probe(const char* name, int cls, int nexpr, const int* npartic
         require(which >= 0 && which < exprProg[nexpr], (std::string(name) + ": program index out of range").c_str());
         CustomBox b = {1.0, 0.0, 1.0, 0.0, 0.0, 1.0};
         if (box) b = CustomBox{box[0], box[3], box[4], box[6], box[7], box[8]};
-        *out = cls == B200MD_CUSTOM_COMPOUND
+        *out = custom_points(cls)
             ? custom_run<B200MD_CUSTOM_COMPOUND_MAX_STACK, true>(code.data(), imm, prog_start[which], prog_start[which+1], vars, params, globals, b,
                                                                   periodic != 0)
             : custom_run<B200MD_CUSTOM_MAX_STACK, false>(code.data(), imm, prog_start[which], prog_start[which+1], vars, params, globals, b);
@@ -608,13 +649,13 @@ extern "C" int b200md_set_bonded_groups(b200md_ctx* ctx, int kind, int n, const 
     API_BEGIN(ctx)
     check_set(ctx, "set_bonded_groups", n);
     require((kind >= B200MD_BONDED_BONDS && kind <= B200MD_BONDED_CUSTOM_EXTERNALS) || kind == B200MD_BONDED_CUSTOM_ANGLES ||
-            kind == B200MD_BONDED_CUSTOM_COMPOUND,
+            kind == B200MD_BONDED_CUSTOM_COMPOUND || kind == B200MD_BONDED_CUSTOM_CENTROID,
             "set_bonded_groups: kind must be 0 (bonds), 1 (angles), 2 (torsions), 3 (RB torsions), 4 (CMAP), 5 (custom torsions), "
-            "6 (custom bonds), 7 (custom externals), 9 (custom angles) or 10 (custom compound bonds)");
+            "6 (custom bonds), 7 (custom externals), 9 (custom angles), 10 (custom compound bonds) or 11 (custom centroid bonds)");
     std::vector<unsigned char>* g = kind == B200MD_BONDED_BONDS ? &ctx->bonds.group : kind == B200MD_BONDED_ANGLES ? &ctx->angles.group :
                                     kind == B200MD_BONDED_TORSIONS ? &ctx->torsions.group : kind == B200MD_BONDED_RB_TORSIONS ? &ctx->rb.group :
                                     &ctx->cmap.group;
-    for (int k = 0; k < 5; k++) if (kind == CUSTOM_NAMES[k].kind) g = &ctx->custom.cls[k].group;
+    for (int k = 0; k < CUSTOM_CLASSES; k++) if (kind == CUSTOM_NAMES[k].kind) g = &ctx->custom.cls[k].group;
     g->resize(n);
     for (int i = 0; i < n; i++) { require(group[i] >= 0 && (group[i] & ~0x80) < 32, "force group out of range"); (*g)[i] = (unsigned char) group[i]; }
     API_END(ctx)
@@ -1404,7 +1445,7 @@ static bool fft_beside_tiles(const b200md_ctx* c) {
 static int layout_custom(b200md_ctx* c, CustomSlots& s, int width, int pad) {
     CustomTable& t = c->custom;
     std::vector<int2> code; std::vector<double> imm;
-    std::vector<int> progStart(1, 0), exprClass, exprParticles, exprPeriodic, exprProg, exprBase(5, 0);
+    std::vector<int> progStart(1, 0), exprClass, exprParticles, exprPeriodic, exprProg, exprBase(CUSTOM_CLASSES, 0);
     int terms = 0;
     s.nslots = 0; s.stride = 0;
     for (int k = s.first; k < s.last; k++) {
@@ -1456,8 +1497,53 @@ static int layout_custom(b200md_ctx* c, CustomSlots& s, int width, int pad) {
     return terms;
 }
 
+// finalize: the classes of s in the layout of k_compound (CompoundDev: 8 atoms, or groups, per slot, unused -1)
+static void layout_compound(b200md_ctx* c, CustomSlots& u, CompoundDev& e) {
+    e = CompoundDev{};
+    e.groupMask = 0xffffffffu;
+    e.globals = c->custom.globalsDev.p;
+    layout_custom(c, u, B200MD_CUSTOM_MAX_PARTICLES, -1);
+    e.nslots = u.nslots; e.paramStride = u.stride;
+    e.atoms = u.atomsDev.p; e.params = u.paramsDev.p; e.group = u.groupDev.p; e.expr = u.exprDev.p;
+    e.exprParticles = u.exprParticlesDev.p; e.exprPeriodic = u.exprPeriodicDev.p; e.exprProg = u.exprProgDev.p;
+    e.code = u.codeDev.p; e.imm = u.immDev.p; e.progStart = u.progStartDev.p;
+}
+
+// finalize: the centroid bonds' groups (CentroidDev): the CSR, room for the centres and the derivatives of every slot, and
+// the scatter entries in slot order, (slot, group position k, atom) of every atom of weight != 0 of every group of every term
+static void upload_centroid(b200md_ctx* c) {
+    CustomTable& t = c->custom;
+    CentroidGroups& g = t.groups;
+    CentroidDev& d = c->cen;
+    d = CentroidDev{};
+    if (c->ccd.nslots == 0) return;
+    const CustomClass& cl = t.cls[B200MD_CUSTOM_CENTROID];
+    const int nslots = c->ccd.nslots;
+    std::vector<int> termOf(nslots, -1);
+    for (int i = 0; i < cl.n; i++) termOf[cl.slot[i]] = i;
+    std::vector<int4> scatter; std::vector<double> weight;
+    for (int s = 0; s < nslots; s++) {
+        const int i = termOf[s];
+        if (i < 0) continue;
+        for (int k = 0; k < cl.nparticles[cl.expr[i]]; k++) {
+            const int grp = cl.atoms[B200MD_CUSTOM_MAX_PARTICLES*(size_t) i + k];
+            for (int a = g.start[grp]; a < g.start[grp+1]; a++)
+                if (g.weight[a] != 0.0) { scatter.push_back(make_int4(s, k, g.atoms[a], 0)); weight.push_back(g.weight[a]); }
+        }
+    }
+    const int ngroups = (int) g.start.size() - 1;
+    g.startDev.upload(g.start); g.atomsDev.upload(g.atoms); g.weightDev.upload(g.weight);
+    g.centerDev.alloc(3*(size_t) ngroups); g.centerDev.zero();
+    g.derivDev.alloc((size_t) nslots*CENTROID_DERIVS); g.derivDev.zero();
+    g.scatterDev.upload(scatter); g.scatterWeightDev.upload(weight);
+    d.ngroups = ngroups; d.nscatter = (int) scatter.size();
+    d.groupStart = g.startDev.p; d.groupAtoms = g.atomsDev.p; d.groupWeight = g.weightDev.p;
+    d.center = g.centerDev.p; d.deriv = g.derivDev.p;
+    d.scatter = g.scatterDev.p; d.scatterWeight = g.scatterWeightDev.p;
+}
+
 // finalize: the custom terms in the layouts of k_custom (CustomDev: int4 atoms, zero-padded) and k_compound (CompoundDev: 8
-// atoms per slot, unused -1), and the global values both read
+// atoms per slot, unused -1; the centroid bonds in a second one), and the global values all read
 static void upload_custom(b200md_ctx* c) {
     CustomTable& t = c->custom;
     // the global values get their buffer even without terms: a custom force with no terms may still name globals, and
@@ -1473,16 +1559,9 @@ static void upload_custom(b200md_ctx* c) {
     d.atoms = (const int4*) s.atomsDev.p; d.params = s.paramsDev.p; d.group = s.groupDev.p; d.expr = s.exprDev.p;
     d.exprClass = s.exprClassDev.p; d.exprProg = s.exprProgDev.p;
     d.code = s.codeDev.p; d.imm = s.immDev.p; d.progStart = s.progStartDev.p;
-    CustomSlots& u = t.kernel[1];
-    CompoundDev& e = c->cpd;
-    e = CompoundDev{};
-    e.groupMask = 0xffffffffu;
-    e.globals = t.globalsDev.p;
-    layout_custom(c, u, B200MD_CUSTOM_MAX_PARTICLES, -1);
-    e.nslots = u.nslots; e.paramStride = u.stride;
-    e.atoms = u.atomsDev.p; e.params = u.paramsDev.p; e.group = u.groupDev.p; e.expr = u.exprDev.p;
-    e.exprParticles = u.exprParticlesDev.p; e.exprPeriodic = u.exprPeriodicDev.p; e.exprProg = u.exprProgDev.p;
-    e.code = u.codeDev.p; e.imm = u.immDev.p; e.progStart = u.progStartDev.p;
+    layout_compound(c, t.kernel[1], c->cpd);
+    layout_compound(c, t.kernel[2], c->ccd);
+    upload_centroid(c);
 }
 
 extern "C" int b200md_finalize(b200md_ctx* ctx) {
@@ -1603,8 +1682,8 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
         }
     }
     // ---- molecules (connected components of bonds, angles, torsions, RB torsions, CMAP terms, custom torsions, bonds and
-    // angles, constraints and exceptions; not custom externals, which act on one particle, nor custom compound bonds, which
-    // read continuous coordinates and may tie two molecules that must keep wrapping apart) for the wrap at list
+    // angles, constraints and exceptions; not custom externals, which act on one particle, nor custom compound and centroid
+    // bonds, which read continuous coordinates and may tie two molecules that must keep wrapping apart) for the wrap at list
     // builds; off for non-periodic systems and with more than one rank (every rank would have to wrap in the same step,
     // and the reciprocal-space rank builds no list) ----
     c->cellOffset.alloc((size_t) 3*NP); c->cellOffset.zero();
@@ -1617,7 +1696,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
         for (const int2& a : c->bonds.atoms) join(a.x, a.y);
         for (const int4& a : c->angles.atoms) { join(a.x, a.y); join(a.y, a.z); }
         for (auto* t : {&c->torsions.atoms, &c->rb.atoms, &c->cmap.atoms}) for (const int4& a : *t) { join(a.x, a.y); join(a.y, a.z); join(a.z, a.w); }
-        for (int k = 0; k < 5; k++) {
+        for (int k = 0; k < CUSTOM_CLASSES; k++) {
             const CustomClass& cl = c->custom.cls[k];
             const int w = CUSTOM_NAMES[k].width;
             if (CUSTOM_NAMES[k].joins)
@@ -1715,7 +1794,7 @@ extern "C" int b200md_update_cmap_params(b200md_ctx* ctx, int nmaps, const int* 
     API_END(ctx)
 }
 
-// CalcCustom{Torsion,Bond,External,Angle,CompoundBond}ForceKernel::copyParametersToContext (kernels.h): same terms and
+// CalcCustom{Torsion,Bond,External,Angle,CompoundBond,CentroidBond}ForceKernel::copyParametersToContext (kernels.h): same terms and
 // programs, new parameters, into the same device buffer.
 static void update_custom(b200md_ctx* ctx, int cls, int n, const double* params) {
     const CustomNames& nm = CUSTOM_NAMES[cls];
@@ -1751,6 +1830,11 @@ extern "C" int b200md_update_custom_angle_params(b200md_ctx* ctx, int n, const d
 extern "C" int b200md_update_custom_compound_params(b200md_ctx* ctx, int n, const double* params) {
     API_BEGIN(ctx)
     update_custom(ctx, B200MD_CUSTOM_COMPOUND, n, params);
+    API_END(ctx)
+}
+extern "C" int b200md_update_custom_centroid_params(b200md_ctx* ctx, int n, const double* params) {
+    API_BEGIN(ctx)
+    update_custom(ctx, B200MD_CUSTOM_CENTROID, n, params);
     API_END(ctx)
 }
 
@@ -1961,18 +2045,19 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     const bool direct = (terms & B200MD_TERM_NB_DIRECT) && c->haveNb && !pmeRank;
     const bool recip = (terms & B200MD_TERM_NB_RECIP) && c->haveNb && c->nb.method == B200MD_NB_PME && !directRank;
     const int customBits = B200MD_TERM_CUSTOM_TORSIONS | B200MD_TERM_CUSTOM_BONDS | B200MD_TERM_CUSTOM_EXTERNALS | B200MD_TERM_CUSTOM_ANGLES |
-                           B200MD_TERM_CUSTOM_COMPOUND;
+                           B200MD_TERM_CUSTOM_COMPOUND | B200MD_TERM_CUSTOM_CENTROID;
     int bterms = terms & (B200MD_TERM_BONDS | B200MD_TERM_ANGLES | B200MD_TERM_TORSIONS | B200MD_TERM_RB_TORSIONS | B200MD_TERM_CMAP |
                           customBits);
     if (c->haveNb) bterms |= terms & B200MD_TERM_NB_DIRECT;
     const int nbonded = c->bd.nbonds + c->bd.nangles + c->bd.ntorsions + c->bd.nrb + c->bd.ncmap + c->bd.nexc;
     // the k_bonded branch is counted as one launch whenever it is taken (even when the selected classes have no terms and
     // launch_bonded skips the kernel); k_custom is counted once when it runs, for any number of custom classes, k_compound
-    // once when it runs
+    // once when it runs, the three centroid kernels when they run
     const bool classic = (bterms & ~customBits) && nbonded > 0;
     const bool custom = (bterms & c->ctd.terms) != 0;
     const bool compound = (bterms & B200MD_TERM_CUSTOM_COMPOUND) && c->cpd.nslots > 0;
-    const bool bonded = (classic || custom || compound) && !pmeRank;
+    const bool centroid = (bterms & B200MD_TERM_CUSTOM_CENTROID) && c->ccd.nslots > 0;
+    const bool bonded = (classic || custom || compound || centroid) && !pmeRank;
     // Reciprocal space (spread -> FFT/convolution -> gather, in USER atom order: independent of the neighbour list) and
     // direct space (list check / rebuild, tile kernel, bonded terms) are independent until the integrator: fork them onto
     // two streams (also inside the captured step graph).  Both accumulate into the same fixed-point force buffer, so the
@@ -2011,8 +2096,9 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
         BondedDev bd = c->bd; bd.groupMask = groupMask;
         CustomDev ct = c->ctd; ct.groupMask = groupMask;
         CompoundDev cp = c->cpd; cp.groupMask = groupMask;
-        launch_bonded(c->nb, bd, ct, cp, bterms, energy, sb);
-        launches += (classic ? 1 : 0) + (custom ? 1 : 0) + (compound ? 1 : 0);
+        CompoundDev cc = c->ccd; cc.groupMask = groupMask;
+        launch_bonded(c->nb, bd, ct, cp, cc, c->cen, bterms, energy, sb);
+        launches += (classic ? 1 : 0) + (custom ? 1 : 0) + (compound ? 1 : 0) + (centroid ? CENTROID_LAUNCHES : 0);
     };
 
     // ---- the schedule, in stream order ----
@@ -2139,7 +2225,7 @@ extern "C" int b200md_compute_groups(b200md_ctx* ctx, int terms, unsigned int bo
         if (terms & B200MD_TERM_RB_TORSIONS) e += h[EN_RBTORSION];
         if (terms & B200MD_TERM_CMAP) e += h[EN_CMAP];
         if (terms & (B200MD_TERM_CUSTOM_TORSIONS | B200MD_TERM_CUSTOM_BONDS | B200MD_TERM_CUSTOM_EXTERNALS | B200MD_TERM_CUSTOM_ANGLES |
-                     B200MD_TERM_CUSTOM_COMPOUND)) e += h[EN_CUSTOM];
+                     B200MD_TERM_CUSTOM_COMPOUND | B200MD_TERM_CUSTOM_CENTROID)) e += h[EN_CUSTOM];
         if (ctx->haveNb) {
             if (terms & B200MD_TERM_NB_DIRECT) {
                 e += h[EN_NB] + h[EN_EXC];
@@ -2409,6 +2495,7 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
     Snapshot state, counter;
     require(phase != 7 || c->ctd.nslots > 0, "time_phase(custom torsions): the System has none");
     require(phase != 8 || c->cpd.nslots > 0, "time_phase(custom compound bonds): the System has none");
+    require(phase != 9 || c->ccd.nslots > 0, "time_phase(custom centroid bonds): the System has none");
     if (phase == 4) {
         require(c->haveIntegrator, "time_phase(integrate) before set_integrator");
         state.parts = state_spans(c, ST_POS | ST_VEL); state.save(s);
@@ -2426,9 +2513,10 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
             case 3: launch_pme_gather(c->nb, pme_for_launch(c), local, s); break;
             case 4: launch_integrate(c->nb, c->units, c->integ, local, s); break;
             case 5: launch_list_build(c->nb, s); break;
-            case 6: launch_bonded(c->nb, c->bd, c->ctd, c->cpd, B200MD_TERM_ALL, false, s); break;
+            case 6: launch_bonded(c->nb, c->bd, c->ctd, c->cpd, c->ccd, c->cen, B200MD_TERM_ALL, false, s); break;
             case 7: launch_custom(c->nb, c->ctd, B200MD_TERM_ALL, false, s); break;
             case 8: launch_compound(c->nb, c->cpd, false, s); break;
+            case 9: launch_centroid(c->nb, c->ccd, c->cen, false, s); break;
             default: throw std::runtime_error("unknown phase");
         }
         CUDA_CHECK(cudaEventRecord(e1, s));

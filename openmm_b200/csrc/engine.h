@@ -228,6 +228,19 @@ struct CompoundDev {
     unsigned int groupMask;
 };
 
+// Custom centroid bonds: their terms are laid out as compound bonds (a second CompoundDev, a slot's "atoms" its groups) and
+// this holds what the groups add (k_centroid_centers, k_centroid_scatter, bonded.cu).  Group g is the atoms
+// groupAtoms[groupStart[g] .. groupStart[g+1]-1] with their normalised weights; center[3g ..] its centre, recomputed every
+// evaluation; deriv[slot][j-1] the value of derivative program j of the slot's term (CENTROID_DERIVS per slot); scatter[e] =
+// (slot, group position k in the term, atom, 0) with weight scatterWeight[e], in slot order.
+#define CENTROID_DERIVS (3*B200MD_CUSTOM_MAX_PARTICLES)
+struct CentroidDev {
+    int ngroups, nscatter;
+    const int* groupStart; const int* groupAtoms; const double* groupWeight;
+    double* center; double* deriv;
+    const int4* scatter; const double* scatterWeight;
+};
+
 // One integration unit = a SETTLE water, a SHAKE cluster (centre + <=3 H) or a free atom.
 struct UnitDev {
     int nunits;
@@ -507,10 +520,14 @@ size_t fft_cta_smem_bytes(const PmeDev& pme);  // largest shared memory of one s
 bool fft_slab_path(const PmeDev& pme);          // the 3-launch slab pipeline is usable for this grid (precondition of the multi-GPU FFT)
 
 // k_bonded (when the classes in `terms` have terms), when a custom class in `terms` has terms (CustomDev::terms) k_custom
-// behind it on the same stream, and when there are compound bonds and their bit is in `terms`, k_compound behind that
-void launch_bonded(const NbDev& nb, const BondedDev& bd, const CustomDev& ct, const CompoundDev& cd, int terms, bool energy, cudaStream_t s);
+// behind it on the same stream, when there are compound bonds (cd) and their bit is in `terms`, k_compound behind that, and
+// when there are centroid bonds (cc, cn) and their bit is in `terms`, the three centroid kernels last
+void launch_bonded(const NbDev& nb, const BondedDev& bd, const CustomDev& ct, const CompoundDev& cd, const CompoundDev& cc, const CentroidDev& cn,
+                   int terms, bool energy, cudaStream_t s);
 void launch_custom(const NbDev& nb, const CustomDev& ct, int terms, bool energy, cudaStream_t s);
 void launch_compound(const NbDev& nb, const CompoundDev& cd, bool energy, cudaStream_t s);
+const int CENTROID_LAUNCHES = 3;
+void launch_centroid(const NbDev& nb, const CompoundDev& cc, const CentroidDev& cn, bool energy, cudaStream_t s);     // centres, programs, scatter
 
 void launch_integrate(const NbDev& nb, const UnitDev& units, const IntegDev& integ, const CommDev& cd, cudaStream_t s);
 void launch_force_push(const NbDev& nb, const CommDev& cd, cudaStream_t s);          // partial forces of foreign atoms -> owners' inboxes

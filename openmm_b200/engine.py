@@ -7,12 +7,13 @@ from .systems import SystemDesc, NB_PME
 
 TERM_BONDS, TERM_ANGLES, TERM_TORSIONS, TERM_NB_DIRECT, TERM_NB_RECIP = 1, 2, 4, 8, 16
 TERM_RB_TORSIONS, TERM_CMAP, TERM_CUSTOM_TORSIONS = 32, 64, 128
-TERM_CUSTOM_BONDS, TERM_CUSTOM_EXTERNALS, TERM_CUSTOM_ANGLES, TERM_CUSTOM_COMPOUND, TERM_ALL = 256, 512, 1024, 2048, 4095
+TERM_CUSTOM_BONDS, TERM_CUSTOM_EXTERNALS, TERM_CUSTOM_ANGLES, TERM_CUSTOM_COMPOUND = 256, 512, 1024, 2048
+TERM_CUSTOM_CENTROID, TERM_ALL = 4096, 8191
 # kinds of b200md_set_bonded_groups
 BONDED_KINDS = {"bonds": 0, "angles": 1, "torsions": 2, "rb_torsions": 3, "cmap": 4, "custom_torsions": 5, "custom_bonds": 6,
-                "custom_externals": 7, "custom_angles": 9, "custom_compound": 10}
+                "custom_externals": 7, "custom_angles": 9, "custom_compound": 10, "custom_centroid": 11}
 PHASES = {"pair": 0, "pme_spread": 1, "pme_fft_conv": 2, "pme_gather": 3, "integrate": 4, "list_build": 5, "bonded": 6,
-          "custom_torsions": 7, "custom_compound": 8}
+          "custom_torsions": 7, "custom_compound": 8, "custom_centroid": 9}
 
 
 class EngineError(RuntimeError):
@@ -105,13 +106,15 @@ class Engine:
                                        _ip(_i32(d.cmap_map)), _ip(_i32(d.cmap_atoms))))
         # the custom classes: field prefix, field of each term's expression, programs per expression (E and dE/dtheta, E and
         # dE/dr, E and dE/dx, dE/dy, dE/dz, E and dE/dtheta; a compound bond's E and its derivatives by every coordinate of its
-        # particles, whose number and periodic flag per expression its call also takes), what messages call the terms
+        # particles, whose number and periodic flag per expression its call also takes; a centroid bond's likewise, by the
+        # coordinates of its group centres, and its call also takes the groups), what messages call the terms
         for prefix, expr_field, nprog, name, call in (
                 ("custom", "_prog", 2, "custom torsions", L.b200md_set_custom_torsions),
                 ("cbond", "_prog", 2, "custom bonds", L.b200md_set_custom_bonds),
                 ("cext", "_prog", 4, "custom externals", L.b200md_set_custom_externals),
                 ("cangle", "_prog", 2, "custom angles", L.b200md_set_custom_angles),
-                ("ccompound", "_expr", None, "custom compound bonds", L.b200md_set_custom_compound)):
+                ("ccompound", "_expr", None, "custom compound bonds", L.b200md_set_custom_compound),
+                ("ccentroid", "_expr", None, "custom centroid bonds", L.b200md_set_custom_centroid)):
             expr = getattr(d, prefix + expr_field)
             if not len(expr):
                 continue
@@ -121,12 +124,17 @@ class Engine:
                                   "plugin's expression translator)" % (name, prefix, prefix, prefix, prefix, prefix))
             params = _f64(getattr(d, prefix + "_params")).reshape(len(expr), -1)
             atoms = _i32(getattr(d, prefix + "_atoms")).reshape(len(expr), -1)
+            tail = ()
             if nprog is None:
-                head = (len(d.ccompound_particles), _ip(_i32(d.ccompound_particles)), _ip(_i32(d.ccompound_periodic)))
+                npart = getattr(d, prefix + ("_groups_per_bond" if prefix == "ccentroid" else "_particles"))
+                head = (len(npart), _ip(_i32(npart)), _ip(_i32(getattr(d, prefix + "_periodic"))))
             else:
                 head = ((len(start) - 1)//nprog,)
+            if prefix == "ccentroid":
+                gs = _i32(d.ccentroid_group_start)
+                tail = (len(gs) - 1, _ip(gs), _ip(_i32(d.ccentroid_group_atoms)), _dp(_f64(d.ccentroid_group_weights)))
             self._ck(call(self.h, *head, _ip(_i32(start)), _ip(_i32(op)), _ip(_i32(arg)), _dp(_f64(imm)), params.shape[1], len(expr),
-                          _ip(_i32(expr)), _ip(atoms), _dp(params)))
+                          _ip(_i32(expr)), _ip(atoms), _dp(params), *tail))
         if len(d.custom_global_values):
             self._ck(L.b200md_set_custom_globals(self.h, len(d.custom_global_values), _dp(_f64(d.custom_global_values))))
         for kind, g in self._bonded_groups.items():
@@ -225,7 +233,7 @@ class Engine:
         size, coeff, cmap_map = _i32(size), _f64(coeff), _i32(cmap_map)
         self._ck(self.lib.b200md_update_cmap_params(self.h, len(size), _ip(size), _dp(coeff), len(cmap_map), _ip(cmap_map)))
 
-    # ---- CalcCustom{Torsion,Bond,External,Angle,CompoundBond}ForceKernel::copyParametersToContext and the global parameters ----
+    # ---- CalcCustom{Torsion,Bond,External,Angle,CompoundBond,CentroidBond}ForceKernel::copyParametersToContext and the globals ----
     def _update_custom(self, call, params):
         p = _f64(params)
         self._ck(call(self.h, len(p), _dp(p)))
@@ -249,6 +257,10 @@ class Engine:
     def update_custom_compound_params(self, params):
         """New per-bond parameters [n, param_stride] for the same custom compound bonds and expressions."""
         self._update_custom(self.lib.b200md_update_custom_compound_params, params)
+
+    def update_custom_centroid_params(self, params):
+        """New per-bond parameters [n, param_stride] for the same custom centroid bonds, groups and expressions."""
+        self._update_custom(self.lib.b200md_update_custom_centroid_params, params)
 
     def set_custom_globals(self, values):
         """The values of the global parameter slots the expressions read (the number of slots is fixed at definition)."""

@@ -133,6 +133,27 @@ class SystemDesc:
     ccompound_op: np.ndarray = field(default_factory=_i)
     ccompound_arg: np.ndarray = field(default_factory=_i)
     ccompound_imm: np.ndarray = field(default_factory=_d)
+    # CustomCentroidBondForce (ccentroid_*), laid out as the compound bonds with groups for particles: per expression its
+    # energy (of g1.., x1, y1, z1, .., distance, angle, dihedral and the point functions), parameter names, groups per bond (at
+    # most 8) and periodic flag; per term its expression, groups ([n,8], unused slots -1) and parameters.  The groups: CSR
+    # (group_start, group_atoms) with the normalised weights of CustomCentroidBondForceImpl::computeNormalizedWeights, and per
+    # group whether its Force gives no weights (mass weighted: the weights are the atoms' masses, normalised).  The programs
+    # are those of a compound bond of the same expression over x1.. of the group centres.
+    ccentroid_energy: tuple = ()
+    ccentroid_param_names: tuple = ()
+    ccentroid_groups_per_bond: np.ndarray = field(default_factory=_i)
+    ccentroid_periodic: np.ndarray = field(default_factory=_i)
+    ccentroid_expr: np.ndarray = field(default_factory=_i)
+    ccentroid_atoms: np.ndarray = field(default_factory=lambda: np.full((0, 8), -1, dtype=np.int32))
+    ccentroid_params: np.ndarray = field(default_factory=lambda: np.zeros((0, 0)))
+    ccentroid_group_start: np.ndarray = field(default_factory=lambda: np.zeros(1, dtype=np.int32))
+    ccentroid_group_atoms: np.ndarray = field(default_factory=_i)
+    ccentroid_group_weights: np.ndarray = field(default_factory=_d)
+    ccentroid_group_mass: np.ndarray = field(default_factory=_i)
+    ccentroid_prog_start: np.ndarray = field(default_factory=_i)
+    ccentroid_op: np.ndarray = field(default_factory=_i)
+    ccentroid_arg: np.ndarray = field(default_factory=_i)
+    ccentroid_imm: np.ndarray = field(default_factory=_d)
     con_i: np.ndarray = field(default_factory=_i)
     con_j: np.ndarray = field(default_factory=_i)
     con_d: np.ndarray = field(default_factory=_d)
@@ -193,7 +214,8 @@ class SystemDesc:
         return d
 
     def save(self, path):
-        names = ("custom_param_names", "cbond_param_names", "cext_param_names", "cangle_param_names", "ccompound_param_names")
+        names = ("custom_param_names", "cbond_param_names", "cext_param_names", "cangle_param_names", "ccompound_param_names",
+                 "ccentroid_param_names")
         d = {k: (np.asarray(v) if v is not None else np.zeros(0)) for k, v in self.__dict__.items()
              if not isinstance(v, str) and k not in names}
         for k in names:
@@ -211,9 +233,11 @@ class SystemDesc:
             v = z[k]
             if k == "name":
                 kw[k] = str(v)
-            elif k in ("custom_energy", "custom_global_names", "cbond_energy", "cext_energy", "cangle_energy", "ccompound_energy"):
+            elif k in ("custom_energy", "custom_global_names", "cbond_energy", "cext_energy", "cangle_energy", "ccompound_energy",
+                       "ccentroid_energy"):
                 kw[k] = tuple(str(x) for x in v)
-            elif k in ("custom_param_names", "cbond_param_names", "cext_param_names", "cangle_param_names", "ccompound_param_names"):
+            elif k in ("custom_param_names", "cbond_param_names", "cext_param_names", "cangle_param_names", "ccompound_param_names",
+                       "ccentroid_param_names"):
                 kw[k] = tuple(tuple(str(y) for y in x if str(y)) for x in v)
             elif k == "box":
                 kw[k] = v if v.size == 9 else None
@@ -419,6 +443,92 @@ def with_orientational_restraint(desc, atoms6, kr=4000.0, ka=400.0, kd=400.0, of
     ref = [np.linalg.norm(x[2] - x[3]) + offset, ang(1, 2, 3) + offset, ang(2, 3, 4) + offset] + [t + offset for t in dih]
     return _add_compound(desc, ORIENTATIONAL_RESTRAINT, ORIENTATIONAL_PARAMS, 6, periodic, np.asarray(atoms6).reshape(1, 6),
                          np.array([[kr, ka, kd] + ref]))
+
+
+def compound_to_centroid(desc):
+    """The same System with every CustomCompoundBondForce bond written as a CustomCentroidBondForce bond of the same expression
+    (p1.. become g1..) over single-atom groups of weight 1, one group per particle of every bond: each group centre is its
+    atom's coordinate, bit for bit"""
+    import copy
+    import re
+    d = copy.copy(desc)
+    ex = np.asarray(desc.ccompound_expr, dtype=np.int64)
+    npart = np.asarray(desc.ccompound_particles, dtype=np.int64)
+    atoms = np.asarray(desc.ccompound_atoms, dtype=np.int32).reshape(-1, 8)
+    groups = np.full((len(ex), 8), -1, dtype=np.int32)
+    flat = []
+    for i, p in enumerate(ex):
+        for k in range(npart[p]):
+            groups[i, k] = len(flat)
+            flat.append(atoms[i, k])
+    d.ccentroid_energy = tuple(re.sub(r"\bp(\d)\b", r"g\1", e) for e in desc.ccompound_energy)
+    d.ccentroid_param_names = tuple(desc.ccompound_param_names)
+    d.ccentroid_groups_per_bond = np.asarray(desc.ccompound_particles, dtype=np.int32)
+    d.ccentroid_periodic = np.asarray(desc.ccompound_periodic, dtype=np.int32)
+    d.ccentroid_expr = np.asarray(desc.ccompound_expr, dtype=np.int32)
+    d.ccentroid_atoms = groups
+    d.ccentroid_params = np.asarray(desc.ccompound_params, dtype=np.float64)
+    d.ccentroid_group_start = np.arange(len(flat) + 1, dtype=np.int32)
+    d.ccentroid_group_atoms = np.array(flat, dtype=np.int32)
+    d.ccentroid_group_weights = np.ones(len(flat))
+    d.ccentroid_group_mass = np.zeros(len(flat), dtype=np.int32)
+    d.ccentroid_prog_start, d.ccentroid_op, d.ccentroid_arg, d.ccentroid_imm = _i(), _i(), _i(), _d()
+    d.ccompound_energy, d.ccompound_param_names = (), ()
+    d.ccompound_particles, d.ccompound_periodic, d.ccompound_expr = _i(), _i(), _i()
+    d.ccompound_atoms, d.ccompound_params = np.full((0, 8), -1, dtype=np.int32), np.zeros((0, 0))
+    d.ccompound_prog_start, d.ccompound_op, d.ccompound_arg, d.ccompound_imm = _i(), _i(), _i(), _d()
+    return d
+
+
+# centre-of-mass distance restraint between two groups, and a flat-bottom restraint of one group's centre to a point
+COM_DISTANCE_RESTRAINT = "0.5*k*(distance(g1,g2)-r0)^2"
+FLAT_BOTTOM_RESTRAINT = "0.5*k*step(dr)*dr^2; dr = pointdistance(x1, y1, z1, x0, y0, z0) - rflat"
+
+
+def with_centroid_restraint(desc, groups, energy, params, param_names, bonds=None, weights=None, periodic=False):
+    """desc plus one CustomCentroidBondForce expression `energy` over `groups` (lists of atoms, new groups after those desc
+    has), with per-bond parameters param_names.  bonds: the group positions of every bond ([n, groups per bond], indices into
+    `groups`; default one bond over all of them in order) and params [n, len(param_names)].  weights: None for mass weighted
+    groups, else one weight list per group (normalised here, as computeNormalizedWeights does)."""
+    import copy
+    d = copy.copy(desc)
+    m = np.asarray(desc.masses, dtype=np.float64)
+    base = len(desc.ccentroid_group_start) - 1
+    bonds = np.arange(len(groups)).reshape(1, -1) if bonds is None else np.asarray(bonds).reshape(-1, np.asarray(bonds).shape[-1])
+    per = bonds.shape[1]
+    start, flat, w = list(desc.ccentroid_group_start), list(desc.ccentroid_group_atoms), list(desc.ccentroid_group_weights)
+    for g, atoms in enumerate(groups):
+        raw = m[np.asarray(atoms)] if weights is None else np.asarray(weights[g], dtype=np.float64)
+        flat += [int(a) for a in atoms]
+        w += (raw/raw.sum()).tolist()
+        start.append(len(flat))
+    n, old = len(bonds), len(desc.ccentroid_expr)
+    width = max([len(p) for p in desc.ccentroid_param_names] + [len(param_names)])
+    par = np.zeros((old + n, width))
+    if old:
+        par[:old, :np.asarray(desc.ccentroid_params).shape[1]] = desc.ccentroid_params
+    par[old:, :len(param_names)] = np.asarray(params, dtype=np.float64).reshape(n, len(param_names))
+    padded = np.full((n, 8), -1, dtype=np.int32)
+    padded[:, :per] = bonds + base
+    d.ccentroid_expr = np.concatenate([desc.ccentroid_expr, np.full(n, len(desc.ccentroid_energy))]).astype(np.int32)
+    d.ccentroid_energy = tuple(desc.ccentroid_energy) + (energy,)
+    d.ccentroid_param_names = tuple(desc.ccentroid_param_names) + (tuple(param_names),)
+    d.ccentroid_groups_per_bond = np.concatenate([desc.ccentroid_groups_per_bond, [per]]).astype(np.int32)
+    d.ccentroid_periodic = np.concatenate([desc.ccentroid_periodic, [int(periodic)]]).astype(np.int32)
+    d.ccentroid_atoms = np.concatenate([np.asarray(desc.ccentroid_atoms, dtype=np.int32).reshape(-1, 8), padded])
+    d.ccentroid_params = par
+    d.ccentroid_group_start = np.array(start, dtype=np.int32)
+    d.ccentroid_group_atoms = np.array(flat, dtype=np.int32)
+    d.ccentroid_group_weights = np.array(w, dtype=np.float64)
+    d.ccentroid_group_mass = np.concatenate([desc.ccentroid_group_mass, np.full(len(groups), int(weights is None))]).astype(np.int32)
+    d.ccentroid_prog_start, d.ccentroid_op, d.ccentroid_arg, d.ccentroid_imm = _i(), _i(), _i(), _d()
+    return d
+
+
+def solute_halves(desc):
+    """The solute heavy atoms (solute_heavy_atoms) split in atom order into two halves: stand-ins for two domains"""
+    h = solute_heavy_atoms(desc)
+    return h[:len(h)//2], h[len(h)//2:]
 
 
 def improper_centres(desc):

@@ -8,7 +8,7 @@
 //
 // Supported: NonbondedForce (NoCutoff, CutoffNonPeriodic, CutoffPeriodic, PME; parameter offsets), HarmonicBondForce,
 // HarmonicAngleForce, PeriodicTorsionForce, RBTorsionForce, CMAPTorsionForce, CustomTorsionForce, CustomBondForce,
-// CustomExternalForce, CustomAngleForce, CustomCompoundBondForce (any number of objects, each in its own force group; custom forces without energy parameter
+// CustomExternalForce, CustomAngleForce, CustomCompoundBondForce, CustomCentroidBondForce (any number of objects, each in its own force group; custom forces without energy parameter
 // derivatives, expressions within the limits of custom_translate.h), CMMotionRemover;
 // Verlet / Langevin / LangevinMiddle integrators; SETTLE + X-H_n SHAKE constraints; MonteCarloBarostat and
 // MonteCarloAnisotropicBarostat (ApplyMonteCarloBarostatKernel; MonteCarloMembraneBarostat is refused).  A Force class without a kernel here
@@ -18,7 +18,7 @@
 // Bonded classes.  Each keeps the terms of all its Force objects in one TermRecord of PlatformData, sent at finalize; what
 // their kernels share (ObjectTerms: the object's range of the record, group tags, updates) exists once.  Bond, angle,
 // periodic-torsion and RB-torsion kernels are one template, B200CalcBondedForceKernel; the custom torsion, bond, external,
-// angle and compound-bond kernels another, B200CalcCustomForceKernel, for their expression programs; CMAP keeps its own for
+// angle, compound-bond and centroid-bond kernels another, B200CalcCustomForceKernel, for their expression programs; CMAP keeps its own for
 // its maps.
 //
 // The hot loop.  Integrator::step(n) of the reference is, per step, updateContextState() -> calcForcesAndEnergy(true,
@@ -44,6 +44,7 @@
 #include "openmm/CustomExternalForce.h"
 #include "openmm/CustomAngleForce.h"
 #include "openmm/CustomCompoundBondForce.h"
+#include "openmm/CustomCentroidBondForce.h"
 #include "openmm/CMMotionRemover.h"
 #include "openmm/VerletIntegrator.h"
 #include "openmm/LangevinIntegrator.h"
@@ -52,6 +53,7 @@
 #include "openmm/internal/ContextImpl.h"
 #include "openmm/internal/NonbondedForceImpl.h"
 #include "openmm/internal/CMAPTorsionForceImpl.h"
+#include "openmm/internal/CustomCentroidBondForceImpl.h"
 #include "../include/b200md.h"
 #include "custom_translate.h"
 #include <algorithm>
@@ -191,15 +193,19 @@ struct PlatformData {
     TermRecord bonds{B200MD_BONDED_BONDS, 2, 0, 2}, angles{B200MD_BONDED_ANGLES, 3, 0, 2}, torsions{B200MD_BONDED_TORSIONS, 4, 1, 2},
                rb{B200MD_BONDED_RB_TORSIONS, 4, 0, 1}, cmap{B200MD_BONDED_CMAP, 1, 1, 0};
     // the custom terms of each class (B200MD_CUSTOM_*): one atom column (a compound bond's B200MD_CUSTOM_MAX_PARTICLES
-    // entries, unused ones -1), the expression, the parameters
-    TermRecord customTerms[5] = {{B200MD_BONDED_CUSTOM_TORSIONS, 1, 1, 1}, {B200MD_BONDED_CUSTOM_BONDS, 1, 1, 1},
+    // entries, unused ones -1; a centroid bond's are groups), the expression, the parameters
+    TermRecord customTerms[6] = {{B200MD_BONDED_CUSTOM_TORSIONS, 1, 1, 1}, {B200MD_BONDED_CUSTOM_BONDS, 1, 1, 1},
                                  {B200MD_BONDED_CUSTOM_EXTERNALS, 1, 1, 1}, {B200MD_BONDED_CUSTOM_ANGLES, 1, 1, 1},
-                                 {B200MD_BONDED_CUSTOM_COMPOUND, 1, 1, 1}};
+                                 {B200MD_BONDED_CUSTOM_COMPOUND, 1, 1, 1}, {B200MD_BONDED_CUSTOM_CENTROID, 1, 1, 1}};
+    // the groups of every CustomCentroidBondForce object, one object's after the other's (a bond's group indices count from the
+    // first group of all objects): CSR over atoms with the normalised weights of computeNormalizedWeights
+    vector<int> centroidGroupStart = vector<int>(1, 0), centroidGroupAtoms;
+    vector<double> centroidGroupWeights;
     // CMAP: the maps of all objects one after the other (a term's map index counts from the first map of all objects);
     // coefficients from CMAPTorsionForceImpl::calcMapDerivatives, [sum size^2][16]
     vector<int> cmapSize; vector<double> cmapCoeff;
     // the programs of each custom class
-    CustomPrograms customPrograms[5];
+    CustomPrograms customPrograms[6];
     // the global parameters the expressions of all custom classes read: slot of every name (shared by all objects) and the
     // value last sent
     map<string, int> customGlobalSlot;
@@ -228,12 +234,17 @@ struct PlatformData {
             if (r->size()) check(b200md_set_bonded_groups(ctx, r->kind, r->size(), r->group.data()));
         typedef int (*SetCustom)(b200md_ctx*, int, const int*, const int*, const int*, const double*, int, int, const int*, const int*, const double*);
         const SetCustom setCustom[4] = {b200md_set_custom_torsions, b200md_set_custom_bonds, b200md_set_custom_externals, b200md_set_custom_angles};
-        for (int k = 0; k < 5; k++) {
+        for (int k = 0; k < 6; k++) {
             const TermRecord& r = customTerms[k];
             if (!r.size()) continue;
             const CustomPrograms& c = customPrograms[k];
             const vector<double> par = c.packed(r);
-            if (k == B200MD_CUSTOM_COMPOUND)
+            if (k == B200MD_CUSTOM_CENTROID)
+                check(b200md_set_custom_centroid(ctx, c.numExpressions(), c.particles.data(), c.periodic.data(), c.progStart.data(), c.op.data(),
+                                                 c.arg.data(), c.imm.data(), c.stride, r.size(), r.ints[0].data(), r.atoms[0].data(), par.data(),
+                                                 (int) centroidGroupStart.size() - 1, centroidGroupStart.data(), centroidGroupAtoms.data(),
+                                                 centroidGroupWeights.data()));
+            else if (k == B200MD_CUSTOM_COMPOUND)
                 check(b200md_set_custom_compound(ctx, c.numExpressions(), c.particles.data(), c.periodic.data(), c.progStart.data(), c.op.data(),
                                                  c.arg.data(), c.imm.data(), c.stride, r.size(), r.ints[0].data(), r.atoms[0].data(), par.data()));
             else
@@ -623,9 +634,14 @@ private:
 
 // What the custom kernels differ in (B200CalcCustomForceKernel below): the Force, its class and term bit, the names in
 // messages, how its expression is translated, its particles per term and whether its point functions take the minimum image
-// (compound bonds only), how term i is read, and the call that sends new parameters.  CustomTerms is what the torsion, bond,
-// external and angle classes share: an expression of the class's variables, translated by translateExpression.
-template<class T> struct CustomTerms {
+// (compound and centroid bonds only), how term i is read, the groups of atoms the object adds (centroid bonds only: addGroups
+// returns the index its first group gets, which read adds to the object's own group indices), and the call that sends new
+// parameters.  CustomTerms is what the torsion, bond, external and angle classes share: an expression of the class's
+// variables, translated by translateExpression.
+struct NoGroups {
+    template<class F> static int addGroups(PlatformData&, const System&, const F&) { return 0; }
+};
+template<class T> struct CustomTerms : NoGroups {
     template<class F> static void translate(const F& force, map<string, int>& globalSlot, vector<b200md_custom::Program>& programs) {
         vector<string> params, globals;
         for (int i = 0; i < T::numParams(force); i++) params.push_back(T::paramName(force, i));
@@ -644,7 +660,7 @@ struct CustomTorsions : CustomTerms<CustomTorsions> {
     static int count(const Force& f) { return f.getNumTorsions(); }
     static int numParams(const Force& f) { return f.getNumPerTorsionParameters(); }
     static string paramName(const Force& f, int i) { return f.getPerTorsionParameterName(i); }
-    static vector<int> read(const Force& f, int i, vector<double>& par) { int a, b, c, e; f.getTorsionParameters(i, a, b, c, e, par); return {a, b, c, e}; }
+    static vector<int> read(const Force& f, int i, vector<double>& par, int) { int a, b, c, e; f.getTorsionParameters(i, a, b, c, e, par); return {a, b, c, e}; }
     static int update(b200md_ctx* c, int n, const double* p) { return b200md_update_custom_torsion_params(c, n, p); }
     static int numParamDerivatives(const Force& f) { return f.getNumEnergyParameterDerivatives(); }
 };
@@ -656,7 +672,7 @@ struct CustomBonds : CustomTerms<CustomBonds> {
     static int count(const Force& f) { return f.getNumBonds(); }
     static int numParams(const Force& f) { return f.getNumPerBondParameters(); }
     static string paramName(const Force& f, int i) { return f.getPerBondParameterName(i); }
-    static vector<int> read(const Force& f, int i, vector<double>& par) { int a, b; f.getBondParameters(i, a, b, par); return {a, b}; }
+    static vector<int> read(const Force& f, int i, vector<double>& par, int) { int a, b; f.getBondParameters(i, a, b, par); return {a, b}; }
     static int update(b200md_ctx* c, int n, const double* p) { return b200md_update_custom_bond_params(c, n, p); }
     static int numParamDerivatives(const Force& f) { return f.getNumEnergyParameterDerivatives(); }
 };
@@ -669,7 +685,7 @@ struct CustomExternals : CustomTerms<CustomExternals> {
     static int count(const Force& f) { return f.getNumParticles(); }
     static int numParams(const Force& f) { return f.getNumPerParticleParameters(); }
     static string paramName(const Force& f, int i) { return f.getPerParticleParameterName(i); }
-    static vector<int> read(const Force& f, int i, vector<double>& par) { int a; f.getParticleParameters(i, a, par); return {a}; }
+    static vector<int> read(const Force& f, int i, vector<double>& par, int) { int a; f.getParticleParameters(i, a, par); return {a}; }
     static int update(b200md_ctx* c, int n, const double* p) { return b200md_update_custom_external_params(c, n, p); }
     static int numParamDerivatives(const Force&) { return 0; }        // CustomExternalForce has none
 };
@@ -681,19 +697,19 @@ struct CustomAngles : CustomTerms<CustomAngles> {
     static int count(const Force& f) { return f.getNumAngles(); }
     static int numParams(const Force& f) { return f.getNumPerAngleParameters(); }
     static string paramName(const Force& f, int i) { return f.getPerAngleParameterName(i); }
-    static vector<int> read(const Force& f, int i, vector<double>& par) { int a, b, c; f.getAngleParameters(i, a, b, c, par); return {a, b, c}; }
+    static vector<int> read(const Force& f, int i, vector<double>& par, int) { int a, b, c; f.getAngleParameters(i, a, b, c, par); return {a, b, c}; }
     static int update(b200md_ctx* c, int n, const double* p) { return b200md_update_custom_angle_params(c, n, p); }
     static int numParamDerivatives(const Force& f) { return f.getNumEnergyParameterDerivatives(); }
 };
 // A compound bond's expression is of the coordinates of its particles: 1 + 3 (particles per bond) programs, which k_compound
 // interprets.  Its atoms are padded to B200MD_CUSTOM_MAX_PARTICLES with -1.
-struct CustomCompounds {
+struct CustomCompounds : NoGroups {
     typedef CustomCompoundBondForce Force; typedef CalcCustomCompoundBondForceKernel Kernel;
     enum { cls = B200MD_CUSTOM_COMPOUND, bit = B200MD_TERM_CUSTOM_COMPOUND };
     static constexpr const char* name = "CustomCompoundBondForce", *terms = "bonds", *aTerm = "a bond", *changed = nullptr;
     static int count(const Force& f) { return f.getNumBonds(); }
     static int numParams(const Force& f) { return f.getNumPerBondParameters(); }
-    static vector<int> read(const Force& f, int i, vector<double>& par) {
+    static vector<int> read(const Force& f, int i, vector<double>& par, int) {
         vector<int> atoms;
         f.getBondParameters(i, atoms, par);
         atoms.resize(B200MD_CUSTOM_MAX_PARTICLES, -1);
@@ -706,6 +722,46 @@ struct CustomCompounds {
     }
     static int particles(const Force& f) { return f.getNumParticlesPerBond(); }
     static bool periodic(const Force& f) { return f.usesPeriodicBoundaryConditions(); }
+};
+// A centroid bond's expression is a compound bond's of the centres of its groups: the same programs, which k_compound runs at
+// the centres k_centroid_centers makes.  Its groups are padded to B200MD_CUSTOM_MAX_PARTICLES with -1, and its objects' groups
+// go into one table, with the weights CustomCentroidBondForceImpl::computeNormalizedWeights makes (masses by default; a
+// group whose weights add to 0 raises the reference's error there).
+struct CustomCentroids {
+    typedef CustomCentroidBondForce Force; typedef CalcCustomCentroidBondForceKernel Kernel;
+    enum { cls = B200MD_CUSTOM_CENTROID, bit = B200MD_TERM_CUSTOM_CENTROID };
+    static constexpr const char* name = "CustomCentroidBondForce", *terms = "bonds", *aTerm = "a bond",
+                                 *changed = "The set of groups in a bond has changed";
+    static int count(const Force& f) { return f.getNumBonds(); }
+    static int numParams(const Force& f) { return f.getNumPerBondParameters(); }
+    static vector<int> read(const Force& f, int i, vector<double>& par, int base) {
+        vector<int> groups;
+        f.getBondParameters(i, groups, par);
+        for (int& g : groups) g += base;
+        groups.resize(B200MD_CUSTOM_MAX_PARTICLES, -1);
+        return groups;
+    }
+    static int update(b200md_ctx* c, int n, const double* p) { return b200md_update_custom_centroid_params(c, n, p); }
+    static int numParamDerivatives(const Force& f) { return f.getNumEnergyParameterDerivatives(); }
+    static void translate(const Force& f, map<string, int>& globalSlot, vector<b200md_custom::Program>& programs) {
+        b200md_custom::translateCentroid(f, globalSlot, programs);
+    }
+    static int particles(const Force& f) { return f.getNumGroupsPerBond(); }
+    static bool periodic(const Force& f) { return f.usesPeriodicBoundaryConditions(); }
+    static int addGroups(PlatformData& d, const System& system, const Force& f) {
+        const int base = (int) d.centroidGroupStart.size() - 1;
+        vector<vector<double> > weights;
+        CustomCentroidBondForceImpl::computeNormalizedWeights(f, system, weights);
+        for (int g = 0; g < f.getNumGroups(); g++) {
+            vector<int> atoms;
+            vector<double> given;
+            f.getGroupParameters(g, atoms, given);
+            d.centroidGroupAtoms.insert(d.centroidGroupAtoms.end(), atoms.begin(), atoms.end());
+            d.centroidGroupWeights.insert(d.centroidGroupWeights.end(), weights[g].begin(), weights[g].end());
+            d.centroidGroupStart.push_back((int) d.centroidGroupAtoms.size());
+        }
+        return base;
+    }
 };
 
 // The global parameters one custom force object's expression reads, and their slots in the Context's shared map
@@ -733,9 +789,10 @@ struct ObjectGlobals {
     }
 };
 
-// CustomTorsionForce, CustomBondForce, CustomExternalForce, CustomAngleForce and CustomCompoundBondForce (T: CustomTorsions,
-// CustomBonds, CustomExternals, CustomAngles, CustomCompounds): the expression becomes 1 + (number of variables) instruction
-// programs, which k_custom interprets (k_compound for compound bonds).
+// CustomTorsionForce, CustomBondForce, CustomExternalForce, CustomAngleForce, CustomCompoundBondForce and
+// CustomCentroidBondForce (T: CustomTorsions, CustomBonds, CustomExternals, CustomAngles, CustomCompounds, CustomCentroids):
+// the expression becomes 1 + (number of variables) instruction programs, which k_custom interprets (k_compound for compound
+// and centroid bonds).
 template<class T>
 class B200CalcCustomForceKernel : public T::Kernel, ObjectTerms {
 public:
@@ -743,7 +800,7 @@ public:
     // the term's parameters: as many as the force declares (the Reference platform reads as many), padded with zeros
     void read(const typename T::Force& force, int i, TermRecord& r) const {
         vector<double> par;
-        const vector<int> atoms = T::read(force, i, par);
+        const vector<int> atoms = T::read(force, i, par, groupBase);
         par.resize(numParams);
         par.resize(B200MD_CUSTOM_MAX_PARAMS, 0.0);
         r.add(atoms, {expr}, par);
@@ -753,6 +810,8 @@ public:
         CustomPrograms& c = d.customPrograms[T::cls];
         expr = c.numExpressions();
         numParams = T::numParams(force);
+        if (d.finalized) throw OpenMMException(string("B200 platform: ") + T::name + " initialised after the Context was finalised");
+        groupBase = T::addGroups(d, system, force);
         add(d, d.customTerms[T::cls], force, T::count(force), T::bit, T::name, [&](int i, TermRecord& r) { read(force, i, r); });
         vector<b200md_custom::Program> programs;
         T::translate(force, d.customGlobalSlot, programs);
@@ -776,6 +835,7 @@ public:
 private:
     ContextImpl& context;
     int expr = 0, numParams = 0;          // this object's expression; its number of per-term parameters
+    int groupBase = 0;                    // the index of this object's first group (centroid bonds)
     ObjectGlobals globals;
 };
 
@@ -911,6 +971,7 @@ public:
         if (name == CalcCustomExternalForceKernel::Name()) return new B200CalcCustomForceKernel<CustomExternals>(name, platform, context);
         if (name == CalcCustomAngleForceKernel::Name()) return new B200CalcCustomForceKernel<CustomAngles>(name, platform, context);
         if (name == CalcCustomCompoundBondForceKernel::Name()) return new B200CalcCustomForceKernel<CustomCompounds>(name, platform, context);
+        if (name == CalcCustomCentroidBondForceKernel::Name()) return new B200CalcCustomForceKernel<CustomCentroids>(name, platform, context);
         if (name == RemoveCMMotionKernel::Name()) return new B200RemoveCMMotionKernel(name, platform, context);
         if (name == IntegrateVerletStepKernel::Name()) return new B200IntegrateVerletStepKernel(name, platform);
         if (name == IntegrateLangevinStepKernel::Name()) return new B200IntegrateLangevinStepKernel(name, platform);
@@ -928,7 +989,7 @@ public:
                                 CalcNonbondedForceKernel::Name(), CalcHarmonicBondForceKernel::Name(), CalcHarmonicAngleForceKernel::Name(),
                                 CalcPeriodicTorsionForceKernel::Name(), CalcRBTorsionForceKernel::Name(), CalcCMAPTorsionForceKernel::Name(),
                                 CalcCustomTorsionForceKernel::Name(), CalcCustomBondForceKernel::Name(), CalcCustomExternalForceKernel::Name(),
-                                CalcCustomAngleForceKernel::Name(), CalcCustomCompoundBondForceKernel::Name(),
+                                CalcCustomAngleForceKernel::Name(), CalcCustomCompoundBondForceKernel::Name(), CalcCustomCentroidBondForceKernel::Name(),
                                 RemoveCMMotionKernel::Name(), IntegrateVerletStepKernel::Name(),
                                 IntegrateLangevinStepKernel::Name(), IntegrateLangevinMiddleStepKernel::Name(), ApplyMonteCarloBarostatKernel::Name()})
             registerKernelFactory(n, factory);
@@ -988,6 +1049,7 @@ public:
             if (const CustomExternalForce* f = dynamic_cast<const CustomExternalForce*>(&force)) validateCustom<CustomExternals>(*f);
             if (const CustomAngleForce* f = dynamic_cast<const CustomAngleForce*>(&force)) validateCustom<CustomAngles>(*f);
             if (const CustomCompoundBondForce* f = dynamic_cast<const CustomCompoundBondForce*>(&force)) validateCustom<CustomCompounds>(*f);
+            if (const CustomCentroidBondForce* f = dynamic_cast<const CustomCentroidBondForce*>(&force)) validateCustom<CustomCentroids>(*f);
         }
         const int nc = system.getNumConstraints();
         if (nc > 0) {

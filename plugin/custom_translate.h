@@ -1,8 +1,8 @@
-// custom_translate.h -- CustomTorsionForce, CustomBondForce, CustomExternalForce, CustomAngleForce and
-// CustomCompoundBondForce expressions -> the instruction programs of b200md_set_custom_torsions / _bonds / _externals /
-// _angles / _compound (B200MD_OP_*, include/b200md.h).  Lepton, part of the host's libOpenMM.so, parses, optimises and
-// differentiates the expression exactly as the Reference platform does
-// (ReferenceCalcCustom{Torsion,Bond,External,Angle,CompoundBond}ForceKernel::initialize) and makes the stack program
+// custom_translate.h -- CustomTorsionForce, CustomBondForce, CustomExternalForce, CustomAngleForce,
+// CustomCompoundBondForce and CustomCentroidBondForce expressions -> the instruction programs of b200md_set_custom_torsions /
+// _bonds / _externals / _angles / _compound / _centroid (B200MD_OP_*, include/b200md.h).  Lepton, part of the host's
+// libOpenMM.so, parses, optimises and differentiates the expression exactly as the Reference platform does
+// (ReferenceCalcCustom{Torsion,Bond,External,Angle,CompoundBond,CentroidBond}ForceKernel::initialize) and makes the stack program
 // (ExpressionProgram); this file only maps every Lepton::Operation to one instruction.  Included by the plugin
 // (B200Platform.cpp) and by its test C API (tests/custom_capi.cpp), so that both make the same programs.
 #ifndef B200MD_CUSTOM_TRANSLATE_H_
@@ -10,6 +10,8 @@
 #include "openmm/OpenMMException.h"
 #include "openmm/CustomCompoundBondForce.h"
 #include "openmm/internal/CustomCompoundBondForceImpl.h"
+#include "openmm/CustomCentroidBondForce.h"
+#include "openmm/internal/CustomCentroidBondForceImpl.h"
 #include "lepton/CustomFunction.h"
 #include "lepton/ExpressionProgram.h"
 #include "lepton/Operation.h"
@@ -206,6 +208,29 @@ inline void translateCompound(const OpenMM::CustomCompoundBondForce& force, std:
     for (int i = 0; i < force.getNumPerBondParameters(); i++) paramNames.push_back(force.getPerBondParameterName(i));
     for (int i = 0; i < force.getNumGlobalParameters(); i++) globalNames.push_back(force.getGlobalParameterName(i));
     detail::translatePrograms(OpenMM::CustomCompoundBondForceImpl::prepareExpression(force, functions), variables, "CustomCompoundBondForce",
+                              B200MD_CUSTOM_COMPOUND_MAX_STACK, paramNames, globalNames, globalSlot, programs);
+}
+
+// A CustomCentroidBondForce: the programs of a compound bond of the same expression, by x1, y1, z1, x2, .. of the group
+// centres (1 + 3 groups per bond).  CustomCentroidBondForceImpl::prepareExpression turns distance, angle and dihedral of
+// g1, g2, .. into the point functions of those coordinates, as for the Reference platform.
+inline void translateCentroid(const OpenMM::CustomCentroidBondForce& force, std::map<std::string, int>& globalSlot, std::vector<Program>& programs) {
+    const int numGroups = force.getNumGroupsPerBond();
+    if (numGroups > B200MD_CUSTOM_MAX_PARTICLES)
+        throw Unsupported("B200 platform: a CustomCentroidBondForce with more than 8 groups per bond is not supported");
+    if (force.getNumPerBondParameters() > B200MD_CUSTOM_MAX_PARAMS)
+        throw Unsupported("B200 platform: a CustomCentroidBondForce with more than 16 per-bond parameters is not supported");
+    if (force.getNumTabulatedFunctions() > 0)
+        throw Unsupported("B200 platform: tabulated functions in a CustomCentroidBondForce expression are not supported");
+    PointFunctionPlaceholder distance(6), angle(9), dihedral(12);
+    std::map<std::string, Lepton::CustomFunction*> functions;
+    functions["pointdistance"] = &distance; functions["pointangle"] = &angle; functions["pointdihedral"] = &dihedral;
+    std::vector<std::string> variables, paramNames, globalNames;
+    for (int i = 1; i <= numGroups; i++)
+        for (const char* axis : {"x", "y", "z"}) variables.push_back(axis + std::to_string(i));
+    for (int i = 0; i < force.getNumPerBondParameters(); i++) paramNames.push_back(force.getPerBondParameterName(i));
+    for (int i = 0; i < force.getNumGlobalParameters(); i++) globalNames.push_back(force.getGlobalParameterName(i));
+    detail::translatePrograms(OpenMM::CustomCentroidBondForceImpl::prepareExpression(force, functions), variables, "CustomCentroidBondForce",
                               B200MD_CUSTOM_COMPOUND_MAX_STACK, paramNames, globalNames, globalSlot, programs);
 }
 
