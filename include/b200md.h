@@ -46,7 +46,8 @@ typedef struct b200md_ctx b200md_ctx;
 #define B200MD_TERM_CUSTOM_ANGLES    1024
 #define B200MD_TERM_CUSTOM_COMPOUND  2048
 #define B200MD_TERM_CUSTOM_CENTROID  4096
-#define B200MD_TERM_ALL        8191
+#define B200MD_TERM_GBSA             8192   /* GBSAOBCForce: OBC II implicit solvent with the ACE surface term */
+#define B200MD_TERM_ALL        16383
 
 /* ---- the bonded classes: kind argument of b200md_set_bonded_groups and b200md_update_bonded_params ---- */
 #define B200MD_BONDED_BONDS           0
@@ -258,6 +259,18 @@ int b200md_update_custom_angle_params(b200md_ctx* ctx, int n, const double* para
 int b200md_update_custom_compound_params(b200md_ctx* ctx, int n, const double* params);
 /* CalcCustomCentroidBondForceKernel::copyParametersToContext: the same for centroid bonds (groups and weights stay).       */
 int b200md_update_custom_centroid_params(b200md_ctx* ctx, int n, const double* params);
+/* CalcGBSAOBCForceKernel::initialize (kernels.h): OBC II generalized Born (Onufriev, Bashford and Case, Proteins 55:383,
+ * 2004; alpha 1, beta 0.8, gamma 4.85, dielectric offset 0.009 nm) with the ACE surface term (probe radius 0.14 nm, energy
+ * 4 pi surface_area_energy (R + 0.14)^2 (R/B)^6 per atom).  One value per atom of charge (e), radius R (nm) and scale s.
+ * method is the GBSAOBCForce's (B200MD_NB_NOCUTOFF, _CUTOFF_NONPERIODIC or _CUTOFF_PERIODIC) and must agree with the
+ * context's nonbonded method at finalize (CutoffPeriodic with CutoffPeriodic or PME), with the same cutoff; without
+ * b200md_set_nonbonded only NoCutoff is accepted.  Every pair within the cutoff counts, excluded pairs included; with a
+ * cutoff the pair energy is shifted by -q_i q_j/cutoff.  A dielectric of 0 turns the polar part off.  Single GPU only. */
+int b200md_set_gbsa(b200md_ctx* ctx, int method, double cutoff, double solute_dielectric, double solvent_dielectric,
+                    double surface_area_energy, const double* charge, const double* radius, const double* scale);
+/* CalcGBSAOBCForceKernel::copyParametersToContext: new charges, radii and scales (n == the number of atoms) into the same
+ * device buffers, so a captured step graph stays valid.                                                                   */
+int b200md_update_gbsa_params(b200md_ctx* ctx, int n, const double* charge, const double* radius, const double* scale);
 /* Test hook, no context and no device: program `which` of a b200md_set_custom_torsions program set, checked as that call
  * checks it (nglobals = the number of global slots), evaluated at (theta, params, globals) on the host by the interpreter
  * source the device kernel runs.  0 and *out on success, -1 with the reason in msg.                                       */
@@ -368,7 +381,8 @@ int b200md_get_stats(b200md_ctx* ctx, b200md_stats* out);
  * phase: 0 pair kernel, 1 pme spread, 2 fft+convolution, 3 pme gather, 4 integrate+constrain, 5 list build,
  * 6 bonded+exceptions (k_bonded and, with custom terms, k_custom and k_compound), 7 custom torsions, bonds, externals and
  * angles alone (k_custom), 8 custom compound bonds alone (k_compound), 9 custom centroid bonds alone (k_centroid_centers,
- * the k_compound instantiation that reads the centres, k_centroid_scatter).
+ * the k_compound instantiation that reads the centres, k_centroid_scatter), 10 the generalized Born chain (k_gb_born,
+ * k_gb_radii, k_gb_pairs, k_gb_fold, k_gb_chain).
  * Runs `reps` isolated launches of that phase on the current state.                                  */
 int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* ms_mean);
 /* stand-alone 3-D FFT entry (the bespoke FFT alone, for parity against fftpack / numpy):

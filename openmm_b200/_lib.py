@@ -65,6 +65,8 @@ SIGNATURES = {
     "b200md_update_custom_angle_params": (C.c_int, [_P, C.c_int, _D]),
     "b200md_update_custom_compound_params": (C.c_int, [_P, C.c_int, _D]),
     "b200md_update_custom_centroid_params": (C.c_int, [_P, C.c_int, _D]),
+    "b200md_set_gbsa": (C.c_int, [_P, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, _D, _D, _D]),
+    "b200md_update_gbsa_params": (C.c_int, [_P, C.c_int, _D, _D, _D]),
     "b200md_custom_program_probe": (C.c_int, [C.c_int, _I, _I, _I, _D, C.c_int, C.c_int, C.c_int, C.c_double, _D, _D, _D,
                                               C.c_char_p, C.c_int]),
     "b200md_custom_term_probe": (C.c_int, [C.c_int, C.c_int, _I, _I, _I, _D, C.c_int, C.c_int, C.c_int, _D, _D, _D, _D, _D,

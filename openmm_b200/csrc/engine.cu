@@ -260,6 +260,19 @@ struct b200md_ctx {
     CompoundDev cpd{};
     CompoundDev ccd{};          // the centroid bonds' programs and slots
     CentroidDev cen{};
+    // generalized Born (b200md_set_gbsa): the force's settings and per-atom parameters as given, their device form and the
+    // stream the chain runs on beside the tile kernel (created at finalize when there is one)
+    struct {
+        bool have = false;
+        int method = 0;
+        double cutoff = 0, solute = 1, solvent = 78.5, surface = 0;
+        std::vector<double> charge, radius, scale;
+        DevBuf<float> chargeDev; DevBuf<double2> radiusDev; DevBuf<double> atomRadiusDev, bornR, chain, bornForce;
+        DevBuf<long long> bornSum, dEdB;
+        cudaStream_t stream = nullptr;
+        cudaEvent_t evFork = nullptr, evJoin = nullptr;
+    } gbsa;
+    GbsaDev gbd{};
     UnitDev units{};
     IntegDev integ{};
     bool haveIntegrator = false;
@@ -303,6 +316,7 @@ struct b200md_ctx {
 static void check_flags(b200md_ctx* c);
 static void sync_velocities(b200md_ctx* c);
 static void sync_positions(b200md_ctx* c);
+static void setup_gbsa(b200md_ctx* c);
 
 extern "C" const char* b200md_version(void) { return "b200md 0.2 (sm_90a)"; }
 extern "C" const char* b200md_last_error(const b200md_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
@@ -361,6 +375,9 @@ extern "C" void b200md_destroy(b200md_ctx* ctx) {
     if (ctx->evJoin) cudaEventDestroy(ctx->evJoin);
     if (ctx->evJoinBonded) cudaEventDestroy(ctx->evJoinBonded);
     if (ctx->evForkGrid) cudaEventDestroy(ctx->evForkGrid);
+    if (ctx->gbsa.stream) cudaStreamDestroy(ctx->gbsa.stream);
+    if (ctx->gbsa.evFork) cudaEventDestroy(ctx->gbsa.evFork);
+    if (ctx->gbsa.evJoin) cudaEventDestroy(ctx->gbsa.evJoin);
     char* window = ctx->window;
     delete ctx;
     if (window) cudaFree(window);
@@ -1674,6 +1691,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     upload_params(c);
     build_units(c);
     build_ccma(c);
+    setup_gbsa(c);
     if (c->mg == MG_P2P) {
         setup_ownership(c);
         if (nb.method == B200MD_NB_PME) {
@@ -1836,6 +1854,88 @@ extern "C" int b200md_update_custom_centroid_params(b200md_ctx* ctx, int n, cons
     API_BEGIN(ctx)
     update_custom(ctx, B200MD_CUSTOM_CENTROID, n, params);
     API_END(ctx)
+}
+
+// ---------------------------------------------------------------- generalized Born (GBSAOBCForce)
+// charge, radius and scale of every atom: finite, radius above the dielectric offset (ObcParameters' rho = R - 0.009 must be
+// positive), scale not negative
+static void check_gbsa_params(const b200md_ctx* c, const char* call, const double* q, const double* r, const double* s) {
+    for (int i = 0; i < c->natoms; i++) {
+        require(std::isfinite(q[i]) && std::isfinite(r[i]) && std::isfinite(s[i]), (std::string(call) + ": a parameter is not finite").c_str());
+        require(r[i] > 0.009, (std::string(call) + ": a radius must exceed the dielectric offset of 0.009 nm").c_str());
+        require(s[i] >= 0.0, (std::string(call) + ": a scale factor must not be negative").c_str());
+    }
+}
+// the device form of the per-atom parameters (GbsaDev), into buffers of a fixed size: a captured step graph keeps its pointers
+static void upload_gbsa_params(b200md_ctx* c) {
+    const int N = c->natoms;
+    std::vector<float> q(c->npad, 0.f); std::vector<double2> rad(c->npad, make_double2(1.0, 0.0)); std::vector<double> R(c->npad, 1.0);
+    for (int i = 0; i < N; i++) {
+        const double rho = c->gbsa.radius[i] - 0.009;
+        q[i] = (float) (c->gbsa.charge[i]*std::sqrt(B200MD_ONE_4PI_EPS0));
+        rad[i] = make_double2(rho, rho*c->gbsa.scale[i]);
+        R[i] = c->gbsa.radius[i];
+    }
+    c->gbsa.chargeDev.upload(q); c->gbsa.radiusDev.upload(rad); c->gbsa.atomRadiusDev.upload(R);
+}
+extern "C" int b200md_set_gbsa(b200md_ctx* ctx, int method, double cutoff, double solute, double solvent, double surface,
+                               const double* charge, const double* radius, const double* scale) {
+    API_BEGIN(ctx)
+    check_set(ctx, "set_gbsa", 0);
+    require(ctx->world == 1, "generalized Born (GBSAOBCForce) is not supported in multi-GPU runs");
+    require(method == B200MD_NB_NOCUTOFF || method == B200MD_NB_CUTOFF_NONPERIODIC || method == B200MD_NB_CUTOFF_PERIODIC,
+            "set_gbsa: method must be NoCutoff, CutoffNonPeriodic or CutoffPeriodic");
+    require(method == B200MD_NB_NOCUTOFF || (std::isfinite(cutoff) && cutoff > 0.0), "set_gbsa: the cutoff must be positive");
+    require(std::isfinite(solute) && std::isfinite(solvent) && std::isfinite(surface), "set_gbsa: the dielectrics and the surface energy must be finite");
+    check_gbsa_params(ctx, "set_gbsa", charge, radius, scale);
+    auto& g = ctx->gbsa;
+    g.have = true; g.method = method; g.cutoff = cutoff; g.solute = solute; g.solvent = solvent; g.surface = surface;
+    g.charge.assign(charge, charge + ctx->natoms); g.radius.assign(radius, radius + ctx->natoms); g.scale.assign(scale, scale + ctx->natoms);
+    API_END(ctx)
+}
+extern "C" int b200md_update_gbsa_params(b200md_ctx* ctx, int n, const double* charge, const double* radius, const double* scale) {
+    API_BEGIN(ctx)
+    require(ctx->finalized, "update_gbsa_params before finalize");
+    require(ctx->gbsa.have, "update_gbsa_params: the context has no generalized Born force");
+    require(n == ctx->natoms, "update_gbsa_params: the number of particles has changed");
+    check_gbsa_params(ctx, "update_gbsa_params", charge, radius, scale);
+    auto& g = ctx->gbsa;
+    g.charge.assign(charge, charge + n); g.radius.assign(radius, radius + n); g.scale.assign(scale, scale + n);
+    CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+    upload_gbsa_params(ctx);
+    API_END(ctx)
+}
+// finalize: the method must agree with the nonbonded one (the chain walks its list), the device state, and the stream
+static void setup_gbsa(b200md_ctx* c) {
+    auto& g = c->gbsa;
+    c->gbd = GbsaDev{};
+    if (!g.have) return;
+    require(c->world == 1, "generalized Born (GBSAOBCForce) is not supported in multi-GPU runs");
+    const int nm = c->haveNb ? c->nbdesc.method : -1;
+    if (!c->haveNb) require(g.method == B200MD_NB_NOCUTOFF, "generalized Born with a cutoff needs a nonbonded force with the same cutoff");
+    else if (g.method == B200MD_NB_NOCUTOFF) require(nm == B200MD_NB_NOCUTOFF, "generalized Born: NoCutoff needs a NoCutoff nonbonded force");
+    else if (g.method == B200MD_NB_CUTOFF_NONPERIODIC) require(nm == B200MD_NB_CUTOFF_NONPERIODIC, "generalized Born: CutoffNonPeriodic needs a CutoffNonPeriodic nonbonded force");
+    else require(nm == B200MD_NB_CUTOFF_PERIODIC || nm == B200MD_NB_PME, "generalized Born: CutoffPeriodic needs a CutoffPeriodic or PME nonbonded force");
+    if (g.method != B200MD_NB_NOCUTOFF)
+        require(std::fabs(g.cutoff - c->nbdesc.cutoff) <= 1e-12*c->nbdesc.cutoff, "generalized Born: the cutoff must be that of the nonbonded force");
+    upload_gbsa_params(c);
+    const int NP = c->npad;
+    g.bornSum.alloc(NP); g.bornSum.zero(); g.dEdB.alloc(NP); g.dEdB.zero();
+    g.bornR.alloc(NP); g.bornR.zero(); g.chain.alloc(NP); g.chain.zero(); g.bornForce.alloc(NP); g.bornForce.zero();
+    GbsaDev& d = c->gbd;
+    d.useCutoff = g.method != B200MD_NB_NOCUTOFF;
+    d.cutoff = d.useCutoff ? g.cutoff : 0.0; d.cutoff2 = d.cutoff*d.cutoff;
+    d.prefactor = (g.solute != 0.0 && g.solvent != 0.0) ? -(1.0/g.solute - 1.0/g.solvent) : 0.0;
+    d.surfaceFactor = 4.0*M_PI*g.surface;
+    d.charge = g.chargeDev.p; d.radius = g.radiusDev.p; d.atomRadius = g.atomRadiusDev.p;
+    d.bornSum = g.bornSum.p; d.dEdB = g.dEdB.p; d.bornR = g.bornR.p; d.chain = g.chain.p; d.bornForce = g.bornForce.p;
+    if (!g.stream) {
+        int hi = 0;
+        CUDA_CHECK(cudaDeviceGetStreamPriorityRange(nullptr, &hi));
+        CUDA_CHECK(cudaStreamCreateWithPriority(&g.stream, cudaStreamNonBlocking, hi));
+        CUDA_CHECK(cudaEventCreateWithFlags(&g.evFork, cudaEventDisableTiming));
+        CUDA_CHECK(cudaEventCreateWithFlags(&g.evJoin, cudaEventDisableTiming));
+    }
 }
 
 // ---------------------------------------------------------------- state
@@ -2077,6 +2177,11 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     // atoms this rank OWNS (k_pme_gather), so when it runs on its own stream the push does not have to wait for it: it goes
     // out right behind the tile kernel and the bonded terms, beside the FFT chain.
     const bool pushEarly = p2p && fork;
+    // Generalized Born: its pair passes walk this evaluation's list, so the chain forks after the list check and build (which
+    // it needs even when direct space is not evaluated, e.g. GB alone in a force group) and joins before the integrator.  It
+    // adds into the user-order fixed-point buffer like everything else, so the overlap cannot change the result.
+    const bool gb = (terms & B200MD_TERM_GBSA) && c->gbsa.have && !pmeRank;
+    const bool forkGb = gb && c->overlapPme;
 
     int launches = 0;
     auto launch_recip = [&]() {
@@ -2114,10 +2219,17 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
         CUDA_CHECK(cudaStreamWaitEvent(sp, c->evForkGrid, 0));
         CUDA_CHECK(cudaMemsetAsync(pme.gridFixed, 0, sizeof(long long)*(size_t) pme.nx*pme.ny*pme.nz, sp));
     }
-    if (direct) {
+    if (direct || gb) {
         launch_check_displacement(c->nb, c->cd, s); launches++;
         launch_list_build(c->nb, s); launches += LIST_BUILD_LAUNCHES;
     }
+    if (forkGb) {
+        CUDA_CHECK(cudaEventRecord(c->gbsa.evFork, s));
+        CUDA_CHECK(cudaStreamWaitEvent(c->gbsa.stream, c->gbsa.evFork, 0));
+        launch_gbsa(c->nb, c->gbd, energy, c->gbsa.stream);
+        CUDA_CHECK(cudaEventRecord(c->gbsa.evJoin, c->gbsa.stream));
+    }
+    if (gb) launches += GBSA_LAUNCHES;
     if (forkAfterList) launch_recip();
     if (forkBonded) {
         CUDA_CHECK(cudaStreamWaitEvent(c->streamBonded, c->evFork, 0));
@@ -2126,9 +2238,11 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     }
     if (direct) { launch_pair(c->nb, energy, s); launches += PAIR_LAUNCHES; }
     if (bonded && !forkBonded) launch_bonded_terms(s);
+    if (gb && !forkGb) launch_gbsa(c->nb, c->gbd, energy, s);
     if (pushEarly) { launch_force_push(c->nb, c->cd, s); launches++; }
     if (fork) CUDA_CHECK(cudaStreamWaitEvent(s, c->evJoin, 0));
     if (forkBonded) CUDA_CHECK(cudaStreamWaitEvent(s, c->evJoinBonded, 0));
+    if (forkGb) CUDA_CHECK(cudaStreamWaitEvent(s, c->gbsa.evJoin, 0));
     if (p2p) {
         if (!pushEarly) { launch_force_push(c->nb, c->cd, s); launches++; }
         // in the step path k_integrate totals own partial + inboxes; here (energies, getState) the owners total and broadcast
@@ -2175,7 +2289,7 @@ static void check_flags(b200md_ctx* c) {
 // After the state was changed from outside (positions, box, parameters, checkpoint): build the list now, synchronously,
 // and size the tile pools from what the build actually used.  The step graphs trust the current list and never grow it.
 static void prepare_list(b200md_ctx* c) {
-    if (!c->listDirty || !c->haveNb) { c->listDirty = false; return; }
+    if (!c->listDirty || !(c->haveNb || c->gbsa.have)) { c->listDirty = false; return; }
     if (c->pmeOnly || nccl_pme_rank(c)) { c->listDirty = false; return; }    // keeps no list
     for (int attempt = 0; attempt < 8; attempt++) {
         launch_check_displacement(c->nb, c->cd, c->stream);
@@ -2226,6 +2340,7 @@ extern "C" int b200md_compute_groups(b200md_ctx* ctx, int terms, unsigned int bo
         if (terms & B200MD_TERM_CMAP) e += h[EN_CMAP];
         if (terms & (B200MD_TERM_CUSTOM_TORSIONS | B200MD_TERM_CUSTOM_BONDS | B200MD_TERM_CUSTOM_EXTERNALS | B200MD_TERM_CUSTOM_ANGLES |
                      B200MD_TERM_CUSTOM_COMPOUND | B200MD_TERM_CUSTOM_CENTROID)) e += h[EN_CUSTOM];
+        if ((terms & B200MD_TERM_GBSA) && ctx->gbsa.have) e += h[EN_GB];
         if (ctx->haveNb) {
             if (terms & B200MD_TERM_NB_DIRECT) {
                 e += h[EN_NB] + h[EN_EXC];
@@ -2496,6 +2611,7 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
     require(phase != 7 || c->ctd.nslots > 0, "time_phase(custom torsions): the System has none");
     require(phase != 8 || c->cpd.nslots > 0, "time_phase(custom compound bonds): the System has none");
     require(phase != 9 || c->ccd.nslots > 0, "time_phase(custom centroid bonds): the System has none");
+    require(phase != 10 || c->gbsa.have, "time_phase(generalized Born): the System has none");
     if (phase == 4) {
         require(c->haveIntegrator, "time_phase(integrate) before set_integrator");
         state.parts = state_spans(c, ST_POS | ST_VEL); state.save(s);
@@ -2517,6 +2633,7 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
             case 7: launch_custom(c->nb, c->ctd, B200MD_TERM_ALL, false, s); break;
             case 8: launch_compound(c->nb, c->cpd, false, s); break;
             case 9: launch_centroid(c->nb, c->ccd, c->cen, false, s); break;
+            case 10: launch_gbsa(c->nb, c->gbd, false, s); break;
             default: throw std::runtime_error("unknown phase");
         }
         CUDA_CHECK(cudaEventRecord(e1, s));

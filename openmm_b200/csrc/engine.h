@@ -160,7 +160,7 @@ struct NbDev {
 };
 
 enum { EN_NB = 0, EN_RECIP = 1, EN_BOND = 2, EN_ANGLE = 3, EN_TORSION = 4, EN_EXC = 5, EN_KE = 6, EN_RBTORSION = 7, EN_CMAP = 8,
-       EN_CUSTOM = 9, B200MD_NUM_ENERGY = 10 };
+       EN_CUSTOM = 9, EN_GB = 10, B200MD_NUM_ENERGY = 11 };
 
 struct PmeDev {
     int nx, ny, nz, nzc;
@@ -239,6 +239,23 @@ struct CentroidDev {
     const int* groupStart; const int* groupAtoms; const double* groupWeight;
     double* center; double* deriv;
     const int4* scatter; const double* scatterWeight;
+};
+
+// Generalized Born (GBSAOBCForce, OBC II + ACE; gbsa.cu).  Per-atom parameters in user order; the pair passes walk the current
+// neighbour list and reach them through sorig.  bornSum and dEdB are 2^32 fixed point, so that the sums do not depend on the
+// order of the atomics: the Born sum sum_j I_ij (k_gb_born, zeroed again by k_gb_radii once read) and dE/dB_i (set by k_gb_radii
+// to the ACE and self terms, accumulated by k_gb_pairs, read by k_gb_fold).  bornR and chain: B_i and
+// C_i = rho_i (alpha - 2 beta Psi_i + 3 gamma Psi_i^2)(1 - T_i^2)/R_i (k_gb_radii); bornForce = dE/dB_i B_i^2 C_i (k_gb_fold).
+struct GbsaDev {
+    int useCutoff;
+    double cutoff, cutoff2;
+    double prefactor;            // -(1/solute - 1/solvent), charges carry sqrt(ONE_4PI_EPS0); 0 when a dielectric is 0
+    double surfaceFactor;        // 4 pi surface_area_energy
+    const float* charge;         // q sqrt(ONE_4PI_EPS0)
+    const double2* radius;       // (rho = R - 0.009, s rho)
+    const double* atomRadius;    // R
+    long long* bornSum; long long* dEdB;
+    double* bornR; double* chain; double* bornForce;
 };
 
 // One integration unit = a SETTLE water, a SHAKE cluster (centre + <=3 H) or a free atom.
@@ -372,6 +389,47 @@ __device__ __forceinline__ long long float_to_fixed(float f) {           // |f| 
     const unsigned int lo = __float2uint_rz((f - fl)*4294967296.0f);
     return ((long long) hi << 32) | (long long) lo;
 }
+
+// minimum image of a displacement in fp32 (ReferenceForce::getDeltaRPeriodic order for triclinic boxes: c, b, a)
+__device__ __forceinline__ float3 min_image(float3 d, const BoxDev& b) {
+    if (b.triclinic) {
+        float s = floorf(d.z*b.invCz + 0.5f);
+        d.x -= s*b.cx; d.y -= s*b.cy; d.z -= s*b.cz;
+        s = floorf(d.y*b.invBy + 0.5f);
+        d.x -= s*b.bx; d.y -= s*b.by;
+        s = floorf(d.x*b.invAx + 0.5f);
+        d.x -= s*b.ax;
+    }
+    else {
+        d.x -= b.ax*rintf(d.x*b.invAx);
+        d.y -= b.by*rintf(d.y*b.invBy);
+        d.z -= b.cz*rintf(d.z*b.invCz);
+    }
+    return d;
+}
+
+// The tiles of a list live in TILE_REGIONS pools (flush_tile, nonbonded.cu).  Flat tile number f -> slot: lane r holds the
+// inclusive prefix sum of the pool counts; the pool of f is the number of prefixes <= f.  Read by the tile kernel and the
+// generalized Born pair passes (gbsa.cu).
+struct TileCursor {
+    int incl, total, cap;
+    __device__ __forceinline__ void init(const NbDev& nb, const ListDev& L, int lane) {
+        cap = nb.maxTiles/TILE_REGIONS;
+        int c = min(L.lc[LC_TILES + lane], cap);
+        for (int off = 1; off < 32; off <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, c, off);
+            if (lane >= off) c += v;
+        }
+        incl = c;
+        total = __shfl_sync(0xffffffffu, c, 31);
+    }
+    __device__ __forceinline__ int slot(int f) const {       // f < total, uniform over the warp
+        const int r = __popc(__ballot_sync(0xffffffffu, incl <= f));
+        const int before = __shfl_sync(0xffffffffu, incl, max(r-1, 0));
+        return r*cap + f - (r > 0 ? before : 0);
+    }
+};
+static_assert(TILE_REGIONS == 32, "TileCursor maps one pool to one lane");
 
 // ---- integration state in the working type R: float (single precision) or double (mixed precision) ----
 // The only place that knows the mixed layout: a position is posq.xyz (hi) + posqCorr.xyz (lo), stored as hi = (float) x,
@@ -528,6 +586,10 @@ void launch_custom(const NbDev& nb, const CustomDev& ct, int terms, bool energy,
 void launch_compound(const NbDev& nb, const CompoundDev& cd, bool energy, cudaStream_t s);
 const int CENTROID_LAUNCHES = 3;
 void launch_centroid(const NbDev& nb, const CompoundDev& cc, const CentroidDev& cn, bool energy, cudaStream_t s);     // centres, programs, scatter
+
+// the generalized Born chain on the current neighbour list: Born sums, radii + ACE + self terms, GB pairs, fold, chain-rule pairs
+const int GBSA_LAUNCHES = 5;
+void launch_gbsa(const NbDev& nb, const GbsaDev& gb, bool energy, cudaStream_t s);
 
 void launch_integrate(const NbDev& nb, const UnitDev& units, const IntegDev& integ, const CommDev& cd, cudaStream_t s);
 void launch_force_push(const NbDev& nb, const CommDev& cd, cudaStream_t s);          // partial forces of foreign atoms -> owners' inboxes

@@ -22,23 +22,6 @@
 
 #define FULL 0xffffffffu
 
-__device__ __forceinline__ float3 min_image(float3 d, const BoxDev& b) {
-    if (b.triclinic) {
-        float s = floorf(d.z*b.invCz + 0.5f);
-        d.x -= s*b.cx; d.y -= s*b.cy; d.z -= s*b.cz;
-        s = floorf(d.y*b.invBy + 0.5f);
-        d.x -= s*b.bx; d.y -= s*b.by;
-        s = floorf(d.x*b.invAx + 0.5f);
-        d.x -= s*b.ax;
-    }
-    else {
-        d.x -= b.ax*rintf(d.x*b.invAx);
-        d.y -= b.by*rintf(d.y*b.invBy);
-        d.z -= b.cz*rintf(d.z*b.invCz);
-    }
-    return d;
-}
-
 // squared distance from the (periodic image of the) point/box centre offset d to an axis-aligned box of half
 // extents h centred at the origin.  Orthorhombic: the per-axis nearest image minimises it.  Triclinic: the 3-step
 // reduction is not guaranteed to pick the image nearest to the BOX, so all 27 neighbouring images are tried
@@ -676,28 +659,6 @@ __device__ __forceinline__ float ewald_g(float w) {
 // slots, denormal/range fix-ups around rsqrtf and __fdividef, switch-function code in the main path).  This version is
 // written FMA-first with ftz approximate rcp/rsqrt (one Newton step restores rsqrt to <1 ulp) and moves the switching
 // function into its own instantiation: ~58 instructions per slot.
-// The tiles of a list live in TILE_REGIONS pools (flush_tile).  Flat tile number f -> slot: lane r holds the inclusive prefix
-// sum of the pool counts; the pool of f is the number of prefixes <= f.
-struct TileCursor {
-    int incl, total, cap;
-    __device__ __forceinline__ void init(const NbDev& nb, const ListDev& L, int lane) {
-        cap = nb.maxTiles/TILE_REGIONS;
-        int c = min(L.lc[LC_TILES + lane], cap);
-        for (int off = 1; off < 32; off <<= 1) {
-            const int v = __shfl_up_sync(FULL, c, off);
-            if (lane >= off) c += v;
-        }
-        incl = c;
-        total = __shfl_sync(FULL, c, 31);
-    }
-    __device__ __forceinline__ int slot(int f) const {       // f < total, uniform over the warp
-        const int r = __popc(__ballot_sync(FULL, incl <= f));
-        const int before = __shfl_sync(FULL, incl, max(r-1, 0));
-        return r*cap + f - (r > 0 ? before : 0);
-    }
-};
-static_assert(TILE_REGIONS == 32, "TileCursor maps one pool to one lane");
-
 __device__ __forceinline__ float wrap_rel(float p, float c, double L, double invL) {
     double r = (double) p - (double) c;
     r -= L*rint(r*invL);

@@ -8,12 +8,12 @@ from .systems import SystemDesc, NB_PME
 TERM_BONDS, TERM_ANGLES, TERM_TORSIONS, TERM_NB_DIRECT, TERM_NB_RECIP = 1, 2, 4, 8, 16
 TERM_RB_TORSIONS, TERM_CMAP, TERM_CUSTOM_TORSIONS = 32, 64, 128
 TERM_CUSTOM_BONDS, TERM_CUSTOM_EXTERNALS, TERM_CUSTOM_ANGLES, TERM_CUSTOM_COMPOUND = 256, 512, 1024, 2048
-TERM_CUSTOM_CENTROID, TERM_ALL = 4096, 8191
+TERM_CUSTOM_CENTROID, TERM_GBSA, TERM_ALL = 4096, 8192, 16383
 # kinds of b200md_set_bonded_groups
 BONDED_KINDS = {"bonds": 0, "angles": 1, "torsions": 2, "rb_torsions": 3, "cmap": 4, "custom_torsions": 5, "custom_bonds": 6,
                 "custom_externals": 7, "custom_angles": 9, "custom_compound": 10, "custom_centroid": 11}
 PHASES = {"pair": 0, "pme_spread": 1, "pme_fft_conv": 2, "pme_gather": 3, "integrate": 4, "list_build": 5, "bonded": 6,
-          "custom_torsions": 7, "custom_compound": 8, "custom_centroid": 9}
+          "custom_torsions": 7, "custom_compound": 8, "custom_centroid": 9, "gbsa": 10}
 
 
 class EngineError(RuntimeError):
@@ -140,6 +140,10 @@ class Engine:
         for kind, g in self._bonded_groups.items():
             g = _i32(g)
             self._ck(L.b200md_set_bonded_groups(self.h, BONDED_KINDS[kind], len(g), _ip(g)))
+        if len(d.gb_charges):
+            self._ck(L.b200md_set_gbsa(self.h, int(d.gb_method), float(d.cutoff), float(d.gb_solute_dielectric),
+                                       float(d.gb_solvent_dielectric), float(d.gb_surface_area_energy), _dp(_f64(d.gb_charges)),
+                                       _dp(_f64(d.gb_radii)), _dp(_f64(d.gb_scales))))
         if len(d.con_i):
             self._ck(L.b200md_set_constraints(self.h, len(d.con_i), _ip(_i32(d.con_i)), _ip(_i32(d.con_j)), _dp(_f64(d.con_d))))
         if d.cm_frequency:
@@ -261,6 +265,14 @@ class Engine:
     def update_custom_centroid_params(self, params):
         """New per-bond parameters [n, param_stride] for the same custom centroid bonds, groups and expressions."""
         self._update_custom(self.lib.b200md_update_custom_centroid_params, params)
+
+    # ---- CalcGBSAOBCForceKernel::copyParametersToContext ----
+    def update_gbsa_params(self, charges, radii, scales):
+        """New per-atom charges, radii and scale factors of the generalized Born force (one per atom, as before)."""
+        q, r, s = _f64(charges), _f64(radii), _f64(scales)
+        if not (len(q) == len(r) == len(s)):
+            raise ValueError("update_gbsa_params: charges, radii and scales differ in length")
+        self._ck(self.lib.b200md_update_gbsa_params(self.h, len(q), _dp(q), _dp(r), _dp(s)))
 
     def set_custom_globals(self, values):
         """The values of the global parameter slots the expressions read (the number of slots is fixed at definition)."""

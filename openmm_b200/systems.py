@@ -154,6 +154,16 @@ class SystemDesc:
     ccentroid_op: np.ndarray = field(default_factory=_i)
     ccentroid_arg: np.ndarray = field(default_factory=_i)
     ccentroid_imm: np.ndarray = field(default_factory=_d)
+    # GBSAOBCForce (gb_*): one charge (e), radius (nm) and scale per atom, or none when the System has no generalized Born
+    # force; its method (NB_NOCUTOFF, NB_CUTOFF_NONPERIODIC or NB_CUTOFF_PERIODIC; the cutoff is `cutoff`), dielectrics and
+    # surface-area energy (kJ/mol/nm^2)
+    gb_charges: np.ndarray = field(default_factory=_d)
+    gb_radii: np.ndarray = field(default_factory=_d)
+    gb_scales: np.ndarray = field(default_factory=_d)
+    gb_method: int = NB_NOCUTOFF
+    gb_solute_dielectric: float = 1.0
+    gb_solvent_dielectric: float = 78.5
+    gb_surface_area_energy: float = 2.25936
     con_i: np.ndarray = field(default_factory=_i)
     con_j: np.ndarray = field(default_factory=_i)
     con_d: np.ndarray = field(default_factory=_d)

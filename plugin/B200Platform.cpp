@@ -9,7 +9,8 @@
 // Supported: NonbondedForce (NoCutoff, CutoffNonPeriodic, CutoffPeriodic, PME; parameter offsets), HarmonicBondForce,
 // HarmonicAngleForce, PeriodicTorsionForce, RBTorsionForce, CMAPTorsionForce, CustomTorsionForce, CustomBondForce,
 // CustomExternalForce, CustomAngleForce, CustomCompoundBondForce, CustomCentroidBondForce (any number of objects, each in its own force group; custom forces without energy parameter
-// derivatives, expressions within the limits of custom_translate.h), CMMotionRemover;
+// derivatives, expressions within the limits of custom_translate.h), GBSAOBCForce (one per System, its method and cutoff
+// matching the NonbondedForce's; NoCutoff also without one), CMMotionRemover;
 // Verlet / Langevin / LangevinMiddle integrators; SETTLE + X-H_n SHAKE constraints; MonteCarloBarostat and
 // MonteCarloAnisotropicBarostat (ApplyMonteCarloBarostatKernel; MonteCarloMembraneBarostat is refused).  A Force class without a kernel here
 // makes Platform::supportsKernels() false; an unsupported OPTION of a supported class is rejected in contextCreated()
@@ -45,6 +46,7 @@
 #include "openmm/CustomAngleForce.h"
 #include "openmm/CustomCompoundBondForce.h"
 #include "openmm/CustomCentroidBondForce.h"
+#include "openmm/GBSAOBCForce.h"
 #include "openmm/CMMotionRemover.h"
 #include "openmm/VerletIntegrator.h"
 #include "openmm/LangevinIntegrator.h"
@@ -839,6 +841,41 @@ private:
     ObjectGlobals globals;
 };
 
+// GBSAOBCForce: the per-atom parameters go to the engine at initialize; execute() only records the term, so the lazy fused
+// step covers it like every other force.  validateSystem has checked the method against the NonbondedForce's.
+class B200CalcGBSAOBCForceKernel : public CalcGBSAOBCForceKernel {
+public:
+    B200CalcGBSAOBCForceKernel(string name, const Platform& platform, ContextImpl& context) : CalcGBSAOBCForceKernel(name, platform), context(context) {}
+    static void read(const GBSAOBCForce& force, vector<double>& q, vector<double>& r, vector<double>& s) {
+        const int n = force.getNumParticles();
+        q.resize(n); r.resize(n); s.resize(n);
+        for (int i = 0; i < n; i++) force.getParticleParameters(i, q[i], r[i], s[i]);
+    }
+    void initialize(const System& system, const GBSAOBCForce& force) {
+        PlatformData& d = getData(context);
+        if (d.finalized) throw OpenMMException("B200 platform: GBSAOBCForce initialised after the Context was finalised");
+        vector<double> q, r, s;
+        read(force, q, r, s);
+        const int method = force.getNonbondedMethod() == GBSAOBCForce::NoCutoff ? B200MD_NB_NOCUTOFF :
+                           force.getNonbondedMethod() == GBSAOBCForce::CutoffNonPeriodic ? B200MD_NB_CUTOFF_NONPERIODIC : B200MD_NB_CUTOFF_PERIODIC;
+        d.check(b200md_set_gbsa(d.ctx, method, force.getCutoffDistance(), force.getSoluteDielectric(), force.getSolventDielectric(),
+                                force.getSurfaceAreaEnergy(), q.data(), r.data(), s.data()));
+        d.systemTerms |= B200MD_TERM_GBSA;
+    }
+    double execute(ContextImpl& context, bool includeForces, bool includeEnergy) { getData(context).pendingTerms |= B200MD_TERM_GBSA; return 0.0; }
+    void copyParametersToContext(ContextImpl& context, const GBSAOBCForce& force) {
+        PlatformData& d = getData(context);
+        d.ensureFinalized();
+        d.dropForces();
+        if (force.getNumParticles() != d.numParticles) throw OpenMMException("updateParametersInContext: The number of particles has changed");
+        vector<double> q, r, s;
+        read(force, q, r, s);
+        d.check(b200md_update_gbsa_params(d.ctx, (int) q.size(), q.data(), r.data(), s.data()));
+    }
+private:
+    ContextImpl& context;
+};
+
 // RemoveCMMotionKernel::execute is called by CMMotionRemoverImpl::updateContextState in EVERY step; the frequency test is
 // the kernel's (ReferenceKernels.cpp:2712-2714).  The removal itself is deferred to the integrator step that follows (the
 // fused step graph removes the centre-of-mass motion itself) or to the next read of the velocities (PlatformData::flushCm).
@@ -972,6 +1009,7 @@ public:
         if (name == CalcCustomAngleForceKernel::Name()) return new B200CalcCustomForceKernel<CustomAngles>(name, platform, context);
         if (name == CalcCustomCompoundBondForceKernel::Name()) return new B200CalcCustomForceKernel<CustomCompounds>(name, platform, context);
         if (name == CalcCustomCentroidBondForceKernel::Name()) return new B200CalcCustomForceKernel<CustomCentroids>(name, platform, context);
+        if (name == CalcGBSAOBCForceKernel::Name()) return new B200CalcGBSAOBCForceKernel(name, platform, context);
         if (name == RemoveCMMotionKernel::Name()) return new B200RemoveCMMotionKernel(name, platform, context);
         if (name == IntegrateVerletStepKernel::Name()) return new B200IntegrateVerletStepKernel(name, platform);
         if (name == IntegrateLangevinStepKernel::Name()) return new B200IntegrateLangevinStepKernel(name, platform);
@@ -990,7 +1028,7 @@ public:
                                 CalcPeriodicTorsionForceKernel::Name(), CalcRBTorsionForceKernel::Name(), CalcCMAPTorsionForceKernel::Name(),
                                 CalcCustomTorsionForceKernel::Name(), CalcCustomBondForceKernel::Name(), CalcCustomExternalForceKernel::Name(),
                                 CalcCustomAngleForceKernel::Name(), CalcCustomCompoundBondForceKernel::Name(), CalcCustomCentroidBondForceKernel::Name(),
-                                RemoveCMMotionKernel::Name(), IntegrateVerletStepKernel::Name(),
+                                CalcGBSAOBCForceKernel::Name(), RemoveCMMotionKernel::Name(), IntegrateVerletStepKernel::Name(),
                                 IntegrateLangevinStepKernel::Name(), IntegrateLangevinMiddleStepKernel::Name(), ApplyMonteCarloBarostatKernel::Name()})
             registerKernelFactory(n, factory);
         platformProperties.push_back(DeviceIndex());
@@ -1029,13 +1067,45 @@ public:
         catch (const b200md_custom::Unsupported&) { throw; }
         catch (const OpenMMException&) {}
     }
+    // A GBSAOBCForce: the generalized Born chain walks the NonbondedForce's neighbour list, so its method and cutoff must be
+    // that list's (CutoffPeriodic goes with CutoffPeriodic or PME, which is what ForceField builds for PME); without a
+    // NonbondedForce only NoCutoff, over the list of all pairs.  Radii at or below the dielectric offset are refused too.
+    static void validateGBSA(const System& system, const GBSAOBCForce& gbsa, const NonbondedForce* nonbonded) {
+        if (gbsa.getNumParticles() != system.getNumParticles())
+            throw OpenMMException("B200 platform: a GBSAOBCForce must have exactly as many particles as the System");
+        const GBSAOBCForce::NonbondedMethod m = gbsa.getNonbondedMethod();
+        if (!nonbonded) {
+            if (m != GBSAOBCForce::NoCutoff) throw OpenMMException("B200 platform: a GBSAOBCForce with a cutoff needs a NonbondedForce with the same cutoff");
+        }
+        else {
+            const NonbondedForce::NonbondedMethod n = nonbonded->getNonbondedMethod();
+            const bool match = m == GBSAOBCForce::NoCutoff ? n == NonbondedForce::NoCutoff :
+                               m == GBSAOBCForce::CutoffNonPeriodic ? n == NonbondedForce::CutoffNonPeriodic :
+                               (n == NonbondedForce::CutoffPeriodic || n == NonbondedForce::PME);
+            if (!match) throw OpenMMException("B200 platform: the GBSAOBCForce's nonbonded method does not match the NonbondedForce's");
+            if (m != GBSAOBCForce::NoCutoff && gbsa.getCutoffDistance() != nonbonded->getCutoffDistance())
+                throw OpenMMException("B200 platform: the GBSAOBCForce's cutoff differs from the NonbondedForce's");
+        }
+        for (int i = 0; i < gbsa.getNumParticles(); i++) {
+            double q, r, s;
+            gbsa.getParticleParameters(i, q, r, s);
+            if (!(r > 0.009)) throw OpenMMException("B200 platform: a GBSAOBCForce radius at or below the dielectric offset (0.009 nm)");
+        }
+    }
     static void validateSystem(const System& system) {
         for (int i = 0; i < system.getNumParticles(); i++)
             if (system.isVirtualSite(i)) throw OpenMMException("B200 platform: virtual sites are not supported");
         int numNonbonded = 0;
+        const NonbondedForce* nonbonded = nullptr;
+        const GBSAOBCForce* gbsa = nullptr;
         for (int f = 0; f < system.getNumForces(); f++) {
             const Force& force = system.getForce(f);
+            if (const GBSAOBCForce* g = dynamic_cast<const GBSAOBCForce*>(&force)) {
+                if (gbsa) throw OpenMMException("B200 platform: only one GBSAOBCForce per System is supported");
+                gbsa = g;
+            }
             if (const NonbondedForce* nb = dynamic_cast<const NonbondedForce*>(&force)) {
+                nonbonded = nb;
                 if (++numNonbonded > 1) throw OpenMMException("B200 platform: only one NonbondedForce per System is supported");
                 const NonbondedForce::NonbondedMethod m = nb->getNonbondedMethod();
                 if (m == NonbondedForce::Ewald || m == NonbondedForce::LJPME)
@@ -1051,6 +1121,7 @@ public:
             if (const CustomCompoundBondForce* f = dynamic_cast<const CustomCompoundBondForce*>(&force)) validateCustom<CustomCompounds>(*f);
             if (const CustomCentroidBondForce* f = dynamic_cast<const CustomCentroidBondForce*>(&force)) validateCustom<CustomCentroids>(*f);
         }
+        if (gbsa) validateGBSA(system, *gbsa, nonbonded);
         const int nc = system.getNumConstraints();
         if (nc > 0) {
             vector<int> ci(nc), cj(nc); vector<double> cd(nc), mass(system.getNumParticles());

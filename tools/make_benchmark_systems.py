@@ -6,13 +6,15 @@ examples/benchmark.py:97-138:
 
   dhfr  : amber99sb.xml + tip3p.xml on examples/5dfr_solv-cube_equil.pdb, PME, cutoff 0.9 nm, constraints=HBonds, rigid water
   apoa1 : amber14/protein.ff14SB + lipid17 + tip3p on examples/apoa1.pdb, PME, cutoff 1.0 nm, HBonds, hydrogenMass 1.5 amu
+  dhfr_gbsa : amber99sb.xml + amber99_obc.xml on examples/5dfr_minimized.pdb, CutoffNonPeriodic, cutoff 2 nm, HBonds (the
+              implicit-solvent protocol of examples/benchmark.py; the GBSA generator sets the reaction-field dielectric to 1)
 
 The stand-in only RECORDS what forcefield.py builds (particles, bonds, angles, torsions, constraints, nonbonded
 parameters); the one piece of C++ logic the application layer calls back into, NonbondedForce::createExceptionsFromBonds,
 is executed by the real reference library (oracle/_ref, oracle.omm.exceptions_from_bonds).  Output: data/<name>.npz
 (generated files are committed; /root/reference does not exist on the GPU box).
 
-Run: python tools/make_benchmark_systems.py [dhfr] [apoa1]
+Run: python tools/make_benchmark_systems.py [dhfr] [apoa1] [dhfr_gbsa]   (dhfr_gbsa -> tests/golden/dhfr_gbsa.npz)
 """
 import os
 import sys
@@ -223,6 +225,37 @@ def _install_mock():
         def setExceptionsUsePeriodicBoundaryConditions(self, p):
             pass
 
+    class GBSAOBCForce(Force):
+        NoCutoff, CutoffNonPeriodic, CutoffPeriodic = range(3)
+
+        def __init__(self):
+            Force.__init__(self)
+            self.particles = []
+            self.method, self.cutoff = 0, 1.0
+            self.solute, self.solvent, self.surface = 1.0, 78.5, 2.25936
+
+        def addParticle(self, q, radius, scale):
+            self.particles.append([float(s(q)), float(s(radius)), float(s(scale))])
+            return len(self.particles)-1
+
+        def getNumParticles(self):
+            return len(self.particles)
+
+        def setNonbondedMethod(self, m):
+            self.method = int(m)
+
+        def setCutoffDistance(self, c):
+            self.cutoff = float(s(c))
+
+        def setSoluteDielectric(self, d):
+            self.solute = float(d)
+
+        def setSolventDielectric(self, d):
+            self.solvent = float(d)
+
+        def setSurfaceAreaEnergy(self, e):
+            self.surface = float(s(e))
+
     class CMMotionRemover(Force):
         def __init__(self, frequency=1):
             Force.__init__(self)
@@ -232,7 +265,7 @@ def _install_mock():
         def __init__(self, *a, **k):
             pass
 
-    for cls in (Force, System, HarmonicBondForce, HarmonicAngleForce, PeriodicTorsionForce, NonbondedForce, CMMotionRemover):
+    for cls in (Force, System, HarmonicBondForce, HarmonicAngleForce, PeriodicTorsionForce, NonbondedForce, GBSAOBCForce, CMMotionRemover):
         setattr(mm, cls.__name__, cls)
     mm.Vec3 = Vec3
 
@@ -260,7 +293,7 @@ def to_desc(system, positions_nm, name):
     d = systems.SystemDesc(masses=np.array(system.masses), charges=p[:, 0], sigmas=p[:, 1], epsilons=p[:, 2],
                            positions=np.asarray(positions_nm, dtype=np.float64), box=system.box, method=nb.method, cutoff=nb.cutoff,
                            ewald_tol=nb.tol, use_switch=nb.switch, switch_distance=max(nb.switch_distance, 0.0),
-                           use_dispersion=nb.dispersion, name=name)
+                           use_dispersion=nb.dispersion, rf_dielectric=nb.rf, name=name)
     d.exc_i, d.exc_j = ex[:, 0].astype(np.int32), ex[:, 1].astype(np.int32)
     d.exc_qq, d.exc_sigma, d.exc_eps = ex[:, 2].copy(), ex[:, 3].copy(), ex[:, 4].copy()
     bonds = [b for f in system.forces if type(f).__name__ == "HarmonicBondForce" for b in f.bonds]
@@ -282,7 +315,18 @@ def to_desc(system, positions_nm, name):
         d.con_i, d.con_j, d.con_d = c[:, 0].astype(np.int32), c[:, 1].astype(np.int32), c[:, 2].copy()
     cm = [f for f in system.forces if type(f).__name__ == "CMMotionRemover"]
     d.cm_frequency = int(cm[0].frequency) if cm else 0
+    gb = [f for f in system.forces if type(f).__name__ == "GBSAOBCForce"]
+    if gb:
+        g = np.array(gb[0].particles)
+        d.gb_charges, d.gb_radii, d.gb_scales = g[:, 0].copy(), g[:, 1].copy(), g[:, 2].copy()
+        d.gb_method = gb[0].method
+        assert gb[0].method == NB_METHOD_OF_GB[nb.method] and (gb[0].method == 0 or gb[0].cutoff == nb.cutoff)
+        d.gb_solute_dielectric, d.gb_solvent_dielectric, d.gb_surface_area_energy = gb[0].solute, gb[0].solvent, gb[0].surface
     return d
+
+
+# GBSAOBCForce method that ForceField builds for each NonbondedForce method (forcefield.py GBSAOBCGenerator)
+NB_METHOD_OF_GB = {0: 0, 1: 1, 2: 2, 3: 2, 4: 2}
 
 
 def build(name):
@@ -302,18 +346,23 @@ def build(name):
         ff = app.ForceField("amber14/protein.ff14SB.xml", "amber14/lipid17.xml", "amber14/tip3p.xml")
         system = ff.createSystem(pdb.topology, nonbondedMethod=app.PME, nonbondedCutoff=1.0*unit.nanometer, constraints=app.HBonds, rigidWater=True,
                                  hydrogenMass=1.5*unit.amu)
+    elif name == "dhfr_gbsa":
+        pdb = app.PDBFile(os.path.join(EXAMPLES, "5dfr_minimized.pdb"))
+        ff = app.ForceField("amber99sb.xml", "amber99_obc.xml")
+        system = ff.createSystem(pdb.topology, nonbondedMethod=app.CutoffNonPeriodic, nonbondedCutoff=2.0*unit.nanometer, constraints=app.HBonds)
     else:
         raise SystemExit("unknown system " + name)
     pos = np.array(pdb.positions.value_in_unit(unit.nanometer))
-    if system.box is None:
+    if system.box is None and pdb.topology.getPeriodicBoxVectors() is not None:
         v = pdb.topology.getPeriodicBoxVectors().value_in_unit(unit.nanometer)
         system.box = np.array([[float(x) for x in row] for row in v])
     d = to_desc(system, pos, name)
-    os.makedirs(os.path.join(ROOT, "data"), exist_ok=True)
-    path = os.path.join(ROOT, "data", name + ".npz")
+    out = os.path.join(ROOT, "tests", "golden") if name == "dhfr_gbsa" else os.path.join(ROOT, "data")
+    os.makedirs(out, exist_ok=True)
+    path = os.path.join(out, name + ".npz")
     d.save(path)
     print("%s: %d atoms, box %s, %d bonds %d angles %d torsions %d exceptions %d constraints, cm_freq %d -> %s (%.1f MB)" % (
-        name, d.natoms, np.diag(d.box), len(d.bond_i), len(d.angle_i), len(d.tor_i), len(d.exc_i), len(d.con_i), d.cm_frequency, path,
+        name, d.natoms, None if d.box is None else np.diag(d.box), len(d.bond_i), len(d.angle_i), len(d.tor_i), len(d.exc_i), len(d.con_i), d.cm_frequency, path,
         os.path.getsize(path)/1e6))
     return d
 
