@@ -382,9 +382,16 @@ int b200md_get_stats(b200md_ctx* ctx, b200md_stats* out);
  * 6 bonded+exceptions (k_bonded and, with custom terms, k_custom and k_compound), 7 custom torsions, bonds, externals and
  * angles alone (k_custom), 8 custom compound bonds alone (k_compound), 9 custom centroid bonds alone (k_centroid_centers,
  * the k_compound instantiation that reads the centres, k_centroid_scatter), 10 the generalized Born chain (k_gb_born,
- * k_gb_radii, k_gb_pairs, k_gb_fold, k_gb_chain).
+ * k_gb_radii, k_gb_pairs, k_gb_fold, k_gb_chain), 11 the first half of the list build alone (k_list_prep: binning, sort,
+ * block bounds), 12 its second half alone (k_build_tiles).
  * Runs `reps` isolated launches of that phase on the current state.                                  */
 int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* ms_mean);
+/* The current neighbour list, read back for identity checks.  *ntiles = its tile count.  sorig (if not NULL): [padded_atoms]
+ * sorted slot -> user atom (-1 for padding).  tile_i / tile_j / tile_mask (all three, or none): the tiles flattened over
+ * the slot pools in pool order, at most `cap` of them: tile_i[t] = i-block, tile_j[32 t + lane] = sorted j-slot (-1 for
+ * an empty lane), tile_mask[32 t + lane] = the lane's mask word (bit k: pair with j-lane k is computed; 0xffffffff for a
+ * tile without a mask).  A tile's position in this flattening depends on the order in which tiles were emitted.      */
+int b200md_get_list(b200md_ctx* ctx, int* sorig, int64_t cap, int* tile_i, int* tile_j, unsigned int* tile_mask, int64_t* ntiles);
 /* stand-alone 3-D FFT entry (the bespoke FFT alone, for parity against fftpack / numpy):
  * in: real [nx][ny][nz] floats (host), out: complex [nx][ny][nz/2+1] (re,im) floats (host).          */
 int b200md_fft3d_r2c(int device, int nx, int ny, int nz, const float* in, float* out);

@@ -102,6 +102,7 @@ SIGNATURES = {
     "b200md_comm_init": (C.c_int, [_P, C.c_int, C.c_int, _P]),
     "b200md_get_stats": (C.c_int, [_P, C.POINTER(Stats)]),
     "b200md_time_phase": (C.c_int, [_P, C.c_int, C.c_int, _D]),
+    "b200md_get_list": (C.c_int, [_P, _I, C.c_int64, _I, _I, C.POINTER(C.c_uint), C.POINTER(C.c_int64)]),
     "b200md_fft3d_r2c": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, _F, _F]),
     "b200md_fft3d_c2r": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, _F, _F]),
     "b200md_pme_create": (C.c_int, [C.POINTER(_P), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double]),

@@ -2594,6 +2594,38 @@ extern "C" int b200md_get_stats(b200md_ctx* ctx, b200md_stats* out) {
     API_END(ctx)
 }
 
+extern "C" int b200md_get_list(b200md_ctx* ctx, int* sorig, int64_t cap, int* tile_i, int* tile_j, unsigned int* tile_mask, int64_t* ntiles) {
+    API_BEGIN(ctx)
+    require(ctx->finalized, "get_list before finalize");
+    const DevFlags f = read_flags(ctx, true);
+    const ListBufs& L = ctx->lists[f.ct[CT_CUR] & 1];
+    const int pool = ctx->nb.maxTiles/TILE_REGIONS;
+    int64_t total = 0;
+    for (int r = 0; r < TILE_REGIONS; r++) total += std::min(f.cur()[LC_TILES + r], pool);
+    *ntiles = total;
+    if (sorig) CUDA_CHECK(cudaMemcpy(sorig, L.sorig.p, sizeof(int)*ctx->npad, cudaMemcpyDeviceToHost));
+    if (tile_i && tile_j && tile_mask) {
+        require(cap >= total, "get_list: the tile arrays are smaller than the list");
+        std::vector<int> ti(ctx->nb.maxTiles), tj((size_t) ctx->nb.maxTiles*32), tm(ctx->nb.maxTiles);
+        std::vector<unsigned int> mp((size_t) ctx->nb.maxTiles*32);
+        CUDA_CHECK(cudaMemcpy(ti.data(), L.tileI.p, sizeof(int)*ti.size(), cudaMemcpyDeviceToHost));
+        CUDA_CHECK(cudaMemcpy(tj.data(), L.tileJ.p, sizeof(int)*tj.size(), cudaMemcpyDeviceToHost));
+        CUDA_CHECK(cudaMemcpy(tm.data(), L.tileMask.p, sizeof(int)*tm.size(), cudaMemcpyDeviceToHost));
+        CUDA_CHECK(cudaMemcpy(mp.data(), L.maskPool.p, sizeof(unsigned int)*mp.size(), cudaMemcpyDeviceToHost));
+        int64_t o = 0;
+        for (int r = 0; r < TILE_REGIONS; r++)
+            for (int k = 0; k < std::min(f.cur()[LC_TILES + r], pool); k++, o++) {
+                const size_t t = (size_t) r*pool + k;
+                tile_i[o] = ti[t];
+                for (int l = 0; l < 32; l++) {
+                    tile_j[o*32 + l] = tj[t*32 + l];
+                    tile_mask[o*32 + l] = tm[t] < 0 ? 0xffffffffu : mp[(size_t) tm[t]*32 + l];
+                }
+            }
+    }
+    API_END(ctx)
+}
+
 extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* ms_mean) {
     API_BEGIN(ctx)
     require(ctx->finalized, "time_phase before finalize");
@@ -2619,8 +2651,9 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
     }
     for (int r = -2; r < reps; r++) {
         if (phase == 4) state.restore(s);
-        if (phase == 5) set_counter(c, CT_REBUILD, 1);     // the list is not marked dirty: the next step adds no synchronous rebuild
+        if (phase == 5 || phase == 11 || phase == 12) set_counter(c, CT_REBUILD, 1);     // the list is not marked dirty: the next step adds no synchronous rebuild
         if (phase == 0) { CUDA_CHECK(cudaMemsetAsync(&c->counters.p[CT_CURSOR], 0, sizeof(int), s)); CUDA_CHECK(cudaMemsetAsync(&c->counters.p[CT_PAIRSTART], 0, sizeof(int), s)); }      // the SM-partitioned tile kernel's cursor starts from tile 0
+        if (phase == 12) launch_list_prep(c->nb, s);        // untimed: the tile pass reads what the prep pass sorted
         CUDA_CHECK(cudaEventRecord(e0, s));
         switch (phase) {
             case 0: launch_pair(c->nb, false, s); break;
@@ -2634,9 +2667,12 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
             case 8: launch_compound(c->nb, c->cpd, false, s); break;
             case 9: launch_centroid(c->nb, c->ccd, c->cen, false, s); break;
             case 10: launch_gbsa(c->nb, c->gbd, false, s); break;
+            case 11: launch_list_prep(c->nb, s); break;
+            case 12: launch_build_tiles(c->nb, s); break;
             default: throw std::runtime_error("unknown phase");
         }
         CUDA_CHECK(cudaEventRecord(e1, s));
+        if (phase == 11) launch_build_tiles(c->nb, s);      // untimed: completes the build (and flips the list) as phase 5 does
         CUDA_CHECK(cudaEventSynchronize(e1));
         float ms = 0; CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
         if (r >= 0) total += ms;

@@ -553,6 +553,8 @@ struct ScaleDev {
 void launch_check_displacement(const NbDev& nb, const CommDev& cd, cudaStream_t s);
 const int LIST_BUILD_LAUNCHES = 2;
 void launch_list_build(const NbDev& nb, cudaStream_t s);     // k_list_prep (grid barriers) + k_build_tiles, gated on counters[CT_REBUILD]
+void launch_list_prep(const NbDev& nb, cudaStream_t s);      // the two halves of launch_list_build (timed apart by b200md_time_phase)
+void launch_build_tiles(const NbDev& nb, cudaStream_t s);
 const int PAIR_LAUNCHES = 2;
 void launch_pair(const NbDev& nb, bool energy, cudaStream_t s);        // k_pair + k_fold_sorted (sorted -> user-order forces)
 void pair_set_carveout(size_t fftSmem, size_t brickSmem);     // shared memory for a chain CTA beside the tile CTAs left on an SM

@@ -143,29 +143,70 @@ __device__ __forceinline__ void bin_atom(const NbDev& nb, int a) {
     atomicAdd(&nb.cellCount[key], 1);
 }
 
-// exclusive scan of cellCount[0..ncells) into cellCount (in place), single block
-__device__ void scan_cells_block(const NbDev& nb, int* partial) {      // one CTA, partial[blockDim.x] in shared memory
-    int n = nb.ncells;
-    int per = (n + blockDim.x - 1)/blockDim.x;
-    int begin = threadIdx.x*per, end = min(begin+per, n);
-    int sum = 0;
-    for (int i = begin; i < end; i++) sum += nb.cellCount[i];
-    partial[threadIdx.x] = sum;
+// exclusive prefix sum over the CTA (blockDim.x a multiple of 32, at most 1,024 threads); *total = the CTA's sum.
+// ws: 32 ints of shared memory.
+__device__ __forceinline__ int block_exclusive_scan(int v, int* ws, int* total) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    int x = v;
+    for (int off = 1; off < 32; off <<= 1) {
+        const int y = __shfl_up_sync(FULL, x, off);
+        if (lane >= off) x += y;
+    }
+    if (lane == 31) ws[w] = x;
     __syncthreads();
-    // Hillis-Steele inclusive scan over the partials
-    for (int off = 1; off < blockDim.x; off <<= 1) {
-        int v = (threadIdx.x >= off) ? partial[threadIdx.x-off] : 0;
-        __syncthreads();
-        partial[threadIdx.x] += v;
-        __syncthreads();
+    if (w == 0) {
+        int t = (lane < nw) ? ws[lane] : 0;
+        for (int off = 1; off < 32; off <<= 1) {
+            const int y = __shfl_up_sync(FULL, t, off);
+            if (lane >= off) t += y;
+        }
+        if (lane < nw) ws[lane] = t;
     }
-    int run = partial[threadIdx.x] - sum;
-    for (int i = begin; i < end; i++) {
-        int c = nb.cellCount[i];
-        nb.cellCount[i] = run;
-        run += c;
+    __syncthreads();
+    const int r = x - v + (w > 0 ? ws[w-1] : 0);
+    *total = ws[nw-1];
+    __syncthreads();          // ws is reused by the next call
+    return r;
+}
+
+// exclusive scan of cellCount[0..ncells) into cellCount (in place), by the whole grid: CTA b scans the contiguous slice
+// [b*per, (b+1)*per) and adds the sums of the slices before it, which every CTA publishes as soon as it has its own (all
+// CTAs are co-resident, so the waits end).  The sums go to tmpSorted[0..G), which the binning phase zeroes (0 = not yet
+// published, else sum + 1) and the fill phase overwrites.  ws: 33 ints of shared memory.
+__device__ void scan_cells_grid(const NbDev& nb, int* ws) {
+    const int n = nb.ncells, per = (n + gridDim.x - 1)/gridDim.x;
+    const int begin = min((int) blockIdx.x*per, n), end = min(begin + per, n);
+    int* sums = nb.tmpSorted;
+    int local = 0;
+    for (int i = begin + threadIdx.x; i < end; i += blockDim.x) local += nb.cellCount[i];
+    int mine;
+    block_exclusive_scan(local, ws, &mine);
+    if (threadIdx.x == 0) atomicExch(&sums[blockIdx.x], mine + 1);
+    if (threadIdx.x < 32) {
+        int before = 0;
+        for (int b = threadIdx.x; b < (int) blockIdx.x; b += 32) {
+            int v;
+            long spins = 0;
+            while ((v = *((volatile int*) &sums[b])) == 0) {
+                __nanosleep(32);
+                if (++spins > (1L << 23)) { nb.counters[CT_OVERFLOW] = 2; v = 1; break; }
+            }
+            before += v - 1;
+        }
+        for (int off = 16; off > 0; off >>= 1) before += __shfl_xor_sync(FULL, before, off);
+        if (threadIdx.x == 0) ws[32] = before;
     }
-    if (threadIdx.x == 0) nb.cellCount[n] = nb.natoms;
+    __syncthreads();
+    int run = ws[32];
+    for (int c0 = begin; c0 < end; c0 += blockDim.x) {
+        const int i = c0 + threadIdx.x;
+        const int c = (i < end) ? nb.cellCount[i] : 0;
+        int chunk;
+        const int r = block_exclusive_scan(c, ws, &chunk);
+        if (i < end) nb.cellCount[i] = run + r;
+        run += chunk;
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) nb.cellCount[n] = nb.natoms;
 }
 
 __device__ __forceinline__ void fill_atom(const NbDev& nb, int a) {
@@ -231,7 +272,7 @@ __device__ __forceinline__ void grid_barrier(const NbDev& nb, int target) {
     __syncthreads();
 }
 
-__device__ void list_prep_phases(const NbDev& nb, const ListDev& L, int* partial) {
+__device__ void list_prep_phases(const NbDev& nb, const ListDev& L, int* ws) {
     const int G = gridDim.x;
     const int gtid = blockIdx.x*blockDim.x + threadIdx.x, gthreads = G*blockDim.x;
     const int lane = threadIdx.x & 31, gwarp = gtid >> 5, gwarps = gthreads >> 5;
@@ -244,9 +285,10 @@ __device__ void list_prep_phases(const NbDev& nb, const ListDev& L, int* partial
     }
     // 1. binning
     for (int a = gtid; a < nb.natoms; a += gthreads) bin_atom(nb, a);
+    if (gtid < G) nb.tmpSorted[gtid] = 0;          // the scan's slice sums (npad >= G)
     grid_barrier(nb, base + G);
-    // 2. exclusive scan of the cell counts (one CTA)
-    if (blockIdx.x == 0) scan_cells_block(nb, partial);
+    // 2. exclusive scan of the cell counts
+    scan_cells_grid(nb, ws);
     grid_barrier(nb, base + 2*G);
     // 3. atoms into their cells
     for (int a = gtid; a < nb.natoms; a += gthreads) fill_atom(nb, a);
@@ -310,31 +352,37 @@ __device__ __forceinline__ void grid_barrier_exit(const NbDev& nb) {
 __global__ void __launch_bounds__(256) k_list_prep(NbDev nb) {
     if (nb.counters[CT_REBUILD] == 0) return;
     const ListDev& L = nb.list[(nb.counters[CT_CUR] & 1) ^ 1];      // the list under construction
-    __shared__ int partial[256];
-    list_prep_phases(nb, L, partial);
+    __shared__ int ws[33];
+    list_prep_phases(nb, L, ws);
     grid_barrier_exit(nb);
 }
 
 #define MAX_CACHED_EXCL 24
+#define TILE_SPAN 1024         // sorted-index span of a tile that flush_tile indexes directly (bytes of shared memory per warp)
 #define SB_MAX 1024            // superblocks listed per pass of k_build_tiles (1024 superblocks = 1.05 M atoms)
 // Emit one tile from the first `count` entries of buf (ascending sorted indices).
 // sexc: this lane's exclusion partners as SORTED indices, cached once per i-block (nexc of them; partners beyond
-// MAX_CACHED_EXCL are looked up in global memory).
+// MAX_CACHED_EXCL are looked up in global memory).  esig: bit (b mod 32) is set for every block b that holds one of them
+// (all bits when some are not cached): the partners are only searched in tiles that hold such a block.  slotOf: this warp's
+// TILE_SPAN bytes of shared memory, all zero on entry and on return; a tile whose j-slots span fewer than TILE_SPAN
+// sorted indices is indexed through it (slotOf[j - first j] = lane + 1), wider ones are searched by bisection.
 // Tile slots come from TILE_REGIONS independent sub-pools (i-block ib allocates from pool ib % TILE_REGIONS): one global
 // counter would take ~14k (DHFR) to ~66k (ApoA1) returning atomics on ONE address per build, which L2 serialises at ~2 ns
 // each.  Pool r owns the slots [r*cap, (r+1)*cap), cap = maxTiles/TILE_REGIONS; consumers flatten the pools with a
 // 32-lane prefix sum (tile_cursor below).
 __device__ void flush_tile(const NbDev& nb, const ListDev& L, int ib, const int* buf, int count, bool diagonal, int lane,
-                           const int* sexc, int nexc, int e0) {
+                           const int* sexc, int nexc, int e0, unsigned int esig, unsigned char* slotOf) {
     const int region = ib % TILE_REGIONS;
     const int cap = nb.maxTiles/TILE_REGIONS;
     int k = 0;
-    if (lane == 0) k = atomicAdd(&L.lc[LC_TILES + region], 1);
-    k = __shfl_sync(FULL, k, 0);
-    if (k >= cap) { if (lane == 0) nb.counters[CT_OVERFLOW] = 1; return; }
-    const int t = region*cap + k;
-    int myj = (lane < count) ? buf[lane] : -1;
-    L.tileJ[t*32 + lane] = myj;
+    if (lane == 0) k = atomicAdd(&L.lc[LC_TILES + region], 1);      // the slot is not needed until the mask is formed
+    const int myj = (lane < count) ? buf[lane] : -1;
+    const unsigned int tsig = __reduce_or_sync(FULL, (lane < count) ? 1u << ((myj >> 5) & 31) : 0u);   // blocks in the tile
+    const bool indexed = (buf[count-1] - buf[0] < TILE_SPAN) && (esig & tsig) != 0u;
+    if (__any_sync(FULL, indexed)) {
+        if (lane < count) slotOf[myj - buf[0]] = (unsigned char) (lane + 1);
+        __syncwarp();
+    }
     unsigned int valid = (count >= 32) ? FULL : ((1u << count) - 1u);
     unsigned int mask = valid;
     bool need = (count < 32);
@@ -345,22 +393,40 @@ __device__ void flush_tile(const NbDev& nb, const ListDev& L, int ib, const int*
         need = true;
     }
     if (si >= nb.natoms) { mask = 0; need = true; }
-    else {
+    else if (esig & tsig) {
         const int jlo = buf[0], jhi = buf[count-1];
-        for (int e = 0; e < nexc; e++) {
-            const int sj = (e < MAX_CACHED_EXCL) ? sexc[e] : nb.sortedOf[nb.exclList[e0 + e]];
-            if (sj < jlo || sj > jhi) continue;
-            int lo = 0, hi = count-1;          // binary search in the ascending tile
-            while (lo < hi) { int mid = (lo+hi) >> 1; if (buf[mid] < sj) lo = mid+1; else hi = mid; }
-            if (buf[lo] == sj) { mask &= ~(1u << lo); need = true; }
+        if (jhi - jlo < TILE_SPAN) {
+            for (int e = 0; e < nexc; e++) {
+                const int sj = (e < MAX_CACHED_EXCL) ? sexc[e] : nb.sortedOf[nb.exclList[e0 + e]];
+                if (!((tsig >> ((sj >> 5) & 31)) & 1u) || sj < jlo || sj > jhi) continue;
+                const int p = slotOf[sj - jlo];
+                if (p) { mask &= ~(1u << (p - 1)); need = true; }
+            }
+        }
+        else {
+            for (int e = 0; e < nexc; e++) {
+                const int sj = (e < MAX_CACHED_EXCL) ? sexc[e] : nb.sortedOf[nb.exclList[e0 + e]];
+                if (!((tsig >> ((sj >> 5) & 31)) & 1u) || sj < jlo || sj > jhi) continue;
+                int lo = 0, hi = count-1;          // binary search in the ascending tile
+                while (lo < hi) { int mid = (lo+hi) >> 1; if (buf[mid] < sj) lo = mid+1; else hi = mid; }
+                if (buf[lo] == sj) { mask &= ~(1u << lo); need = true; }
+            }
         }
     }
     need = __any_sync(FULL, need);
+    if (__any_sync(FULL, indexed)) {
+        __syncwarp();
+        if (lane < count) slotOf[myj - buf[0]] = 0;
+    }
+    k = __shfl_sync(FULL, k, 0);
+    if (k >= cap) { if (lane == 0) nb.counters[CT_OVERFLOW] = 1; return; }
+    const int t = region*cap + k;
+    L.tileJ[t*32 + lane] = myj;
     int mi = -1;
-    if (need) {
-        if (lane == 0) mi = atomicAdd(&L.lc[LC_MASKS + region], 1);
-        mi = region*cap + __shfl_sync(FULL, mi, 0);          // mask tiles <= tiles in every pool
-        L.maskPool[mi*32 + lane] = mask;     // capacity == maxTiles, and mask tiles <= tiles
+    if (need) {             // the mask takes the tile's own slot of maskPool (capacity == maxTiles): no second returning atomic
+        if (lane == 0) atomicAdd(&L.lc[LC_MASKS + region], 1);
+        mi = t;
+        L.maskPool[mi*32 + lane] = mask;
     }
     if (lane == 0) { L.tileI[t] = ib; L.tileMask[t] = mi; }
 }
@@ -388,8 +454,11 @@ struct BuildSmem {
     int sbuf[NW][64];
     int sstage[NW][64];                           // j-atoms that passed the box test and wait for the exact cull
     int sexcAll[32][MAX_CACHED_EXCL + 1];         // +1: odd stride, conflict-free per-lane rows
+    unsigned int sexcSigPart[NW][32];             // blocks (mod 32) of the partners each warp translated ...
+    unsigned int sexcSig[32];                     // ... and of all of a lane's partners (flush_tile's esig)
     float4 sipos[32];                             // the i-block's atoms, relative to the block centre
     int sleft[NW];
+    __align__(16) unsigned char sslotOf[NW][TILE_SPAN];          // flush_tile's j-slot -> lane index, kept all zero between flushes
     int sbList[SB_MAX];                           // superblocks within range of this i-block
     int sbCount;
     int smerged[NW*32];
@@ -403,19 +472,30 @@ __device__ __forceinline__ void group_sync(int barId, int nthreads) {
 template <int NW>
 __device__ void build_tiles_iblock(const NbDev& nb, const ListDev& L, int ib, int w, int lane, BuildSmem<NW>& S, int barId) {
     int* buf = S.sbuf[w];
-    // this lane's exclusion partners, translated to sorted indices ONCE per i-block
+    // this lane's exclusion partners, translated to sorted indices ONCE per i-block; the warps share the dependent
+    // exclList -> sortedOf look-ups (up to MAX_CACHED_EXCL per lane for protein atoms), warp w taking partners w, w+NW, ..
     int* sexc = S.sexcAll[lane];
     int nexc = 0, e0 = 0;
     {
         const int si = ib*32 + lane;
+        unsigned int sig = 0;
         if (si < nb.natoms) {
             const int a = L.sorig[si];
             e0 = nb.exclStart[a];
             nexc = nb.exclStart[a+1] - e0;
-            if (w == 0)
-                for (int e = 0; e < nexc && e < MAX_CACHED_EXCL; e++) sexc[e] = nb.sortedOf[nb.exclList[e0 + e]];
+            for (int e = w; e < nexc && e < MAX_CACHED_EXCL; e += NW) {
+                const int sj = nb.sortedOf[nb.exclList[e0 + e]];
+                sexc[e] = sj;
+                sig |= 1u << ((sj >> 5) & 31);
+            }
+            if (nexc > MAX_CACHED_EXCL) sig = FULL;
         }
+        S.sexcSigPart[w][lane] = sig;
+        for (int i = threadIdx.x; i < NW*TILE_SPAN/16; i += NW*32) reinterpret_cast<int4*>(&S.sslotOf[0][0])[i] = make_int4(0, 0, 0, 0);
     }
+    auto flush = [&](const int* tile, int count, bool diagonal) {
+        flush_tile(nb, L, ib, tile, count, diagonal, lane, sexc, nexc, e0, S.sexcSig[lane], S.sslotOf[w]);
+    };
     const float4 ci = L.blockCenter[ib];
     const float4 hi = L.blockHalf[ib];
     if (w == 0) {
@@ -424,6 +504,11 @@ __device__ void build_tiles_iblock(const NbDev& nb, const ListDev& L, int ib, in
         S.sipos[lane] = make_float4(qx, qy, qz, qx*qx + qy*qy + qz*qz);
     }
     group_sync(barId, NW*32);
+    if (w == 0) {                 // read after the group barrier that opens the superblock pass
+        unsigned int sig = 0;
+        for (int q = 0; q < NW; q++) sig |= S.sexcSigPart[q][lane];
+        S.sexcSig[lane] = sig;
+    }
     const bool periodic = nb.box.periodic != 0;
     const bool allPairs = (nb.method == B200MD_NB_NOCUTOFF);
     // same condition as the pair kernel's SHIFT mode (lc[LC_MAXHALF] = max block half extent of THIS build)
@@ -447,9 +532,15 @@ __device__ void build_tiles_iblock(const NbDev& nb, const ListDev& L, int ib, in
             const float3 d = min_image(make_float3(pj.x-ci.x, pj.y-ci.y, pj.z-ci.z), nb.box);
             const float mx = -2.0f*d.x, my = -2.0f*d.y, mz = -2.0f*d.z;
             const float thr = nb.paddedCutoff2*1.00001f - (d.x*d.x + d.y*d.y + d.z*d.z);
-            for (int k = 0; k < 32; k++) {
-                const float4 q = S.sipos[k];
-                if (fmaf(mx, q.x, fmaf(my, q.y, fmaf(mz, q.z, q.w))) < thr) { inc = true; break; }
+            // four i-atoms per step: their loads and FMA chains overlap, and only the step's verdict branches
+            for (int k = 0; k < 32; k += 4) {
+                bool hit = false;
+#pragma unroll
+                for (int u = 0; u < 4; u++) {
+                    const float4 q = S.sipos[k + u];
+                    hit |= (fmaf(mx, q.x, fmaf(my, q.y, fmaf(mz, q.z, q.w))) < thr);
+                }
+                if (hit) { inc = true; break; }
             }
         }
         const unsigned int m = __ballot_sync(FULL, inc);
@@ -458,7 +549,7 @@ __device__ void build_tiles_iblock(const NbDev& nb, const ListDev& L, int ib, in
         nbuf += __popc(m);
         __syncwarp();
         if (nbuf >= 32) {
-            flush_tile(nb, L, ib, buf, 32, false, lane, sexc, nexc, e0);
+            flush(buf, 32, false);
             const int v = (lane + 32 < nbuf) ? buf[lane+32] : 0;
             __syncwarp();
             buf[lane] = v;
@@ -556,12 +647,12 @@ __device__ void build_tiles_iblock(const NbDev& nb, const ListDev& L, int ib, in
             __syncwarp();
             if (jblk == ib) {
                 // the diagonal tile is always emitted on its own so that its mask is the simple j>i triangle
-                flush_tile(nb, L, ib, buf, nbuf, true, lane, sexc, nexc, e0);
+                flush(buf, nbuf, true);
                 nbuf = 0;
                 __syncwarp();
             }
             else if (nbuf >= 32) {
-                flush_tile(nb, L, ib, buf, 32, false, lane, sexc, nexc, e0);
+                flush(buf, 32, false);
                 int v = (lane + 32 < nbuf) ? buf[lane+32] : 0;
                 __syncwarp();
                 buf[lane] = v;
@@ -572,7 +663,8 @@ __device__ void build_tiles_iblock(const NbDev& nb, const ListDev& L, int ib, in
     }
     }   // superblock chunks
     if (exactCull && nstg > 0) exact_stage(nstg);
-    // merge the four partial buffers (each ascending, < 32 entries): rank sort into S.smerged, flush by warp 0
+    // merge the NW partial buffers (each ascending, < 32 entries): rank sort into S.smerged, flushed by the warps in turn.
+    // A value's rank in buffer q is found by binary search (5 steps, not a scan of the whole buffer).
     if (lane == 0) S.sleft[w] = nbuf;
     group_sync(barId, NW*32);
     int total = 0;
@@ -581,14 +673,16 @@ __device__ void build_tiles_iblock(const NbDev& nb, const ListDev& L, int ib, in
         const int v = buf[lane];
         int rank = 0;
         for (int q = 0; q < NW; q++) {
-            const int nq = S.sleft[q];
-            for (int k = 0; k < nq; k++) rank += (S.sbuf[q][k] < v);
+            const int* bq = S.sbuf[q];
+            int lo = 0, hi = S.sleft[q];
+            while (lo < hi) { const int mid = (lo + hi) >> 1; if (bq[mid] < v) lo = mid + 1; else hi = mid; }
+            rank += lo;
         }
         S.smerged[rank] = v;                 // sorted indices are unique, so ranks are a permutation
     }
     group_sync(barId, NW*32);
     for (int off = 32*w; off < total; off += 32*NW)
-        flush_tile(nb, L, ib, S.smerged + off, min(32, total - off), false, lane, sexc, nexc, e0);
+        flush(S.smerged + off, min(32, total - off), false);
     group_sync(barId, NW*32);          // the group's shared memory is reused by its next i-block
 }
 
@@ -610,16 +704,24 @@ void launch_check_displacement(const NbDev& nb, const CommDev& cd, cudaStream_t 
     k_check_gather<<<(nb.npad+255)/256, 256, 0, s>>>(nb, cd);
 }
 
-void launch_list_build(const NbDev& nb, cudaStream_t s) {
-    // LIST_BUILD_LAUNCHES kernels, each returns immediately unless counters[CT_REBUILD] is set
+void launch_list_prep(const NbDev& nb, cudaStream_t s) {
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     k_list_prep<<<std::max(1, std::min((nb.npad + 255)/256, 2*sms)), 256, 0, s>>>(nb);
+}
+
+void launch_build_tiles(const NbDev& nb, cudaStream_t s) {
     // 8 warps per i-block shorten the dependent chain while the grid is under one wave (measured: DHFR 108 -> 98 us per
     // build); above that the extra CTAs only add waves (ApoA1 225 -> 244 us), so large systems keep 4
     if (nb.nblocks <= 1200) k_build_tiles<8><<<nb.nblocks, 256, 0, s>>>(nb);
     else k_build_tiles<4><<<nb.nblocks, 128, 0, s>>>(nb);
+}
+
+void launch_list_build(const NbDev& nb, cudaStream_t s) {
+    // LIST_BUILD_LAUNCHES kernels, each returns immediately unless counters[CT_REBUILD] is set
+    launch_list_prep(nb, s);
+    launch_build_tiles(nb, s);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -13,7 +13,7 @@ TERM_CUSTOM_CENTROID, TERM_GBSA, TERM_ALL = 4096, 8192, 16383
 BONDED_KINDS = {"bonds": 0, "angles": 1, "torsions": 2, "rb_torsions": 3, "cmap": 4, "custom_torsions": 5, "custom_bonds": 6,
                 "custom_externals": 7, "custom_angles": 9, "custom_compound": 10, "custom_centroid": 11}
 PHASES = {"pair": 0, "pme_spread": 1, "pme_fft_conv": 2, "pme_gather": 3, "integrate": 4, "list_build": 5, "bonded": 6,
-          "custom_torsions": 7, "custom_compound": 8, "custom_centroid": 9, "gbsa": 10}
+          "custom_torsions": 7, "custom_compound": 8, "custom_centroid": 9, "gbsa": 10, "list_prep": 11, "list_tiles": 12}
 
 
 class EngineError(RuntimeError):
@@ -319,6 +319,17 @@ class Engine:
         s = _lib.Stats()
         self._ck(self.lib.b200md_get_stats(self.h, C.byref(s)))
         return {k: (list(getattr(s, k)) if k == "pme_grid" else getattr(s, k)) for k, _ in s._fields_}
+
+    def get_list(self):
+        """(sorig [padded atoms], tile_i [T], tile_j [T, 32], tile_mask [T, 32] uint32) of the current neighbour list; the
+        tiles in the order of the slot pools, which depends on the order in which they were emitted"""
+        n = C.c_int64()
+        sorig = np.empty(self.stats()["padded_atoms"], dtype=np.int32)
+        self._ck(self.lib.b200md_get_list(self.h, _ip(sorig), 0, None, None, None, C.byref(n)))
+        t = n.value
+        ti, tj, tm = np.empty(t, np.int32), np.empty((t, 32), np.int32), np.empty((t, 32), np.uint32)
+        self._ck(self.lib.b200md_get_list(self.h, None, t, _ip(ti), _ip(tj), tm.ctypes.data_as(C.POINTER(C.c_uint)), C.byref(n)))
+        return sorig, ti, tj, tm
 
     def time_phase(self, phase, reps=20):
         ms = C.c_double()
