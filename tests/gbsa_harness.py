@@ -83,17 +83,23 @@ def hello_nacl():
     return d
 
 
-def ion_box(n=400, edge=3.2, cutoff=1.2, method=systems.NB_CUTOFF_PERIODIC, seed=11):
-    """n ions of alternating charge +-1 on a jittered lattice in a cubic box, GBSA radii 0.15-0.2 nm; periodic methods
-    keep the box, NB_NOCUTOFF and NB_CUTOFF_NONPERIODIC drop it.  The GBSAOBCForce takes CutoffPeriodic for PME."""
+def ion_box(n=400, edge=3.2, cutoff=1.2, method=systems.NB_CUTOFF_PERIODIC, seed=11, box=None):
+    """n ions of alternating charge +-1 on a jittered lattice in a cubic box of edge `edge`, or of the cell `box` (rows a,
+    b, c; reduced form) when given; GBSA radii 0.15-0.2 nm.  Periodic methods keep the box, NB_NOCUTOFF and
+    NB_CUTOFF_NONPERIODIC drop it.  The GBSAOBCForce takes CutoffPeriodic for PME."""
     rng = np.random.default_rng(seed)
     m = int(np.ceil(n**(1/3)))
     g = np.stack(np.meshgrid(*[np.arange(m)]*3, indexing="ij"), -1).reshape(-1, 3)[:n]
-    pos = (g + 0.5 + 0.25*rng.uniform(-1, 1, (n, 3)))*(edge/m)
+    if box is None:
+        pos = (g + 0.5 + 0.25*rng.uniform(-1, 1, (n, 3)))*(edge/m)
+        box = np.eye(3)*edge
+    else:
+        box = np.asarray(box, dtype=np.float64)
+        pos = ((g + 0.5 + 0.25*rng.uniform(-1, 1, (n, 3)))/m) @ box
     q = np.where(np.arange(n) % 2 == 0, 1.0, -1.0)
     periodic = method in (systems.NB_CUTOFF_PERIODIC, systems.NB_PME)
     d = systems.SystemDesc(masses=np.full(n, 30.0), charges=q, sigmas=np.full(n, 0.3), epsilons=np.full(n, 0.4), positions=pos,
-                           box=np.eye(3)*edge if periodic else None, method=method, cutoff=cutoff, rf_dielectric=1.0,
+                           box=box if periodic else None, method=method, cutoff=cutoff, rf_dielectric=1.0,
                            use_dispersion=False, name="ion_box")
     d.gb_charges = q.copy()
     d.gb_radii = rng.uniform(0.15, 0.2, n)
@@ -102,12 +108,31 @@ def ion_box(n=400, edge=3.2, cutoff=1.2, method=systems.NB_CUTOFF_PERIODIC, seed
     return d
 
 
+# the edges of OpenMM's reduced form (a = 3 nm, b.x = +-a/2, c.x = -+a/2, c.y = +-b/2), as tests/test_gpu_oracle_edges.py
+TRICLINIC_LIMITS = {"pmp": (1.5, -1.5, 1.5), "mpm": (-1.5, 1.5, -1.5)}
+
+
+def triclinic_ion_box(sign):
+    """400 ions in the reduced-form limit cell `sign` (a key of TRICLINIC_LIMITS), CutoffPeriodic at 0.49 times the
+    smallest cell width (1.09 nm of 2.23): every pair within the cutoff has one image that the single-pass reduction of
+    ReferenceForce::getDeltaRPeriodic finds"""
+    bx, cx, cy = TRICLINIC_LIMITS[sign]
+    box = np.array([[3.0, 0, 0], [bx, 3.0, 0], [cx, cy, 3.0]])
+    a, b, c = box
+    v = abs(np.dot(a, np.cross(b, c)))
+    width = min(v/np.linalg.norm(np.cross(b, c)), v/np.linalg.norm(np.cross(c, a)), v/np.linalg.norm(np.cross(a, b)))
+    d = ion_box(cutoff=round(0.49*width, 2), box=box, seed=12)
+    d.name = "ion_box_tri_" + sign
+    return d
+
+
 def golden_cases():
     """The cases of tests/golden/reference_gbsa.npz (make_golden_gbsa.py), by name"""
     custom = ion_box(method=systems.NB_NOCUTOFF)
     custom.gb_surface_area_energy, custom.gb_solute_dielectric, custom.gb_solvent_dielectric = 0.0, 4.0, 40.0
     return {"dhfr_nocutoff": dhfr_gbsa(systems.NB_NOCUTOFF), "dhfr_cutoff": dhfr_gbsa(), "hello_nacl": hello_nacl(),
-            "ion_box": ion_box(), "ion_box_custom": custom}
+            "ion_box": ion_box(), "ion_box_custom": custom,
+            "ion_box_tri_pmp": triclinic_ion_box("pmp"), "ion_box_tri_mpm": triclinic_ion_box("mpm")}
 
 
 # ---------------------------------------------------------------- the restatement

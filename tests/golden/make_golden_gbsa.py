@@ -6,6 +6,8 @@ against:
   hello_nacl       the six ions of the reference's HelloSodiumChloride example
   ion_box          400 ions in a 3.2 nm periodic box, CutoffPeriodic, 1.2 nm
   ion_box_custom   the same ions at NoCutoff, surface-area energy 0, dielectrics 4 and 40
+  ion_box_tri_pmp  400 ions in the triclinic cell at the (+, -, +) limits of the reduced form, CutoffPeriodic 1.09 nm
+  ion_box_tri_mpm  the same at the (-, +, -) limits
 Each case stores the positions it was evaluated at and the GBSAOBCForce's energy and forces.
 
 Run: python tests/golden/make_golden_gbsa.py

@@ -11,7 +11,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import gbsa_harness as H  # noqa: E402
 from openmm_b200 import systems  # noqa: E402
 
-CASES = ("dhfr_nocutoff", "dhfr_cutoff", "hello_nacl", "ion_box", "ion_box_custom")
+CASES = ("dhfr_nocutoff", "dhfr_cutoff", "hello_nacl", "ion_box", "ion_box_custom", "ion_box_tri_pmp", "ion_box_tri_mpm")
 
 
 @pytest.mark.parametrize("name", CASES)

@@ -66,10 +66,13 @@ def test_dhfr_gbsa_plugin_matches_reference(H, method):
     assert err <= FORCE_BAR and abs(e - er) <= ENERGY_BAR*abs(er), (err, e, er)
 
 
-@pytest.mark.parametrize("case", ["dhfr_nocutoff", "dhfr_cutoff", "ion_box_periodic", "ion_box_pme", "ion_box_custom", "hello_nacl"])
+@pytest.mark.parametrize("case", ["dhfr_nocutoff", "dhfr_cutoff", "ion_box_periodic", "ion_box_pme", "ion_box_custom", "hello_nacl",
+                                  "ion_box_tri_pmp", "ion_box_tri_mpm"])
 def test_engine_matches_the_restatement(H, case):
     from openmm_b200 import Engine, systems
-    if case.startswith("dhfr"):
+    if case.startswith("ion_box_tri"):
+        d = H.triclinic_ion_box(case.split("_")[-1])
+    elif case.startswith("dhfr"):
         d = H.dhfr_gbsa(systems.NB_NOCUTOFF if case == "dhfr_nocutoff" else systems.NB_CUTOFF_NONPERIODIC)
     elif case == "ion_box_pme":
         d = H.ion_box(method=systems.NB_PME)
@@ -85,6 +88,118 @@ def test_engine_matches_the_restatement(H, case):
     err = H.force_error(f, fr)
     print("%s engine vs restatement: force %.2e, energy %.2e" % (case, err, abs(e - er)/abs(er)))
     assert err <= FORCE_BAR and abs(e - er) <= ENERGY_BAR*abs(er), (err, e, er)
+
+
+@pytest.mark.parametrize("case", ["ion_box", "ion_box_tri_pmp", "ion_box_tri_mpm"])
+def test_periodic_ion_boxes_plugin_matches_reference(H, case):
+    """the plugin against the Reference platform on the cubic and the two triclinic periodic ion boxes"""
+    d = H.golden_cases()[case].rounded()
+    ref, b200 = H.Simulation(d, "Reference"), H.Simulation(d, "B200")
+    assert b200.platform() == "B200"
+    (f, e), (fr, er) = H.gb_only(b200), H.gb_only(ref)
+    err = H.force_error(f, fr)
+    print("%s plugin vs Reference: force %.2e, energy %.2e" % (case, err, abs(e - er)/abs(er)))
+    assert err <= FORCE_BAR and abs(e - er) <= ENERGY_BAR*abs(er), (err, e, er)
+
+
+def _to_aged_state(eng, nsteps):
+    """Step one step at a time, a compute() after each, until a state after nsteps steps whose list was built neither in
+    its last step nor in that compute (test_gpu_oracle_edges._age without the pair counts); returns the steps taken"""
+    steps = 0
+    while steps < nsteps + 100:
+        b0 = eng.stats()["list_builds"]
+        eng.step(1)
+        steps += 1
+        b1 = eng.stats()["list_builds"]
+        eng.compute(energy=False)
+        if steps >= nsteps and eng.stats()["list_builds"] == b1 == b0:
+            return steps
+    pytest.fail("no aged state within %d steps" % steps)
+
+
+def _check_against_restatement_and_fresh(H, eng, d, label, precision="single", fresh_positions=None):
+    """GB forces and energy of eng's current state against the restatement at its positions (the fp32 hi part in mixed
+    precision) and against a fresh engine at the same positions; returns the force error against the restatement.
+    fresh_positions: the engine's own wrapped fp32 coordinates, for atoms that set_positions put whole box lengths out.
+    The fresh engine wraps those again and rounds differently, so the two are held to the relative bound of an aged list
+    against a fresh one (test_gpu_oracle_edges.AGED_BOUND), not to the 1e-6 absolute bound of identical coordinates."""
+    from openmm_b200 import Engine
+    import copy
+    f, e = _engine_gb(eng)
+    x = eng.get_positions()
+    xo = x.astype(np.float32).astype(np.float64) if precision == "mixed" else x
+    fr, er = H.obc_forces_energy(d, xo)
+    err = H.force_error(f, fr)
+    d2 = copy.copy(d)
+    d2.positions = x if fresh_positions is None else fresh_positions
+    fresh = Engine(d2, precision=precision)
+    f2, e2 = _engine_gb(fresh)
+    fresh.close()
+    print("%s: force %.2e, energy %.2e against the restatement; fresh list %.2e, energy %.2e"
+          % (label, err, abs(e - er)/abs(er), np.abs(f - f2).max(), abs(e - e2)/abs(e2)))
+    assert err <= FORCE_BAR and abs(e - er) <= ENERGY_BAR*abs(er), (err, e, er)
+    if fresh_positions is None:
+        # same forces as a fresh Context; not to the bit, since that one's list was built at x in another order
+        assert np.abs(f - f2).max() < 1e-6 and abs(e - e2) <= 1e-9*abs(e2), (np.abs(f - f2).max(), e, e2)
+    else:
+        rel = H.force_error(f, f2)
+        print("  fresh engine from the wrapped coordinates: force %.2e relative" % rel)
+        assert rel < 1.5e-5 and abs(e - e2) <= 1e-8*abs(e2), (rel, e, e2)
+    return err
+
+
+@pytest.mark.parametrize("case", ["dhfr_cutoff", "dhfr_nocutoff", "ion_box_pad002"])
+def test_aged_list_matches_the_restatement(H, monkeypatch, record_property, case):
+    """GB on the list as it stands after a Langevin run (not rebuilt in the last step): the mask-free pair sweeps rely on
+    the aged list still holding every pair within the cutoff once"""
+    from openmm_b200 import Engine, systems
+    if case == "ion_box_pad002":
+        monkeypatch.setenv("B200MD_PAD_FRACTION", "0.02")
+        d, dt, nsteps = H.ion_box().rounded(), 0.001, 80
+    else:
+        d = H.dhfr_gbsa(systems.NB_NOCUTOFF if case == "dhfr_nocutoff" else systems.NB_CUTOFF_NONPERIODIC).rounded()
+        dt, nsteps = 0.002, 40
+    eng = Engine(d)
+    eng.set_integrator(systems.INT_LANGEVIN, dt, 300.0, 1.0, 13)
+    eng.set_velocities(np.random.default_rng(13).standard_normal((d.natoms, 3))*np.sqrt(0.0083144626*300.0/np.asarray(d.masses))[:, None])
+    eng.apply_velocity_constraints()
+    steps = _to_aged_state(eng, nsteps)
+    builds = eng.stats()["list_builds"]
+    err = _check_against_restatement_and_fresh(H, eng, d, "%s after %d steps, %d list builds" % (case, steps, builds))
+    eng.close()
+    record_property("force_error", err)
+    if case == "ion_box_pad002":
+        assert builds > 3
+
+
+@pytest.mark.parametrize("n", [2, 31, 33, 65])
+def test_small_periodic_ion_boxes(H, n):
+    """N that leaves the last 32-atom block partly empty, then the same ions moved by 1-3 lattice vectors through
+    set_positions (the list build moves them back in fp32)."""
+    from openmm_b200 import Engine
+    from test_gpu_oracle_edges import _inner_positions
+    d = H.ion_box(n=n, edge=2.6, cutoff=1.2, seed=n).rounded()
+    eng = Engine(d)
+    _check_against_restatement_and_fresh(H, eng, d, "%d ions" % n)
+    k = np.random.default_rng(n).integers(-3, 4, (n, 3))
+    eng.set_positions(d.positions + k @ d.box)
+    eng.compute(energy=False)
+    _check_against_restatement_and_fresh(H, eng, d, "%d ions moved by lattice vectors" % n,
+                                         fresh_positions=_inner_positions(eng, n))
+    eng.close()
+
+
+def test_mixed_precision_matches_the_restatement(H):
+    """DHFR-GBSA in mixed precision after 10 Langevin steps: the pair sweeps read the fp32 hi part of the positions"""
+    from openmm_b200 import Engine, systems
+    d = H.dhfr_gbsa().rounded()
+    eng = Engine(d, precision="mixed")
+    assert eng.precision == "mixed"
+    eng.set_integrator(systems.INT_LANGEVIN, 0.002, 300.0, 1.0, 17)
+    eng.step(10)
+    eng.compute(energy=False)
+    _check_against_restatement_and_fresh(H, eng, d, "DHFR-GBSA mixed", precision="mixed")
+    eng.close()
 
 
 def _gb_forces(d, overlap):
