@@ -901,6 +901,15 @@ extern "C" int b200md_restore_coordinates(b200md_ctx* ctx) {
     API_END(ctx)
 }
 
+// The current charges into posq.w (times sqrt(ONE_4PI_EPS0)), positions kept.  Synchronous: the caller has drained the stream.
+static void stamp_charges(b200md_ctx* c) {
+    const double sk = std::sqrt(B200MD_ONE_4PI_EPS0);
+    std::vector<float4> p(c->npad);
+    CUDA_CHECK(cudaMemcpy(p.data(), c->posq.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToHost));
+    for (int i = 0; i < c->natoms; i++) p[i].w = (float) (c->charge[i]*sk);
+    CUDA_CHECK(cudaMemcpy(c->posq.p, p.data(), sizeof(float4)*c->npad, cudaMemcpyHostToDevice));
+}
+
 // per-atom and per-exception parameters -> device (computeParameters, ReferenceKernels.cpp:1077-1121)
 static void upload_params(b200md_ctx* c) {
     const int N = c->natoms;
@@ -914,11 +923,7 @@ static void upload_params(b200md_ctx* c) {
         c->chargeD.upload(qd); c->sigepsD.upload(sd);
         c->nb.chargeD = c->pmeOnly ? nullptr : c->chargeD.p; c->nb.sigepsD = c->sigepsD.p;     // stand-alone PME: the charges arrive with every call (posq.w)
     }
-    // charges live in posq.w; keep positions
-    std::vector<float4> p(c->npad);
-    CUDA_CHECK(cudaMemcpy(p.data(), c->posq.p, sizeof(float4)*c->npad, cudaMemcpyDeviceToHost));
-    for (int i = 0; i < N; i++) p[i].w = (float) (c->charge[i]*sk);
-    CUDA_CHECK(cudaMemcpy(c->posq.p, p.data(), sizeof(float4)*c->npad, cudaMemcpyHostToDevice));
+    stamp_charges(c);
     const int ne = (int) c->exc.atoms.size();
     std::vector<double4> ep(ne);
     for (int e = 0; e < ne; e++) {
@@ -2112,6 +2117,9 @@ extern "C" int b200md_checkpoint_load(b200md_ctx* ctx, const void* buf, int64_t 
     for (int i = 0; i < 3; i++) { ctx->boxA[i] = h.box[i]; ctx->boxB[i] = h.box[3+i]; ctx->boxC[i] = h.box[6+i]; }
     const char* p = (const char*) buf + sizeof(h);
     for (const DevSpan& s : state_spans(ctx)) { CUDA_CHECK(cudaMemcpy(s.p, p, s.bytes, cudaMemcpyHostToDevice)); p += s.bytes; }
+    // the blob's posq.w holds the charges of when it was saved; every other copy of the parameters is the context's own
+    // (a checkpoint carries no force-field parameters, ContextImpl::loadCheckpoint)
+    stamp_charges(ctx);
     CUDA_CHECK(cudaMemcpy(ctx->stepCounter.p, &h.rngStep, sizeof(unsigned long long), cudaMemcpyHostToDevice));
     host_set_state(ctx); ctx->velStale = false;
     if (ctx->haveBox) apply_box(ctx);

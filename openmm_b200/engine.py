@@ -228,6 +228,21 @@ class Engine:
         self._ck(self.lib.b200md_compute_groups(self.h, terms, groups, 1, C.byref(e)))
         return e.value
 
+    # ---- CalcNonbondedForceKernel::copyParametersToContext (and Context::setParameter of its parameter offsets) ----
+    def update_nonbonded_params(self, desc, dispersion_coefficient=None):
+        """The per-atom charges, sigmas and epsilons and the per-exception (chargeProd, sigma, epsilon) of `desc` for the same
+        atoms and exceptions.  dispersion_coefficient defaults to desc.dispersion_coefficient(), as at definition; parameter
+        offsets pass the one of the parameters' default values instead (NonbondedForceImpl::calcDispersionCorrection)."""
+        q, sig, eps = _f64(desc.charges), _f64(desc.sigmas), _f64(desc.epsilons)
+        eqq, esig, eeps = _f64(desc.exc_qq), _f64(desc.exc_sigma), _f64(desc.exc_eps)
+        if not (len(q) == len(sig) == len(eps) == self.natoms):
+            raise ValueError("update_nonbonded_params: charges, sigmas and epsilons need one value per atom (%d)" % self.natoms)
+        if not (len(eqq) == len(esig) == len(eeps) == len(desc.exc_i)):
+            raise ValueError("update_nonbonded_params: exc_qq, exc_sigma and exc_eps need one value per exception")
+        disp = desc.dispersion_coefficient() if dispersion_coefficient is None else dispersion_coefficient
+        self._ck(self.lib.b200md_update_nonbonded_params(self.h, _dp(q), _dp(sig), _dp(eps), len(eqq), _dp(eqq), _dp(esig), _dp(eeps),
+                                                         float(disp)))
+
     # ---- Calc{RBTorsion,CMAPTorsion}ForceKernel::copyParametersToContext ----
     def update_rb_torsion_params(self, c):
         c = _f64(c)

@@ -63,6 +63,31 @@ def lib():
     return _lib
 
 
+# parameter updates and checkpoints through a buffer (plugin/tests/nonbonded_capi.cpp, built by plugin/Makefile `all`
+# against the headers oracle/Makefile stages, so that it builds wherever oracle/_ref/ is present)
+NB_LIB = os.path.join(REF_DIR, "tests", "libnonbonded_capi.so")
+_nb_lib = None
+
+
+def nb_lib():
+    global _nb_lib
+    if _nb_lib is None:
+        lib()
+        L = C.CDLL(NB_LIB)
+        P, D, I = C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int)
+        sig = {
+            "nbc_last_error": (C.c_char_p, []), "nbc_set_particles": (C.c_int, [P, C.c_int, D, D, D]),
+            "nbc_set_exceptions": (C.c_int, [P, C.c_int, I, I, D, D, D]), "nbc_update_in_context": (C.c_int, [P, P]),
+            "nbc_create_checkpoint": (C.c_longlong, [P, C.c_char_p, C.c_longlong]),
+            "nbc_load_checkpoint": (C.c_int, [P, C.c_char_p, C.c_longlong]),
+        }
+        for name, (res, args) in sig.items():
+            f = getattr(L, name)
+            f.restype, f.argtypes = res, args
+        _nb_lib = L
+    return _nb_lib
+
+
 def _dp(a):
     return a.ctypes.data_as(C.POINTER(C.c_double))
 
@@ -232,6 +257,34 @@ class Simulation:
 
     def checkpoint_roundtrip(self):
         self._ck(self.L.omm_context_checkpoint_roundtrip(self.ctx))
+
+    def _nbck(self, rc):
+        if rc != 0:
+            raise RuntimeError(nb_lib().nbc_last_error().decode())
+
+    def update_nonbonded(self, desc):
+        """desc's per-atom and per-exception parameters as the NonbondedForce's new base values (same particles and
+        exceptions; the parameter offsets stay), then NonbondedForce::updateParametersInContext."""
+        L = nb_lib()
+        self._nbck(L.nbc_set_particles(self.nb, self.n, _dp(_f64(desc.charges)), _dp(_f64(desc.sigmas)), _dp(_f64(desc.epsilons))))
+        if len(desc.exc_i):
+            self._nbck(L.nbc_set_exceptions(self.nb, len(desc.exc_i), _ip(_i32(desc.exc_i)), _ip(_i32(desc.exc_j)), _dp(_f64(desc.exc_qq)),
+                                            _dp(_f64(desc.exc_sigma)), _dp(_f64(desc.exc_eps))))
+        self._nbck(L.nbc_update_in_context(self.nb, self.ctx))
+
+    def checkpoint(self):
+        """Context::createCheckpoint, as bytes"""
+        L = nb_lib()
+        n = L.nbc_create_checkpoint(self.ctx, None, 0)
+        if n < 0:
+            raise RuntimeError(L.nbc_last_error().decode())
+        buf = C.create_string_buffer(n)
+        if L.nbc_create_checkpoint(self.ctx, buf, n) != n:
+            raise RuntimeError(L.nbc_last_error().decode() or "the checkpoint changed size")
+        return buf.raw
+
+    def load_checkpoint(self, blob):
+        self._nbck(nb_lib().nbc_load_checkpoint(self.ctx, blob, len(blob)))
 
     def close(self):
         if getattr(self, "ctx", None):

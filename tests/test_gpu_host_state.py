@@ -154,14 +154,6 @@ def test_timed_list_build_adds_no_rebuild_to_the_next_step(precision):
     assert eng.stats()["list_builds"] == builds       # the positions have not moved since the last timed build
 
 
-def _update_nonbonded_params(eng, d):
-    """the same parameters again (the Python Engine has no wrapper for this call)"""
-    from openmm_b200.engine import _dp, _f64
-    a = [_f64(p) for p in (d.charges, d.sigmas, d.epsilons, d.exc_qq, d.exc_sigma, d.exc_eps)]
-    eng._ck(eng.lib.b200md_update_nonbonded_params(eng.h, _dp(a[0]), _dp(a[1]), _dp(a[2]), len(d.exc_i), _dp(a[3]), _dp(a[4]),
-                                                   _dp(a[5]), d.dispersion_coefficient()))
-
-
 @pytest.mark.parametrize("call", ["set_positions", "set_box", "update_nonbonded_params", "load_checkpoint"])
 def test_state_changes_rebuild_the_list(call):
     d = _system()
@@ -175,7 +167,7 @@ def test_state_changes_rebuild_the_list(call):
     elif call == "set_box":
         eng.set_box(d.box)
     elif call == "update_nonbonded_params":
-        _update_nonbonded_params(eng, d)
+        eng.update_nonbonded_params(d)          # the same parameters again
     else:
         eng.load_checkpoint(blob)
     # the list is marked dirty (a synchronous list pass first) and the device's rebuild flag is raised (one build)
