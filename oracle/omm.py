@@ -138,9 +138,11 @@ class Simulation:
     """System + Integrator + Context on one platform, from a SystemDesc."""
 
     def __init__(self, desc, platform="Reference", integrator=(0, 0.0, 0.0, 0.001), seed=7, constraint_tol=1e-5,
-                 pme=None, props="", recip_group=None, bonded_periodic=False, nb_globals=None, particle_offsets=(), exception_offsets=()):
+                 pme=None, props="", recip_group=None, bonded_periodic=False, nb_globals=None, particle_offsets=(), exception_offsets=(),
+                 bonded_group=None):
         """integrator = (kind, temperature, friction, dt); pme = (alpha, nx, ny, nz) to pin the PME parameters;
-        bonded_periodic: setUsesPeriodicBoundaryConditions(true) on the three bonded forces; nb_globals = {name: default},
+        bonded_periodic: setUsesPeriodicBoundaryConditions(true) on the three bonded forces; bonded_group: the force group of
+        the three bonded forces (default 0, the NonbondedForce's); nb_globals = {name: default},
         particle_offsets = [(name, particle, dq, dsigma, deps)], exception_offsets = [(name, exception index, dqq, dsigma, deps)]
         (NonbondedForce parameter offsets)."""
         L = lib()
@@ -176,16 +178,22 @@ class Simulation:
         if len(desc.bond_i):
             f = L.omm_bonds_create(len(desc.bond_i), _ip(_i32(desc.bond_i)), _ip(_i32(desc.bond_j)), _dp(_f64(desc.bond_r0)), _dp(_f64(desc.bond_k)))
             L.omm_bonded_set_periodic(f, 0, int(bonded_periodic))
+            if bonded_group is not None:
+                L.omm_force_set_group(f, bonded_group)
             L.omm_system_add_force(self.sys, f)
         if len(desc.angle_i):
             f = L.omm_angles_create(len(desc.angle_i), _ip(_i32(desc.angle_i)), _ip(_i32(desc.angle_j)), _ip(_i32(desc.angle_k)),
                                     _dp(_f64(desc.angle_t0)), _dp(_f64(desc.angle_kk)))
             L.omm_bonded_set_periodic(f, 1, int(bonded_periodic))
+            if bonded_group is not None:
+                L.omm_force_set_group(f, bonded_group)
             L.omm_system_add_force(self.sys, f)
         if len(desc.tor_i):
             f = L.omm_torsions_create(len(desc.tor_i), _ip(_i32(desc.tor_i)), _ip(_i32(desc.tor_j)), _ip(_i32(desc.tor_k)), _ip(_i32(desc.tor_l)),
                                       _ip(_i32(desc.tor_n)), _dp(_f64(desc.tor_phase)), _dp(_f64(desc.tor_kk)))
             L.omm_bonded_set_periodic(f, 2, int(bonded_periodic))
+            if bonded_group is not None:
+                L.omm_force_set_group(f, bonded_group)
             L.omm_system_add_force(self.sys, f)
         if desc.cm_frequency:
             L.omm_system_add_force(self.sys, L.omm_cmmotion_create(desc.cm_frequency))
@@ -209,6 +217,11 @@ class Simulation:
 
     def set_positions(self, x):
         self._ck(self.L.omm_context_set_positions(self.ctx, self.n, _dp(_f64(x))))
+
+    def set_box(self, box):
+        """Context::setPeriodicBoxVectors, as MonteCarloBarostatImpl calls it after scaling the coordinates"""
+        b = _f64(box)
+        self._ck(self.L.omm_context_set_box(self.ctx, _dp(b[0]), _dp(b[1]), _dp(b[2])))
 
     def set_velocities(self, v):
         self._ck(self.L.omm_context_set_velocities(self.ctx, self.n, _dp(_f64(v))))
