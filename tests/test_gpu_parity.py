@@ -77,8 +77,12 @@ def _compare(mods, name, tol=TOL, etol=TOL):
 
 
 # ---- the bespoke FFT against numpy (template: platforms/cuda/tests/TestCudaFFT3D.cpp:52-135, same odd sizes) ----
+# Above 160 points along y or z two copies of a (y, z) plane no longer fit in shared memory and the line-batched FFT takes
+# over (fft.cu FftLaunch): the cubic edges of the supercell grids (tests/test_gpu_supercell.py), a non-cubic grid on that
+# path, and 224-point x lines on the slab path.
 @pytest.mark.parametrize("shape", [(28, 25, 30), (28, 25, 25), (25, 28, 25), (25, 25, 28), (21, 25, 27), (56, 56, 56), (88, 88, 88), (90, 90, 90), (128, 128, 128), (6, 6, 6),
-                                   (26, 39, 13), (27, 45, 33), (12, 40, 24), (144, 20, 36)])
+                                   (26, 39, 13), (27, 45, 33), (12, 40, 24), (144, 20, 36),
+                                   (168, 168, 168), (176, 176, 176), (192, 192, 192), (224, 224, 224), (112, 168, 224), (224, 168, 112)])
 def test_fft3d_matches_numpy(mods, shape):
     _, _, engine, _, _ = mods
     rng = np.random.default_rng(sum(shape))
