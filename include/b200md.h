@@ -47,7 +47,9 @@ typedef struct b200md_ctx b200md_ctx;
 #define B200MD_TERM_CUSTOM_COMPOUND  2048
 #define B200MD_TERM_CUSTOM_CENTROID  4096
 #define B200MD_TERM_GBSA             8192   /* GBSAOBCForce: OBC II implicit solvent with the ACE surface term */
-#define B200MD_TERM_ALL        16383
+#define B200MD_TERM_RMSD             16384  /* RMSDForce */
+#define B200MD_TERM_CV_FORCES        32768  /* CustomCVForce: force += sum_i dE/dCV_i F_i (b200md_set_cv_coefficients) */
+#define B200MD_TERM_ALL        65535
 
 /* ---- the bonded classes: kind argument of b200md_set_bonded_groups and b200md_update_bonded_params ---- */
 #define B200MD_BONDED_BONDS           0
@@ -271,6 +273,37 @@ int b200md_set_gbsa(b200md_ctx* ctx, int method, double cutoff, double solute_di
 /* CalcGBSAOBCForceKernel::copyParametersToContext: new charges, radii and scales (n == the number of atoms) into the same
  * device buffers, so a captured step graph stays valid.                                                                   */
 int b200md_update_gbsa_params(b200md_ctx* ctx, int n, const double* charge, const double* radius, const double* scale);
+/* CalcRMSDForceKernel::initialize (kernels.h): nforces RMSDForce objects.  Object o is the particles particles[start[o] ..
+ * start[o+1]-1] (start has nforces + 1 entries, start[0] = 0; at least one particle, each at most once; the caller expands an
+ * empty RMSDForce particle list to every particle) with the reference positions ref[3k .. 3k+2] of entry k, in force group
+ * group[o].  Its energy is the RMSD between the continuous coordinates of its particles and the reference positions, both
+ * centred, after the optimal rotation (Coutsias, Seok and Dill, J. Comput. Chem. 25:1849, 2004).  Where the mean square
+ * deviation is below 1e-20 the energy and the forces are 0, as on the Reference platform.  Single GPU only.              */
+int b200md_set_rmsd(b200md_ctx* ctx, int nforces, const int* start, const int* particles, const double* ref, const int* group);
+/* CalcRMSDForceKernel::copyParametersToContext: new particle lists and reference positions for the same number of objects
+ * (groups stay).  With the same total number of entries a captured step graph stays valid.                              */
+int b200md_update_rmsd(b200md_ctx* ctx, int nforces, const int* start, const int* particles, const double* ref);
+/* CustomCVForce (CalcCustomCVForceKernel).  The collective variables are evaluated by an inner context of the same number of
+ * particles on the same device, one force group per variable; the caller evaluates the energy expression.
+ * set_cv_forces (before finalize): the number n of collective variables, one force slot each.  Single GPU only.
+ * cv_copy_state: the continuous user-order positions (hi and lo in mixed precision) and the box of `from` into `to`, with the
+ * effect of b200md_set_positions on `to` (its list is rebuilt at its next evaluation), but no host round trip: stream-ordered
+ * on `from`'s stream, and `to`'s stream waits on an event.  The two contexts must be on one device.
+ * cv_snapshot_forces: the fixed-point user-order force buffer of `inner` (its last evaluation) into slot `slot` of `outer`;
+ * `outer`'s stream waits for the copy.
+ * set_cv_coefficients: dE/dCV_i of the n variables, a stream-ordered copy into the buffer the step graphs read.  The term bit
+ * B200MD_TERM_CV_FORCES then adds sum_i dE/dCV_i F_i to the forces, in fixed point and a fixed order.  b200md_step with more
+ * than one step is refused on a context with collective variables: the coefficients change every step.                 */
+int b200md_set_cv_forces(b200md_ctx* ctx, int n);
+int b200md_cv_copy_state(b200md_ctx* from, b200md_ctx* to);
+int b200md_cv_snapshot_forces(b200md_ctx* inner, b200md_ctx* outer, int slot);
+int b200md_set_cv_coefficients(b200md_ctx* ctx, int n, const double* d);
+/* Test hooks, no context and no device: the RMSD arithmetic of the device kernels run on the host.  rmsd_probe: the RMSD of n
+ * positions pos[3k ..] from n reference positions ref[3k ..] (both centred here) and the force on each position, forces[3k ..].
+ * rmsd_eigen_probe: the largest eigenvalue of the symmetric 4x4 matrix a (row-major) and a unit eigenvector q of it, by the
+ * cyclic Jacobi iteration k_rmsd_solve runs; returns the number of sweeps.                                               */
+int b200md_rmsd_probe(int n, const double* pos, const double* ref, double* rmsd, double* forces);
+int b200md_rmsd_eigen_probe(const double* a, double* lambda, double* q);
 /* Test hook, no context and no device: program `which` of a b200md_set_custom_torsions program set, checked as that call
  * checks it (nglobals = the number of global slots), evaluated at (theta, params, globals) on the host by the interpreter
  * source the device kernel runs.  0 and *out on success, -1 with the reason in msg.                                       */
@@ -383,7 +416,7 @@ int b200md_get_stats(b200md_ctx* ctx, b200md_stats* out);
  * angles alone (k_custom), 8 custom compound bonds alone (k_compound), 9 custom centroid bonds alone (k_centroid_centers,
  * the k_compound instantiation that reads the centres, k_centroid_scatter), 10 the generalized Born chain (k_gb_born,
  * k_gb_radii, k_gb_pairs, k_gb_fold, k_gb_chain), 11 the first half of the list build alone (k_list_prep: binning, sort,
- * block bounds), 12 its second half alone (k_build_tiles).
+ * block bounds), 12 its second half alone (k_build_tiles), 13 the RMSD forces (k_rmsd_sums, k_rmsd_solve, k_rmsd_forces).
  * Runs `reps` isolated launches of that phase on the current state.                                  */
 int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* ms_mean);
 /* The current neighbour list, read back for identity checks.  *ntiles = its tile count.  sorig (if not NULL): [padded_atoms]

@@ -67,6 +67,14 @@ SIGNATURES = {
     "b200md_update_custom_centroid_params": (C.c_int, [_P, C.c_int, _D]),
     "b200md_set_gbsa": (C.c_int, [_P, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, _D, _D, _D]),
     "b200md_update_gbsa_params": (C.c_int, [_P, C.c_int, _D, _D, _D]),
+    "b200md_set_rmsd": (C.c_int, [_P, C.c_int, _I, _I, _D, _I]),
+    "b200md_update_rmsd": (C.c_int, [_P, C.c_int, _I, _I, _D]),
+    "b200md_rmsd_probe": (C.c_int, [C.c_int, _D, _D, _D, _D]),
+    "b200md_set_cv_forces": (C.c_int, [_P, C.c_int]),
+    "b200md_cv_copy_state": (C.c_int, [_P, _P]),
+    "b200md_cv_snapshot_forces": (C.c_int, [_P, _P, C.c_int]),
+    "b200md_set_cv_coefficients": (C.c_int, [_P, C.c_int, _D]),
+    "b200md_rmsd_eigen_probe": (C.c_int, [_D, _D, _D]),
     "b200md_custom_program_probe": (C.c_int, [C.c_int, _I, _I, _I, _D, C.c_int, C.c_int, C.c_int, C.c_double, _D, _D, _D,
                                               C.c_char_p, C.c_int]),
     "b200md_custom_term_probe": (C.c_int, [C.c_int, C.c_int, _I, _I, _I, _D, C.c_int, C.c_int, C.c_int, _D, _D, _D, _D, _D,

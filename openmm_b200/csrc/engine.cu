@@ -2,6 +2,7 @@
 // No CPU fallback exists: every compute entry point needs a CUDA device and fails loudly without one.
 #include "engine.h"
 #include "custom_interp.h"
+#include "rmsd.h"
 #include "../../include/b200md.h"
 #include <stdexcept>
 #include <algorithm>
@@ -273,6 +274,21 @@ struct b200md_ctx {
         cudaEvent_t evFork = nullptr, evJoin = nullptr;
     } gbsa;
     GbsaDev gbd{};
+    // RMSDForce objects (b200md_set_rmsd): their particle lists one after the other, the reference position of every entry
+    // centred over its object, and the device form
+    struct {
+        std::vector<int> start, atoms, entryObj; std::vector<double> ref, refSq; std::vector<unsigned char> group;
+        DevBuf<int> startDev, atomsDev, entryObjDev; DevBuf<double> refDev, refSqDev, sums, solved; DevBuf<unsigned char> groupDev;
+    } rmsd;
+    RmsdDev rmd{};
+    // CustomCVForce (b200md_set_cv_forces): the number of collective variables, their force snapshots and coefficients; evCv
+    // orders this context's stream against another's (state copies and force snapshots)
+    struct {
+        int n = 0;
+        DevBuf<long long> forces; DevBuf<double> coeff; std::vector<double> hcoeff;
+    } cv;
+    CvDev cvd{};
+    cudaEvent_t evCv = nullptr;
     UnitDev units{};
     IntegDev integ{};
     bool haveIntegrator = false;
@@ -317,6 +333,9 @@ static void check_flags(b200md_ctx* c);
 static void sync_velocities(b200md_ctx* c);
 static void sync_positions(b200md_ctx* c);
 static void setup_gbsa(b200md_ctx* c);
+static void setup_rmsd(b200md_ctx* c);
+static void setup_cv(b200md_ctx* c);
+static void host_set_state(b200md_ctx* c);
 
 extern "C" const char* b200md_version(void) { return "b200md 0.2 (sm_90a)"; }
 extern "C" const char* b200md_last_error(const b200md_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
@@ -375,6 +394,7 @@ extern "C" void b200md_destroy(b200md_ctx* ctx) {
     if (ctx->evJoin) cudaEventDestroy(ctx->evJoin);
     if (ctx->evJoinBonded) cudaEventDestroy(ctx->evJoinBonded);
     if (ctx->evForkGrid) cudaEventDestroy(ctx->evForkGrid);
+    if (ctx->evCv) cudaEventDestroy(ctx->evCv);
     if (ctx->gbsa.stream) cudaStreamDestroy(ctx->gbsa.stream);
     if (ctx->gbsa.evFork) cudaEventDestroy(ctx->gbsa.evFork);
     if (ctx->gbsa.evJoin) cudaEventDestroy(ctx->gbsa.evJoin);
@@ -1697,6 +1717,8 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     build_units(c);
     build_ccma(c);
     setup_gbsa(c);
+    setup_rmsd(c);
+    setup_cv(c);
     if (c->mg == MG_P2P) {
         setup_ownership(c);
         if (nb.method == B200MD_NB_PME) {
@@ -1943,6 +1965,162 @@ static void setup_gbsa(b200md_ctx* c) {
     }
 }
 
+// ---------------------------------------------------------------- RMSDForce
+// nforces objects: object o is the particles particles[start[o] .. start[o+1]-1] (at least one, each at most once, in range)
+// with the reference positions ref[3 k ..] of entry k; kept on the host with every reference position centred over its object
+static void read_rmsd(b200md_ctx* c, const char* call, int nforces, const int* start, const int* particles, const double* ref) {
+    require(nforces >= 0, (std::string(call) + ": negative count").c_str());
+    require(nforces == 0 || start[0] == 0, (std::string(call) + ": start[0] must be 0").c_str());
+    auto& r = c->rmsd;
+    std::vector<int> st(start, start + nforces + 1), atoms, obj;
+    std::vector<double> pos, sq;
+    for (int o = 0; o < nforces; o++) {
+        require(st[o+1] > st[o], (std::string(call) + ": an RMSD force has no particles").c_str());
+        std::set<int> seen;
+        double cen[3] = {0.0, 0.0, 0.0};
+        for (int k = st[o]; k < st[o+1]; k++) {
+            const int a = particles[k];
+            require(a >= 0 && a < c->natoms, (std::string(call) + ": particle index out of range").c_str());
+            require(seen.insert(a).second, (std::string(call) + ": a particle appears twice in one RMSD force").c_str());
+            for (int d = 0; d < 3; d++) {
+                require(std::isfinite(ref[3*k + d]), (std::string(call) + ": a reference position is not finite").c_str());
+                cen[d] += ref[3*k + d];
+            }
+        }
+        const int n = st[o+1] - st[o];
+        double s2 = 0.0;
+        for (int k = st[o]; k < st[o+1]; k++) {
+            atoms.push_back(particles[k]); obj.push_back(o);
+            for (int d = 0; d < 3; d++) { const double x = ref[3*k + d] - cen[d]/n; pos.push_back(x); s2 += x*x; }
+        }
+        sq.push_back(s2);
+    }
+    r.start.swap(st); r.atoms.swap(atoms); r.entryObj.swap(obj); r.ref.swap(pos); r.refSq.swap(sq);
+}
+static void upload_rmsd(b200md_ctx* c) {
+    auto& r = c->rmsd;
+    r.startDev.upload(r.start); r.atomsDev.upload(r.atoms); r.entryObjDev.upload(r.entryObj); r.refDev.upload(r.ref); r.refSqDev.upload(r.refSq);
+}
+extern "C" int b200md_set_rmsd(b200md_ctx* ctx, int nforces, const int* start, const int* particles, const double* ref, const int* group) {
+    API_BEGIN(ctx)
+    check_set(ctx, "set_rmsd", nforces);
+    require(ctx->world == 1, "RMSDForce is not supported in multi-GPU runs");
+    read_rmsd(ctx, "set_rmsd", nforces, start, particles, ref);
+    ctx->rmsd.group.assign(nforces, 0);
+    for (int o = 0; o < nforces; o++) {
+        require(group[o] >= 0 && group[o] <= 31, "set_rmsd: force group out of range");
+        ctx->rmsd.group[o] = (unsigned char) group[o];
+    }
+    API_END(ctx)
+}
+extern "C" int b200md_update_rmsd(b200md_ctx* ctx, int nforces, const int* start, const int* particles, const double* ref) {
+    API_BEGIN(ctx)
+    require(ctx->finalized, "update_rmsd before finalize");
+    require(nforces == (int) ctx->rmsd.group.size(), "update_rmsd: the number of RMSD forces has changed");
+    const size_t before = ctx->rmsd.atoms.size();
+    CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+    read_rmsd(ctx, "update_rmsd", nforces, start, particles, ref);
+    upload_rmsd(ctx);
+    ctx->rmd.atoms = ctx->rmsd.atomsDev.p; ctx->rmd.entryObj = ctx->rmsd.entryObjDev.p; ctx->rmd.ref = ctx->rmsd.refDev.p;
+    ctx->rmd.nentries = (int) ctx->rmsd.atoms.size();
+    // the same number of entries keeps the buffers and the launch shapes, so a captured step graph stays valid
+    if (ctx->rmsd.atoms.size() != before) invalidate_graph(ctx);
+    API_END(ctx)
+}
+static void setup_rmsd(b200md_ctx* c) {
+    auto& r = c->rmsd;
+    c->rmd = RmsdDev{};
+    if (r.group.empty()) return;
+    require(c->world == 1, "RMSDForce is not supported in multi-GPU runs");
+    upload_rmsd(c);
+    r.groupDev.upload(r.group);
+    const size_t n = r.group.size();
+    r.sums.alloc(16*n); r.sums.zero(); r.solved.alloc(16*n); r.solved.zero();
+    RmsdDev& d = c->rmd;
+    d.nobj = (int) n; d.nentries = (int) r.atoms.size();
+    d.objStart = r.startDev.p; d.atoms = r.atomsDev.p; d.entryObj = r.entryObjDev.p; d.ref = r.refDev.p; d.refSq = r.refSqDev.p;
+    d.group = r.groupDev.p; d.sums = r.sums.p; d.solved = r.solved.p;
+    d.groupMask = 0xffffffffu;
+}
+
+// ---------------------------------------------------------------- CustomCVForce
+extern "C" int b200md_set_cv_forces(b200md_ctx* ctx, int n) {
+    API_BEGIN(ctx)
+    check_set(ctx, "set_cv_forces", n);
+    require(ctx->world == 1, "CustomCVForce is not supported in multi-GPU runs");
+    ctx->cv.n = n;
+    API_END(ctx)
+}
+static void setup_cv(b200md_ctx* c) {
+    auto& v = c->cv;
+    c->cvd = CvDev{};
+    if (!v.n) return;
+    require(c->world == 1, "CustomCVForce is not supported in multi-GPU runs");
+    v.forces.alloc((size_t) v.n*3*c->npad); v.forces.zero();
+    v.coeff.alloc(v.n); v.coeff.zero(); v.hcoeff.assign(v.n, 0.0);
+    c->cvd.n = v.n; c->cvd.forces = v.forces.p; c->cvd.coeff = v.coeff.p;
+    if (!c->evCv) CUDA_CHECK(cudaEventCreateWithFlags(&c->evCv, cudaEventDisableTiming));
+}
+static b200md_ctx* cv_pair(b200md_ctx* a, b200md_ctx* b, const char* call) {
+    require(a && b && a != b, (std::string(call) + ": two different contexts are needed").c_str());
+    require(a->finalized && b->finalized, (std::string(call) + " before finalize").c_str());
+    require(a->device == b->device, (std::string(call) + ": the two contexts are on different devices").c_str());
+    require(a->natoms == b->natoms && a->npad == b->npad, (std::string(call) + ": the two contexts differ in their number of particles").c_str());
+    require(a->world == 1 && b->world == 1, (std::string(call) + ": not supported in multi-GPU runs").c_str());
+    for (b200md_ctx* c : {a, b})
+        if (!c->evCv) CUDA_CHECK(cudaEventCreateWithFlags(&c->evCv, cudaEventDisableTiming));
+    return a;
+}
+extern "C" int b200md_cv_copy_state(b200md_ctx* from, b200md_ctx* to) {
+    API_BEGIN(from)
+    {
+        cv_pair(from, to, "cv_copy_state");
+        sync_positions(from);
+        // stream-ordered on `from`'s stream, behind whatever `to` still has queued; `to` waits for the copy
+        CUDA_CHECK(cudaEventRecord(to->evCv, to->stream));
+        CUDA_CHECK(cudaStreamWaitEvent(from->stream, to->evCv, 0));
+        launch_cv_copy_state(from->nb, to->nb, from->natoms, from->stream);
+        from->kernelLaunches++;
+        CUDA_CHECK(cudaEventRecord(from->evCv, from->stream));
+        CUDA_CHECK(cudaStreamWaitEvent(to->stream, from->evCv, 0));
+        if (from->haveBox) {
+            bool same = to->haveBox;
+            for (int i = 0; i < 3; i++) same = same && to->boxA[i] == from->boxA[i] && to->boxB[i] == from->boxB[i] && to->boxC[i] == from->boxC[i];
+            if (!same) {
+                for (int i = 0; i < 3; i++) { to->boxA[i] = from->boxA[i]; to->boxB[i] = from->boxB[i]; to->boxC[i] = from->boxC[i]; }
+                to->haveBox = true;
+                apply_box(to);
+            }
+        }
+        // what b200md_set_positions does besides the upload
+        to->stepStateValid = false;
+        host_set_state(to);
+        request_rebuild(to);
+    }
+    API_END(from)
+}
+extern "C" int b200md_cv_snapshot_forces(b200md_ctx* inner, b200md_ctx* outer, int slot) {
+    API_BEGIN(outer)
+    cv_pair(inner, outer, "cv_snapshot_forces");
+    require(slot >= 0 && slot < outer->cv.n, "cv_snapshot_forces: slot out of range");
+    const size_t n = 3*(size_t) outer->npad;
+    // on the inner stream, behind the evaluation that produced the forces and before the next one; the outer stream waits
+    CUDA_CHECK(cudaMemcpyAsync(outer->cv.forces.p + slot*n, inner->force.p, sizeof(long long)*n, cudaMemcpyDeviceToDevice, inner->stream));
+    CUDA_CHECK(cudaEventRecord(inner->evCv, inner->stream));
+    CUDA_CHECK(cudaStreamWaitEvent(outer->stream, inner->evCv, 0));
+    API_END(outer)
+}
+extern "C" int b200md_set_cv_coefficients(b200md_ctx* ctx, int n, const double* d) {
+    API_BEGIN(ctx)
+    require(ctx->finalized, "set_cv_coefficients before finalize");
+    require(n == ctx->cv.n, "set_cv_coefficients: n must be the number of collective variables");
+    for (int i = 0; i < n; i++) require(std::isfinite(d[i]), "set_cv_coefficients: a coefficient is not finite");
+    ctx->cv.hcoeff.assign(d, d + n);
+    // stream ordered, into the buffer the step graphs read: no graph is captured or instantiated again
+    if (n) CUDA_CHECK(cudaMemcpyAsync(ctx->cv.coeff.p, ctx->cv.hcoeff.data(), sizeof(double)*n, cudaMemcpyHostToDevice, ctx->stream));
+    API_END(ctx)
+}
+
 // ---------------------------------------------------------------- state
 // Multi-GPU (peer-memory data plane): only the owner integrates an atom.  Positions reach every rank with the step itself;
 // velocities stay with the owner until somebody reads them from the host side.
@@ -2165,7 +2343,9 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     const bool custom = (bterms & c->ctd.terms) != 0;
     const bool compound = (bterms & B200MD_TERM_CUSTOM_COMPOUND) && c->cpd.nslots > 0;
     const bool centroid = (bterms & B200MD_TERM_CUSTOM_CENTROID) && c->ccd.nslots > 0;
-    const bool bonded = (classic || custom || compound || centroid) && !pmeRank;
+    const bool rmsd = (terms & B200MD_TERM_RMSD) && c->rmd.nobj > 0;
+    const bool bonded = (classic || custom || compound || centroid || rmsd) && !pmeRank;
+    const bool cvForces = (terms & B200MD_TERM_CV_FORCES) && c->cvd.n > 0;
     // Reciprocal space (spread -> FFT/convolution -> gather, in USER atom order: independent of the neighbour list) and
     // direct space (list check / rebuild, tile kernel, bonded terms) are independent until the integrator: fork them onto
     // two streams (also inside the captured step graph).  Both accumulate into the same fixed-point force buffer, so the
@@ -2212,12 +2392,18 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
         CompoundDev cc = c->ccd; cc.groupMask = groupMask;
         launch_bonded(c->nb, bd, ct, cp, cc, c->cen, bterms, energy, sb);
         launches += (classic ? 1 : 0) + (custom ? 1 : 0) + (compound ? 1 : 0) + (centroid ? CENTROID_LAUNCHES : 0);
+        if (rmsd) {
+            RmsdDev rd = c->rmd; rd.groupMask = groupMask;
+            launch_rmsd(c->nb, rd, energy, sb);
+            launches += RMSD_LAUNCHES;
+        }
     };
 
     // ---- the schedule, in stream order ----
     if (!forcesAlreadyZero) CUDA_CHECK(cudaMemsetAsync(c->force.p, 0, sizeof(long long)*3*c->npad, s));
     if (energy) CUDA_CHECK(cudaMemsetAsync(c->energy.p, 0, sizeof(double)*B200MD_NUM_ENERGY, s));
     if (p2p && !direct) { launch_pos_wait(c->nb, c->cd, s); launches++; }       // nobody else on this stream waits for the owners' position stores
+    if (cvForces) { launch_cv_combine(c->nb, c->cvd, s); launches++; }
     if (!forkAfterList) launch_recip();
     else {
         // the charge grid is zeroed at the head of the step on the chain's stream, beside the list check and build: it needs
@@ -2349,6 +2535,7 @@ extern "C" int b200md_compute_groups(b200md_ctx* ctx, int terms, unsigned int bo
         if (terms & (B200MD_TERM_CUSTOM_TORSIONS | B200MD_TERM_CUSTOM_BONDS | B200MD_TERM_CUSTOM_EXTERNALS | B200MD_TERM_CUSTOM_ANGLES |
                      B200MD_TERM_CUSTOM_COMPOUND | B200MD_TERM_CUSTOM_CENTROID)) e += h[EN_CUSTOM];
         if ((terms & B200MD_TERM_GBSA) && ctx->gbsa.have) e += h[EN_GB];
+        if (terms & B200MD_TERM_RMSD) e += h[EN_RMSD];
         if (ctx->haveNb) {
             if (terms & B200MD_TERM_NB_DIRECT) {
                 e += h[EN_NB] + h[EN_EXC];
@@ -2441,6 +2628,8 @@ static void capture_steps(b200md_ctx* c, int nsteps, cudaGraphExec_t* exec, int*
 extern "C" int b200md_step(b200md_ctx* ctx, int nsteps) {
     API_BEGIN(ctx)
     require(ctx->finalized && ctx->haveIntegrator, "step before finalize / set_integrator");
+    // the coefficients of the collective-variable forces come from the host before every step
+    require(ctx->cv.n == 0 || nsteps <= 1, "step: a context with CustomCVForce terms takes one step per call");
     b200md_ctx* c = ctx;
     int remaining = nsteps;
     prepare_list(c);      // the state was changed from outside: the step graphs trust the current list
@@ -2652,6 +2841,7 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
     require(phase != 8 || c->cpd.nslots > 0, "time_phase(custom compound bonds): the System has none");
     require(phase != 9 || c->ccd.nslots > 0, "time_phase(custom centroid bonds): the System has none");
     require(phase != 10 || c->gbsa.have, "time_phase(generalized Born): the System has none");
+    require(phase != 13 || c->rmd.nobj > 0, "time_phase(RMSD): the System has none");
     if (phase == 4) {
         require(c->haveIntegrator, "time_phase(integrate) before set_integrator");
         state.parts = state_spans(c, ST_POS | ST_VEL); state.save(s);
@@ -2677,6 +2867,7 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
             case 10: launch_gbsa(c->nb, c->gbd, false, s); break;
             case 11: launch_list_prep(c->nb, s); break;
             case 12: launch_build_tiles(c->nb, s); break;
+            case 13: launch_rmsd(c->nb, c->rmd, false, s); break;
             default: throw std::runtime_error("unknown phase");
         }
         CUDA_CHECK(cudaEventRecord(e1, s));

@@ -160,7 +160,7 @@ struct NbDev {
 };
 
 enum { EN_NB = 0, EN_RECIP = 1, EN_BOND = 2, EN_ANGLE = 3, EN_TORSION = 4, EN_EXC = 5, EN_KE = 6, EN_RBTORSION = 7, EN_CMAP = 8,
-       EN_CUSTOM = 9, EN_GB = 10, B200MD_NUM_ENERGY = 11 };
+       EN_CUSTOM = 9, EN_GB = 10, EN_RMSD = 11, B200MD_NUM_ENERGY = 12 };
 
 struct PmeDev {
     int nx, ny, nz, nzc;
@@ -256,6 +256,26 @@ struct GbsaDev {
     const double* atomRadius;    // R
     long long* bornSum; long long* dEdB;
     double* bornR; double* chain; double* bornForce;
+};
+
+// RMSDForce objects (rmsd.cu).  Object o is the entries [objStart[o], objStart[o+1]) of atoms (user atoms) and ref (the
+// reference position of each entry, centred over the object's entries on the host), in force group group[o]; entryObj maps an
+// entry back to its object and refSq[o] = sum |r|^2.  Per evaluation k_rmsd_sums writes sums[16 o ..] = (centre, sum |x - c|^2,
+// R row-major) and k_rmsd_solve solved[16 o ..] = (U row-major, 1/(N rmsd), rmsd).
+struct RmsdDev {
+    int nobj, nentries;
+    const int* objStart; const int* atoms; const int* entryObj;
+    const double* ref; const double* refSq;
+    const unsigned char* group;
+    double* sums; double* solved;
+    unsigned int groupMask;
+};
+
+// CustomCVForce (cv.cu): n collective variables; forces[i][3][npad] the fixed-point forces of variable i, snapshot from the inner
+// context; coeff[i] = dE/dCV_i, uploaded by the host before every evaluation
+struct CvDev {
+    int n;
+    const long long* forces; const double* coeff;
 };
 
 // One integration unit = a SETTLE water, a SHAKE cluster (centre + <=3 H) or a free atom.
@@ -592,6 +612,14 @@ void launch_centroid(const NbDev& nb, const CompoundDev& cc, const CentroidDev& 
 // the generalized Born chain on the current neighbour list: Born sums, radii + ACE + self terms, GB pairs, fold, chain-rule pairs
 const int GBSA_LAUNCHES = 5;
 void launch_gbsa(const NbDev& nb, const GbsaDev& gb, bool energy, cudaStream_t s);
+
+// RMSDForce: centre and sums, eigen solve, forces (launched behind the bonded terms, on their stream)
+const int RMSD_LAUNCHES = 3;
+void launch_rmsd(const NbDev& nb, const RmsdDev& rd, bool energy, cudaStream_t s);
+
+// CustomCVForce: the outer context's positions into the inner one; force += sum_i coeff_i F_i
+void launch_cv_copy_state(const NbDev& from, const NbDev& to, int natoms, cudaStream_t s);
+void launch_cv_combine(const NbDev& nb, const CvDev& cv, cudaStream_t s);
 
 void launch_integrate(const NbDev& nb, const UnitDev& units, const IntegDev& integ, const CommDev& cd, cudaStream_t s);
 void launch_force_push(const NbDev& nb, const CommDev& cd, cudaStream_t s);          // partial forces of foreign atoms -> owners' inboxes

@@ -8,12 +8,13 @@ from .systems import SystemDesc, NB_PME
 TERM_BONDS, TERM_ANGLES, TERM_TORSIONS, TERM_NB_DIRECT, TERM_NB_RECIP = 1, 2, 4, 8, 16
 TERM_RB_TORSIONS, TERM_CMAP, TERM_CUSTOM_TORSIONS = 32, 64, 128
 TERM_CUSTOM_BONDS, TERM_CUSTOM_EXTERNALS, TERM_CUSTOM_ANGLES, TERM_CUSTOM_COMPOUND = 256, 512, 1024, 2048
-TERM_CUSTOM_CENTROID, TERM_GBSA, TERM_ALL = 4096, 8192, 16383
+TERM_CUSTOM_CENTROID, TERM_GBSA, TERM_RMSD, TERM_CV_FORCES, TERM_ALL = 4096, 8192, 16384, 32768, 65535
 # kinds of b200md_set_bonded_groups
 BONDED_KINDS = {"bonds": 0, "angles": 1, "torsions": 2, "rb_torsions": 3, "cmap": 4, "custom_torsions": 5, "custom_bonds": 6,
                 "custom_externals": 7, "custom_angles": 9, "custom_compound": 10, "custom_centroid": 11}
 PHASES = {"pair": 0, "pme_spread": 1, "pme_fft_conv": 2, "pme_gather": 3, "integrate": 4, "list_build": 5, "bonded": 6,
-          "custom_torsions": 7, "custom_compound": 8, "custom_centroid": 9, "gbsa": 10, "list_prep": 11, "list_tiles": 12}
+          "custom_torsions": 7, "custom_compound": 8, "custom_centroid": 9, "gbsa": 10, "list_prep": 11, "list_tiles": 12,
+          "rmsd": 13}
 
 
 class EngineError(RuntimeError):
@@ -144,6 +145,11 @@ class Engine:
             self._ck(L.b200md_set_gbsa(self.h, int(d.gb_method), float(d.cutoff), float(d.gb_solute_dielectric),
                                        float(d.gb_solvent_dielectric), float(d.gb_surface_area_energy), _dp(_f64(d.gb_charges)),
                                        _dp(_f64(d.gb_radii)), _dp(_f64(d.gb_scales))))
+        if d.cv_count:
+            self._ck(L.b200md_set_cv_forces(self.h, int(d.cv_count)))
+        if len(d.rmsd_group):
+            self._ck(L.b200md_set_rmsd(self.h, len(d.rmsd_group), _ip(_i32(d.rmsd_start)), _ip(_i32(d.rmsd_atoms)),
+                                       _dp(_f64(d.rmsd_ref)), _ip(_i32(d.rmsd_group))))
         if len(d.con_i):
             self._ck(L.b200md_set_constraints(self.h, len(d.con_i), _ip(_i32(d.con_i)), _ip(_i32(d.con_j)), _dp(_f64(d.con_d))))
         if d.cm_frequency:
@@ -288,6 +294,12 @@ class Engine:
         if not (len(q) == len(r) == len(s)):
             raise ValueError("update_gbsa_params: charges, radii and scales differ in length")
         self._ck(self.lib.b200md_update_gbsa_params(self.h, len(q), _dp(q), _dp(r), _dp(s)))
+
+    # ---- CalcRMSDForceKernel::copyParametersToContext ----
+    def update_rmsd(self, start, atoms, ref):
+        """New particle lists and reference positions ([entries, 3]) for the same number of RMSD forces."""
+        start, atoms, ref = _i32(start), _i32(atoms), _f64(ref)
+        self._ck(self.lib.b200md_update_rmsd(self.h, len(start) - 1, _ip(start), _ip(atoms), _dp(ref)))
 
     def set_custom_globals(self, values):
         """The values of the global parameter slots the expressions read (the number of slots is fixed at definition)."""

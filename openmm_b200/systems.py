@@ -164,6 +164,14 @@ class SystemDesc:
     gb_solute_dielectric: float = 1.0
     gb_solvent_dielectric: float = 78.5
     gb_surface_area_energy: float = 2.25936
+    # RMSDForce objects (rmsd_*): object o is the atoms rmsd_atoms[rmsd_start[o]:rmsd_start[o+1]] with the reference position
+    # rmsd_ref[k] of entry k, in force group rmsd_group[o]; no objects when rmsd_group is empty
+    rmsd_start: np.ndarray = field(default_factory=_i)
+    rmsd_atoms: np.ndarray = field(default_factory=_i)
+    rmsd_ref: np.ndarray = field(default_factory=_d)
+    rmsd_group: np.ndarray = field(default_factory=_i)
+    # CustomCVForce: the number of collective variables whose forces the context combines (0: none)
+    cv_count: int = 0
     con_i: np.ndarray = field(default_factory=_i)
     con_j: np.ndarray = field(default_factory=_i)
     con_d: np.ndarray = field(default_factory=_d)

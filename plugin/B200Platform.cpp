@@ -10,7 +10,7 @@
 // HarmonicAngleForce, PeriodicTorsionForce, RBTorsionForce, CMAPTorsionForce, CustomTorsionForce, CustomBondForce,
 // CustomExternalForce, CustomAngleForce, CustomCompoundBondForce, CustomCentroidBondForce (any number of objects, each in its own force group; custom forces without energy parameter
 // derivatives, expressions within the limits of custom_translate.h), GBSAOBCForce (one per System, its method and cutoff
-// matching the NonbondedForce's; NoCutoff also without one), CMMotionRemover;
+// matching the NonbondedForce's; NoCutoff also without one), RMSDForce (any number of objects), CMMotionRemover;
 // Verlet / Langevin / LangevinMiddle integrators; SETTLE + X-H_n SHAKE constraints; MonteCarloBarostat and
 // MonteCarloAnisotropicBarostat (ApplyMonteCarloBarostatKernel; MonteCarloMembraneBarostat is refused).  A Force class without a kernel here
 // makes Platform::supportsKernels() false; an unsupported OPTION of a supported class is rejected in contextCreated()
@@ -47,6 +47,13 @@
 #include "openmm/CustomCompoundBondForce.h"
 #include "openmm/CustomCentroidBondForce.h"
 #include "openmm/GBSAOBCForce.h"
+#include "openmm/RMSDForce.h"
+#include "openmm/CustomCVForce.h"
+#include "openmm/TabulatedFunction.h"
+#include "lepton/CustomFunction.h"
+#include "lepton/ExpressionProgram.h"
+#include "lepton/ParsedExpression.h"
+#include "lepton/Parser.h"
 #include "openmm/CMMotionRemover.h"
 #include "openmm/VerletIntegrator.h"
 #include "openmm/LangevinIntegrator.h"
@@ -67,6 +74,10 @@
 
 using namespace OpenMM;
 using namespace std;
+
+// the Reference platform's spline of a TabulatedFunction as a Lepton function, exported by libOpenMM.so
+// (platforms/reference/include/ReferenceTabulatedFunction.h)
+extern "C" Lepton::CustomFunction* createReferenceTabulatedFunction(const TabulatedFunction& function);
 
 namespace {
 
@@ -206,6 +217,18 @@ struct PlatformData {
     // CMAP: the maps of all objects one after the other (a term's map index counts from the first map of all objects);
     // coefficients from CMAPTorsionForceImpl::calcMapDerivatives, [sum size^2][16]
     vector<int> cmapSize; vector<double> cmapCoeff;
+    // RMSDForce objects in the order their kernels were initialised: particle lists (an empty list expanded to every particle)
+    // with the reference position of each listed particle, and the force groups
+    int cvCount = 0;                // collective variables of the System's CustomCVForce
+    vector<vector<int> > rmsdParticles; vector<vector<double> > rmsdRef; vector<int> rmsdGroup;
+    void rmsdArrays(vector<int>& start, vector<int>& atoms, vector<double>& ref) const {
+        start.assign(1, 0); atoms.clear(); ref.clear();
+        for (size_t o = 0; o < rmsdParticles.size(); o++) {
+            atoms.insert(atoms.end(), rmsdParticles[o].begin(), rmsdParticles[o].end());
+            ref.insert(ref.end(), rmsdRef[o].begin(), rmsdRef[o].end());
+            start.push_back((int) atoms.size());
+        }
+    }
     // the programs of each custom class
     CustomPrograms customPrograms[6];
     // the global parameters the expressions of all custom classes read: slot of every name (shared by all objects) and the
@@ -255,6 +278,11 @@ struct PlatformData {
             check(b200md_set_bonded_groups(ctx, r.kind, r.size(), r.group.data()));
         }
         if (!customGlobals.empty()) check(b200md_set_custom_globals(ctx, (int) customGlobals.size(), customGlobals.data()));
+        if (!rmsdGroup.empty()) {
+            vector<int> start, atoms; vector<double> ref;
+            rmsdArrays(start, atoms, ref);
+            check(b200md_set_rmsd(ctx, (int) rmsdGroup.size(), start.data(), atoms.data(), ref.data(), rmsdGroup.data()));
+        }
         check(b200md_finalize(ctx));
         finalized = true;
     }
@@ -876,6 +904,125 @@ private:
     ContextImpl& context;
 };
 
+// RMSDForce: the particle list and reference positions go to the engine at finalize, with those of every other RMSDForce;
+// execute() only records the term, so the step graph covers it.  RMSDForceImpl has checked the particle indices and the
+// number of reference positions.
+class B200CalcRMSDForceKernel : public CalcRMSDForceKernel {
+public:
+    B200CalcRMSDForceKernel(string name, const Platform& platform, ContextImpl& context) : CalcRMSDForceKernel(name, platform), context(context) {}
+    // the particle list (empty: every particle, as ReferenceCalcRMSDForceKernel) and the reference position of each
+    static void read(const RMSDForce& force, int numParticles, vector<int>& particles, vector<double>& ref) {
+        particles = force.getParticles();
+        if (particles.empty())
+            for (int i = 0; i < numParticles; i++) particles.push_back(i);
+        const vector<Vec3>& pos = force.getReferencePositions();
+        ref.clear();
+        for (int i : particles) for (int k = 0; k < 3; k++) ref.push_back(pos[i][k]);
+    }
+    void initialize(const System& system, const RMSDForce& force) {
+        PlatformData& d = getData(context);
+        if (d.finalized) throw OpenMMException("B200 platform: RMSDForce initialised after the Context was finalised");
+        index = (int) d.rmsdGroup.size();
+        numReference = (int) force.getReferencePositions().size();
+        d.rmsdParticles.emplace_back(); d.rmsdRef.emplace_back();
+        read(force, system.getNumParticles(), d.rmsdParticles.back(), d.rmsdRef.back());
+        d.rmsdGroup.push_back(force.getForceGroup());
+        d.systemTerms |= B200MD_TERM_RMSD; d.bondedGroupsUsed |= 1u << force.getForceGroup();
+    }
+    double execute(ContextImpl& context, bool includeForces, bool includeEnergy) { getData(context).pendingTerms |= B200MD_TERM_RMSD; return 0.0; }
+    void copyParametersToContext(ContextImpl& context, const RMSDForce& force) {
+        PlatformData& d = getData(context);
+        d.ensureFinalized();
+        d.dropForces();
+        if ((int) force.getReferencePositions().size() != numReference)
+            throw OpenMMException("updateParametersInContext: The number of reference positions has changed");
+        read(force, d.numParticles, d.rmsdParticles[index], d.rmsdRef[index]);
+        vector<int> start, atoms; vector<double> ref;
+        d.rmsdArrays(start, atoms, ref);
+        d.check(b200md_update_rmsd(d.ctx, (int) d.rmsdGroup.size(), start.data(), atoms.data(), ref.data()));
+    }
+private:
+    ContextImpl& context;
+    int index = 0, numReference = 0;
+};
+
+// CustomCVForce: CustomCVForceImpl (the reference's, untouched) builds an inner System of the collective variables, one force
+// group each, and a linked Context on this platform, so the inner Context is an ordinary engine on the same device.  execute()
+// copies the state to it on the device, evaluates each variable's group there and snapshots its forces into the outer
+// context's slot, evaluates the energy expression and its derivatives on the host with Lepton (one host sync per variable, as
+// on the reference's GPU platforms), uploads dE/dCV_i and records the term: the forces are combined inside the outer
+// evaluation, the fused step graph included.
+class B200CalcCustomCVForceKernel : public CalcCustomCVForceKernel {
+public:
+    B200CalcCustomCVForceKernel(string name, const Platform& platform, ContextImpl& context) : CalcCustomCVForceKernel(name, platform), context(context) {}
+    void initialize(const System& system, const CustomCVForce& force, ContextImpl& innerContext) {
+        PlatformData& d = getData(context);
+        if (d.finalized) throw OpenMMException("B200 platform: CustomCVForce initialised after the Context was finalised");
+        if (d.cvCount) throw OpenMMException("B200 platform: only one CustomCVForce per System is supported");
+        if (force.getNumEnergyParameterDerivatives() > 0) throw OpenMMException("B200 platform: energy parameter derivatives of a CustomCVForce are not supported");
+        for (int i = 0; i < force.getNumCollectiveVariables(); i++) variableNames.push_back(force.getCollectiveVariableName(i));
+        for (int i = 0; i < force.getNumGlobalParameters(); i++) globalNames.push_back(force.getGlobalParameterName(i));
+        build(force);
+        d.cvCount = (int) variableNames.size();
+        d.check(b200md_set_cv_forces(d.ctx, d.cvCount));
+        d.systemTerms |= B200MD_TERM_CV_FORCES;
+    }
+    double execute(ContextImpl& context, ContextImpl& innerContext, bool includeForces, bool includeEnergy) {
+        PlatformData& d = getData(context);
+        d.ensureFinalized();
+        copyState(context, innerContext);
+        PlatformData& inner = getData(innerContext);
+        map<string, double> variables;
+        for (const string& name : globalNames) variables[name] = context.getParameter(name);
+        const int n = (int) variableNames.size();
+        for (int i = 0; i < n; i++) {
+            variables[variableNames[i]] = innerContext.calcForcesAndEnergy(true, true, 1 << i);
+            if (includeForces) d.check(b200md_cv_snapshot_forces(inner.ctx, d.ctx, i));
+        }
+        if (includeForces) {
+            vector<double> coeff(n);
+            for (int i = 0; i < n; i++) coeff[i] = derivs[i].evaluate(variables);
+            d.check(b200md_set_cv_coefficients(d.ctx, n, coeff.data()));
+            d.pendingTerms |= B200MD_TERM_CV_FORCES;
+        }
+        return includeEnergy ? energy.evaluate(variables) : 0.0;
+    }
+    // the positions, box and global parameters of the outer Context into the inner one (getCollectiveVariableValues reads it)
+    void copyState(ContextImpl& context, ContextImpl& innerContext) {
+        PlatformData& d = getData(context);
+        d.ensureFinalized();
+        PlatformData& inner = getData(innerContext);
+        inner.ensureFinalized();
+        inner.dropForces();
+        for (auto& p : innerContext.getParameters()) innerContext.setParameter(p.first, context.getParameter(p.first));
+        if (b200md_cv_copy_state(d.ctx, inner.ctx) != 0) d.check(-1);
+        inner.boxError = d.boxError;
+    }
+    void copyParametersToContext(ContextImpl& context, const CustomCVForce& force) { build(force); }
+private:
+    // the energy expression and its derivatives by the variables, with the force's tabulated functions as the Reference
+    // platform's splines (ReferenceCustomCVForce)
+    void build(const CustomCVForce& force) {
+        map<string, Lepton::CustomFunction*> functions;
+        for (int i = 0; i < force.getNumTabulatedFunctions(); i++)
+            functions[force.getTabulatedFunctionName(i)] = createReferenceTabulatedFunction(force.getTabulatedFunction(i));
+        try {
+            Lepton::ParsedExpression expr = Lepton::Parser::parse(force.getEnergyFunction(), functions);
+            energy = expr.createProgram();
+            derivs.clear();
+            for (const string& name : variableNames) derivs.push_back(expr.differentiate(name).optimize().createProgram());
+        } catch (...) {
+            for (auto& f : functions) delete f.second;
+            throw;
+        }
+        for (auto& f : functions) delete f.second;
+    }
+    ContextImpl& context;
+    vector<string> variableNames, globalNames;
+    Lepton::ExpressionProgram energy;
+    vector<Lepton::ExpressionProgram> derivs;
+};
+
 // RemoveCMMotionKernel::execute is called by CMMotionRemoverImpl::updateContextState in EVERY step; the frequency test is
 // the kernel's (ReferenceKernels.cpp:2712-2714).  The removal itself is deferred to the integrator step that follows (the
 // fused step graph removes the centre-of-mass motion itself) or to the next read of the velocities (PlatformData::flushCm).
@@ -1010,6 +1157,8 @@ public:
         if (name == CalcCustomCompoundBondForceKernel::Name()) return new B200CalcCustomForceKernel<CustomCompounds>(name, platform, context);
         if (name == CalcCustomCentroidBondForceKernel::Name()) return new B200CalcCustomForceKernel<CustomCentroids>(name, platform, context);
         if (name == CalcGBSAOBCForceKernel::Name()) return new B200CalcGBSAOBCForceKernel(name, platform, context);
+        if (name == CalcRMSDForceKernel::Name()) return new B200CalcRMSDForceKernel(name, platform, context);
+        if (name == CalcCustomCVForceKernel::Name()) return new B200CalcCustomCVForceKernel(name, platform, context);
         if (name == RemoveCMMotionKernel::Name()) return new B200RemoveCMMotionKernel(name, platform, context);
         if (name == IntegrateVerletStepKernel::Name()) return new B200IntegrateVerletStepKernel(name, platform);
         if (name == IntegrateLangevinStepKernel::Name()) return new B200IntegrateLangevinStepKernel(name, platform);
@@ -1028,7 +1177,7 @@ public:
                                 CalcPeriodicTorsionForceKernel::Name(), CalcRBTorsionForceKernel::Name(), CalcCMAPTorsionForceKernel::Name(),
                                 CalcCustomTorsionForceKernel::Name(), CalcCustomBondForceKernel::Name(), CalcCustomExternalForceKernel::Name(),
                                 CalcCustomAngleForceKernel::Name(), CalcCustomCompoundBondForceKernel::Name(), CalcCustomCentroidBondForceKernel::Name(),
-                                CalcGBSAOBCForceKernel::Name(), RemoveCMMotionKernel::Name(), IntegrateVerletStepKernel::Name(),
+                                CalcGBSAOBCForceKernel::Name(), CalcRMSDForceKernel::Name(), CalcCustomCVForceKernel::Name(), RemoveCMMotionKernel::Name(), IntegrateVerletStepKernel::Name(),
                                 IntegrateLangevinStepKernel::Name(), IntegrateLangevinMiddleStepKernel::Name(), ApplyMonteCarloBarostatKernel::Name()})
             registerKernelFactory(n, factory);
         platformProperties.push_back(DeviceIndex());
@@ -1092,14 +1241,36 @@ public:
             if (!(r > 0.009)) throw OpenMMException("B200 platform: a GBSAOBCForce radius at or below the dielectric offset (0.009 nm)");
         }
     }
-    static void validateSystem(const System& system) {
-        for (int i = 0; i < system.getNumParticles(); i++)
-            if (system.isVirtualSite(i)) throw OpenMMException("B200 platform: virtual sites are not supported");
+    // the Force classes this platform has a kernel for; a CustomCVForce's variables must be among them, since its inner
+    // Context is created on this platform explicitly and cannot fall back on its own
+    static bool hasKernel(const Force& f) {
+        return dynamic_cast<const NonbondedForce*>(&f) || dynamic_cast<const HarmonicBondForce*>(&f) || dynamic_cast<const HarmonicAngleForce*>(&f) ||
+               dynamic_cast<const PeriodicTorsionForce*>(&f) || dynamic_cast<const RBTorsionForce*>(&f) || dynamic_cast<const CMAPTorsionForce*>(&f) ||
+               dynamic_cast<const CustomTorsionForce*>(&f) || dynamic_cast<const CustomBondForce*>(&f) || dynamic_cast<const CustomExternalForce*>(&f) ||
+               dynamic_cast<const CustomAngleForce*>(&f) || dynamic_cast<const CustomCompoundBondForce*>(&f) ||
+               dynamic_cast<const CustomCentroidBondForce*>(&f) || dynamic_cast<const GBSAOBCForce*>(&f) || dynamic_cast<const RMSDForce*>(&f) ||
+               dynamic_cast<const CustomCVForce*>(&f);
+    }
+    // The checks of one System's forces: the System's own, or the collective variables of a CustomCVForce, which become the
+    // forces of its inner System (same particles, one force group per variable), checked the same way, recursively
+    static void validateForces(const System& system, const vector<const Force*>& forces) {
         int numNonbonded = 0;
         const NonbondedForce* nonbonded = nullptr;
         const GBSAOBCForce* gbsa = nullptr;
-        for (int f = 0; f < system.getNumForces(); f++) {
-            const Force& force = system.getForce(f);
+        for (const Force* fp : forces) {
+            const Force& force = *fp;
+            if (const CustomCVForce* cv = dynamic_cast<const CustomCVForce*>(&force)) {
+                if (cv->getNumEnergyParameterDerivatives() > 0)
+                    throw OpenMMException("B200 platform: energy parameter derivatives of a CustomCVForce are not supported");
+                if (cv->getNumCollectiveVariables() > 31) throw OpenMMException("B200 platform: a CustomCVForce has more than 31 collective variables");
+                vector<const Force*> variables;
+                for (int i = 0; i < cv->getNumCollectiveVariables(); i++) {
+                    const Force& v = cv->getCollectiveVariable(i);
+                    if (!hasKernel(v)) throw OpenMMException("B200 platform: a collective variable of a CustomCVForce is of a Force class this platform does not run");
+                    variables.push_back(&v);
+                }
+                validateForces(system, variables);
+            }
             if (const GBSAOBCForce* g = dynamic_cast<const GBSAOBCForce*>(&force)) {
                 if (gbsa) throw OpenMMException("B200 platform: only one GBSAOBCForce per System is supported");
                 gbsa = g;
@@ -1122,6 +1293,18 @@ public:
             if (const CustomCentroidBondForce* f = dynamic_cast<const CustomCentroidBondForce*>(&force)) validateCustom<CustomCentroids>(*f);
         }
         if (gbsa) validateGBSA(system, *gbsa, nonbonded);
+    }
+    static void validateSystem(const System& system) {
+        for (int i = 0; i < system.getNumParticles(); i++)
+            if (system.isVirtualSite(i)) throw OpenMMException("B200 platform: virtual sites are not supported");
+        int numCV = 0;
+        vector<const Force*> forces;
+        for (int f = 0; f < system.getNumForces(); f++) {
+            forces.push_back(&system.getForce(f));
+            if (dynamic_cast<const CustomCVForce*>(&system.getForce(f)) && ++numCV > 1)
+                throw OpenMMException("B200 platform: only one CustomCVForce per System is supported");
+        }
+        validateForces(system, forces);
         const int nc = system.getNumConstraints();
         if (nc > 0) {
             vector<int> ci(nc), cj(nc); vector<double> cd(nc), mass(system.getNumParticles());
