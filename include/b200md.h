@@ -49,7 +49,8 @@ typedef struct b200md_ctx b200md_ctx;
 #define B200MD_TERM_GBSA             8192   /* GBSAOBCForce: OBC II implicit solvent with the ACE surface term */
 #define B200MD_TERM_RMSD             16384  /* RMSDForce */
 #define B200MD_TERM_CV_FORCES        32768  /* CustomCVForce: force += sum_i dE/dCV_i F_i (b200md_set_cv_coefficients) */
-#define B200MD_TERM_ALL        65535
+#define B200MD_TERM_CUSTOM_NONBONDED 65536  /* CustomNonbondedForce (b200md_set_custom_nonbonded) */
+#define B200MD_TERM_ALL        131071
 
 /* ---- the bonded classes: kind argument of b200md_set_bonded_groups and b200md_update_bonded_params ---- */
 #define B200MD_BONDED_BONDS           0
@@ -72,6 +73,8 @@ typedef struct b200md_ctx b200md_ctx;
 #define B200MD_CUSTOM_ANGLE    3      /* THETA = the angle in [0, pi]             */
 #define B200MD_CUSTOM_COMPOUND 4      /* VAR 3i, 3i+1, 3i+2 = x, y, z of particle i; POINT_DIST, POINT_ANGLE, POINT_DIHEDRAL */
 #define B200MD_CUSTOM_CENTROID 5      /* as COMPOUND, with the centre of group i for particle i */
+#define B200MD_CUSTOM_NONBONDED 6     /* VAR 0 = r; PARAM k = parameter k of the first particle, PARAM P+k of the second (P per-particle
+                                       * parameters, P <= B200MD_CUSTOM_MAX_PARAMS/2); DISCRETE1..3 */
 
 /* ---- instructions of a custom-term expression program (b200md_set_custom_torsions / _bonds / _externals / _angles /
  * _compound) ----
@@ -86,7 +89,11 @@ typedef struct b200md_ctx b200md_ctx;
  * k in 0..5 its derivative by argument k (ReferencePointDistanceFunction, periodic), every one of them 0 at distance 0.
  * POINT_DIST (6 arguments), POINT_ANGLE (9) and POINT_DIHEDRAL (12) are pointdistance, pointangle and pointdihedral of a
  * CustomCompoundBondForce (ReferencePointFunctions.cpp) with the same operand convention: -1 the value, k >= 0 the first
- * derivative by argument k.  They take the minimum image of every displacement iff their expression is periodic. */
+ * derivative by argument k.  They take the minimum image of every displacement iff their expression is periodic.
+ * DISCRETE1, DISCRETE2 and DISCRETE3 (CustomNonbondedForce only) are Discrete1D/2D/3DFunction tables of b200md_set_custom_tables
+ * with 1, 2 or 3 arguments: operand t >= 0 looks up table t at the arguments rounded to the nearest integer (round(), halves away
+ * from zero), x + xsize (y + ysize z), as ReferenceDiscrete{1,2,3}DFunction::evaluate; an index outside the table gives NaN.
+ * Operand -1 is a derivative of the function, which is 0 (evaluateDerivative). */
 enum {
     B200MD_OP_CONST = 0, B200MD_OP_THETA, B200MD_OP_PARAM, B200MD_OP_GLOBAL,
     B200MD_OP_ADD, B200MD_OP_SUB, B200MD_OP_MUL, B200MD_OP_DIV, B200MD_OP_POW, B200MD_OP_NEG, B200MD_OP_SQRT, B200MD_OP_EXP,
@@ -95,6 +102,7 @@ enum {
     B200MD_OP_ERFC, B200MD_OP_STEP, B200MD_OP_DELTA, B200MD_OP_SQUARE, B200MD_OP_CUBE, B200MD_OP_RECIP, B200MD_OP_ADD_CONST,
     B200MD_OP_MUL_CONST, B200MD_OP_POW_CONST, B200MD_OP_MIN, B200MD_OP_MAX, B200MD_OP_ABS, B200MD_OP_FLOOR, B200MD_OP_CEIL,
     B200MD_OP_SELECT, B200MD_OP_VAR, B200MD_OP_PERIODIC_DIST, B200MD_OP_POINT_DIST, B200MD_OP_POINT_ANGLE, B200MD_OP_POINT_DIHEDRAL,
+    B200MD_OP_DISCRETE1, B200MD_OP_DISCRETE2, B200MD_OP_DISCRETE3,
     B200MD_OP_COUNT
 };
 /* hard limits of a custom-term program: stack depth (of a compound-bond program: B200MD_CUSTOM_COMPOUND_MAX_STACK, a
@@ -273,6 +281,28 @@ int b200md_set_gbsa(b200md_ctx* ctx, int method, double cutoff, double solute_di
 /* CalcGBSAOBCForceKernel::copyParametersToContext: new charges, radii and scales (n == the number of atoms) into the same
  * device buffers, so a captured step graph stays valid.                                                                   */
 int b200md_update_gbsa_params(b200md_ctx* ctx, int n, const double* charge, const double* radius, const double* scale);
+/* CalcCustomNonbondedForceKernel::initialize (kernels.h): nobj CustomNonbondedForce objects that share one method
+ * (B200MD_NB_NOCUTOFF, _CUTOFF_NONPERIODIC or _CUTOFF_PERIODIC), one cutoff and one set of excluded pairs.  Programs 2o and 2o+1
+ * are the energy of object o and its dE/dr (class B200MD_CUSTOM_NONBONDED), as for b200md_set_custom_torsions.  Object o has
+ * nparams[o] <= B200MD_CUSTOM_MAX_PARAMS/2 per-particle parameters, params[(o natoms + i) param_stride + k] (param_stride >=
+ * every nparams[o]); a switching distance switch_distance[o] (< 0: none; else 0 <= it < cutoff), applied as
+ * S = 1 - 10 x^3 + 15 x^4 - 6 x^5, x = (r - switch)/(cutoff - switch), to the energy and the force; and force group group[o]
+ * (0..31).  Every pair of distinct particles within the cutoff (r < cutoff; every pair with NoCutoff), but the nexcl pairs
+ * (excl_p1[k], excl_p2[k]), interacts; CutoffPeriodic takes the minimum image.  With b200md_set_nonbonded the method must
+ * agree with it (CutoffPeriodic with CutoffPeriodic or PME), the cutoff must be its cutoff and the excluded pairs its
+ * exceptions; without it the neighbour list is built at this method and cutoff with these exclusions.  Single GPU only.   */
+int b200md_set_custom_nonbonded(b200md_ctx* ctx, int method, double cutoff, int nobj, const int* prog_start, const int* op, const int* arg,
+                                const double* imm, const int* nparams, int param_stride, const double* params,
+                                const double* switch_distance, const int* group, int nexcl, const int* excl_p1, const int* excl_p2);
+/* The Discrete1D/2D/3DFunction tables the DISCRETE instructions read, before finalize: ntables tables, table t of dims[4t]
+ * (1, 2 or 3) dimensions of sizes dims[4t+1 ..] (unused ones 1), its values values[start[t] .. start[t+1]-1], x fastest.      */
+int b200md_set_custom_tables(b200md_ctx* ctx, int ntables, const int* dims, const int* start, const double* values);
+/* CalcCustomNonbondedForceKernel::copyParametersToContext: new per-particle parameters of every object (same layout) into the
+ * same device buffers, so a captured step graph stays valid.                                                              */
+int b200md_update_custom_nonbonded_params(b200md_ctx* ctx, int n, const double* params);
+/* The long-range correction of every object (CustomNonbondedForceImpl::calcLongRangeCorrection, 0 for none): coefficient[o]/V
+ * is added to the energy of object o's group at every energy evaluation, V the volume of the current box.                   */
+int b200md_set_custom_nonbonded_lrc(b200md_ctx* ctx, int nobj, const double* coefficient);
 /* CalcRMSDForceKernel::initialize (kernels.h): nforces RMSDForce objects.  Object o is the particles particles[start[o] ..
  * start[o+1]-1] (start has nforces + 1 entries, start[0] = 0; at least one particle, each at most once; the caller expands an
  * empty RMSDForce particle list to every particle) with the reference positions ref[3k .. 3k+2] of entry k, in force group
@@ -316,6 +346,12 @@ int b200md_custom_program_probe(int nprog, const int* prog_start, const int* op,
 int b200md_custom_term_probe(int cls, int nprog, const int* prog_start, const int* op, const int* arg, const double* imm,
                              int param_stride, int nglobals, int which, const double* vars, const double* box,
                              const double* params, const double* globals, double* out, char* msg, int msglen);
+/* The same for a CustomNonbondedForce program set (2 programs per object) of objects with nparams parameters each: program
+ * `which` at r = vars[0] with params[0 .. 2 nparams-1] (the first particle's, then the second's), reading the tables of
+ * b200md_set_custom_tables given here (ntables, dims, start, values).                                                     */
+int b200md_custom_nonbonded_probe(int nprog, const int* prog_start, const int* op, const int* arg, const double* imm, int nparams,
+                                  int nglobals, int which, double r, const double* params, const double* globals, int ntables,
+                                  const int* dims, const int* start, const double* values, double* out, char* msg, int msglen);
 /* The same for ONE compound-bond expression of nparticles particles (1 + 3 nparticles programs), periodic or not, at the 3
  * nparticles coordinates vars[].                                                                                          */
 int b200md_custom_compound_probe(int nparticles, int periodic, const int* prog_start, const int* op, const int* arg, const double* imm,
@@ -416,7 +452,8 @@ int b200md_get_stats(b200md_ctx* ctx, b200md_stats* out);
  * angles alone (k_custom), 8 custom compound bonds alone (k_compound), 9 custom centroid bonds alone (k_centroid_centers,
  * the k_compound instantiation that reads the centres, k_centroid_scatter), 10 the generalized Born chain (k_gb_born,
  * k_gb_radii, k_gb_pairs, k_gb_fold, k_gb_chain), 11 the first half of the list build alone (k_list_prep: binning, sort,
- * block bounds), 12 its second half alone (k_build_tiles), 13 the RMSD forces (k_rmsd_sums, k_rmsd_solve, k_rmsd_forces).
+ * block bounds), 12 its second half alone (k_build_tiles), 13 the RMSD forces (k_rmsd_sums, k_rmsd_solve, k_rmsd_forces),
+ * 14 the CustomNonbondedForce pairs (k_custom_nonbonded).
  * Runs `reps` isolated launches of that phase on the current state.                                  */
 int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* ms_mean);
 /* The current neighbour list, read back for identity checks.  *ntiles = its tile count.  sorig (if not NULL): [padded_atoms]

@@ -67,6 +67,12 @@ SIGNATURES = {
     "b200md_update_custom_centroid_params": (C.c_int, [_P, C.c_int, _D]),
     "b200md_set_gbsa": (C.c_int, [_P, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, _D, _D, _D]),
     "b200md_update_gbsa_params": (C.c_int, [_P, C.c_int, _D, _D, _D]),
+    "b200md_set_custom_nonbonded": (C.c_int, [_P, C.c_int, C.c_double, C.c_int, _I, _I, _I, _D, _I, C.c_int, _D, _D, _I, C.c_int, _I, _I]),
+    "b200md_set_custom_tables": (C.c_int, [_P, C.c_int, _I, _I, _D]),
+    "b200md_update_custom_nonbonded_params": (C.c_int, [_P, C.c_int, _D]),
+    "b200md_set_custom_nonbonded_lrc": (C.c_int, [_P, C.c_int, _D]),
+    "b200md_custom_nonbonded_probe": (C.c_int, [C.c_int, _I, _I, _I, _D, C.c_int, C.c_int, C.c_int, C.c_double, _D, _D, C.c_int, _I, _I,
+                                                _D, _D, C.c_char_p, C.c_int]),
     "b200md_set_rmsd": (C.c_int, [_P, C.c_int, _I, _I, _D, _I]),
     "b200md_update_rmsd": (C.c_int, [_P, C.c_int, _I, _I, _D]),
     "b200md_rmsd_probe": (C.c_int, [C.c_int, _D, _D, _D, _D]),

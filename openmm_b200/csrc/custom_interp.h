@@ -1,9 +1,10 @@
 // custom_interp.h -- the interpreter of custom-term expression programs (B200MD_OP_*, include/b200md.h), one source for
-// the device kernels (k_custom and k_compound, bonded.cu) and the host (the program checks of engine.cu and the
+// the device kernels (k_custom and k_compound, bonded.cu; k_custom_nonbonded, custom_nonbonded.cu) and the host (the program checks of engine.cu and the
 // b200md_custom_*_probe calls).  A program is a Lepton ExpressionProgram flattened to (opcode, operand, immediate); this file
 // restates ExpressionProgram::evaluate (ExpressionProgram.cpp:100-110), every Operation::evaluate (lepton/Operation.h) and,
 // for PERIODIC_DIST and the POINT_* opcodes, ReferencePointDistanceFunction, ReferencePointAngleFunction and
-// ReferencePointDihedralFunction (ReferencePointFunctions.cpp) over a fixed-size double stack.
+// ReferencePointDihedralFunction (ReferencePointFunctions.cpp) and, for the DISCRETE opcodes, ReferenceDiscrete{1,2,3}DFunction
+// (ReferenceTabulatedFunction.cpp) over a fixed-size double stack.
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>
@@ -21,7 +22,8 @@ CUSTOM_HD int custom_op_args(int op) {
         case B200MD_OP_CONST: case B200MD_OP_THETA: case B200MD_OP_PARAM: case B200MD_OP_GLOBAL: case B200MD_OP_VAR: return 0;
         case B200MD_OP_ADD: case B200MD_OP_SUB: case B200MD_OP_MUL: case B200MD_OP_DIV: case B200MD_OP_POW:
         case B200MD_OP_ATAN2: case B200MD_OP_MIN: case B200MD_OP_MAX: return 2;
-        case B200MD_OP_SELECT: return 3;
+        case B200MD_OP_SELECT: case B200MD_OP_DISCRETE3: return 3;
+        case B200MD_OP_DISCRETE2: return 2;
         case B200MD_OP_PERIODIC_DIST: case B200MD_OP_POINT_DIST: return 6;
         case B200MD_OP_POINT_ANGLE: return 9;
         case B200MD_OP_POINT_DIHEDRAL: return 12;
@@ -132,15 +134,31 @@ CUSTOM_HD double custom_point_dihedral(const double* a, int which, const CustomB
     return which < 3 ? -i0 : which < 6 ? i0 - s : which < 9 ? i3 + s : -i3;
 }
 
+// The Discrete1D/2D/3DFunction tables of a context (b200md_set_custom_tables): table t has dims[t] = (dimensions, xsize, ysize,
+// zsize) and the values [start[t], start[t+1]) of values, x fastest.
+struct CustomTables { int n; const int4* dims; const int* start; const double* values; };
+
+// A DISCRETE instruction of nargs arguments a[] and operand t: table t at the arguments rounded to the nearest integer, as
+// ReferenceDiscrete{1,2,3}DFunction::evaluate, or NaN for an index outside the table (the Reference platform throws there; the
+// NaN reaches the energy and the forces instead of a clamped, silently wrong value).  Operand -1 is a derivative: 0.
+CUSTOM_HD double custom_discrete(const double* a, int nargs, int t, const CustomTables& tb) {
+    if (t < 0) return 0.0;
+    const int4 d = tb.dims[t];
+    const double x = round(a[0]), y = nargs > 1 ? round(a[1]) : 0.0, z = nargs > 2 ? round(a[2]) : 0.0;
+    if (!(x >= 0.0 && x < d.y && y >= 0.0 && y < d.z && z >= 0.0 && z < d.w)) return NAN;
+    return tb.values[tb.start[t] + (int) x + d.y*((int) y + d.z*(int) z)];
+}
+
 // Program [begin, end) of `code` (x = opcode, y = operand) and `imm`, at the term's variables vars[] (THETA reads vars[0]).
 // Argument k of an operation is st[sp + k]: argument 0 is the value pushed last, as in ExpressionProgram::evaluate.  The
 // program must have passed custom_check_program (no underflow, depth <= STACK, one value left, VAR operands within the
 // class's variables).  STACK is the capacity of the stack (B200MD_CUSTOM_MAX_STACK; B200MD_CUSTOM_COMPOUND_MAX_STACK for a
 // compound bond); POINTS: the program may hold POINT_* instructions (a compound bond's), which take the minimum image iff
-// `periodic`.  Without POINTS their code is not generated: the other classes' programs cannot hold them.
-template <int STACK, bool POINTS>
+// `periodic`.  Without POINTS their code is not generated: the other classes' programs cannot hold them.  TABLES: the program
+// may hold DISCRETE instructions (a custom nonbonded force's), which read `tables`; likewise not generated without it.
+template <int STACK, bool POINTS, bool TABLES = false>
 CUSTOM_HD double custom_run(const int2* code, const double* imm, int begin, int end, const double* vars, const double* params,
-                            const double* globals, const CustomBox& box, bool periodic = false) {
+                            const double* globals, const CustomBox& box, bool periodic = false, const CustomTables* tables = nullptr) {
     double st[STACK];
     int sp = STACK;
     for (int pc = begin; pc < end; pc++) {
@@ -195,7 +213,8 @@ CUSTOM_HD double custom_run(const int2* code, const double* imm, int begin, int 
             case B200MD_OP_PERIODIC_DIST: r = custom_periodic_dist(st + sp, in.y, box); break;
             case B200MD_OP_SELECT: r = a != 0.0 ? b : st[sp + 2]; break;
             default:
-                if (!POINTS) r = 0.0;
+                if (TABLES && in.x >= B200MD_OP_DISCRETE1) r = custom_discrete(st + sp, nargs, in.y, *tables);
+                else if (!POINTS) r = 0.0;
                 else if (in.x == B200MD_OP_POINT_DIST) r = custom_point_dist(st + sp, in.y, box, periodic);
                 else if (in.x == B200MD_OP_POINT_ANGLE) r = custom_point_angle(st + sp, in.y, box, periodic);
                 else r = custom_point_dihedral(st + sp, in.y, box, periodic);
@@ -212,15 +231,19 @@ CUSTOM_HD double custom_run(const int2* code, const double* imm, int begin, int 
 // operand in -1..5; a compound bond of nparticles particles: VAR 0..3 nparticles-1 and the POINT_* opcodes with an operand
 // from -1 to their number of arguments - 1), PARAM operands < param_stride, GLOBAL operands < nglobals (nglobals < 0: not
 // checked yet), no stack underflow, depth <= the class's stack capacity, exactly one value left, at most
-// B200MD_CUSTOM_MAX_CODE instructions.  nullptr if the program passes, else the reason.  An opcode of another class's is an
+// B200MD_CUSTOM_MAX_CODE instructions.  A custom nonbonded program reads VAR 0 (r) and may hold the DISCRETE opcodes, with an
+// operand from -1 to ntables - 1 (ntables < 0: not checked yet); they are unknown opcodes for every other class.  nullptr if the program passes, else the reason.  An opcode of another class's is an
 // unknown opcode for a torsion or an angle program, as is a POINT_* opcode for every class but the compound bond.  A centroid
 // bond's program (of nparticles group centres) is checked as a compound bond's.
-inline const char* custom_check_program(int cls, const int2* code, int begin, int end, int param_stride, int nglobals, int nparticles = 0) {
+inline const char* custom_check_program(int cls, const int2* code, int begin, int end, int param_stride, int nglobals, int nparticles = 0,
+                                        int ntables = -1) {
     const bool torsion = cls == B200MD_CUSTOM_TORSION, bond = cls == B200MD_CUSTOM_BOND, angle = cls == B200MD_CUSTOM_ANGLE,
-               centroid = cls == B200MD_CUSTOM_CENTROID, compound = cls == B200MD_CUSTOM_COMPOUND || centroid;
+               centroid = cls == B200MD_CUSTOM_CENTROID, compound = cls == B200MD_CUSTOM_COMPOUND || centroid,
+               nonbonded = cls == B200MD_CUSTOM_NONBONDED;
 #define CUSTOM_WHY(what) (torsion ? "custom torsion program: " what : bond ? "custom bond program: " what : \
                           angle ? "custom angle program: " what : centroid ? "custom centroid program: " what : \
-                          compound ? "custom compound program: " what : "custom external program: " what)
+                          compound ? "custom compound program: " what : nonbonded ? "custom nonbonded program: " what : \
+                          "custom external program: " what)
     if (end <= begin) return CUSTOM_WHY("empty program");
     if (end - begin > B200MD_CUSTOM_MAX_CODE) return CUSTOM_WHY("more than 256 instructions");
     const int numVars = compound ? 3*nparticles : custom_num_vars(cls);
@@ -229,10 +252,13 @@ inline const char* custom_check_program(int cls, const int2* code, int begin, in
         const int op = code[pc].x, arg = code[pc].y;
         const int nargs = custom_op_args(op);
         const bool point = op == B200MD_OP_POINT_DIST || op == B200MD_OP_POINT_ANGLE || op == B200MD_OP_POINT_DIHEDRAL;
-        if (nargs < 0 || ((torsion || angle) && (op == B200MD_OP_VAR || op == B200MD_OP_PERIODIC_DIST)) || (point && !compound))
+        const bool table = op == B200MD_OP_DISCRETE1 || op == B200MD_OP_DISCRETE2 || op == B200MD_OP_DISCRETE3;
+        if (nargs < 0 || ((torsion || angle) && (op == B200MD_OP_VAR || op == B200MD_OP_PERIODIC_DIST)) || (point && !compound) ||
+            (table && !nonbonded))
             return CUSTOM_WHY("unknown opcode");
         if (!torsion && !angle && op == B200MD_OP_THETA) return CUSTOM_WHY("THETA outside a torsion program");
-        if ((bond || compound) && op == B200MD_OP_PERIODIC_DIST) return CUSTOM_WHY("PERIODIC_DIST outside an external program");
+        if ((bond || compound || nonbonded) && op == B200MD_OP_PERIODIC_DIST) return CUSTOM_WHY("PERIODIC_DIST outside an external program");
+        if (table && (arg < -1 || (ntables >= 0 && arg >= ntables))) return CUSTOM_WHY("table index out of range");
         if (op == B200MD_OP_VAR && (arg < 0 || arg >= numVars)) return CUSTOM_WHY("variable index out of range for the class");
         if (op == B200MD_OP_PERIODIC_DIST && (arg < -1 || arg > 5)) return CUSTOM_WHY("periodic distance operand outside -1..5");
         if (point && (arg < -1 || arg >= nargs)) return CUSTOM_WHY("point function operand out of range");

@@ -274,6 +274,22 @@ struct b200md_ctx {
         cudaEvent_t evFork = nullptr, evJoin = nullptr;
     } gbsa;
     GbsaDev gbd{};
+    // CustomNonbondedForce objects (b200md_set_custom_nonbonded): the shared method, cutoff and excluded pairs, every object's
+    // programs, parameters, switching distance, group and long-range coefficient as given, the tables, their device form and the
+    // stream the pair kernel runs on beside the tile kernel (created at finalize when there are objects)
+    struct {
+        bool have = false;
+        int method = 0, nobj = 0, stride = 0;
+        double cutoff = 0;
+        std::vector<int> progStart, op, arg, nparams, group; std::vector<double> imm, params, switchDist, lrc;
+        std::vector<int2> excl;
+        std::vector<int4> tableDims; std::vector<int> tableStart; std::vector<double> tableValues;
+        DevBuf<int> progStartDev, nparamsDev, groupDev, tableStartDev; DevBuf<int2> codeDev; DevBuf<int4> tableDimsDev;
+        DevBuf<double> immDev, paramsDev, switchDev, tableValuesDev;
+        cudaStream_t stream = nullptr;
+        cudaEvent_t evFork = nullptr, evJoin = nullptr;
+    } cnb;
+    CnbDev cnd{};
     // RMSDForce objects (b200md_set_rmsd): their particle lists one after the other, the reference position of every entry
     // centred over its object, and the device form
     struct {
@@ -333,6 +349,7 @@ static void check_flags(b200md_ctx* c);
 static void sync_velocities(b200md_ctx* c);
 static void sync_positions(b200md_ctx* c);
 static void setup_gbsa(b200md_ctx* c);
+static void setup_custom_nonbonded(b200md_ctx* c);
 static void setup_rmsd(b200md_ctx* c);
 static void setup_cv(b200md_ctx* c);
 static void host_set_state(b200md_ctx* c);
@@ -398,6 +415,9 @@ extern "C" void b200md_destroy(b200md_ctx* ctx) {
     if (ctx->gbsa.stream) cudaStreamDestroy(ctx->gbsa.stream);
     if (ctx->gbsa.evFork) cudaEventDestroy(ctx->gbsa.evFork);
     if (ctx->gbsa.evJoin) cudaEventDestroy(ctx->gbsa.evJoin);
+    if (ctx->cnb.stream) cudaStreamDestroy(ctx->cnb.stream);
+    if (ctx->cnb.evFork) cudaEventDestroy(ctx->cnb.evFork);
+    if (ctx->cnb.evJoin) cudaEventDestroy(ctx->cnb.evJoin);
     char* window = ctx->window;
     delete ctx;
     if (window) cudaFree(window);
@@ -1611,7 +1631,12 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     require(!ctx->finalized, "finalize called twice");
     b200md_ctx* c = ctx;
     const int N = c->natoms, NP = c->npad;
-    if (!c->haveNb) { c->nbdesc = b200md_nonbonded_desc{}; c->nbdesc.method = B200MD_NB_NOCUTOFF; }
+    if (!c->haveNb) {
+        // no NonbondedForce: the list is built for the custom nonbonded force alone, at its method and cutoff
+        c->nbdesc = b200md_nonbonded_desc{};
+        c->nbdesc.method = c->cnb.have ? c->cnb.method : B200MD_NB_NOCUTOFF;
+        if (c->cnb.have) c->nbdesc.cutoff = c->cnb.cutoff;
+    }
     NbDev& nb = c->nb;
     nb.natoms = N; nb.npad = NP; nb.nblocks = c->nblocks;
     nb.method = c->nbdesc.method;
@@ -1689,6 +1714,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     {
         std::vector<std::vector<int> > ex(N);
         for (const int2& a : c->exc.atoms) { ex[a.x].push_back(a.y); ex[a.y].push_back(a.x); }
+        if (!c->haveNb) for (const int2& a : c->cnb.excl) { ex[a.x].push_back(a.y); ex[a.y].push_back(a.x); }
         std::vector<int> start(N+1, 0), list;
         for (int i = 0; i < N; i++) {
             std::sort(ex[i].begin(), ex[i].end());
@@ -1717,6 +1743,7 @@ extern "C" int b200md_finalize(b200md_ctx* ctx) {
     build_units(c);
     build_ccma(c);
     setup_gbsa(c);
+    setup_custom_nonbonded(c);
     setup_rmsd(c);
     setup_cv(c);
     if (c->mg == MG_P2P) {
@@ -1883,6 +1910,193 @@ extern "C" int b200md_update_custom_centroid_params(b200md_ctx* ctx, int n, cons
     API_END(ctx)
 }
 
+// ---------------------------------------------------------------- CustomNonbondedForce
+// The programs of nobj objects, 2 each (energy, dE/dr), every one passing custom_check_program for its object's nparams[o] <=
+// B200MD_CUSTOM_MAX_PARAMS/2 parameters per particle (nglobals, ntables < 0: checked at finalize).  Returns the instructions.
+static std::vector<int2> check_nonbonded_programs(const std::string& call, int nobj, const int* prog_start, const int* op, const int* arg,
+                                                  const int* nparams, int nglobals, int ntables) {
+    require(nobj >= 1, (call + ": at least one object").c_str());
+    require(prog_start[0] == 0, (call + ": prog_start[0] must be 0").c_str());
+    for (int q = 0; q < 2*nobj; q++) require(prog_start[q+1] >= prog_start[q], (call + ": prog_start must not decrease").c_str());
+    std::vector<int2> code(prog_start[2*nobj]);
+    for (size_t k = 0; k < code.size(); k++) code[k] = make_int2(op[k], arg[k]);
+    for (int o = 0; o < nobj; o++) {
+        require(nparams[o] >= 0 && nparams[o] <= B200MD_CUSTOM_MAX_PARAMS/2, (call + ": more than 8 per-particle parameters").c_str());
+        for (int q = 2*o; q < 2*o + 2; q++) {
+            const char* why = custom_check_program(B200MD_CUSTOM_NONBONDED, code.data(), prog_start[q], prog_start[q+1], 2*nparams[o], nglobals, 0, ntables);
+            if (why) throw std::runtime_error(std::string(why) + " (program " + std::to_string(q) + ")");
+        }
+    }
+    return code;
+}
+// ntables tables: 1 to 3 dimensions of at least one entry each (unused ones 1), start[t+1] - start[t] entries each
+static void check_tables(const std::string& call, int ntables, const int* dims, const int* start) {
+    require(ntables >= 0, (call + ": negative number of tables").c_str());
+    require(ntables == 0 || start[0] == 0, (call + ": start[0] must be 0").c_str());
+    for (int t = 0; t < ntables; t++) {
+        const int nd = dims[4*t];
+        require(nd >= 1 && nd <= 3, (call + ": a table has 1, 2 or 3 dimensions").c_str());
+        long long size = 1;
+        for (int k = 0; k < 3; k++) {
+            require(dims[4*t + 1 + k] >= 1 && (k < nd || dims[4*t + 1 + k] == 1), (call + ": a table size must be at least 1 (1 for an unused dimension)").c_str());
+            size *= dims[4*t + 1 + k];
+        }
+        require(start[t+1] - start[t] == size, (call + ": a table's number of values does not match its sizes").c_str());
+    }
+}
+static void check_cnb_params(const b200md_ctx* c, const char* call, int nobj, int stride, const double* params) {
+    for (size_t k = 0; k < (size_t) nobj*c->natoms*stride; k++)
+        require(std::isfinite(params[k]), (std::string(call) + ": a per-particle parameter is not finite").c_str());
+}
+extern "C" int b200md_set_custom_nonbonded(b200md_ctx* ctx, int method, double cutoff, int nobj, const int* prog_start, const int* op, const int* arg,
+                                           const double* imm, const int* nparams, int stride, const double* params,
+                                           const double* switch_distance, const int* group, int nexcl, const int* excl_p1, const int* excl_p2) {
+    API_BEGIN(ctx)
+    check_set(ctx, "set_custom_nonbonded", nobj);
+    check_set(ctx, "set_custom_nonbonded", nexcl);
+    require(ctx->world == 1, "CustomNonbondedForce is not supported in multi-GPU runs");
+    require(method == B200MD_NB_NOCUTOFF || method == B200MD_NB_CUTOFF_NONPERIODIC || method == B200MD_NB_CUTOFF_PERIODIC,
+            "set_custom_nonbonded: method must be NoCutoff, CutoffNonPeriodic or CutoffPeriodic");
+    require(method == B200MD_NB_NOCUTOFF || (std::isfinite(cutoff) && cutoff > 0.0), "set_custom_nonbonded: the cutoff must be positive");
+    require(stride >= 0 && stride <= B200MD_CUSTOM_MAX_PARAMS/2, "set_custom_nonbonded: more than 8 per-particle parameters");
+    const std::vector<int2> code = check_nonbonded_programs("set_custom_nonbonded", nobj, prog_start, op, arg, nparams, -1, -1);
+    for (int o = 0; o < nobj; o++) {
+        require(nparams[o] <= stride, "set_custom_nonbonded: an object has more parameters than param_stride");
+        const double sw = switch_distance[o];
+        require(sw < 0.0 || (method != B200MD_NB_NOCUTOFF && sw < cutoff), "set_custom_nonbonded: the switching distance must be below the cutoff");
+        require(group[o] >= 0 && group[o] < 32, "set_custom_nonbonded: force group out of range");
+    }
+    for (int k = 0; k < nexcl; k++)
+        require(excl_p1[k] >= 0 && excl_p1[k] < ctx->natoms && excl_p2[k] >= 0 && excl_p2[k] < ctx->natoms && excl_p1[k] != excl_p2[k],
+                "set_custom_nonbonded: an excluded pair must be two different particles");
+    check_cnb_params(ctx, "set_custom_nonbonded", nobj, stride, params);
+    auto& g = ctx->cnb;
+    g.have = true; g.method = method; g.cutoff = method == B200MD_NB_NOCUTOFF ? 0.0 : cutoff; g.nobj = nobj; g.stride = stride;
+    const int total = prog_start[2*nobj];
+    g.progStart.assign(prog_start, prog_start + 2*nobj + 1);
+    g.op.assign(op, op + total); g.arg.assign(arg, arg + total); g.imm.assign(imm, imm + total);
+    g.nparams.assign(nparams, nparams + nobj); g.group.assign(group, group + nobj);
+    g.switchDist.assign(switch_distance, switch_distance + nobj);
+    g.params.assign(params, params + (size_t) nobj*ctx->natoms*stride);
+    g.lrc.assign(nobj, 0.0);
+    g.excl.resize(nexcl);
+    for (int k = 0; k < nexcl; k++) g.excl[k] = make_int2(excl_p1[k], excl_p2[k]);
+    API_END(ctx)
+}
+extern "C" int b200md_set_custom_tables(b200md_ctx* ctx, int ntables, const int* dims, const int* start, const double* values) {
+    API_BEGIN(ctx)
+    check_set(ctx, "set_custom_tables", ntables);
+    check_tables("set_custom_tables", ntables, dims, start);
+    auto& g = ctx->cnb;
+    g.tableDims.resize(ntables);
+    for (int t = 0; t < ntables; t++) g.tableDims[t] = make_int4(dims[4*t], dims[4*t + 1], dims[4*t + 2], dims[4*t + 3]);
+    g.tableStart.assign(start, start + ntables + 1);
+    g.tableValues.assign(values, values + (ntables ? start[ntables] : 0));
+    API_END(ctx)
+}
+// the parameters of every object, [nobj][npad][stride] (padding atoms 0), into buffers of a fixed size: a captured step graph
+// keeps its pointers
+static void upload_cnb_params(b200md_ctx* c) {
+    auto& g = c->cnb;
+    const int st = std::max(g.stride, 1);
+    std::vector<double> p((size_t) g.nobj*c->npad*st, 0.0);
+    for (int o = 0; o < g.nobj; o++)
+        for (int i = 0; i < c->natoms; i++)
+            for (int k = 0; k < g.stride; k++) p[((size_t) o*c->npad + i)*st + k] = g.params[((size_t) o*c->natoms + i)*g.stride + k];
+    g.paramsDev.upload(p);
+}
+extern "C" int b200md_update_custom_nonbonded_params(b200md_ctx* ctx, int n, const double* params) {
+    API_BEGIN(ctx)
+    require(ctx->finalized, "update_custom_nonbonded_params before finalize");
+    require(ctx->cnb.have, "update_custom_nonbonded_params: the context has no custom nonbonded force");
+    require(n == ctx->natoms, "update_custom_nonbonded_params: the number of particles has changed");
+    auto& g = ctx->cnb;
+    check_cnb_params(ctx, "update_custom_nonbonded_params", g.nobj, g.stride, params);
+    g.params.assign(params, params + (size_t) g.nobj*n*g.stride);
+    CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+    upload_cnb_params(ctx);
+    API_END(ctx)
+}
+extern "C" int b200md_set_custom_nonbonded_lrc(b200md_ctx* ctx, int nobj, const double* coefficient) {
+    API_BEGIN(ctx)
+    require(ctx->cnb.have && nobj == ctx->cnb.nobj, "set_custom_nonbonded_lrc: one coefficient per custom nonbonded object");
+    for (int o = 0; o < nobj; o++) require(std::isfinite(coefficient[o]), "set_custom_nonbonded_lrc: a coefficient is not finite");
+    ctx->cnb.lrc.assign(coefficient, coefficient + nobj);
+    API_END(ctx)
+}
+// finalize: the method, cutoff and exclusions must be the list's (those of the nonbonded force, when there is one), the
+// programs' global and table operands in range; the device state and the stream
+static void setup_custom_nonbonded(b200md_ctx* c) {
+    auto& g = c->cnb;
+    c->cnd = CnbDev{};
+    if (!g.have) return;
+    require(c->world == 1, "CustomNonbondedForce is not supported in multi-GPU runs");
+    if (c->haveNb) {
+        const int nm = c->nbdesc.method;
+        require(g.method == B200MD_NB_CUTOFF_PERIODIC ? (nm == B200MD_NB_CUTOFF_PERIODIC || nm == B200MD_NB_PME) : nm == g.method,
+                "custom nonbonded force: its method does not match the nonbonded force's (CutoffPeriodic goes with CutoffPeriodic or PME)");
+        if (g.method != B200MD_NB_NOCUTOFF)
+            require(std::fabs(g.cutoff - c->nbdesc.cutoff) <= 1e-12*c->nbdesc.cutoff, "custom nonbonded force: the cutoff must be that of the nonbonded force");
+        auto pairs = [](const std::vector<int2>& v) {
+            std::vector<std::pair<int, int> > p;
+            for (const int2& a : v) p.push_back(std::make_pair(std::min(a.x, a.y), std::max(a.x, a.y)));
+            std::sort(p.begin(), p.end());
+            p.erase(std::unique(p.begin(), p.end()), p.end());
+            return p;
+        };
+        require(pairs(g.excl) == pairs(c->exc.atoms), "custom nonbonded force: its exclusions must be the nonbonded force's exceptions");
+    }
+    const int ntables = (int) g.tableDims.size();
+    check_nonbonded_programs("custom nonbonded force", g.nobj, g.progStart.data(), g.op.data(), g.arg.data(), g.nparams.data(),
+                             (int) c->custom.globals.size(), ntables);
+    std::vector<int2> code(g.op.size());
+    for (size_t k = 0; k < code.size(); k++) code[k] = make_int2(g.op[k], g.arg[k]);
+    g.codeDev.upload(code); g.immDev.upload(g.imm); g.progStartDev.upload(g.progStart);
+    g.nparamsDev.upload(g.nparams); g.groupDev.upload(g.group); g.switchDev.upload(g.switchDist);
+    upload_cnb_params(c);
+    g.tableDimsDev.alloc(std::max(ntables, 1)); g.tableDimsDev.upload(g.tableDims);
+    g.tableStartDev.alloc(ntables + 1); g.tableStartDev.upload(ntables ? g.tableStart : std::vector<int>(1, 0));
+    g.tableValuesDev.alloc(std::max<size_t>(g.tableValues.size(), 1)); g.tableValuesDev.upload(g.tableValues);
+    CnbDev& d = c->cnd;
+    d.nobj = g.nobj; d.stride = std::max(g.stride, 1);
+    d.useCutoff = g.method != B200MD_NB_NOCUTOFF;
+    d.cutoff = g.cutoff; d.cutoff2 = g.cutoff*g.cutoff;
+    d.nparams = g.nparamsDev.p; d.switchDist = g.switchDev.p; d.group = g.groupDev.p; d.params = g.paramsDev.p;
+    d.code = g.codeDev.p; d.imm = g.immDev.p; d.progStart = g.progStartDev.p;
+    d.globals = c->custom.globalsDev.p;
+    d.ntables = ntables; d.tableDims = g.tableDimsDev.p; d.tableStart = g.tableStartDev.p; d.tableValues = g.tableValuesDev.p;
+    d.groupMask = 0xffffffffu;
+    if (!g.stream) {
+        int hi = 0;
+        CUDA_CHECK(cudaDeviceGetStreamPriorityRange(nullptr, &hi));
+        CUDA_CHECK(cudaStreamCreateWithPriority(&g.stream, cudaStreamNonBlocking, hi));
+        CUDA_CHECK(cudaEventCreateWithFlags(&g.evFork, cudaEventDisableTiming));
+        CUDA_CHECK(cudaEventCreateWithFlags(&g.evJoin, cudaEventDisableTiming));
+    }
+}
+extern "C" int b200md_custom_nonbonded_probe(int nprog, const int* prog_start, const int* op, const int* arg, const double* imm, int nparams,
+                                             int nglobals, int which, double r, const double* params, const double* globals, int ntables,
+                                             const int* dims, const int* start, const double* values, double* out, char* msg, int msglen) {
+    try {
+        require(nprog >= 2 && nprog % 2 == 0, "custom_nonbonded_probe: two programs per object");
+        require(nglobals >= 0, "custom_nonbonded_probe: negative number of globals");
+        check_tables("custom_nonbonded_probe", ntables, dims, start);
+        const std::vector<int> np(nprog/2, nparams);
+        const std::vector<int2> code = check_nonbonded_programs("custom_nonbonded_probe", nprog/2, prog_start, op, arg, np.data(), nglobals, ntables);
+        require(which >= 0 && which < nprog, "custom_nonbonded_probe: program index out of range");
+        std::vector<int4> d(ntables);
+        for (int t = 0; t < ntables; t++) d[t] = make_int4(dims[4*t], dims[4*t + 1], dims[4*t + 2], dims[4*t + 3]);
+        const CustomTables tables = {ntables, d.data(), start, values};
+        const CustomBox b = {1.0, 0.0, 1.0, 0.0, 0.0, 1.0};
+        *out = custom_run<B200MD_CUSTOM_MAX_STACK, false, true>(code.data(), imm, prog_start[which], prog_start[which+1], &r, params, globals, b,
+                                                                 false, &tables);
+        return 0;
+    } catch (std::exception& e) {
+        if (msg && msglen > 0) { strncpy(msg, e.what(), msglen - 1); msg[msglen - 1] = 0; }
+        return -1;
+    }
+}
+
 // ---------------------------------------------------------------- generalized Born (GBSAOBCForce)
 // charge, radius and scale of every atom: finite, radius above the dielectric offset (ObcParameters' rho = R - 0.009 must be
 // positive), scale not negative
@@ -1939,6 +2153,9 @@ static void setup_gbsa(b200md_ctx* c) {
     if (!g.have) return;
     require(c->world == 1, "generalized Born (GBSAOBCForce) is not supported in multi-GPU runs");
     const int nm = c->haveNb ? c->nbdesc.method : -1;
+    // without a nonbonded force the list is the custom nonbonded force's: the chain needs it to hold every pair
+    if (!c->haveNb && c->cnb.have)
+        require(c->cnb.method == B200MD_NB_NOCUTOFF, "generalized Born at NoCutoff beside a custom nonbonded force with a cutoff needs a nonbonded force");
     if (!c->haveNb) require(g.method == B200MD_NB_NOCUTOFF, "generalized Born with a cutoff needs a nonbonded force with the same cutoff");
     else if (g.method == B200MD_NB_NOCUTOFF) require(nm == B200MD_NB_NOCUTOFF, "generalized Born: NoCutoff needs a NoCutoff nonbonded force");
     else if (g.method == B200MD_NB_CUTOFF_NONPERIODIC) require(nm == B200MD_NB_CUTOFF_NONPERIODIC, "generalized Born: CutoffNonPeriodic needs a CutoffNonPeriodic nonbonded force");
@@ -2370,6 +2587,10 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     // adds into the user-order fixed-point buffer like everything else, so the overlap cannot change the result.
     const bool gb = (terms & B200MD_TERM_GBSA) && c->gbsa.have && !pmeRank;
     const bool forkGb = gb && c->overlapPme;
+    // CustomNonbondedForce: one pair kernel over this evaluation's list, forked and joined as the generalized Born chain is
+    const bool cnb = (terms & B200MD_TERM_CUSTOM_NONBONDED) && c->cnb.have && !pmeRank;
+    const bool forkCnb = cnb && c->overlapPme;
+    CnbDev cnd = c->cnd; cnd.groupMask = groupMask;
 
     int launches = 0;
     auto launch_recip = [&]() {
@@ -2413,7 +2634,7 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
         CUDA_CHECK(cudaStreamWaitEvent(sp, c->evForkGrid, 0));
         CUDA_CHECK(cudaMemsetAsync(pme.gridFixed, 0, sizeof(long long)*(size_t) pme.nx*pme.ny*pme.nz, sp));
     }
-    if (direct || gb) {
+    if (direct || gb || cnb) {
         launch_check_displacement(c->nb, c->cd, s); launches++;
         launch_list_build(c->nb, s); launches += LIST_BUILD_LAUNCHES;
     }
@@ -2424,6 +2645,13 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
         CUDA_CHECK(cudaEventRecord(c->gbsa.evJoin, c->gbsa.stream));
     }
     if (gb) launches += GBSA_LAUNCHES;
+    if (forkCnb) {
+        CUDA_CHECK(cudaEventRecord(c->cnb.evFork, s));
+        CUDA_CHECK(cudaStreamWaitEvent(c->cnb.stream, c->cnb.evFork, 0));
+        launch_custom_nonbonded(c->nb, cnd, energy, c->cnb.stream);
+        CUDA_CHECK(cudaEventRecord(c->cnb.evJoin, c->cnb.stream));
+    }
+    if (cnb) launches++;
     if (forkAfterList) launch_recip();
     if (forkBonded) {
         CUDA_CHECK(cudaStreamWaitEvent(c->streamBonded, c->evFork, 0));
@@ -2433,10 +2661,12 @@ static int enqueue_forces(b200md_ctx* c, int terms, bool energy, bool forcesAlre
     if (direct) { launch_pair(c->nb, energy, s); launches += PAIR_LAUNCHES; }
     if (bonded && !forkBonded) launch_bonded_terms(s);
     if (gb && !forkGb) launch_gbsa(c->nb, c->gbd, energy, s);
+    if (cnb && !forkCnb) launch_custom_nonbonded(c->nb, cnd, energy, s);
     if (pushEarly) { launch_force_push(c->nb, c->cd, s); launches++; }
     if (fork) CUDA_CHECK(cudaStreamWaitEvent(s, c->evJoin, 0));
     if (forkBonded) CUDA_CHECK(cudaStreamWaitEvent(s, c->evJoinBonded, 0));
     if (forkGb) CUDA_CHECK(cudaStreamWaitEvent(s, c->gbsa.evJoin, 0));
+    if (forkCnb) CUDA_CHECK(cudaStreamWaitEvent(s, c->cnb.evJoin, 0));
     if (p2p) {
         if (!pushEarly) { launch_force_push(c->nb, c->cd, s); launches++; }
         // in the step path k_integrate totals own partial + inboxes; here (energies, getState) the owners total and broadcast
@@ -2483,7 +2713,7 @@ static void check_flags(b200md_ctx* c) {
 // After the state was changed from outside (positions, box, parameters, checkpoint): build the list now, synchronously,
 // and size the tile pools from what the build actually used.  The step graphs trust the current list and never grow it.
 static void prepare_list(b200md_ctx* c) {
-    if (!c->listDirty || !(c->haveNb || c->gbsa.have)) { c->listDirty = false; return; }
+    if (!c->listDirty || !(c->haveNb || c->gbsa.have || c->cnb.have)) { c->listDirty = false; return; }
     if (c->pmeOnly || nccl_pme_rank(c)) { c->listDirty = false; return; }    // keeps no list
     for (int attempt = 0; attempt < 8; attempt++) {
         launch_check_displacement(c->nb, c->cd, c->stream);
@@ -2536,6 +2766,11 @@ extern "C" int b200md_compute_groups(b200md_ctx* ctx, int terms, unsigned int bo
                      B200MD_TERM_CUSTOM_COMPOUND | B200MD_TERM_CUSTOM_CENTROID)) e += h[EN_CUSTOM];
         if ((terms & B200MD_TERM_GBSA) && ctx->gbsa.have) e += h[EN_GB];
         if (terms & B200MD_TERM_RMSD) e += h[EN_RMSD];
+        if ((terms & B200MD_TERM_CUSTOM_NONBONDED) && ctx->cnb.have) {
+            e += h[EN_CNB];
+            for (int o = 0; o < ctx->cnb.nobj; o++)        // ReferenceCalcCustomNonbondedForceKernel::execute
+                if ((bonded_group_mask >> ctx->cnb.group[o]) & 1u) e += ctx->cnb.lrc[o]/ctx->nb.box.volume;
+        }
         if (ctx->haveNb) {
             if (terms & B200MD_TERM_NB_DIRECT) {
                 e += h[EN_NB] + h[EN_EXC];
@@ -2842,6 +3077,7 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
     require(phase != 9 || c->ccd.nslots > 0, "time_phase(custom centroid bonds): the System has none");
     require(phase != 10 || c->gbsa.have, "time_phase(generalized Born): the System has none");
     require(phase != 13 || c->rmd.nobj > 0, "time_phase(RMSD): the System has none");
+    require(phase != 14 || c->cnb.have, "time_phase(custom nonbonded): the System has none");
     if (phase == 4) {
         require(c->haveIntegrator, "time_phase(integrate) before set_integrator");
         state.parts = state_spans(c, ST_POS | ST_VEL); state.save(s);
@@ -2868,6 +3104,7 @@ extern "C" int b200md_time_phase(b200md_ctx* ctx, int phase, int reps, double* m
             case 11: launch_list_prep(c->nb, s); break;
             case 12: launch_build_tiles(c->nb, s); break;
             case 13: launch_rmsd(c->nb, c->rmd, false, s); break;
+            case 14: launch_custom_nonbonded(c->nb, c->cnd, false, s); break;
             default: throw std::runtime_error("unknown phase");
         }
         CUDA_CHECK(cudaEventRecord(e1, s));

@@ -160,7 +160,7 @@ struct NbDev {
 };
 
 enum { EN_NB = 0, EN_RECIP = 1, EN_BOND = 2, EN_ANGLE = 3, EN_TORSION = 4, EN_EXC = 5, EN_KE = 6, EN_RBTORSION = 7, EN_CMAP = 8,
-       EN_CUSTOM = 9, EN_GB = 10, EN_RMSD = 11, B200MD_NUM_ENERGY = 12 };
+       EN_CUSTOM = 9, EN_GB = 10, EN_RMSD = 11, EN_CNB = 12, B200MD_NUM_ENERGY = 13 };
 
 struct PmeDev {
     int nx, ny, nz, nzc;
@@ -256,6 +256,21 @@ struct GbsaDev {
     const double* atomRadius;    // R
     long long* bornSum; long long* dEdB;
     double* bornR; double* chain; double* bornForce;
+};
+
+// CustomNonbondedForce objects (custom_nonbonded.cu), sharing one method, cutoff and exclusion set.  Object o runs the programs
+// 2o (energy) and 2o+1 (dE/dr), the instructions [progStart[q], progStart[q+1]) of code and imm, with nparams[o] parameters per
+// particle, params[(o npad + atom) stride + k]; switchDist[o] < 0: no switching function; group[o] its force group.  The
+// Discrete1D/2D/3DFunction tables: table t has tableDims[t] = (dimensions, xsize, ysize, zsize), values from tableStart[t].
+struct CnbDev {
+    int nobj, stride, useCutoff;
+    double cutoff, cutoff2;
+    const int* nparams; const double* switchDist; const int* group;
+    const double* params;
+    const int2* code; const double* imm; const int* progStart;
+    const double* globals;
+    int ntables; const int4* tableDims; const int* tableStart; const double* tableValues;
+    unsigned int groupMask;
 };
 
 // RMSDForce objects (rmsd.cu).  Object o is the entries [objStart[o], objStart[o+1]) of atoms (user atoms) and ref (the
@@ -451,6 +466,53 @@ struct TileCursor {
 };
 static_assert(TILE_REGIONS == 32, "TileCursor maps one pool to one lane");
 
+#ifdef __CUDACC__
+// displacement b - a in double, minimum image as ReferenceForce::getDeltaRPeriodic (triclinic order c, b, a).  Read by the pair
+// sweeps over the list (gbsa.cu, custom_nonbonded.cu).
+__device__ __forceinline__ double3 tile_delta(const BoxDev& bx, float4 a, float4 b) {
+    double dx = (double) b.x - (double) a.x, dy = (double) b.y - (double) a.y, dz = (double) b.z - (double) a.z;
+    if (bx.periodic) {
+        if (bx.triclinic) {
+            double k = floor(dz*bx.recip[8] + 0.5);
+            dx -= k*(double) bx.cx; dy -= k*(double) bx.cy; dz -= k*bx.dcz;
+            k = floor(dy*bx.recip[4] + 0.5);
+            dx -= k*(double) bx.bx; dy -= k*bx.dby;
+            k = floor(dx*bx.recip[0] + 0.5);
+            dx -= k*bx.dax;
+        }
+        else {
+            dx -= bx.dax*rint(dx*bx.recip[0]); dy -= bx.dby*rint(dy*bx.recip[4]); dz -= bx.dcz*rint(dz*bx.recip[8]);
+        }
+    }
+    return make_double3(dx, dy, dz);
+}
+
+// v in 2^32 fixed point into *p (integer atomics: the sum does not depend on the order of the additions)
+__device__ __forceinline__ void add_fixed(long long* p, double v) {
+    if (v != 0.0) atomicAdd((unsigned long long*) p, (unsigned long long) __double2ll_rn(v*B200MD_FORCE_SCALE));
+}
+__device__ __forceinline__ double shfl_d(double v, int src) { return __shfl_sync(0xffffffffu, v, src); }
+
+// Every tile of the current list, one warp per tile: body(L, t, si, ai, sj, aj) with the tile's slot t, this lane's i slot and
+// user atom (-1 for padding) and the j slot and user atom it holds at the start (the body rotates the j side through the lanes
+// itself).  The pair sweeps of gbsa.cu and custom_nonbonded.cu walk the list with it.
+template <class Body>
+__device__ __forceinline__ void walk_tiles(const NbDev& nb, Body body) {
+    const ListDev& L = nb.list[nb.counters[CT_CUR] & 1];
+    const int lane = threadIdx.x & 31;
+    const int gwarp = (blockIdx.x*blockDim.x + threadIdx.x) >> 5;
+    const int nwarps = (gridDim.x*blockDim.x) >> 5;
+    TileCursor cursor;
+    cursor.init(nb, L, lane);
+    for (int f = gwarp; f < cursor.total; f += nwarps) {
+        const int t = cursor.slot(f);
+        const int si = L.tileI[t]*32 + lane;
+        const int sj = L.tileJ[t*32 + lane];
+        body(L, t, si, si < nb.natoms ? L.sorig[si] : -1, sj, sj >= 0 ? L.sorig[sj] : -1);
+    }
+}
+#endif
+
 // ---- integration state in the working type R: float (single precision) or double (mixed precision) ----
 // The only place that knows the mixed layout: a position is posq.xyz (hi) + posqCorr.xyz (lo), stored as hi = (float) x,
 // lo = (float) (x - hi), about 48 significant bits; velocities and 1/mass live in velmD.  The fp32 posq the force kernels
@@ -612,6 +674,9 @@ void launch_centroid(const NbDev& nb, const CompoundDev& cc, const CentroidDev& 
 // the generalized Born chain on the current neighbour list: Born sums, radii + ACE + self terms, GB pairs, fold, chain-rule pairs
 const int GBSA_LAUNCHES = 5;
 void launch_gbsa(const NbDev& nb, const GbsaDev& gb, bool energy, cudaStream_t s);
+
+// CustomNonbondedForce: every object's pairs over the current neighbour list, one kernel
+void launch_custom_nonbonded(const NbDev& nb, const CnbDev& cn, bool energy, cudaStream_t s);
 
 // RMSDForce: centre and sums, eigen solve, forces (launched behind the bonded terms, on their stream)
 const int RMSD_LAUNCHES = 3;

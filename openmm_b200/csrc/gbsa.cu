@@ -37,25 +37,6 @@
 #define GB_BETA 0.8
 #define GB_GAMMA 4.85
 
-// displacement b - a in double, minimum image as ReferenceForce::getDeltaRPeriodic (triclinic order c, b, a)
-__device__ __forceinline__ double3 gb_delta(const BoxDev& bx, float4 a, float4 b) {
-    double dx = (double) b.x - (double) a.x, dy = (double) b.y - (double) a.y, dz = (double) b.z - (double) a.z;
-    if (bx.periodic) {
-        if (bx.triclinic) {
-            double k = floor(dz*bx.recip[8] + 0.5);
-            dx -= k*(double) bx.cx; dy -= k*(double) bx.cy; dz -= k*bx.dcz;
-            k = floor(dy*bx.recip[4] + 0.5);
-            dx -= k*(double) bx.bx; dy -= k*bx.dby;
-            k = floor(dx*bx.recip[0] + 0.5);
-            dx -= k*bx.dax;
-        }
-        else {
-            dx -= bx.dax*rint(dx*bx.recip[0]); dy -= bx.dby*rint(dy*bx.recip[4]); dz -= bx.dcz*rint(dz*bx.recip[8]);
-        }
-    }
-    return make_double3(dx, dy, dz);
-}
-
 // I(r, rho_i, s_j rho_j) of the header, 0 when the scaled sphere of j does not reach the offset sphere of i
 __device__ __forceinline__ double obc_integral(double r, double rInv, double rho, double sr) {
     if (rho >= r + sr) return 0.0;
@@ -73,33 +54,10 @@ __device__ __forceinline__ double obc_integral_deriv(double r, double r2Inv, dou
     return 0.125*(1.0 + sr*sr*r2Inv)*(l*l - u*u) + 0.25*log(u/l)*r2Inv;
 }
 
-__device__ __forceinline__ void add_fixed(long long* p, double v) {
-    if (v != 0.0) atomicAdd((unsigned long long*) p, (unsigned long long) __double2ll_rn(v*B200MD_FORCE_SCALE));
-}
-__device__ __forceinline__ double shfl_d(double v, int src) { return __shfl_sync(FULL, v, src); }
-
-// Every tile of the current list, one warp per tile: body(L, t, si, ai, sj, aj) with this lane's i slot and user atom (-1 for
-// padding) and the j slot and user atom it holds at the start (the body rotates the j side through the lanes itself).
-template <class Body>
-__device__ __forceinline__ void gb_tiles(const NbDev& nb, Body body) {
-    const ListDev& L = nb.list[nb.counters[CT_CUR] & 1];
-    const int lane = threadIdx.x & 31;
-    const int gwarp = (blockIdx.x*blockDim.x + threadIdx.x) >> 5;
-    const int nwarps = (gridDim.x*blockDim.x) >> 5;
-    TileCursor cursor;
-    cursor.init(nb, L, lane);
-    for (int f = gwarp; f < cursor.total; f += nwarps) {
-        const int t = cursor.slot(f);
-        const int si = L.tileI[t]*32 + lane;
-        const int sj = L.tileJ[t*32 + lane];
-        body(L, si, si < nb.natoms ? L.sorig[si] : -1, sj, sj >= 0 ? L.sorig[sj] : -1);
-    }
-}
-
 // pass 1: the Born sums
 __global__ void __launch_bounds__(256) k_gb_born(NbDev nb, GbsaDev gb) {
     const int src = ((threadIdx.x & 31) + 1) & 31;
-    gb_tiles(nb, [&](const ListDev& L, int si, int ai, int sj, int aj) {
+    walk_tiles(nb, [&](const ListDev& L, int, int si, int ai, int sj, int aj) {
         const float4 pi = L.sposq[si];
         const double2 ri = ai >= 0 ? gb.radius[ai] : make_double2(1.0, 0.0);
         float4 pj = L.sposq[max(sj, 0)];
@@ -107,7 +65,7 @@ __global__ void __launch_bounds__(256) k_gb_born(NbDev nb, GbsaDev gb) {
         double sumI = 0.0, sumJ = 0.0;
         for (int k = 0; k < 32; k++) {
             if (ai >= 0 && sj > si) {
-                const double3 d = gb_delta(nb.box, pi, pj);
+                const double3 d = tile_delta(nb.box, pi, pj);
                 const double r2 = d.x*d.x + d.y*d.y + d.z*d.z;
                 if (!gb.useCutoff || r2 <= gb.cutoff2) {
                     const double r = sqrt(r2), rInv = 1.0/r;
@@ -167,7 +125,7 @@ __global__ void __launch_bounds__(256) k_gb_pairs(NbDev nb, GbsaDev gb) {
     const int src = ((threadIdx.x & 31) + 1) & 31;
     double e = 0.0;
     const double shift = gb.useCutoff ? 1.0/gb.cutoff : 0.0;
-    gb_tiles(nb, [&](const ListDev& L, int si, int ai, int sj, int aj) {
+    walk_tiles(nb, [&](const ListDev& L, int, int si, int ai, int sj, int aj) {
         const float4 pi = L.sposq[si];
         const double qi = ai >= 0 ? gb.prefactor*gb.charge[ai] : 0.0, bi = ai >= 0 ? gb.bornR[ai] : 1.0;
         float4 pj = L.sposq[max(sj, 0)];
@@ -175,7 +133,7 @@ __global__ void __launch_bounds__(256) k_gb_pairs(NbDev nb, GbsaDev gb) {
         double fix = 0.0, fiy = 0.0, fiz = 0.0, fjx = 0.0, fjy = 0.0, fjz = 0.0, dI = 0.0, dJ = 0.0;
         for (int k = 0; k < 32; k++) {
             if (ai >= 0 && sj > si) {
-                const double3 d = gb_delta(nb.box, pi, pj);
+                const double3 d = tile_delta(nb.box, pi, pj);
                 const double r2 = d.x*d.x + d.y*d.y + d.z*d.z;
                 if (!gb.useCutoff || r2 <= gb.cutoff2) {
                     const double a2 = bi*bj, D = 0.25*r2/a2, ex = exp(-D);
@@ -218,7 +176,7 @@ __global__ void __launch_bounds__(256) k_gb_fold(NbDev nb, GbsaDev gb) {
 // pass 5: the forces of the chain rule through the Born sums of both atoms of every pair
 __global__ void __launch_bounds__(256) k_gb_chain(NbDev nb, GbsaDev gb) {
     const int src = ((threadIdx.x & 31) + 1) & 31;
-    gb_tiles(nb, [&](const ListDev& L, int si, int ai, int sj, int aj) {
+    walk_tiles(nb, [&](const ListDev& L, int, int si, int ai, int sj, int aj) {
         const float4 pi = L.sposq[si];
         const double2 ri = ai >= 0 ? gb.radius[ai] : make_double2(1.0, 0.0);
         const double bfi = ai >= 0 ? gb.bornForce[ai] : 0.0;
@@ -228,7 +186,7 @@ __global__ void __launch_bounds__(256) k_gb_chain(NbDev nb, GbsaDev gb) {
         double fix = 0.0, fiy = 0.0, fiz = 0.0, fjx = 0.0, fjy = 0.0, fjz = 0.0;
         for (int k = 0; k < 32; k++) {
             if (ai >= 0 && sj > si) {
-                const double3 d = gb_delta(nb.box, pi, pj);
+                const double3 d = tile_delta(nb.box, pi, pj);
                 const double r2 = d.x*d.x + d.y*d.y + d.z*d.z;
                 if (!gb.useCutoff || r2 <= gb.cutoff2) {
                     const double r = sqrt(r2), rInv = 1.0/r, r2Inv = rInv*rInv;

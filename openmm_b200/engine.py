@@ -8,13 +8,14 @@ from .systems import SystemDesc, NB_PME
 TERM_BONDS, TERM_ANGLES, TERM_TORSIONS, TERM_NB_DIRECT, TERM_NB_RECIP = 1, 2, 4, 8, 16
 TERM_RB_TORSIONS, TERM_CMAP, TERM_CUSTOM_TORSIONS = 32, 64, 128
 TERM_CUSTOM_BONDS, TERM_CUSTOM_EXTERNALS, TERM_CUSTOM_ANGLES, TERM_CUSTOM_COMPOUND = 256, 512, 1024, 2048
-TERM_CUSTOM_CENTROID, TERM_GBSA, TERM_RMSD, TERM_CV_FORCES, TERM_ALL = 4096, 8192, 16384, 32768, 65535
+TERM_CUSTOM_CENTROID, TERM_GBSA, TERM_RMSD, TERM_CV_FORCES, TERM_CUSTOM_NONBONDED = 4096, 8192, 16384, 32768, 65536
+TERM_ALL = 131071
 # kinds of b200md_set_bonded_groups
 BONDED_KINDS = {"bonds": 0, "angles": 1, "torsions": 2, "rb_torsions": 3, "cmap": 4, "custom_torsions": 5, "custom_bonds": 6,
                 "custom_externals": 7, "custom_angles": 9, "custom_compound": 10, "custom_centroid": 11}
 PHASES = {"pair": 0, "pme_spread": 1, "pme_fft_conv": 2, "pme_gather": 3, "integrate": 4, "list_build": 5, "bonded": 6,
           "custom_torsions": 7, "custom_compound": 8, "custom_centroid": 9, "gbsa": 10, "list_prep": 11, "list_tiles": 12,
-          "rmsd": 13}
+          "rmsd": 13, "custom_nonbonded": 14}
 
 
 class EngineError(RuntimeError):
@@ -145,6 +146,17 @@ class Engine:
             self._ck(L.b200md_set_gbsa(self.h, int(d.gb_method), float(d.cutoff), float(d.gb_solute_dielectric),
                                        float(d.gb_solvent_dielectric), float(d.gb_surface_area_energy), _dp(_f64(d.gb_charges)),
                                        _dp(_f64(d.gb_radii)), _dp(_f64(d.gb_scales))))
+        if len(d.cnb_group):
+            p = np.ascontiguousarray(d.cnb_params, dtype=np.float64)
+            ex = _i32(np.asarray(d.cnb_excl).reshape(-1, 2))
+            self._ck(L.b200md_set_custom_nonbonded(self.h, int(d.cnb_method), float(d.cnb_cutoff), len(d.cnb_group), _ip(_i32(d.cnb_prog_start)),
+                                                   _ip(_i32(d.cnb_op)), _ip(_i32(d.cnb_arg)), _dp(_f64(d.cnb_imm)), _ip(_i32(d.cnb_nparams)),
+                                                   p.shape[2], _dp(p), _dp(_f64(d.cnb_switch)), _ip(_i32(d.cnb_group)), len(ex),
+                                                   _ip(_i32(ex[:, 0])), _ip(_i32(ex[:, 1]))))
+            dims = _i32(np.asarray(d.cnb_table_dims).reshape(-1, 4))
+            self._ck(L.b200md_set_custom_tables(self.h, len(dims), _ip(dims), _ip(_i32(d.cnb_table_start)), _dp(_f64(d.cnb_table_values))))
+            if len(d.cnb_lrc):
+                self._ck(L.b200md_set_custom_nonbonded_lrc(self.h, len(d.cnb_lrc), _dp(_f64(d.cnb_lrc))))
         if d.cv_count:
             self._ck(L.b200md_set_cv_forces(self.h, int(d.cv_count)))
         if len(d.rmsd_group):
@@ -294,6 +306,17 @@ class Engine:
         if not (len(q) == len(r) == len(s)):
             raise ValueError("update_gbsa_params: charges, radii and scales differ in length")
         self._ck(self.lib.b200md_update_gbsa_params(self.h, len(q), _dp(q), _dp(r), _dp(s)))
+
+    # ---- CalcCustomNonbondedForceKernel::copyParametersToContext ----
+    def update_custom_nonbonded_params(self, params):
+        """New per-particle parameters [objects, N, stride] of the custom nonbonded objects, into the same device buffers."""
+        p = np.ascontiguousarray(params, dtype=np.float64)
+        self._ck(self.lib.b200md_update_custom_nonbonded_params(self.h, p.shape[1], _dp(p)))
+
+    def set_custom_nonbonded_lrc(self, coefficients):
+        """The long-range coefficient of every custom nonbonded object (energy += coefficient/volume)."""
+        c = _f64(coefficients)
+        self._ck(self.lib.b200md_set_custom_nonbonded_lrc(self.h, len(c), _dp(c)))
 
     # ---- CalcRMSDForceKernel::copyParametersToContext ----
     def update_rmsd(self, start, atoms, ref):

@@ -164,6 +164,28 @@ class SystemDesc:
     gb_solute_dielectric: float = 1.0
     gb_solvent_dielectric: float = 78.5
     gb_surface_area_energy: float = 2.25936
+    # CustomNonbondedForce objects (cnb_*), none when cnb_group is empty: one method (NB_NOCUTOFF, NB_CUTOFF_NONPERIODIC or
+    # NB_CUTOFF_PERIODIC), cutoff and set of excluded pairs cnb_excl [m, 2] shared by all; per object o its energy and dE/dr
+    # programs (programs 2o and 2o+1 of cnb_prog_start / op / arg / imm, class B200MD_CUSTOM_NONBONDED: the plugin's translator
+    # makes them, or they are written by hand), its number of per-particle parameters cnb_nparams[o], switching distance
+    # cnb_switch[o] (< 0: none), force group cnb_group[o] and long-range coefficient cnb_lrc[o] (energy += coefficient/volume);
+    # cnb_params [objects, N, stride]; the Discrete1D/2D/3DFunction tables: cnb_table_dims [t, 4] = (dimensions, xsize, ysize,
+    # zsize), values cnb_table_values[cnb_table_start[t]:cnb_table_start[t+1]], x fastest
+    cnb_method: int = NB_NOCUTOFF
+    cnb_cutoff: float = 1.0
+    cnb_excl: np.ndarray = field(default_factory=lambda: np.zeros((0, 2), dtype=np.int32))
+    cnb_prog_start: np.ndarray = field(default_factory=_i)
+    cnb_op: np.ndarray = field(default_factory=_i)
+    cnb_arg: np.ndarray = field(default_factory=_i)
+    cnb_imm: np.ndarray = field(default_factory=_d)
+    cnb_nparams: np.ndarray = field(default_factory=_i)
+    cnb_switch: np.ndarray = field(default_factory=_d)
+    cnb_group: np.ndarray = field(default_factory=_i)
+    cnb_lrc: np.ndarray = field(default_factory=_d)
+    cnb_params: np.ndarray = field(default_factory=lambda: np.zeros((0, 0, 0)))
+    cnb_table_dims: np.ndarray = field(default_factory=lambda: np.zeros((0, 4), dtype=np.int32))
+    cnb_table_start: np.ndarray = field(default_factory=lambda: np.zeros(1, dtype=np.int32))
+    cnb_table_values: np.ndarray = field(default_factory=_d)
     # RMSDForce objects (rmsd_*): object o is the atoms rmsd_atoms[rmsd_start[o]:rmsd_start[o+1]] with the reference position
     # rmsd_ref[k] of entry k, in force group rmsd_group[o]; no objects when rmsd_group is empty
     rmsd_start: np.ndarray = field(default_factory=_i)

@@ -10,7 +10,9 @@
 // HarmonicAngleForce, PeriodicTorsionForce, RBTorsionForce, CMAPTorsionForce, CustomTorsionForce, CustomBondForce,
 // CustomExternalForce, CustomAngleForce, CustomCompoundBondForce, CustomCentroidBondForce (any number of objects, each in its own force group; custom forces without energy parameter
 // derivatives, expressions within the limits of custom_translate.h), GBSAOBCForce (one per System, its method and cutoff
-// matching the NonbondedForce's; NoCutoff also without one), RMSDForce (any number of objects), CMMotionRemover;
+// matching the NonbondedForce's; NoCutoff also without one), RMSDForce (any number of objects), CustomNonbondedForce (any
+// number of objects sharing one method, cutoff and exclusion set, which are the NonbondedForce's when there is one; discrete
+// tables, switching function, long-range correction; no interaction groups), CMMotionRemover;
 // Verlet / Langevin / LangevinMiddle integrators; SETTLE + X-H_n SHAKE constraints; MonteCarloBarostat and
 // MonteCarloAnisotropicBarostat (ApplyMonteCarloBarostatKernel; MonteCarloMembraneBarostat is refused).  A Force class without a kernel here
 // makes Platform::supportsKernels() false; an unsupported OPTION of a supported class is rejected in contextCreated()
@@ -49,6 +51,8 @@
 #include "openmm/GBSAOBCForce.h"
 #include "openmm/RMSDForce.h"
 #include "openmm/CustomCVForce.h"
+#include "openmm/CustomNonbondedForce.h"
+#include "openmm/internal/CustomNonbondedForceImpl.h"
 #include "openmm/TabulatedFunction.h"
 #include "lepton/CustomFunction.h"
 #include "lepton/ExpressionProgram.h"
@@ -67,6 +71,7 @@
 #include "custom_translate.h"
 #include <algorithm>
 #include <map>
+#include <set>
 #include <string>
 #include <vector>
 #include <sstream>
@@ -229,6 +234,23 @@ struct PlatformData {
             start.push_back((int) atoms.size());
         }
     }
+    // CustomNonbondedForce objects in the order their kernels were initialised: programs, tables, per-particle parameters
+    // ([particle][P] per object), switching distance (-1: none), force group and long-range coefficient; the method, cutoff and
+    // excluded pairs they share (validateSystem has checked that they do)
+    CustomPrograms cnbPrograms;
+    b200md_custom::Tables cnbTables;
+    vector<vector<double> > cnbParams; vector<int> cnbNumParams, cnbGroup; vector<double> cnbSwitch, cnbLrc;
+    int cnbMethod = 0; double cnbCutoff = 0; vector<int> cnbExcl1, cnbExcl2;
+    int cnbStride() const { int s = 0; for (int p : cnbNumParams) s = max(s, p); return s; }
+    // the parameters of every object as b200md_set_custom_nonbonded takes them: [object][particle][stride]
+    vector<double> cnbPacked() const {
+        const int stride = cnbStride();
+        vector<double> p(cnbParams.size()*numParticles*stride, 0.0);
+        for (size_t o = 0; o < cnbParams.size(); o++)
+            for (int i = 0; i < numParticles; i++)
+                for (int k = 0; k < cnbNumParams[o]; k++) p[(o*numParticles + i)*stride + k] = cnbParams[o][(size_t) i*cnbNumParams[o] + k];
+        return p;
+    }
     // the programs of each custom class
     CustomPrograms customPrograms[6];
     // the global parameters the expressions of all custom classes read: slot of every name (shared by all objects) and the
@@ -278,6 +300,14 @@ struct PlatformData {
             check(b200md_set_bonded_groups(ctx, r.kind, r.size(), r.group.data()));
         }
         if (!customGlobals.empty()) check(b200md_set_custom_globals(ctx, (int) customGlobals.size(), customGlobals.data()));
+        if (!cnbGroup.empty()) {
+            const CustomPrograms& c = cnbPrograms;
+            const vector<double> par = cnbPacked();
+            check(b200md_set_custom_nonbonded(ctx, cnbMethod, cnbCutoff, (int) cnbGroup.size(), c.progStart.data(), c.op.data(), c.arg.data(),
+                                              c.imm.data(), cnbNumParams.data(), cnbStride(), par.data(), cnbSwitch.data(), cnbGroup.data(),
+                                              (int) cnbExcl1.size(), cnbExcl1.data(), cnbExcl2.data()));
+            check(b200md_set_custom_tables(ctx, cnbTables.count(), cnbTables.dims.data(), cnbTables.start.data(), cnbTables.values.data()));
+        }
         if (!rmsdGroup.empty()) {
             vector<int> start, atoms; vector<double> ref;
             rmsdArrays(start, atoms, ref);
@@ -946,6 +976,103 @@ private:
     int index = 0, numReference = 0;
 };
 
+// CustomNonbondedForce: the programs, tables, parameters and exclusions go to the engine at finalize, with those of every other
+// CustomNonbondedForce; execute() only records the term, so the step graph covers it.  The long-range correction is computed
+// on the host as ReferenceCalcCustomNonbondedForceKernel does (CutoffPeriodic only): at the first evaluation, again when a
+// global parameter the force declares changes and at copyParametersToContext; the engine adds coefficient/volume.
+class B200CalcCustomNonbondedForceKernel : public CalcCustomNonbondedForceKernel {
+public:
+    B200CalcCustomNonbondedForceKernel(string name, const Platform& platform, ContextImpl& context) : CalcCustomNonbondedForceKernel(name, platform), context(context) {}
+    ~B200CalcCustomNonbondedForceKernel() { delete forceCopy; }
+    static void read(const CustomNonbondedForce& force, vector<double>& params) {
+        const int n = force.getNumParticles(), np = force.getNumPerParticleParameters();
+        params.assign((size_t) n*np, 0.0);
+        vector<double> p;
+        for (int i = 0; i < n; i++) {
+            force.getParticleParameters(i, p);
+            for (int k = 0; k < np && k < (int) p.size(); k++) params[(size_t) i*np + k] = p[k];
+        }
+    }
+    void initialize(const System& system, const CustomNonbondedForce& force) {
+        PlatformData& d = getData(context);
+        if (d.finalized) throw OpenMMException("B200 platform: CustomNonbondedForce initialised after the Context was finalised");
+        if (force.getNumParticles() != system.getNumParticles())
+            throw OpenMMException("CustomNonbondedForce must have exactly as many particles as the System it belongs to.");
+        index = (int) d.cnbGroup.size();
+        vector<b200md_custom::Program> programs;
+        b200md_custom::translateNonbonded(force, d.customGlobalSlot, programs, d.cnbTables);
+        d.cnbPrograms.add(programs, 0, false);
+        globals.init(d, force);
+        d.cnbParams.emplace_back();
+        read(force, d.cnbParams.back());
+        d.cnbNumParams.push_back(force.getNumPerParticleParameters());
+        const CustomNonbondedForce::NonbondedMethod m = force.getNonbondedMethod();
+        d.cnbMethod = m == CustomNonbondedForce::NoCutoff ? B200MD_NB_NOCUTOFF : m == CustomNonbondedForce::CutoffNonPeriodic ?
+                      B200MD_NB_CUTOFF_NONPERIODIC : B200MD_NB_CUTOFF_PERIODIC;
+        d.cnbCutoff = force.getCutoffDistance();
+        d.cnbSwitch.push_back(m != CustomNonbondedForce::NoCutoff && force.getUseSwitchingFunction() ? force.getSwitchingDistance() : -1.0);
+        d.cnbGroup.push_back(force.getForceGroup());
+        d.cnbLrc.push_back(0.0);
+        if (index == 0)
+            for (int k = 0; k < force.getNumExclusions(); k++) {
+                int a, b;
+                force.getExclusionParticles(k, a, b);
+                d.cnbExcl1.push_back(a); d.cnbExcl2.push_back(b);
+            }
+        if (m == CustomNonbondedForce::CutoffPeriodic && force.getUseLongRangeCorrection()) {
+            forceCopy = new CustomNonbondedForce(force);
+            lrcPending = true;
+        }
+        for (int i = 0; i < force.getNumGlobalParameters(); i++) {
+            globalNames.push_back(force.getGlobalParameterName(i));
+            globalValues.push_back(force.getGlobalParameterDefaultValue(i));
+        }
+        d.systemTerms |= B200MD_TERM_CUSTOM_NONBONDED; d.bondedGroupsUsed |= 1u << force.getForceGroup();
+    }
+    double execute(ContextImpl& context, bool includeForces, bool includeEnergy) {
+        PlatformData& d = getData(context);
+        globals.send(d, context);
+        for (size_t i = 0; i < globalNames.size(); i++) {
+            const double v = context.getParameter(globalNames[i]);
+            if (v != globalValues[i]) { globalValues[i] = v; lrcPending = lrcPending || forceCopy != nullptr; }
+        }
+        if (lrcPending) sendLongRangeCorrection(d, context);
+        d.pendingTerms |= B200MD_TERM_CUSTOM_NONBONDED;
+        return 0.0;
+    }
+    void copyParametersToContext(ContextImpl& context, const CustomNonbondedForce& force) {
+        PlatformData& d = getData(context);
+        d.ensureFinalized();
+        d.dropForces();
+        if (force.getNumParticles() != d.numParticles) throw OpenMMException("updateParametersInContext: The number of particles has changed");
+        if (force.getNumPerParticleParameters() != d.cnbNumParams[index])
+            throw OpenMMException("updateParametersInContext: The number of per-particle parameters has changed");
+        read(force, d.cnbParams[index]);
+        const vector<double> par = d.cnbPacked();
+        d.check(b200md_update_custom_nonbonded_params(d.ctx, d.numParticles, par.data()));
+        if (forceCopy != nullptr) {
+            // a new deep copy: CustomNonbondedForce's assignment would share the tabulated functions, which both then delete
+            delete forceCopy;
+            forceCopy = new CustomNonbondedForce(force);
+            sendLongRangeCorrection(d, context);
+        }
+    }
+private:
+    // CustomNonbondedForceImpl::calcLongRangeCorrection at the Context's current global parameter values
+    void sendLongRangeCorrection(PlatformData& d, ContextImpl& context) {
+        vector<double> derivatives;
+        CustomNonbondedForceImpl::calcLongRangeCorrection(*forceCopy, context.getOwner(), d.cnbLrc[index], derivatives);
+        lrcPending = false;
+        d.check(b200md_set_custom_nonbonded_lrc(d.ctx, (int) d.cnbLrc.size(), d.cnbLrc.data()));
+    }
+    ContextImpl& context;
+    int index = 0;                                  // this object among the Context's CustomNonbondedForce objects
+    CustomNonbondedForce* forceCopy = nullptr;      // for the long-range correction (CutoffPeriodic with it on)
+    bool lrcPending = false;
+    vector<string> globalNames; vector<double> globalValues;
+    ObjectGlobals globals;
+};
+
 // CustomCVForce: CustomCVForceImpl (the reference's, untouched) builds an inner System of the collective variables, one force
 // group each, and a linked Context on this platform, so the inner Context is an ordinary engine on the same device.  execute()
 // copies the state to it on the device, evaluates each variable's group there and snapshots its forces into the outer
@@ -1158,6 +1285,7 @@ public:
         if (name == CalcCustomCentroidBondForceKernel::Name()) return new B200CalcCustomForceKernel<CustomCentroids>(name, platform, context);
         if (name == CalcGBSAOBCForceKernel::Name()) return new B200CalcGBSAOBCForceKernel(name, platform, context);
         if (name == CalcRMSDForceKernel::Name()) return new B200CalcRMSDForceKernel(name, platform, context);
+        if (name == CalcCustomNonbondedForceKernel::Name()) return new B200CalcCustomNonbondedForceKernel(name, platform, context);
         if (name == CalcCustomCVForceKernel::Name()) return new B200CalcCustomCVForceKernel(name, platform, context);
         if (name == RemoveCMMotionKernel::Name()) return new B200RemoveCMMotionKernel(name, platform, context);
         if (name == IntegrateVerletStepKernel::Name()) return new B200IntegrateVerletStepKernel(name, platform);
@@ -1177,7 +1305,8 @@ public:
                                 CalcPeriodicTorsionForceKernel::Name(), CalcRBTorsionForceKernel::Name(), CalcCMAPTorsionForceKernel::Name(),
                                 CalcCustomTorsionForceKernel::Name(), CalcCustomBondForceKernel::Name(), CalcCustomExternalForceKernel::Name(),
                                 CalcCustomAngleForceKernel::Name(), CalcCustomCompoundBondForceKernel::Name(), CalcCustomCentroidBondForceKernel::Name(),
-                                CalcGBSAOBCForceKernel::Name(), CalcRMSDForceKernel::Name(), CalcCustomCVForceKernel::Name(), RemoveCMMotionKernel::Name(), IntegrateVerletStepKernel::Name(),
+                                CalcGBSAOBCForceKernel::Name(), CalcRMSDForceKernel::Name(), CalcCustomCVForceKernel::Name(), CalcCustomNonbondedForceKernel::Name(),
+                                RemoveCMMotionKernel::Name(), IntegrateVerletStepKernel::Name(),
                                 IntegrateLangevinStepKernel::Name(), IntegrateLangevinMiddleStepKernel::Name(), ApplyMonteCarloBarostatKernel::Name()})
             registerKernelFactory(n, factory);
         platformProperties.push_back(DeviceIndex());
@@ -1241,6 +1370,66 @@ public:
             if (!(r > 0.009)) throw OpenMMException("B200 platform: a GBSAOBCForce radius at or below the dielectric offset (0.009 nm)");
         }
     }
+    // A CustomNonbondedForce on its own: interaction groups, energy parameter derivatives, continuous tables, more than 8
+    // per-particle parameters and programs beyond the interpreter's limits are refused (an unknown variable is left to the
+    // kernel's initialize, as for the other custom forces)
+    static void validateCustomNonbonded(const System& system, const CustomNonbondedForce& force) {
+        if (force.getNumInteractionGroups() > 0) throw OpenMMException("B200 platform: interaction groups of a CustomNonbondedForce are not supported");
+        if (force.getNumEnergyParameterDerivatives() > 0)
+            throw OpenMMException("B200 platform: energy parameter derivatives of a CustomNonbondedForce are not supported");
+        if (force.getNumParticles() != system.getNumParticles())
+            throw OpenMMException("CustomNonbondedForce must have exactly as many particles as the System it belongs to.");
+        map<string, int> slots;
+        vector<b200md_custom::Program> programs;
+        b200md_custom::Tables tables;
+        try { b200md_custom::translateNonbonded(force, slots, programs, tables); }
+        catch (const b200md_custom::Unsupported&) { throw; }
+        catch (const OpenMMException&) {}
+    }
+    // the excluded pairs of a CustomNonbondedForce, or the exception pairs of a NonbondedForce, as a set
+    static set<pair<int, int> > pairSet(const CustomNonbondedForce* c, const NonbondedForce* n) {
+        set<pair<int, int> > s;
+        const int count = c ? c->getNumExclusions() : n->getNumExceptions();
+        for (int k = 0; k < count; k++) {
+            int a, b;
+            double q, sig, eps;
+            if (c) c->getExclusionParticles(k, a, b);
+            else n->getExceptionParameters(k, a, b, q, sig, eps);
+            s.insert(make_pair(min(a, b), max(a, b)));
+        }
+        return s;
+    }
+    // The CustomNonbondedForce objects together: the pair kernel walks one neighbour list, so they share one method, one cutoff
+    // and one exclusion set, and with a NonbondedForce those are its method (CutoffPeriodic with CutoffPeriodic or PME), its
+    // cutoff and its exception pairs, from which the list's masks are built.  Without one the list is built at the custom
+    // force's method and cutoff, which a GBSAOBCForce (at NoCutoff) can share only at NoCutoff.
+    static void validateCustomNonbondedSet(const vector<const CustomNonbondedForce*>& forces, const NonbondedForce* nonbonded,
+                                           const GBSAOBCForce* gbsa) {
+        const CustomNonbondedForce& first = *forces[0];
+        const CustomNonbondedForce::NonbondedMethod m = first.getNonbondedMethod();
+        const set<pair<int, int> > excl = pairSet(&first, nullptr);
+        for (const CustomNonbondedForce* f : forces) {
+            if (f->getNonbondedMethod() != m || (m != CustomNonbondedForce::NoCutoff && f->getCutoffDistance() != first.getCutoffDistance()))
+                throw OpenMMException("B200 platform: CustomNonbondedForce objects with different methods or cutoffs are not supported");
+            if (f != &first && pairSet(f, nullptr) != excl)
+                throw OpenMMException("B200 platform: CustomNonbondedForce objects with different exclusions are not supported");
+        }
+        if (!nonbonded) {
+            // the list is then the custom force's own; a GBSAOBCForce (NoCutoff here, validateGBSA) needs every pair in it
+            if (gbsa && m != CustomNonbondedForce::NoCutoff)
+                throw OpenMMException("B200 platform: a GBSAOBCForce beside a CustomNonbondedForce with a cutoff needs a NonbondedForce");
+            return;
+        }
+        const NonbondedForce::NonbondedMethod n = nonbonded->getNonbondedMethod();
+        const bool match = m == CustomNonbondedForce::NoCutoff ? n == NonbondedForce::NoCutoff :
+                           m == CustomNonbondedForce::CutoffNonPeriodic ? n == NonbondedForce::CutoffNonPeriodic :
+                           (n == NonbondedForce::CutoffPeriodic || n == NonbondedForce::PME);
+        if (!match) throw OpenMMException("B200 platform: the CustomNonbondedForce's nonbonded method does not match the NonbondedForce's");
+        if (m != CustomNonbondedForce::NoCutoff && first.getCutoffDistance() != nonbonded->getCutoffDistance())
+            throw OpenMMException("B200 platform: the CustomNonbondedForce's cutoff differs from the NonbondedForce's");
+        if (excl != pairSet(nullptr, nonbonded))
+            throw OpenMMException("B200 platform: the CustomNonbondedForce's exclusions differ from the NonbondedForce's exceptions");
+    }
     // the Force classes this platform has a kernel for; a CustomCVForce's variables must be among them, since its inner
     // Context is created on this platform explicitly and cannot fall back on its own
     static bool hasKernel(const Force& f) {
@@ -1257,6 +1446,7 @@ public:
         int numNonbonded = 0;
         const NonbondedForce* nonbonded = nullptr;
         const GBSAOBCForce* gbsa = nullptr;
+        vector<const CustomNonbondedForce*> customNonbonded;
         for (const Force* fp : forces) {
             const Force& force = *fp;
             if (const CustomCVForce* cv = dynamic_cast<const CustomCVForce*>(&force)) {
@@ -1291,8 +1481,13 @@ public:
             if (const CustomAngleForce* f = dynamic_cast<const CustomAngleForce*>(&force)) validateCustom<CustomAngles>(*f);
             if (const CustomCompoundBondForce* f = dynamic_cast<const CustomCompoundBondForce*>(&force)) validateCustom<CustomCompounds>(*f);
             if (const CustomCentroidBondForce* f = dynamic_cast<const CustomCentroidBondForce*>(&force)) validateCustom<CustomCentroids>(*f);
+            if (const CustomNonbondedForce* f = dynamic_cast<const CustomNonbondedForce*>(&force)) {
+                validateCustomNonbonded(system, *f);
+                customNonbonded.push_back(f);
+            }
         }
         if (gbsa) validateGBSA(system, *gbsa, nonbonded);
+        if (!customNonbonded.empty()) validateCustomNonbondedSet(customNonbonded, nonbonded, gbsa);
     }
     static void validateSystem(const System& system) {
         for (int i = 0; i < system.getNumParticles(); i++)

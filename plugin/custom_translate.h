@@ -1,6 +1,6 @@
 // custom_translate.h -- CustomTorsionForce, CustomBondForce, CustomExternalForce, CustomAngleForce,
-// CustomCompoundBondForce and CustomCentroidBondForce expressions -> the instruction programs of b200md_set_custom_torsions /
-// _bonds / _externals / _angles / _compound / _centroid (B200MD_OP_*, include/b200md.h).  Lepton, part of the host's
+// CustomCompoundBondForce, CustomCentroidBondForce and CustomNonbondedForce expressions -> the instruction programs of
+// b200md_set_custom_torsions / _bonds / _externals / _angles / _compound / _centroid / _nonbonded (B200MD_OP_*, include/b200md.h).  Lepton, part of the host's
 // libOpenMM.so, parses, optimises and differentiates the expression exactly as the Reference platform does
 // (ReferenceCalcCustom{Torsion,Bond,External,Angle,CompoundBond,CentroidBond}ForceKernel::initialize) and makes the stack program
 // (ExpressionProgram); this file only maps every Lepton::Operation to one instruction.  Included by the plugin
@@ -12,6 +12,8 @@
 #include "openmm/internal/CustomCompoundBondForceImpl.h"
 #include "openmm/CustomCentroidBondForce.h"
 #include "openmm/internal/CustomCentroidBondForceImpl.h"
+#include "openmm/CustomNonbondedForce.h"
+#include "openmm/TabulatedFunction.h"
 #include "lepton/CustomFunction.h"
 #include "lepton/ExpressionProgram.h"
 #include "lepton/Operation.h"
@@ -21,6 +23,10 @@
 #include <map>
 #include <string>
 #include <vector>
+
+// the Reference platform's evaluation of a TabulatedFunction as a Lepton function, exported by libOpenMM.so
+// (platforms/reference/include/ReferenceTabulatedFunction.h)
+extern "C" Lepton::CustomFunction* createReferenceTabulatedFunction(const OpenMM::TabulatedFunction& function);
 
 namespace b200md_custom {
 
@@ -65,10 +71,13 @@ private:
 // custom force; a name seen for the first time gets the next slot).  Any other variable is an error, as on the Reference
 // platform.  periodicdistance and its first derivatives -> PERIODIC_DIST, pointdistance / pointangle / pointdihedral and
 // theirs -> POINT_DIST / POINT_ANGLE / POINT_DIHEDRAL (the parser knows these names only for the classes that have them).
-// forceName names the class in messages; maxStack is the stack capacity of the class's interpreter.
+// forceName names the class in messages; maxStack is the stack capacity of the class's interpreter.  tables (a custom nonbonded
+// force's): the name of every discrete tabulated function -> (its table index, its number of arguments); it becomes DISCRETE1..3
+// with the table as operand, any derivative of it DISCRETE with operand -1 (the value 0).
 inline Program translateProgram(const Lepton::ExpressionProgram& prog, const std::vector<std::string>& variables, const std::string& forceName,
                                 const std::vector<std::string>& paramNames, const std::vector<std::string>& globalNames,
-                                std::map<std::string, int>& globalSlot, int maxStack = B200MD_CUSTOM_MAX_STACK) {
+                                std::map<std::string, int>& globalSlot, int maxStack = B200MD_CUSTOM_MAX_STACK,
+                                const std::map<std::string, std::pair<int, int> >* tables = nullptr) {
     typedef Lepton::Operation Op;
     if (prog.getStackSize() > maxStack)
         throw Unsupported("B200 platform: a " + forceName + " expression needs a stack deeper than " + std::to_string(maxStack));
@@ -99,6 +108,15 @@ inline Program translateProgram(const Lepton::ExpressionProgram& prog, const std
             }
             case Op::CUSTOM: {
                 const std::string& fn = o.getName();
+                if (tables && tables->count(fn)) {
+                    const std::pair<int, int>& t = tables->at(fn);
+                    const std::vector<int>& order = dynamic_cast<const Op::Custom&>(o).getDerivOrder();
+                    bool deriv = false;
+                    for (int k : order) deriv = deriv || k != 0;
+                    code = B200MD_OP_DISCRETE1 + t.second - 1;
+                    arg = deriv ? -1 : t.first;
+                    break;
+                }
                 code = fn == "periodicdistance" ? B200MD_OP_PERIODIC_DIST : fn == "pointdistance" ? B200MD_OP_POINT_DIST :
                        fn == "pointangle" ? B200MD_OP_POINT_ANGLE : fn == "pointdihedral" ? B200MD_OP_POINT_DIHEDRAL : -1;
                 if (code < 0)
@@ -161,12 +179,13 @@ namespace detail {
 // .optimize()).  The global slots new names take are committed to globalSlot only when every program translates.
 inline void translatePrograms(const Lepton::ParsedExpression& expr, const std::vector<std::string>& variables, const std::string& forceName,
                               int maxStack, const std::vector<std::string>& paramNames, const std::vector<std::string>& globalNames,
-                              std::map<std::string, int>& globalSlot, std::vector<Program>& programs) {
+                              std::map<std::string, int>& globalSlot, std::vector<Program>& programs,
+                              const std::map<std::string, std::pair<int, int> >* tables = nullptr) {
     std::map<std::string, int> slots = globalSlot;
-    std::vector<Program> out(1, translateProgram(expr.createProgram(), variables, forceName, paramNames, globalNames, slots, maxStack));
+    std::vector<Program> out(1, translateProgram(expr.createProgram(), variables, forceName, paramNames, globalNames, slots, maxStack, tables));
     for (const std::string& v : variables)
         out.push_back(translateProgram(expr.differentiate(v).optimize().createProgram(), variables, forceName, paramNames, globalNames, slots,
-                                       maxStack));
+                                       maxStack, tables));
     programs.swap(out);
     globalSlot.swap(slots);
 }
@@ -232,6 +251,59 @@ inline void translateCentroid(const OpenMM::CustomCentroidBondForce& force, std:
     for (int i = 0; i < force.getNumGlobalParameters(); i++) globalNames.push_back(force.getGlobalParameterName(i));
     detail::translatePrograms(OpenMM::CustomCentroidBondForceImpl::prepareExpression(force, functions), variables, "CustomCentroidBondForce",
                               B200MD_CUSTOM_COMPOUND_MAX_STACK, paramNames, globalNames, globalSlot, programs);
+}
+
+// The Discrete1D/2D/3DFunction tables of b200md_set_custom_tables: table t has dims[4t] dimensions of sizes dims[4t+1 ..]
+// (unused ones 1) and the values [start[t], start[t+1]), x fastest.
+struct Tables {
+    std::vector<int> dims, start = std::vector<int>(1, 0);
+    std::vector<double> values;
+    int count() const { return (int) start.size() - 1; }
+    void add(int ndim, int xsize, int ysize, int zsize, const std::vector<double>& v) {
+        dims.insert(dims.end(), {ndim, xsize, ysize, zsize});
+        values.insert(values.end(), v.begin(), v.end());
+        start.push_back((int) values.size());
+    }
+};
+
+// A CustomNonbondedForce: the energy program and dE/dr (VAR 0 = r), with p1 of per-particle parameter k as PARAM k and p2 as
+// PARAM P+k (P parameters).  Its Discrete1D/2D/3DFunction tables are appended to `tables` and read by DISCRETE instructions;
+// for parsing (and Lepton's constant folding) they are the Reference platform's functions, as in
+// ReferenceCalcCustomNonbondedForceKernel::initialize.  Continuous functions are refused: they need splines on the device.
+inline void translateNonbonded(const OpenMM::CustomNonbondedForce& force, std::map<std::string, int>& globalSlot, std::vector<Program>& programs,
+                               Tables& tables) {
+    const int numParams = force.getNumPerParticleParameters();
+    if (numParams > B200MD_CUSTOM_MAX_PARAMS/2)
+        throw Unsupported("B200 platform: a CustomNonbondedForce with more than 8 per-particle parameters is not supported");
+    Tables mine = tables;
+    std::map<std::string, std::pair<int, int> > index;
+    for (int i = 0; i < force.getNumTabulatedFunctions(); i++) {
+        const OpenMM::TabulatedFunction& f = force.getTabulatedFunction(i);
+        std::vector<double> v;
+        int xs = 1, ys = 1, zs = 1, nd = 0;
+        if (const OpenMM::Discrete1DFunction* d = dynamic_cast<const OpenMM::Discrete1DFunction*>(&f)) { d->getFunctionParameters(v); xs = (int) v.size(); nd = 1; }
+        else if (const OpenMM::Discrete2DFunction* d = dynamic_cast<const OpenMM::Discrete2DFunction*>(&f)) { d->getFunctionParameters(xs, ys, v); nd = 2; }
+        else if (const OpenMM::Discrete3DFunction* d = dynamic_cast<const OpenMM::Discrete3DFunction*>(&f)) { d->getFunctionParameters(xs, ys, zs, v); nd = 3; }
+        else throw Unsupported("B200 platform: continuous tabulated functions in a CustomNonbondedForce expression are not supported");
+        index[force.getTabulatedFunctionName(i)] = std::make_pair(mine.count(), nd);
+        mine.add(nd, xs, ys, zs, v);
+    }
+    std::map<std::string, Lepton::CustomFunction*> functions;
+    for (int i = 0; i < force.getNumTabulatedFunctions(); i++)
+        functions[force.getTabulatedFunctionName(i)] = createReferenceTabulatedFunction(force.getTabulatedFunction(i));
+    std::vector<std::string> paramNames, globalNames;
+    for (const char* suffix : {"1", "2"})
+        for (int i = 0; i < numParams; i++) paramNames.push_back(force.getPerParticleParameterName(i) + suffix);
+    for (int i = 0; i < force.getNumGlobalParameters(); i++) globalNames.push_back(force.getGlobalParameterName(i));
+    try {
+        detail::translatePrograms(Lepton::Parser::parse(force.getEnergyFunction(), functions).optimize(), {"r"}, "CustomNonbondedForce",
+                                  B200MD_CUSTOM_MAX_STACK, paramNames, globalNames, globalSlot, programs, &index);
+    } catch (...) {
+        for (auto& f : functions) delete f.second;
+        throw;
+    }
+    for (auto& f : functions) delete f.second;
+    tables = mine;
 }
 
 } // namespace b200md_custom
